@@ -9,10 +9,11 @@ device-resident replay shard (sum-tree descent + IS weights + 7-frame window gat
 fused IQN loss, backward, (gradient all-reduce when N > 1), Adam, priority update of the sampled leaves.
 N > 1 is the data-parallel learner of config 5 (512 transitions per GPU, weak scaling).
 
-Timing: W untimed warm-up steps, then `--blocks` regions of EXACTLY K steps each, every one bracketed by barrier +
-torch.cuda.synchronize(), CUDA events on the launching stream, max over ranks; the headline is the median block.  A
-`sustained` leg (>= 3 s of steps, clocks sampled) and the end-to-end leg (pinned host batches, H2D / D2H inside the timed
-region) follow.  Inputs are larger than L2: every step draws a fresh prioritized minibatch from a multi-GB replay shard
+Timing: W untimed warm-up steps, then `--blocks` regions (default 1) of EXACTLY K steps each, every one bracketed by
+barrier + torch.cuda.synchronize(), CUDA events on the launching stream, max over ranks; the headline is the median block.
+The end-to-end leg (K steps from pinned host batches, H2D / D2H inside the timed region) follows, and on request a
+`--sustained-seconds` leg with clocks sampled.  `--dump-outputs DIR` writes what the last headline step returned
+(sampled tree indices and per-transition losses) and a fixed sample of the updated online parameters as DIR/<name>.npy.  Inputs are larger than L2: every step draws a fresh prioritized minibatch from a multi-GB replay shard
 and streams > 1 GB of activations.  Also in the line: rooflines of the hidden products (tensor), the embedding producer,
 the conv trunk and the loss kernel (HBM), the Rainbow-only (C51, configs[2]) leg, and the CPU port timed on the host cores.
 `--topology apex` (N >= 2) runs configs[3] instead: 1 learner rank + N-1 actor GPUs with sharded replay.
@@ -49,26 +50,14 @@ def make_args(device, capacity, rainbow_only=0):
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
-
-
-def ncu_traffic(key="dominant_kernel_dram_bytes_per_launch"):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of a kernel, from the committed `ncu --set full` capture
-    (profiles/r02_traffic.json, else round 1's); None if absent."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            return json.load(open(p)).get(key)
-    return None
+    """NVIDIA's H100 SXM data-sheet figures (dense bf16, HBM3) for a card allowed 700 W: the denominators of the
+    roofline fractions, not rates this benchmark has reached.  A card set to a lower power limit clocks lower."""
+    return dict(hbm=3350.0, tf=989.0, src="H100 SXM data sheet (700 W)")
 
 
 def config_dict(world, capacity):
     """The workload description shared by both arms (the driver compares them key by key)."""
-    return {"workload": "configs[1]: 1xB200 learner, synthetic 84x84x4 replay, batch=512/GPU, N=N'=64, K=32, n-step=3",
+    return {"workload": "configs[1]: 1xH100 learner, synthetic 84x84x4 replay, batch=512/GPU, N=N'=64, K=32, n-step=3",
             "batch_per_gpu": B, "global_batch": B * world, "n_tau": N_TAU, "n_tau_prime": N_TAU_P, "n_quantile": K_Q,
             "replay_capacity_per_gpu": capacity, "parallelism": f"dp{world}" if world > 1 else "single",
             "l2": "inputs larger than L2 (fresh prioritized minibatch from a %.1f GB replay shard each step; "
@@ -166,7 +155,7 @@ def run_ours(args):
         torch.cuda.synchronize()
 
     def step():
-        return learner.learn_and_update(mem)[1]
+        return learner.learn_and_update(mem)
 
     # ---- pass 1 (eager, not the headline): per-entry-point device times for the roofline section
     for _ in range(3):
@@ -208,10 +197,12 @@ def run_ours(args):
         barrier()
         e0.record()
         for _ in range(args.steps):
-            loss = step()
+            idxs, loss = step()
         e1.record()
         barrier()
         block_ms.append(parallel.allreduce_max(e0.elapsed_time(e1), dev))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, idxs, loss, learner.online_net._flat)
     launches = launches_per_step * args.steps          # kernels executed in ONE timed region (graph replays them)
     clk = clocks.stop()
     ms = float(np.median(block_ms))
@@ -247,18 +238,15 @@ def run_ours(args):
     evs = [e for e in timers["riqn_gemm_bf16_tc"] if _is_head(e[2])]
     # the weight gradient runs through the MN-major entry point (single-bf16 product): mark it as one MMA pass
     evs += [(a_, b_, tuple(g_[:4]) + (None,)) for a_, b_, g_ in timers["riqn_gemm_bf16_tc_mn"] if _is_head(g_)]
-    label = "gemm_tc_kernel (tcgen05.mma + TMA; NoisyLinear fwd x3 / dgrad / wgrad, %d launches/step)" % (len(evs) // prof_steps)
+    label = "gemm_tc_kernel (wgmma + TMA; NoisyLinear fwd x3 / dgrad / wgrad, %d launches/step)" % (len(evs) // prof_steps)
     flops = sum(2.0 * a_[0] * a_[1] * a_[2] for _, _, a_ in evs)
     passes = sum((3 if a_[4] else 1) * 2.0 * a_[0] * a_[1] * a_[2] for _, _, a_ in evs) / max(flops, 1.0)
     hms = sum(a_.elapsed_time(b_) for a_, b_, _ in evs)
     head_tf = flops / (hms * 1e-3) / 1e12 if hms > 0 else 0.0
-    # denominator: the timed blocks are tens of ms at full clocks -> the BURST cuBLAS figure (VERDICT r1 item 11); the
-    # fraction against the seconds-long sustained figure is reported beside it, with the sustained leg's own clocks
-    roof = {"kernel": label, "bound": "tensor", "achieved": head_tf, "peak": pk["tf_burst"], "unit": "TFLOP/s",
-            "frac": head_tf / pk["tf_burst"], "frac_of_sustained_peak": head_tf / pk["tf_sust"], "traffic": ncu_traffic(),
-            "peak_source": pk["src"] + " bf16 burst (cuBLAS best-of-10; fp16 and bf16 share the tensor rate)",
+    roof = {"kernel": label, "bound": "tensor", "achieved": head_tf, "peak": pk["tf"], "unit": "TFLOP/s",
+            "frac": head_tf / pk["tf"], "peak_source": pk["src"] + ", dense bf16 (fp16 and bf16 share the tensor rate)",
             "share_of_step": hms / (eager_ms * prof_steps), "mma_passes": passes,
-            "tensor_pipe_frac": passes * head_tf / pk["tf_burst"], "precision": dict(_model.PRECISION),
+            "tensor_pipe_frac": passes * head_tf / pk["tf"], "precision": dict(_model.PRECISION),
             "us_per_launch": hms * 1e3 / max(len(evs), 1), "timed": "CUDA events around each launch, eager pass"}
     # HBM-bound producers (VERDICT r1 missing 6): algorithmic bytes per SURVEY 8d / measured launch time
     ek = timers["riqn_quantile_embed_fwd_tc"]
@@ -269,9 +257,9 @@ def run_ours(args):
         emb_bytes += 2.0 * images * nq * bsz * FEAT + 4.0 * nq * bsz + 4.0 * bsz * FEAT + 4.0 * (64 * FEAT + FEAT)
         emb_ms += a_.elapsed_time(b_)
     emb_gbs = emb_bytes / (emb_ms * 1e-3) / 1e9 if emb_ms > 0 else 0.0
-    roof_embed = {"kernel": "riqn_quantile_embed_fwd_tc (cos + tcgen05 product + Hadamard epilogue writing the head's operand "
+    roof_embed = {"kernel": "riqn_quantile_embed_fwd_tc (cos + wgmma product + Hadamard epilogue writing the head's operand "
                             "images; 3 launches/step)", "bound": "hbm", "achieved": emb_gbs, "peak": pk["hbm"], "unit": "GB/s",
-                  "frac": emb_gbs / pk["hbm"], "traffic": ncu_traffic("embed_kernel_dram_bytes_per_launch"),
+                  "frac": emb_gbs / pk["hbm"],
                   "algorithmic_bytes_per_step": emb_bytes / prof_steps, "ms_per_step": emb_ms / prof_steps,
                   "formula": "2*images*Nq*B*F + 4*Nq*B + 4*B*F + 4*(E*F+F)  (SURVEY 8d, materialised output)"}
     cv_ms = sum(a_.elapsed_time(b_) for a_, b_, _ in timers["riqn_conv_fwd_strip"]) + \
@@ -280,7 +268,7 @@ def run_ours(args):
     cv_bytes = n_trunks * (B * 4 * 7056 + 4.0 * B * FEAT)                # uint8 frame stack in, fp32 features out
     cv_gbs = cv_bytes / (cv_ms * 1e-3) / 1e9 if cv_ms > 0 else 0.0
     roof_conv = {"kernel": "conv trunk forward (riqn_s2d_u8 + riqn_conv_fwd_strip: 3 network passes in 6 launches per step)", "bound": "hbm",
-                 "achieved": cv_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": cv_gbs / pk["hbm"], "traffic": None,
+                 "achieved": cv_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": cv_gbs / pk["hbm"],
                  "algorithmic_bytes_per_step": cv_bytes / prof_steps, "ms_per_step": cv_ms / prof_steps,
                  "formula": "B*4*7056 (uint8 frames) + 4*B*3136 (features) per pass: intermediates are not algorithmic"}
     lk = per["riqn_iqn_loss_fwd_bwd"]
@@ -288,7 +276,7 @@ def run_ours(args):
     loss_us = lk["ms_total"] * 1e3 / max(lk["calls"], 1)
     roof_loss = {"kernel": "riqn_iqn_loss_fwd_bwd", "bound": "hbm", "achieved": loss_bytes / (loss_us * 1e-6) / 1e9,
                  "peak": pk["hbm"], "unit": "GB/s", "frac": loss_bytes / (loss_us * 1e-6) / 1e9 / pk["hbm"],
-                 "traffic": None, "us_per_launch": loss_us, "algorithmic_bytes": loss_bytes,
+                 "us_per_launch": loss_us, "algorithmic_bytes": loss_bytes,
                  "note": "0.54 MB per launch: latency-bound at B=512 (SURVEY 8d note)"}
     roof_loss_4096 = loss_kernel_point(dev, 4096, pk) if rank == 0 else None
 
@@ -331,7 +319,7 @@ def run_ours(args):
     out = {
         "metric": METRIC, "value": value, "unit": "grad-steps/s", "n_gpus": world, "steps": args.steps,
         "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": None, "dtype": "%s fwd / %s bwd tensor-core products, fp32 accumulate in TMEM; fp32 elsewhere" % (_model.PRECISION["fwd"], _model.PRECISION["bwd"]), "data": "synthetic", "impl": "ours",
+        "vs_baseline": None, "dtype": "%s fwd / %s bwd tensor-core products, fp32 accumulate; fp32 elsewhere" % (_model.PRECISION["fwd"], _model.PRECISION["bwd"]), "data": "synthetic", "impl": "ours",
         "config": config_dict(world, args.replay_capacity),
         "blocks": {"n": len(block_ms), "steps_per_block": args.steps, "ms": block_ms, "min_ms_per_step": min(block_ms) / args.steps,
                    "max_ms_per_step": max(block_ms) / args.steps, "headline": "median block"},
@@ -357,6 +345,19 @@ def run_ours(args):
     if rank == 0:
         print(json.dumps(out))
     finish(world)
+
+
+def dump_outputs(out_dir, idxs, loss, flat_params, n_sample=1 << 20):
+    """What the last timed step handed back: the sampled tree indices and per-transition losses (float64 / float32),
+    and a fixed, seeded sample of the updated online parameter arena (float32, 4 MB), for output-by-output comparison
+    of two builds run with the same arguments."""
+    os.makedirs(out_dir, exist_ok=True)
+    flat = flat_params.detach().float().cpu()
+    pick = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n_sample].sort().values
+    arrays = {"tree_idxs": idxs.detach().cpu().double().numpy(), "loss": loss.detach().float().cpu().numpy(),
+              "online_params_sample": flat[pick].numpy(), "online_params_sample_index": pick.double().numpy()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def finish(world):
@@ -430,7 +431,7 @@ def c51_leg(dev, args):
             learner.learn_and_update(mem)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    n = max(args.steps, 20)
+    n = args.steps
     e0.record()
     for _ in range(n):
         loss = learner.learn_and_update(mem)[1]
@@ -438,7 +439,7 @@ def c51_leg(dev, args):
     torch.cuda.synchronize()
     assert torch.isfinite(loss).all()
     ms = e0.elapsed_time(e1) / n
-    return {"workload": "configs[2]: 1xB200 Rainbow-only (C51, 51 atoms), batch=512, n-step=3", "ms_per_step": ms,
+    return {"workload": "configs[2]: 1xH100 Rainbow-only (C51, 51 atoms), batch=512, n-step=3", "ms_per_step": ms,
             "value": 1000.0 / ms, "unit": "grad-steps/s", "steps": n, "mode": mode, "replay_capacity": cap}
 
 
@@ -480,7 +481,7 @@ def run_apex(args):
         nonlocal states
         # all ranks: ONE gather of the shards' (pre-sampled, packed) parts; the GPUs are otherwise idle at this point, so the
         # collective does not compete with the persistent GEMMs for SMs (a side-stream prefetch under the learner's step
-        # measured 7.5 ms/step on 8 GPUs: NCCL's CTAs wait for the 148-CTA kernels to end)
+        # waits: NCCL's CTAs cannot start until the one-CTA-per-SM kernels end)
         batch = topo.sample(mem, beta=0.4, device=dev)
         if topo.is_learner:
             _, _, st, ac, rt, nx, nt, w = batch
@@ -680,11 +681,15 @@ def main():
     ap.add_argument("--actor-envs", type=int, default=128, help="apex: environments per actor GPU")
     ap.add_argument("--actor-buffer", type=int, default=200, help="apex: steps per actor buffer flush (reference: 1000)")
     ap.add_argument("--acts-per-step", type=int, default=1, help="apex: batched acting iterations per learner step")
-    ap.add_argument("--blocks", type=int, default=5, help="timed regions of --steps steps each; the median is the headline")
-    ap.add_argument("--sustained-seconds", type=float, default=3.0, help="length of the sustained leg (0 = skip)")
+    ap.add_argument("--blocks", type=int, default=1, help="timed regions of --steps steps each; the median is the headline")
+    ap.add_argument("--sustained-seconds", type=float, default=0.0, help="length of the sustained leg (0 = skip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--no-graph", action="store_true", help="eager launches instead of CUDA-graph replay")
     ap.add_argument("--max-seconds", type=int, default=900, help="watchdog: abort the process after this long")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.topology == "apex"):
+        ap.error("--dump-outputs writes the outputs of the data-parallel learner step (--impl ours --topology dp)")
     watchdog(args.max_seconds)
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* riqn_b200.h -- C-ABI of the B200-native Rainbow-IQN Ape-X learner hot path.
+/* riqn_b200.h -- C-ABI of the H100-native (sm_90a) Rainbow-IQN Ape-X learner hot path.
  *
  * The reference (valeoai/rainbow-iqn-apex) is pure Python/PyTorch and has no FFI or operator registry:
  * its boundary for this path is the Python class surface Agent / Learner / DQN / NoisyLinear /
@@ -7,16 +7,21 @@
  * re-creates the reference classes on top.
  *
  * Conventions
- *   - every function returns 0 on success or a cudaError_t value; nothing is allocated inside, all
- *     buffers are caller-owned DEVICE pointers unless stated; work is enqueued on `stream`
- *     (a cudaStream_t passed as void*) and is stream-ordered, re-entrant per stream;
+ *   - every function returns 0 on success or a cudaError_t value; all buffers are caller-owned DEVICE pointers
+ *     unless stated; work is enqueued on `stream` (a cudaStream_t passed as void*) and is stream-ordered,
+ *     re-entrant per stream.  The only memory a call takes itself is temporary scratch for partial sums, allocated
+ *     from the device's stream-ordered pool on `stream` and released on `stream` before the call returns
+ *     (cudaMallocAsync / cudaFreeAsync): no host synchronisation, no state shared between calls or streams, and
+ *     inside a CUDA graph capture it becomes part of the graph;
+ *   - results are bitwise reproducible: no sum across thread blocks uses float atomics (except in the fp32
+ *     CUDA-core cross-check GEMM and the col2im of riqn_conv_bwd / riqn_conv_bwd_tc);
  *   - fp32 tensors row-major.  tau, q and dtheta use the reference's quantile-major rows r = q * batch + b
  *     (rainbowiqn/model.py:149, compute_loss_iqn.py:238-310); the head-internal matrices (cos, x, h, dh, dz and
  *     their bf16 images) use sample-major rows r' = b * num_quantiles + q, which makes the Hadamard operand
  *     feat[b,:] a warp-broadcast and the reduction over a sample's quantiles contiguous;
  *   - `long long*` index buffers are int64 like the reference's torch.int64 / numpy int64.
  *
- * Each entry point cites the reference code it replaces (paths relative to /root/reference).
+ * Each entry point cites the reference code it replaces (paths relative to the reference repository).
  */
 #ifndef RIQN_B200_H
 #define RIQN_B200_H
@@ -31,7 +36,7 @@ extern "C" {
 int riqn_version(void);
 /* Number of CUDA kernels this library has launched in this process (bench.py's gpu_launches). */
 long long riqn_launch_count(void);
-/* 1 if the running device is compute capability 10.x (sm_100a cubins only), else 0; <0 on CUDA error. */
+/* 1 if the running device is compute capability 9.x (sm_90a cubins only), else 0; <0 on CUDA error. */
 int riqn_device_ok(void);
 
 /* Per-step scalars that change from one learner step to the next, kept in DEVICE memory so that a whole step can be
@@ -73,7 +78,7 @@ int riqn_conv_bwd(const riqn_conv_geom* g, const float* dout, const float* out, 
 /* fp32 im2col alone: col (B*OH*OW, Cin*KH*KW), the workspace riqn_conv_bwd expects. */
 int riqn_im2col_f32(const riqn_conv_geom* g, const void* in, int in_is_u8, float* col, void* stream);
 
-/* Tensor-core variants (tcgen05 GEMM on bf16 im2col operands written straight from the uint8 / fp32 input).
+/* Tensor-core variants (wgmma GEMM on bf16 im2col operands written straight from the uint8 / fp32 input).
  * w_hi / w_lo: bf16 images of the (Cout, Cin*KH*KW) weight (riqn_split_bf16); col_lo == NULL selects the
  * single-bf16 product, otherwise split-bf16 x3 (fp32-faithful).  col_hi/col_lo (M, K) bf16 workspaces; colT_hi
  * (K, M), if non-NULL, is also written for riqn_conv_bwd_tc (needs B*OH*OW % 8 == 0). */
@@ -205,7 +210,7 @@ int riqn_quantile_embed_bwd(int batch, int num_quantiles, int embed_dim, int fea
                             const float* feat, const float* cosv, float* dx_inout, float* dfeat, float* grad_iqn_w,
                             float* grad_iqn_b, void* stream);
 
-/* Tensor-core variants.  Forward: the tcgen05 GEMM's epilogue applies relu / bias / the Hadamard with feat and writes
+/* Tensor-core variants.  Forward: the wgmma GEMM's epilogue applies relu / bias / the Hadamard with feat and writes
  * the bf16 operand images of x directly: x_hi, x_lo (rows, feat_dim) for the NoisyLinear product, x_hi_t / x_lo_t
  * (feat_dim, rows) for its weight gradient in the cross-check arithmetic modes (each may be NULL; the transposed images
  * are split from x32 by a second launch and therefore need x32 != NULL); x32 (may be NULL) is the fp32 matrix.  cos_hi / cos_lo
@@ -359,7 +364,7 @@ int riqn_frame_gather(int batch, int actor_capacity, int history, int n_step, co
                       long long* actions, float* returns, float* nonterminals, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Tensor-core building blocks of the NoisyLinear products (tcgen05.mma + TMA; csrc/gemm_tc.cu).
+ * Tensor-core building blocks of the NoisyLinear products (wgmma + TMA; csrc/gemm_tc.cu).
  * ---------------------------------------------------------------------------------------------- */
 /* fp32 (rows, cols) -> bf16 hi and lo = bf16(x - hi) (either may be NULL); hi_t / lo_t (may be NULL) receive the
  * transposed (cols, rows) copies the weight-gradient product consumes. */
@@ -379,7 +384,7 @@ typedef struct riqn_split_job {
   void* hi_t;
 } riqn_split_job;
 int riqn_split_bf16_multi(int n_jobs, const riqn_split_job* jobs, void* stream);
-/* C (+)= A B^T with A (M,K), B (N,K) row-major bf16, K % 8 == 0, fp32 accumulation in TMEM.  a_lo/b_lo non-NULL
+/* C (+)= A B^T with A (M,K), B (N,K) row-major bf16, K % 8 == 0, fp32 accumulation in registers.  a_lo/b_lo non-NULL
  * selects the split-bf16 x3 (fp32-faithful) product.  epilogue: 0 store, 1 relu(acc+bias[n]), 2 atomicAdd into C,
  * 3 atomicAdd into C and acc*eps[m,n] into out2 (NoisyLinear dmu / dsigma).  split_k > 1 needs 2 or 3.
  * c_t_bf16 / c_bf16 (may be NULL; epilogue 1 only): bf16 transposed (N, M) / row-major (M, N) images of the result. */
@@ -387,8 +392,8 @@ int riqn_gemm_bf16_tc(int M, int N, int K, const void* a_hi, const void* a_lo, c
                       float* c, long ldc, int epilogue, const float* bias, float* out2, const float* eps, int split_k,
                       void* c_t_bf16, void* c_bf16, int fmt, void* stream);
 /* fmt (both GEMM entry points): 0 = both operand images hold bf16, 3 = both hold fp16 (single-pass: a_lo == b_lo == NULL).
- * 1 / 2 (mixed) are rejected: tcgen05 kind::f16 raises an illegal-instruction fault when A and B formats differ. */
-/* Products whose B operand is (K, N) row-major bf16 (MN-major tcgen05 operand, N % 8 == 0) -- no transposed copies:
+ * 1 / 2 (mixed) are rejected: wgmma takes a single 16-bit format for A and B. */
+/* Products whose B operand is (K, N) row-major bf16 (MN-major wgmma operand, N % 8 == 0) -- no transposed copies:
  *   a_is_km != 0: C (+)= A^T B with A (K, M) row-major (M % 8 == 0): the reduction runs over the ROWS of both, i.e. a
  *                 weight gradient dW = dY^T X straight from the row-major activations;
  *   a_is_km == 0: C (+)= A B with A (M, K) row-major (K % 8 == 0): a data gradient dX = dY W from the untransposed W.

@@ -1,9 +1,9 @@
-"""rainbow_iqn_apex_b200 -- B200-native (sm_100a) learner hot path of Rainbow-IQN Ape-X.
+"""rainbow_iqn_apex_b200 -- H100-native (sm_90a) learner hot path of Rainbow-IQN Ape-X.
 
 Same class surface as the reference package ``rainbowiqn`` for this path (SURVEY.md section 8b):
 ``Agent`` / ``Learner`` / ``Actor``, ``DQN`` / ``NoisyLinear``, ``ReplayMemory`` (= ReplayRedisMemory).
 All arithmetic runs in hand-written CUDA kernels behind the C-ABI of include/riqn_b200.h; importing this
-package never falls back to PyTorch or the CPU -- without the built library or a B200 it raises.
+package never falls back to PyTorch or the CPU -- without the built library or an H100 it raises.
 """
 from . import _lib  # noqa: F401
 from .model import DQN, NoisyLinear  # noqa: F401

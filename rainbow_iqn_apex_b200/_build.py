@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library (sm_100a only).  `python -m rainbow_iqn_apex_b200._build`."""
+"""In-tree build of the CUDA library (sm_90a only).  `python -m rainbow_iqn_apex_b200._build`."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libriqn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -40,7 +41,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src}:\n{out.decode()}")
     if procs or force or not os.path.exists(LIB) or any(os.path.getmtime(o) > os.path.getmtime(LIB) for o in objs):
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static",
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, *ARCH, "-lcudart_static",
                "-ldl", "-lrt", "-lpthread"]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
         if r.returncode != 0:

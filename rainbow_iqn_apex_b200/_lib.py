@@ -160,10 +160,10 @@ def launch_count():
 
 
 def require_device():
-    """Fail loudly unless a CUDA device of compute capability 10.x is current."""
+    """Fail loudly unless a CUDA device of compute capability 9.x is current."""
     if not torch.cuda.is_available():
-        raise RiqnError("rainbow_iqn_apex_b200 needs a CUDA device (B200, sm_100a); there is no CPU path")
+        raise RiqnError("rainbow_iqn_apex_b200 needs a CUDA device (H100, sm_90a); there is no CPU path")
     lib = load()
     ok = lib.riqn_device_ok()
     if ok != 1:
-        raise RiqnError(f"libriqn_b200.so holds sm_100a code only; riqn_device_ok() returned {ok}")
+        raise RiqnError(f"libriqn_b200.so holds sm_90a code only; riqn_device_ok() returned {ok}")

@@ -7,7 +7,7 @@ from .model import FEAT
 
 
 def _tc_mode(B):
-    """Hidden NoisyLinear products on the tcgen05 path (same arithmetic modes as the IQN head, model.PRECISION)."""
+    """Hidden NoisyLinear products on the wgmma path (same arithmetic modes as the IQN head, model.PRECISION)."""
     from .model import PRECISION
     return PRECISION["fwd"] != "fp32" and PRECISION["bwd"] == "bf16" and B % 8 == 0
 

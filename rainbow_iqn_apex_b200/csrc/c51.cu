@@ -7,7 +7,7 @@
 #include "../../include/riqn_b200.h"
 
 namespace riqn {
-int colsum_atomic(long M, int N, const float* X, float* out, cudaStream_t s);
+int colsum_add(long M, int N, const float* X, float* out, cudaStream_t s);
 
 // One block per sample.  q[a,j] = v[j] + a[a,j] - mean_a a[.,j]; p = softmax_j q, logp = log_softmax_j q.
 // Optionally the double-DQN action argmax_a sum_j support[j] p[a,j]  (agent.py:92-99).
@@ -195,7 +195,7 @@ RIQN_API int riqn_noisy_wgrad_ld(long rows, int in_features, int out_features, c
   e.out2 = grad_sigma;
   e.eps = weight_epsilon;
   const int tiles = ((out_features + 127) / 128) * ((in_features + 127) / 128);
-  int split = (148 + tiles - 1) / tiles;
+  int split = (riqn_sms() + tiles - 1) / tiles;
   if ((long)split * 64 > rows) split = (int)((rows + 63) / 64);
   return gemm_f32(out_features, in_features, (int)rows, dy, 1, lddy, x, 1, ldx, grad_mu, in_features, EPI_NOISY_WGRAD, e, split,
                   (cudaStream_t)stream);

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the Rainbow-IQN Ape-X learner hot path (sm_100a only).
+// Shared device/host helpers for the Rainbow-IQN Ape-X learner hot path (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -19,9 +19,34 @@
     if (_e != cudaSuccess) return (int)_e;                    \
   } while (0)
 
-namespace riqn { void note_launches(int n); }   // bookkeeping for riqn_launch_count()
+namespace riqn {
+void note_launches(int n);   // bookkeeping for riqn_launch_count()
+
+// Deterministic cross-block sums.  A float atomicAdd makes a sum depend on which block arrives first, and the learner
+// feeds its losses back into the prioritized sampler, so last-bit differences would change which transitions later
+// steps draw.  Instead every contributing block writes its partial to its own slot of a scratch buffer and
+// sum_slots_add() adds the slots in slot order.
+// out[i] += sum_{k < slots} part[k * n + i], k ascending
+int sum_slots_add(int slots, int n, const float* part, float* out, cudaStream_t s);
+}  // namespace riqn
 
 static inline int riqn_cdiv(long a, long b) { return (int)((a + b - 1) / b); }
+
+// Scratch memory of one entry-point call: taken from the device's stream-ordered memory pool on the calling stream and
+// handed back on the same stream when the call returns, i.e. after every kernel that uses it has been enqueued
+// (cudaMallocAsync / cudaFreeAsync).  No host synchronisation, no state shared between calls or streams; inside a CUDA
+// graph capture it becomes an allocation node of the graph.
+struct StreamScratch {
+  float* p = nullptr;
+  cudaStream_t s = nullptr;
+  cudaError_t alloc(size_t n, cudaStream_t stream) {
+    s = stream;
+    return cudaMallocAsync(reinterpret_cast<void**>(&p), n * sizeof(float), stream);
+  }
+  ~StreamScratch() {
+    if (p != nullptr) cudaFreeAsync(p, s);
+  }
+};
 
 // ----------------------------------------------------------------------------------------------
 // Philox4x32-10 counter RNG (Salmon et al. 2011); stateless: value = f(seed, stream, index).
@@ -69,3 +94,15 @@ struct PerDeviceOnce {
     return d & 63;
   }
 };
+
+// SM count of the current device: grid size of the persistent kernels and the split-K choices.
+inline int riqn_sms() {
+  static int sms[64] = {};
+  const int d = PerDeviceOnce::device();
+  if (sms[d] == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d) != cudaSuccess || n < 1) n = 132;   // H100 SXM
+    sms[d] = n;
+  }
+  return sms[d];
+}

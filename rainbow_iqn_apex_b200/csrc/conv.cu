@@ -110,28 +110,35 @@ static int col2im(const riqn_conv_geom* g, const float* dcol, float* din, cudaSt
   } else {
     long total = (long)g->B * g->Cin * hw;
     long blocks = (total + 255) / 256;
-    col2im_kernel<<<(int)(blocks > 148L * 32 ? 148L * 32 : blocks), 256, 0, s>>>(*g, dcol, din);
+    col2im_kernel<<<(int)(blocks > 32L * riqn_sms() ? 32L * riqn_sms() : blocks), 256, 0, s>>>(*g, dcol, din);
   }
   return (int)cudaGetLastError();
 }
 
-// out[n] += sum_m X[m, n]
-__global__ void colsum_atomic_kernel(long M, int N, const float* __restrict__ X, float* __restrict__ out, int rows_per_block) {
+// part[blockIdx.y * N + n] = sum of X[m, n] over this block's rows (two row halves combined in a fixed order)
+__global__ void colsum_part_kernel(long M, int N, const float* __restrict__ X, float* __restrict__ part, int rows_per_block) {
+  __shared__ float upper[128];
   const int n = blockIdx.x * 128 + (threadIdx.x & 127);
   const int half = threadIdx.x >> 7;
-  if (n >= N) return;
   const long r0 = (long)blockIdx.y * rows_per_block;
   const long r1 = min(M, r0 + rows_per_block);
   float acc = 0.f;
-  for (long r = r0 + half; r < r1; r += 2) acc += X[r * N + n];
-  atomicAdd(&out[n], acc);
+  if (n < N)
+    for (long r = r0 + half; r < r1; r += 2) acc += X[r * N + n];
+  if (half) upper[threadIdx.x & 127] = acc;
+  __syncthreads();
+  if (!half && n < N) part[(long)blockIdx.y * N + n] = acc + upper[threadIdx.x];
 }
 
-int colsum_atomic(long M, int N, const float* X, float* out, cudaStream_t s) {
+// out[n] += sum_m X[m, n], in a fixed order
+int colsum_add(long M, int N, const float* X, float* out, cudaStream_t s) {
   int rows_per_block = 256;
   dim3 grid((N + 127) / 128, (unsigned)((M + rows_per_block - 1) / rows_per_block));
-  colsum_atomic_kernel<<<grid, 256, 0, s>>>(M, N, X, out, rows_per_block);
-  return (int)cudaGetLastError();
+  StreamScratch part;
+  RIQN_CUDA(part.alloc((size_t)grid.y * N, s));
+  colsum_part_kernel<<<grid, 256, 0, s>>>(M, N, X, part.p, rows_per_block);
+  RIQN_LAUNCH_CHECK();
+  return sum_slots_add((int)grid.y, N, part.p, out, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -381,7 +388,7 @@ __global__ void im2col_bf16_t_kernel(riqn_conv_geom g, const T* __restrict__ in,
 // dY = dout * (out > 0) from NCHW into the two bf16 operand layouts: dY (M, Cout) and dYT (Cout, M); the bias
 // gradient (sum over b, p) is reduced per channel on the way.
 __global__ void conv_dy_bf16_kernel(int B, int Cout, int ohw, const float* __restrict__ dout, const float* __restrict__ out,
-                                    bf16* __restrict__ dY, bf16* __restrict__ dYT, float* __restrict__ dbias) {
+                                    bf16* __restrict__ dY, bf16* __restrict__ dYT, float* __restrict__ dbias_part) {
   const int c = blockIdx.y;
   const long M = (long)B * ohw;
   float acc = 0.f;
@@ -402,7 +409,7 @@ __global__ void conv_dy_bf16_kernel(int B, int Cout, int ohw, const float* __res
   if (threadIdx.x < 32) {
     float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
     v = warp_sum(v);
-    if (threadIdx.x == 0) atomicAdd(&dbias[c], v);
+    if (threadIdx.x == 0) dbias_part[(long)blockIdx.x * Cout + c] = v;   // summed in block order
   }
 }
 
@@ -410,7 +417,7 @@ __global__ void conv_dy_bf16_kernel(int B, int Cout, int ohw, const float* __res
 // writes are coalesced along the pixels; the (M, Cout) image leaves through a shared tile as 16-byte row pieces.
 __global__ void __launch_bounds__(256) conv_dy_tile_kernel(int B, int Cout, int ohw, const float* __restrict__ dout,
                                                            const float* __restrict__ out, bf16* __restrict__ dY,
-                                                           bf16* __restrict__ dYT, float* __restrict__ dbias) {
+                                                           bf16* __restrict__ dYT, float* __restrict__ dbias_part) {
   __shared__ __align__(16) unsigned short tile[64][66];
   __shared__ float bsum[64];
   const long M = (long)B * ohw;
@@ -459,7 +466,7 @@ __global__ void __launch_bounds__(256) conv_dy_tile_kernel(int B, int Cout, int 
     }
     __syncthreads();
   }
-  if (threadIdx.x < Cout) atomicAdd(&dbias[threadIdx.x], bsum[threadIdx.x]);
+  if (threadIdx.x < Cout) dbias_part[(long)blockIdx.x * Cout + threadIdx.x] = bsum[threadIdx.x];   // summed in block order
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -528,7 +535,7 @@ __global__ void __launch_bounds__(256) s2d_u8_kernel(riqn_conv_geom g, int G, co
 
 static inline int grid_for(long total) {
   long b = (total + 255) / 256;
-  return (int)(b > 148L * 32 ? 148L * 32 : (b < 1 ? 1 : b));
+  return (int)(b > 32L * riqn_sms() ? 32L * riqn_sms() : (b < 1 ? 1 : b));
 }
 
 }  // namespace riqn
@@ -569,12 +576,12 @@ RIQN_API int riqn_conv_bwd(const riqn_conv_geom* g, const float* dout, const flo
   const int ohw = g->OH * g->OW;
   conv_dy_kernel<<<grid_for(M * g->Cout), 256, 0, s>>>(g->B, g->Cout, ohw, dout, out, dY);
   RIQN_LAUNCH_CHECK();
-  int rc = colsum_atomic(M, g->Cout, dY, dbias, s);
+  int rc = colsum_add(M, g->Cout, dY, dbias, s);
   if (rc) return rc;
   // dW[c, k] += sum_m dY[m, c] * col[m, k]
   EpiArgs e;
   const int tiles = ((g->Cout + 127) / 128) * ((K + 127) / 128);
-  int split = (2 * 148 + tiles - 1) / tiles;
+  int split = (2 * riqn_sms() + tiles - 1) / tiles;
   if ((long)split * 64 > M) split = (int)((M + 63) / 64);
   rc = gemm_f32(g->Cout, K, (int)M, dY, 1, g->Cout, col, 1, K, dw, K, EPI_ATOMIC, e, split, s);
   if (rc) return rc;
@@ -590,7 +597,7 @@ RIQN_API int riqn_conv_bwd(const riqn_conv_geom* g, const float* dout, const flo
 
 
 // ---------------------------------------------------------------------------------------------------------------
-// Tensor-core conv entry points (tcgen05 GEMM on bf16 hi/lo im2col operands)
+// Tensor-core conv entry points (wgmma GEMM on bf16 hi/lo im2col operands)
 // ---------------------------------------------------------------------------------------------------------------
 RIQN_API int riqn_conv_fwd_tc(const riqn_conv_geom* g, const void* in, int in_is_u8, const void* w_hi, const void* w_lo,
                               const float* bias, void* col_hi, void* col_lo, void* colT_hi, float* out, void* stream) {
@@ -655,7 +662,7 @@ RIQN_API int riqn_conv_fwd_tc_u8(const riqn_conv_geom* g, const unsigned char* i
 // (gy < OH, gx < OW) and zeros elsewhere; dbias accumulated.  One block = 64 grid rows x all channels (Cout <= 64).
 __global__ void __launch_bounds__(256) conv_dy_grid_kernel(int B, int Cout, int OH, int OW, int G,
                                                            const float* __restrict__ dout, const float* __restrict__ out,
-                                                           bf16* __restrict__ dYg, float* __restrict__ dbias) {
+                                                           bf16* __restrict__ dYg, float* __restrict__ dbias_part) {
   __shared__ __align__(16) unsigned short tile[64][66];
   __shared__ float bsum[64];
   const long Mg = (long)B * G * G;
@@ -714,7 +721,7 @@ __global__ void __launch_bounds__(256) conv_dy_grid_kernel(int B, int Cout, int 
     }
     __syncthreads();
   }
-  if (threadIdx.x < Cout) atomicAdd(&dbias[threadIdx.x], bsum[threadIdx.x]);
+  if (threadIdx.x < Cout) dbias_part[(long)blockIdx.x * Cout + threadIdx.x] = bsum[threadIdx.x];   // summed in block order
 }
 
 // dw[c, perm[k']] += dwp[c, k']: the strip weight gradient back into the (Cout, Cin*KH*KW) parameter order
@@ -781,6 +788,33 @@ RIQN_API int riqn_conv_fwd_strip(const riqn_conv_geom* g, const void* a_hi, cons
 //   dW'[c, (shift, within)] = sum_m' dYg[m', c] * a_hi[m' + shift offset, within]   (MN-major operands, shifted rows)
 //   dw[c, perm[k']] += wgrad_scale * dW'[c, k']
 //   din += col2im(dYg * W)   (W (Cout, K) as MN-major operand; fused epilogue, pad == 0 only; din may be NULL)
+// din[b, c, ih, iw] = sum over (kh, kw) of dcol[(b, oh, ow) on the G x G strip grid, (c, kh, kw)] with
+// ih = oh * stride + kh, iw = ow * stride + kw (pad == 0), kh and kw ascending.  Threads run channel-fastest, so a warp
+// reads neighbouring columns of the same dcol rows.
+__global__ void col2im_gather_kernel(riqn_conv_geom g, int G, const float* __restrict__ dcol, float* __restrict__ din) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long n = (long)g.B * g.Cin * g.H * g.W;
+  if (i >= n) return;
+  const int c = (int)(i % g.Cin), iw = (int)((i / g.Cin) % g.W), ih = (int)((i / ((long)g.Cin * g.W)) % g.H);
+  const long b = i / ((long)g.Cin * g.W * g.H);
+  const int K = g.Cin * g.KH * g.KW;
+  float acc = 0.f;
+  for (int kh = 0; kh < g.KH; ++kh) {
+    const int oy = ih - kh;
+    if (oy < 0 || oy % g.stride) continue;
+    const int oh = oy / g.stride;
+    if (oh >= g.OH) continue;
+    for (int kw = 0; kw < g.KW; ++kw) {
+      const int ox = iw - kw;
+      if (ox < 0 || ox % g.stride) continue;
+      const int ow = ox / g.stride;
+      if (ow >= g.OW) continue;
+      acc += dcol[((b * G + oh) * G + ow) * K + (c * g.KH + kh) * g.KW + kw];
+    }
+  }
+  din[((b * g.Cin + c) * g.H + ih) * g.W + iw] = acc;
+}
+
 RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, const float* out, const void* a_hi,
                                  const void* w_hi, const int* perm, void* dYg, float* dwp_scratch, float* dw, float* dbias,
                                  float* din, float wgrad_scale, void* stream) {
@@ -791,15 +825,18 @@ RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, con
   const long Mg = (long)g->B * G * G;
   const int K = g->Cin * g->KH * g->KW;
   const long tiles = (Mg + 63) / 64;
-  conv_dy_grid_kernel<<<(unsigned)(tiles < 148 * 4 ? tiles : 148 * 4), 256, 0, s>>>(g->B, g->Cout, g->OH, g->OW, G, dout, out,
-                                                                                (bf16*)dYg, dbias);
+  const int dy_grid = (int)(tiles < 4L * riqn_sms() ? tiles : 4L * riqn_sms());
+  StreamScratch dbias_part;
+  RIQN_CUDA(dbias_part.alloc((size_t)dy_grid * g->Cout, s));
+  conv_dy_grid_kernel<<<dy_grid, 256, 0, s>>>(g->B, g->Cout, g->OH, g->OW, G, dout, out, (bf16*)dYg, dbias_part.p);
   RIQN_LAUNCH_CHECK();
+  if (int rc_ = sum_slots_add(dy_grid, g->Cout, dbias_part.p, dbias, s)) return rc_;
   RIQN_CUDA(cudaMemsetAsync(dwp_scratch, 0, sizeof(float) * g->Cout * K, s));
   TcExtra ex;
   ex.mn_major = 3;
   ex.wg_t = t; ex.wg_G = G; ex.wg_kc = kc;
   ex.alpha = wgrad_scale;
-  const int n_tiles = (K + 255) / 256;
+  const int n_tiles = (K + 127) / 128;
   const int split = tc_pick_split(n_tiles, (Mg + 63) / 64);
   int rc = gemm_bf16_tc(g->Cout, K, (int)Mg, (const bf16*)dYg, nullptr, (const bf16*)a_hi, nullptr, dwp_scratch, K, TC_ATOMIC,
                         nullptr, nullptr, nullptr, split, s, &ex);
@@ -807,15 +844,18 @@ RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, con
   unpermute_add_kernel<<<(g->Cout * K + 255) / 256, 256, 0, s>>>(g->Cout, K, dwp_scratch, perm, dw);
   RIQN_LAUNCH_CHECK();
   if (din) {
-    RIQN_CUDA(cudaMemsetAsync(din, 0, sizeof(float) * (size_t)g->B * g->Cin * g->H * g->W, s));
+    // dcol = dYg W on the strip grid, then every input pixel gathers its (kh, kw) contributions in a fixed order
+    StreamScratch dcol_buf;
+    RIQN_CUDA(dcol_buf.alloc((size_t)Mg * K, s));
+    float* dcol = dcol_buf.p;
     TcExtra ci;
-    ci.ohw = G * G;
-    ci.ci_h = g->H; ci.ci_w = g->W; ci.ci_cin = g->Cin; ci.ci_kh = g->KH; ci.ci_kw = g->KW;
-    ci.ci_stride = g->stride; ci.ci_ow = g->OW; ci.ci_oh = g->OH; ci.ci_G = G;
     ci.mn_major = 2;               // B = the (Cout, K) weight itself, read as an MN-major operand (no transposed copy)
-    rc = gemm_bf16_tc((int)Mg, K, g->Cout, (const bf16*)dYg, nullptr, (const bf16*)w_hi, nullptr, din, K, TC_COL2IM, nullptr,
+    rc = gemm_bf16_tc((int)Mg, K, g->Cout, (const bf16*)dYg, nullptr, (const bf16*)w_hi, nullptr, dcol, K, TC_STORE, nullptr,
                       nullptr, nullptr, 1, s, &ci);
     if (rc) return rc;
+    const long n_in = (long)g->B * g->Cin * g->H * g->W;
+    col2im_gather_kernel<<<riqn_cdiv(n_in, 256), 256, 0, s>>>(*g, G, dcol, din);
+    RIQN_LAUNCH_CHECK();
   }
   return 0;
 }
@@ -853,18 +893,23 @@ RIQN_API int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const 
   const int K = g->Cin * g->KH * g->KW;
   const int ohw = g->OH * g->OW;
   if (M % 8 || g->Cout % 8) return (int)cudaErrorInvalidValue;
+  const long tiles = (M + 63) / 64;
+  const int slots = g->Cout <= 64 ? (int)(tiles < 4L * riqn_sms() ? tiles : 4L * riqn_sms()) : (int)((M + 256 * 8 - 1) / (256 * 8));
+  StreamScratch dbias_part;
+  RIQN_CUDA(dbias_part.alloc((size_t)slots * g->Cout, s));
   if (g->Cout <= 64) {
-    const long tiles = (M + 63) / 64;
-    conv_dy_tile_kernel<<<(unsigned)(tiles < 148 * 4 ? tiles : 148 * 4), 256, 0, s>>>(g->B, g->Cout, ohw, dout, out,
-                                                                 din ? (bf16*)dY_hi : nullptr, (bf16*)dYT_hi, dbias);
+    conv_dy_tile_kernel<<<slots, 256, 0, s>>>(g->B, g->Cout, ohw, dout, out, din ? (bf16*)dY_hi : nullptr, (bf16*)dYT_hi,
+                                              dbias_part.p);
   } else {
-    dim3 grid((unsigned)((M + 256 * 8 - 1) / (256 * 8)), g->Cout);
-    conv_dy_bf16_kernel<<<grid, 256, 0, s>>>(g->B, g->Cout, ohw, dout, out, din ? (bf16*)dY_hi : nullptr, (bf16*)dYT_hi, dbias);
+    dim3 grid((unsigned)slots, g->Cout);
+    conv_dy_bf16_kernel<<<grid, 256, 0, s>>>(g->B, g->Cout, ohw, dout, out, din ? (bf16*)dY_hi : nullptr, (bf16*)dYT_hi,
+                                             dbias_part.p);
   }
   RIQN_LAUNCH_CHECK();
+  if (int rc_ = sum_slots_add(slots, g->Cout, dbias_part.p, dbias, s)) return rc_;
   // dW[c, k] += sum_m dY[m, c] * col[m, k]      (K' = M is long: split it over every SM)
-  const int n_tiles = (K + 255) / 256;
-  int split = (148 + n_tiles - 1) / n_tiles;
+  const int n_tiles = (K + 127) / 128;
+  int split = (riqn_sms() + n_tiles - 1) / n_tiles;
   TcExtra ex;
   ex.alpha = wgrad_scale;          // 1/255 when colT holds raw pixel values
   int rc = gemm_bf16_tc(g->Cout, K, (int)M, (const bf16*)dYT_hi, nullptr, (const bf16*)colT_hi, nullptr, dw, K, TC_ATOMIC,

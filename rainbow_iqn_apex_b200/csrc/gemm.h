@@ -3,6 +3,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include "common.cuh"
+
 namespace riqn {
 
 // C[m,n] (+)= epi( sum_k A[m*sAm + k*sAk] * B[n*sBn + k*sBk] )
@@ -30,7 +32,7 @@ struct EpiArgs {
 int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,
              float* C, long ldc, int epi, const EpiArgs& e, int split_k, cudaStream_t stream);
 
-// ---- tcgen05 / TMA path (gemm_tc.cu) ---------------------------------------------------------------------------
+// ---- wgmma / TMA path (gemm_tc.cu) ---------------------------------------------------------------------------
 enum TcEpi { TC_STORE = 0, TC_BIAS_RELU = 1, TC_ATOMIC = 2, TC_NOISY_WGRAD = 3, TC_BIAS_RELU_NCHW = 4, TC_EMBED = 5,
              TC_COL2IM = 6, TC_CONV = 7 };
 
@@ -72,21 +74,18 @@ struct TcExtra {
 int gemm_bf16_tc(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, const __nv_bfloat16* B_hi,
                  const __nv_bfloat16* B_lo, float* C, long ldc, int epi, const float* bias, float* out2, const float* eps,
                  int split_k, cudaStream_t s, const TcExtra* ex);
-// Split-K factor for a persistent grid of `sms` CTAs: `tiles` output tiles, `kb` reduction blocks of 64.  Minimises
-// (rounds of CTAs) x (k-blocks per unit), e.g. 25 tiles -> 11 splits (275 units, two full rounds) rather than 6
-// (150 units: a second round for two stragglers).
-inline int tc_pick_split(int tiles, long kb, int sms = 148) {
+// Split-K over a persistent grid of one CTA per SM: every split writes its partial product to scratch and one pass adds
+// them in split order, so splits beyond one round of CTAs only add partial sums.  tc_max_split is the most splits that
+// still fit in one round for `tiles` output tiles; tc_pick_split takes that many, but no more than the `kb` reduction
+// blocks of 64 (e.g. 25 tiles on 132 SMs -> 5 splits, 125 units).
+inline int tc_max_split(long tiles) {
   if (tiles < 1) tiles = 1;
-  if (kb < 1) kb = 1;
-  long best_cost = -1;
-  int best = 1;
-  const int smax = (int)(kb < 4L * sms ? kb : 4L * sms);
-  for (int s = 1; s <= smax; ++s) {
-    const long units = (long)tiles * s, rounds = (units + sms - 1) / sms, per = (kb + s - 1) / s;
-    const long cost = rounds * (per + 2);          // +2: fixed per-unit cost (pipeline fill, epilogue)
-    if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = s; }
-  }
-  return best;
+  const long s = riqn_sms() / tiles;
+  return s < 1 ? 1 : (int)s;
+}
+inline int tc_pick_split(int tiles, long kb) {
+  const int s = tc_max_split(tiles);
+  return kb < s ? (int)(kb < 1 ? 1 : kb) : s;
 }
 
 int split_bf16(long rows, int cols, const float* src, __nv_bfloat16* hi, __nv_bfloat16* lo, __nv_bfloat16* hiT,

@@ -1,6 +1,6 @@
 // fp32 CUDA-core GEMM with fused epilogues.  Used for the small / oddly-shaped products on the
 // learner path (conv im2col products, quantile embedding K=64, z-layers, weight-gradient
-// reductions) and as the fp32 cross-check for the tcgen05 path (gemm_tc.cu).
+// reductions) and as the fp32 cross-check for the wgmma path (gemm_tc.cu).
 //
 // Tile 128x128x16, 256 threads, 8x8 register micro-tile (4+4 split so shared-memory reads are
 // 128-bit and conflict-free), global->register prefetch of the next k-slab overlapped with the

@@ -1,18 +1,21 @@
-// tcgen05 / TMA GEMM for the NoisyLinear hidden layers of the IQN head (the >90% of the learner step's FLOPs:
-// reference model.py:153-154 forward, and its dgrad / wgrad), sm_100a only.
+// wgmma / TMA GEMM for the NoisyLinear hidden layers of the IQN head (the >90% of the learner step's FLOPs:
+// reference model.py:153-154 forward, and its dgrad / wgrad), sm_90a.
 //
-//   C[m,n] = sum_k A[m,k] * B[n,k]        A (M,K) and B (N,K) both K-major bf16 in HBM, fp32 accumulate in TMEM
+//   C[m,n] = sum_k A[m,k] * B[n,k]        A (M,K) and B (N,K) both K-major bf16 in HBM, fp32 accumulate in registers
 //
-// * operands arrive by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) into a multi-stage shared-memory ring,
-// * one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (UMMA 128x256x16) on shared-memory descriptors,
-// * accumulators live in TMEM, double buffered (2 x 256 columns = all 512) so the epilogue of tile i overlaps the
-//   MMAs of tile i+1; 4 epilogue warps read them back with tcgen05.ld and apply the fused epilogue,
+// * operands arrive by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) into a multi-stage shared-memory ring, issued by
+//   one thread of the producer warpgroup,
+// * two consumer warpgroups each own 64 rows of the 128-row tile and issue wgmma.mma_async (m64nBNk16) on shared-memory
+//   descriptors; the accumulator lives in their registers,
+// * after a tile's last k-block the consumers pass the accumulator through a shared-memory slab, 64 columns at a time,
+//   so that each warp holds 32 rows x 32 columns with one ROW per lane, and apply the fused epilogue from there while
+//   the producer already fetches the next tile's operands,
 // * persistent CTAs (one per SM) walk (m-tile, n-tile, k-split) work units round-robin.
 //
 // Precision: NSPLIT == 1 multiplies bf16(A) * bf16(B).  NSPLIT == 3 takes each operand as hi + lo bf16 pairs
-// (a = a_hi + a_lo exactly to ~2^-17) and accumulates a_hi*b_hi + a_hi*b_lo + a_lo*b_hi into the same TMEM
-// accumulator: an fp32-faithful product (rel. error ~1e-5 per term) at 3 MMAs per k-step, which keeps the IQN
-// loss within 1e-6 of the fp32 reference instead of bf16's 1e-4.
+// (a = a_hi + a_lo exactly to ~2^-17) and accumulates a_hi*b_hi + a_hi*b_lo + a_lo*b_hi into the same accumulator: an
+// fp32-faithful product (rel. error ~1e-5 per term) at 3 MMAs per k-step, which keeps the IQN loss within 1e-6 of the
+// fp32 reference instead of bf16's 1e-4.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <map>
@@ -27,14 +30,15 @@ namespace riqn {
 
 using bf16 = __nv_bfloat16;
 
-constexpr int TBM = 128, TBK = 64, UMMA_K = 16;   // tile N (BN) is a template parameter: 256, or 64 / 32 for narrow outputs
-// Epilogue warps: a warp may only read the TMEM lane quarter (warp % 4), so they come in sets of four; each set drains an
-// equal share of the accumulator columns.  Two sets (8 warps) for the MMA-bound products; FOUR sets for the embedding
-// product, whose k = 64 mainloop is over in a microsecond and whose time is all epilogue latency (104 registers per
-// thread leave room for 18 warps per SM).
-constexpr int epi_warps(int epi) { return epi == TC_EMBED ? 16 : 8; }
-constexpr int tc_threads(int epi) { return 64 + 32 * epi_warps(epi); }  // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner
-
+constexpr int TBM = 128, TBK = 64, MMA_K = 16;   // tile N (BN) is a template parameter: 128, or 64 / 32 for narrow outputs
+constexpr int kConsumerWGs = 2;                   // consumer warpgroup g owns tile rows [64 g, 64 g + 64)
+constexpr int kEpiWarps = 4 * kConsumerWGs;
+constexpr int kTcThreads = 128 * (1 + kConsumerWGs);   // warpgroup 0: TMA producer (one thread issues), then the consumers
+// Accumulator slab of one consumer warpgroup: 64 rows x 64 columns fp32, rows padded to 72 words so that the fragment
+// deposit (a half-warp = 4 rows x 8 columns) is bank-conflict free.  Once read back it holds the four 4 KB per-warp
+// staging tiles of the store helpers below.
+constexpr uint32_t kSlabStride = 72, kSlabBytes = 64 * kSlabStride * 4;
+constexpr uint32_t kSmemLimit = 232448;           // 227 KB of opt-in shared memory per CTA
 
 // NSPLIT 1: a_hi*b_hi.  NSPLIT 3: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi.  NSPLIT 2: A is exact in bf16 (e.g. uint8 pixels),
 // only B is split: a_hi*b_hi + a_hi*b_lo.
@@ -43,15 +47,13 @@ struct TcCfg {
   static constexpr int kAOps = NSPLIT == 3 ? 2 : 1, kBOps = NSPLIT == 1 ? 1 : 2;     // hi (+ lo) images per operand
   static constexpr int kOps = kAOps;                                                 // (A images; B tile starts after them)
   static constexpr uint32_t kABytes = TBM * TBK * 2, kBBytes = BN * TBK * 2;
-  static constexpr uint32_t kStageBytes = kAOps * kABytes + kBOps * kBBytes;         // 48 / 80 / 96 KB at BN = 256
-  static constexpr uint32_t kEpiStage = 32 * 32 * 4;  // per epilogue warp: 32 rows x 32 words for the store transpose
-  static constexpr uint32_t kFbBytes = EPI == TC_EMBED ? epi_warps(EPI) * 256 : 0;   // per-warp feat / bias broadcast patches
-  static constexpr uint32_t kRingBytes = 224 * 1024 - epi_warps(EPI) * kEpiStage - kFbBytes;   // 192 KB with two warp sets
+  static constexpr uint32_t kStageBytes = kAOps * kABytes + kBOps * kBBytes;         // 32 / 48 / 64 KB at BN = 128
+  static constexpr uint32_t kEpiBytes = kConsumerWGs * kSlabBytes;
+  static constexpr uint32_t kFbBytes = EPI == TC_EMBED ? kEpiWarps * 256 : 0;       // per-warp feat / bias broadcast patches
+  static constexpr uint32_t kRingBytes = kSmemLimit - 1024 /*align*/ - kEpiBytes - 256 /*barriers*/ - kFbBytes;
   static constexpr int kStages = kRingBytes / kStageBytes > 6 ? 6 : kRingBytes / kStageBytes;
-  static constexpr uint32_t kTmemCols = 2 * BN < 32 ? 32 : 2 * BN;                   // two accumulator buffers (power of 2)
-  static constexpr uint32_t kSmemBytes =
-      kStages * kStageBytes + 1024 /*align*/ + epi_warps(EPI) * kEpiStage + 256 /*barriers*/ + kFbBytes;
-  static_assert(kSmemBytes <= 232448 && kStages >= 1, "exceeds the 227 KB per-CTA shared memory limit");
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + kEpiBytes + 256 + kFbBytes;
+  static_assert(kSmemBytes <= kSmemLimit && kStages >= 2, "exceeds the 227 KB per-CTA shared memory limit");
 };
 
 // ---------------------------------------------------------------------------------------------- PTX wrappers
@@ -93,57 +95,106 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t sr
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// named barrier over the 128 threads of one warpgroup (id 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// wgmma m64nNk16, fp32 accumulators d[N / 2] in the standard fragment layout (register 4j + 2h + e holds row
+// 16 * warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e).  F16: fp16 operands, else bf16 (A and B always share the
+// format).  TA / TB: the A / B tile is MN-major (transposed) instead of K-major.  acc == 0 overwrites d.
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<32> {
+  template <int F16, int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
+#define RIQN_WGMMA(TY) \
+    asm volatile( \
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n" \
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n}\n" \
+        : \
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB))
+    if constexpr (F16) RIQN_WGMMA("f16"); else RIQN_WGMMA("bf16");
+#undef RIQN_WGMMA
+  }
+};
+
+template <>
+struct Wgmma<64> {
+  template <int F16, int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+#define RIQN_WGMMA(TY) \
+    asm volatile( \
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n" \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n" \
+        : \
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB))
+    if constexpr (F16) RIQN_WGMMA("f16"); else RIQN_WGMMA("bf16");
+#undef RIQN_WGMMA
+  }
+};
+
+template <>
+struct Wgmma<128> {
+  template <int F16, int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+#define RIQN_WGMMA(TY) \
+    asm volatile( \
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n" \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n" \
+        : \
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB))
+    if constexpr (F16) RIQN_WGMMA("f16"); else RIQN_WGMMA("bf16");
+#undef RIQN_WGMMA
+  }
+};
+
+template <int N>
+__device__ __forceinline__ void wgmma_tile(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc, bool f16, int mn) {
+  const bool ta = (mn & 1) != 0, tb = (mn & 2) != 0;   // bit 0: A MN-major, bit 1: B MN-major
+  if (f16) {
+    if (ta) { if (tb) Wgmma<N>::template mma<1, 1, 1>(d, da, db, acc); else Wgmma<N>::template mma<1, 1, 0>(d, da, db, acc); }
+    else    { if (tb) Wgmma<N>::template mma<1, 0, 1>(d, da, db, acc); else Wgmma<N>::template mma<1, 0, 0>(d, da, db, acc); }
+  } else {
+    if (ta) { if (tb) Wgmma<N>::template mma<0, 1, 1>(d, da, db, acc); else Wgmma<N>::template mma<0, 1, 0>(d, da, db, acc); }
+    else    { if (tb) Wgmma<N>::template mma<0, 0, 1>(d, da, db, acc); else Wgmma<N>::template mma<0, 0, 0>(d, da, db, acc); }
+  }
 }
 
-// K-major, 128-byte-swizzled operand tile: rows of 64 bf16 (128 B), 8-row swizzle atoms 1024 B apart.
-// Descriptor fields (cute/arch/mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30) (=1, unused for swizzled
-// K-major), SBO>>4 [32,46) (=1024>>4), version=1 [46,48), layout SWIZZLE_128B=2 [61,64).
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
+// Shared-memory matrix descriptor of wgmma: start >> 4 [0,14), leading byte offset >> 4 [16,30), stride byte offset
+// >> 4 [32,46), swizzle [62,64) (1 = 128-byte swizzle).
+// K-major, 128-byte-swizzled operand tile: rows of 64 16-bit values (128 B), 8-row swizzle atoms SBO = 1024 B apart
+// (LBO unused).
+__device__ __forceinline__ uint64_t gmma_desc_k128(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// MN-major, 128-byte-swizzled operand tile (cute/atom/mma_traits_sm100.hpp, make_umma_desc<Major::MN>): k-rows of 64
-// MN-elements (128 B), 8-row swizzle atoms SBO = 1024 B apart along K, further 64-element MN slabs LBO = 8192 B apart.
-__device__ __forceinline__ uint64_t umma_desc_mn128(uint32_t saddr) {
+// MN-major, 128-byte-swizzled operand tile: k-rows of 64 MN-elements (128 B), 8-row swizzle atoms SBO = 1024 B apart
+// along K, further 64-element MN slabs LBO = 8192 B apart.
+__device__ __forceinline__ uint64_t gmma_desc_mn128(uint32_t saddr) {
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// kind::f16 instruction descriptor: D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1, K-major both, N>>3 [17,23), M>>4 [24,29)
-// (format field: 0 = fp16, 1 = bf16.  The descriptor has separate A / B fields, but a product that MIXES them is an
-  // illegal instruction on sm_100a (measured, round 2): both operands must share the format -> fmt is 0 or 3)
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int m, int n, int fmt = 0) {
-  return (1u << 4) | ((fmt & 1) ? 0u : (1u << 7)) | ((fmt & 2) ? 0u : (1u << 10)) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
+         ((uint64_t)1 << 62);
 }
 // two floats -> packed 16-bit pair (low half = a), fp16 or bf16
 __device__ __forceinline__ uint32_t pack16x2(float a, float b, bool f16) {
@@ -155,7 +206,7 @@ __device__ __forceinline__ uint32_t pack16x2(float a, float b, bool f16) {
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// The accumulator arrives with one ROW per lane (tcgen05.ld 32x32b): storing it directly makes every store instruction
+// The epilogue holds the accumulator with one ROW per lane (read back from the slab): storing it directly makes every store instruction
 // touch 32 different lines with 16-byte pieces (~2 TB/s).  These helpers transpose a 32x32 chunk through a padded
 // per-warp shared-memory tile so that each store instruction writes one full row segment (128 B fp32 / 64 B bf16).
 // Tile rows are 32 words (128 B) apart and the 16-byte piece j of row r lives at piece slot j ^ (r & 7), so that both the
@@ -209,10 +260,10 @@ __device__ __forceinline__ void warp_store_rows_bf16(uint32_t st, const uint32_t
 }
 
 // C += alpha * acc (and out2 += alpha * acc * eps for the NoisyLinear weight gradient) on full 128-byte row segments:
-// plain 16-byte read-modify-writes when this CTA is the only contributor, red.global.add.v4.f32 under split-K.
+// 16-byte read-modify-writes (one CTA per tile: split-K products go through per-split partials instead).
 template <bool NOISY>
 __device__ __forceinline__ void warp_accum_rows_f32(uint32_t st, const uint32_t (&w)[32], int lane, float* c, float* out2,
-                                                    const float* eps, long ld, int rows_valid, bool atomic, float alpha) {
+                                                    const float* eps, long ld, int rows_valid, float alpha) {
   stage_row(st, w, lane);
   const int sub = lane >> 3, piece = lane & 7;
 #pragma unroll
@@ -220,30 +271,17 @@ __device__ __forceinline__ void warp_accum_rows_f32(uint32_t st, const uint32_t 
     const int r = r0 + sub;
     if (r < rows_valid) {
       const uint4 au = staged_piece(st, r, piece);
-      float4 a = make_float4(__uint_as_float(au.x) * alpha, __uint_as_float(au.y) * alpha, __uint_as_float(au.z) * alpha,
-                             __uint_as_float(au.w) * alpha);
+      const float4 a = make_float4(__uint_as_float(au.x) * alpha, __uint_as_float(au.y) * alpha,
+                                   __uint_as_float(au.z) * alpha, __uint_as_float(au.w) * alpha);
       const long off = (long)r * ld + piece * 4;
-      float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 o = *reinterpret_cast<const float4*>(c + off);
+      o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
+      *reinterpret_cast<float4*>(c + off) = o;
       if (NOISY) {
-        e = *reinterpret_cast<const float4*>(eps + off);
-        e.x *= a.x; e.y *= a.y; e.z *= a.z; e.w *= a.w;
-      }
-      if (!atomic) {
-        float4 o = *reinterpret_cast<const float4*>(c + off);
-        o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-        *reinterpret_cast<float4*>(c + off) = o;
-        if (NOISY) {
-          float4 o2 = *reinterpret_cast<const float4*>(out2 + off);
-          o2.x += e.x; o2.y += e.y; o2.z += e.z; o2.w += e.w;
-          *reinterpret_cast<float4*>(out2 + off) = o2;
-        }
-      } else {
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(c + off), "f"(a.x), "f"(a.y), "f"(a.z), "f"(a.w)
-                     : "memory");
-        if (NOISY)
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out2 + off), "f"(e.x), "f"(e.y), "f"(e.z),
-                       "f"(e.w)
-                       : "memory");
+        const float4 e = *reinterpret_cast<const float4*>(eps + off);
+        float4 o2 = *reinterpret_cast<const float4*>(out2 + off);
+        o2.x += a.x * e.x; o2.y += a.y * e.y; o2.z += a.z * e.z; o2.w += a.w * e.w;
+        *reinterpret_cast<float4*>(out2 + off) = o2;
       }
     }
   }
@@ -288,53 +326,42 @@ struct alignas(64) TcArgs {
   int fmt;               // bit 0: A image is fp16, bit 1: B image is fp16 (else bf16), bit 2: o_hi is written as fp16
   int grp_mt, a_wrap;    // TC_CONV, two weight sets (gemm.h): group 1's B maps live in mapO[0] / mapO[1]
   const float* bias2;
+  long part_stride;      // TC_STORE of split-K partials: split ks writes C + ks * part_stride (0 otherwise)
 };
 
 template <int NSPLIT, int EPI, int BN>
-__global__ void __launch_bounds__(tc_threads(EPI), 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                const __grid_constant__ CUtensorMap mapB_hi, const __grid_constant__ CUtensorMap mapB_lo,
                const __grid_constant__ TcArgs p) {
   using Cfg = TcCfg<NSPLIT, BN, EPI>;
   constexpr int TBN = BN;
-  constexpr uint32_t TMEM_COLS = Cfg::kTmemCols;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // layout: operand ring | per-warp epilogue staging tiles (4 KB each, 4 KB aligned) | barriers | feat / bias patches
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + epi_warps(EPI) * Cfg::kEpiStage);
+  // layout: operand ring | accumulator slabs (one per consumer warpgroup, 1 KB aligned) | barriers | feat / bias patches
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kEpiBytes);
   uint64_t* full = bars;                       // [kStages]  TMA -> MMA
-  uint64_t* empty = bars + Cfg::kStages;       // [kStages]  MMA -> TMA
-  uint64_t* tfull = bars + 2 * Cfg::kStages;   // [2]        MMA -> epilogue
-  uint64_t* tempty = tfull + 2;                // [2]        epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  const uint32_t epi_stage = (uint32_t)__cvta_generic_to_shared(smem + Cfg::kStages * Cfg::kStageBytes);
-  const uint32_t epi_fb = epi_stage + epi_warps(EPI) * Cfg::kEpiStage + 256;
+  uint64_t* empty = bars + Cfg::kStages;       // [kStages]  MMA -> TMA (one arrival per consumer warp)
+  const uint32_t epi_base = (uint32_t)__cvta_generic_to_shared(smem + Cfg::kStages * Cfg::kStageBytes);
+  const uint32_t epi_fb = epi_base + Cfg::kEpiBytes + 256;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_units = p.m_tiles * p.n_tiles * p.k_splits;
 
-  if (warp == 0 && lane == 0) {
-    // descriptor fetch overlaps the barrier / TMEM prologue instead of delaying the first TMA load
+  if (threadIdx.x == 0) {
+    // descriptor fetch overlaps the barrier prologue instead of delaying the first TMA load
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapA_hi)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapB_hi)) : "memory");
     if (NSPLIT == 3) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapA_lo)) : "memory");
     if (NSPLIT >= 2) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapB_lo)) : "memory");
-    for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], epi_warps(EPI)); }
+    for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kEpiWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer (one thread)
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
@@ -396,354 +423,352 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one thread)
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(TBM, TBN, p.fmt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++local) {
-        const int ks = u / (p.m_tiles * p.n_tiles);
-        const int kb0 = ks * p.kb_per_split, kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        const int as = local & 1;
-        const uint32_t aphase = (local >> 1) & 1;
-        mbar_wait(&tempty[as], aphase ^ 1);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * TBN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kOps * Cfg::kABytes;
-          if (NSPLIT == 1 && p.mn_major) {
-            const uint32_t idesc_mn = idesc | ((p.mn_major & 1) ? (1u << 15) : 0u) | ((p.mn_major & 2) ? (1u << 16) : 0u);
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups (wgmma + epilogue)
+  const int g = (warp >> 2) - 1;                // this warpgroup's 64 tile rows start at 64 g
+  const int wq = warp & 3;                      // warp in the warpgroup: fragment rows [16 wq, +16)
+  const int band = wq & 1, colhalf = wq >> 1;   // epilogue: 32-row band of the slab, 32-column half of each 64-column chunk
+  const int quarter = 2 * g + band;             // the tile rows [32 quarter, +32) this warp's lanes hold in the epilogue
+  const int ew = warp - 4;                      // epilogue warp index
+  const uint32_t slab = epi_base + g * kSlabBytes;
+  const uint32_t st = slab + wq * (32 * kStRow * 4);   // this warp's staging tile (overlays the slab once it is read)
+  const bool f16 = (p.fmt & 3) != 0;
+  float conv_bias[32];
+  if (EPI == TC_CONV) {                         // one n-tile (N <= 64): this warp's 32 columns never change
 #pragma unroll
-            for (int k = 0; k < TBK / UMMA_K; ++k) {
-              const uint32_t koff_mn = k * (UMMA_K / 8) * 1024;   // MN-major: 16 reduction rows = two 8-row swizzle atoms
-              const uint32_t koff_k = k * UMMA_K * 2;             // K-major: bytes inside the 128 B swizzle row
-              const uint64_t da = (p.mn_major & 1) ? umma_desc_mn128(sa + koff_mn) : umma_desc_k128(sa + koff_k);
-              const uint64_t db = (p.mn_major & 2) ? umma_desc_mn128(sb + koff_mn) : umma_desc_k128(sb + koff_k);
-              umma_bf16(tmem_d, da, db, idesc_mn, (kb > kb0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit(&empty[stage]);
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-            continue;
-          }
+    for (int j = 0; j < 32; ++j) conv_bias[j] = (32 * colhalf + j < p.N && 32 * colhalf < TBN) ? p.bias[32 * colhalf + j] : 0.f;
+  }
+  bool conv_grp1 = false;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+    const int tiles = p.m_tiles * p.n_tiles;
+    const int ks = u / tiles, t = u - ks * tiles;
+    const int nt = t % p.n_tiles, mt = t / p.n_tiles;
+    const int kb0 = ks * p.kb_per_split, kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+    if (EPI == TC_CONV && p.grp_mt && (mt >= p.grp_mt) != conv_grp1) {   // a CTA's tiles ascend: this happens at most once
+      conv_grp1 = mt >= p.grp_mt;
+      const float* bsrc = conv_grp1 ? p.bias2 : p.bias;
 #pragma unroll
-          for (int k = 0; k < TBK / UMMA_K; ++k) {
-            const uint32_t koff = k * UMMA_K * 2;   // bytes along K inside the 128 B swizzle row
-            const uint64_t a_hi = umma_desc_k128(sa + koff), b_hi = umma_desc_k128(sb + koff);
-            umma_bf16(tmem_d, a_hi, b_hi, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            if (NSPLIT >= 2) umma_bf16(tmem_d, a_hi, umma_desc_k128(sb + Cfg::kBBytes + koff), idesc, 1u);
-            if (NSPLIT == 3) umma_bf16(tmem_d, umma_desc_k128(sa + Cfg::kABytes + koff), b_hi, idesc, 1u);
-          }
-          umma_commit(&empty[stage]);             // smem slot free once these MMAs retire
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      for (int j = 0; j < 32; ++j) conv_bias[j] = (32 * colhalf + j < p.N && 32 * colhalf < TBN) ? bsrc[32 * colhalf + j] : 0.f;
+    }
+    // ---- mainloop: the wgmma groups of one k-block stay in flight while the next k-block's operands are awaited; a
+    // ring slot is released once the groups that read it have retired
+    float acc[TBN / 2];
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t s0 = smem_u32(smem + stage * Cfg::kStageBytes);
+      const uint32_t sa = s0 + g * 8192;        // this warpgroup's 64 rows (K-major) or 64-row MN slab (MN-major) of A
+      const uint32_t sb = s0 + Cfg::kOps * Cfg::kABytes;
+      wgmma_fence();
+      if (NSPLIT == 1 && p.mn_major) {
+#pragma unroll
+        for (int k = 0; k < TBK / MMA_K; ++k) {
+          const uint32_t koff_mn = k * (MMA_K / 8) * 1024;   // MN-major: 16 reduction rows = two 8-row swizzle atoms
+          const uint32_t koff_k = k * MMA_K * 2;             // K-major: bytes inside the 128 B swizzle row
+          const uint64_t da = (p.mn_major & 1) ? gmma_desc_mn128(sa + koff_mn) : gmma_desc_k128(sa + koff_k);
+          const uint64_t db = (p.mn_major & 2) ? gmma_desc_mn128(sb + koff_mn) : gmma_desc_k128(sb + koff_k);
+          wgmma_tile<TBN>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u, f16, p.mn_major);
         }
-        umma_commit(&tfull[as]);                  // accumulator complete
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps (TMEM -> registers -> HBM)
-    const int quarter = warp & 3;                 // TMEM lanes [32*quarter, +32) are the ones this warp may read
-    const int chalf = (warp - 2) >> 2;            // which half of the accumulator columns this warp drains
-    float conv_bias[32];
-    if (EPI == TC_CONV) {                         // one n-tile (N <= 64): this warp's 32 columns never change
-      constexpr int CH0 = TBN >= 64 ? TBN / 2 : TBN;     // (TC_CONV runs two warp sets)
+      } else {
 #pragma unroll
-      for (int j = 0; j < 32; ++j) conv_bias[j] = (chalf * CH0 + j < p.N && chalf * CH0 < TBN) ? p.bias[chalf * CH0 + j] : 0.f;
-    }
-    int local = 0;
-    bool conv_grp1 = false;
-    for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++local) {
-      const int t = u % (p.m_tiles * p.n_tiles);
-      const int nt = t % p.n_tiles, mt = t / p.n_tiles;
-      if (EPI == TC_CONV && p.grp_mt && (mt >= p.grp_mt) != conv_grp1) {   // a CTA's tiles ascend: this happens at most once
-        conv_grp1 = mt >= p.grp_mt;
-        constexpr int CH1 = TBN >= 64 ? TBN / 2 : TBN;
-        const float* bsrc = conv_grp1 ? p.bias2 : p.bias;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) conv_bias[j] = (chalf * CH1 + j < p.N && chalf * CH1 < TBN) ? bsrc[chalf * CH1 + j] : 0.f;
+        for (int k = 0; k < TBK / MMA_K; ++k) {
+          const uint32_t koff = k * MMA_K * 2;   // bytes along K inside the 128 B swizzle row
+          const uint64_t a_hi = gmma_desc_k128(sa + koff), b_hi = gmma_desc_k128(sb + koff);
+          wgmma_tile<TBN>(acc, a_hi, b_hi, (kb > kb0 || k > 0) ? 1u : 0u, f16, 0);
+          if (NSPLIT >= 2) wgmma_tile<TBN>(acc, a_hi, gmma_desc_k128(sb + Cfg::kBBytes + koff), 1u, false, 0);
+          if (NSPLIT == 3) wgmma_tile<TBN>(acc, gmma_desc_k128(sa + Cfg::kABytes + koff), b_hi, 1u, false, 0);
+        }
       }
-      const int as = local & 1;
-      const uint32_t aphase = (local >> 1) & 1;
+      wgmma_commit();
+      wgmma_wait<1>();                          // the previous k-block's groups have retired: its slot is free
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+
+    // ---- epilogue, one 64-column chunk at a time: fragment -> slab -> (row per lane) v[32] -> fused epilogue
+#pragma unroll
+    for (int h = 0; h < (TBN + 63) / 64; ++h) {
+      if (EPI == TC_EMBED && lane == 0) tma_store_wait_read();   // bulk stores of the previous chunk read the staging tiles
+      wg_bar(1 + g);
+      {
+        const uint32_t r0 = slab + ((16 * wq + (lane >> 2)) * kSlabStride + 2 * (lane & 3)) * 4;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int jj = 8 * h + j;
+          if (jj * 8 < TBN) {
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + j * 32), "f"(acc[4 * jj]), "f"(acc[4 * jj + 1]) : "memory");
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + 8 * kSlabStride * 4 + j * 32), "f"(acc[4 * jj + 2]),
+                         "f"(acc[4 * jj + 3]) : "memory");
+          }
+        }
+      }
+      wg_bar(1 + g);
+      const int c = 64 * h + 32 * colhalf;
+      uint32_t v[32];
+      if (c < TBN) {
+        const uint32_t rr = slab + ((32 * band + lane) * kSlabStride + 32 * colhalf) * 4;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const uint4 x = lds128(rr + 16 * j);
+          v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
+        }
+      }
+      wg_bar(1 + g);                            // the slab is read: from here on it holds the per-warp staging tiles
+      if (c >= TBN) continue;
       const int m = mt * TBM + quarter * 32 + lane;
-      constexpr int SETS = epi_warps(EPI) / 4;
-      constexpr int HALF = TBN >= 32 * SETS ? TBN / SETS : TBN;   // columns per warp set (BN = 32: only the first set has columns)
-      // embedding epilogue: lane = row.  The 32 feat / bias values of a chunk are fetched by ONE coalesced load per warp
-      // (lane j loads column j) and broadcast through a 256-byte shared-memory patch; the finished 16-bit tiles are staged
-      // in the TMA 64-byte-swizzle layout and leave through cp.async.bulk.tensor stores -- no per-thread global stores and
-      // no read-back of the staging tile (round 2: the LSU data pipe was the limiter of this kernel)
-      const int e_mbase = mt * TBM + quarter * 32;
-      const bool e_one_sample = (p.batch & 31) == 0;          // sample-major rows: a warp's 32 rows share one feature row
-      const float* embed_feat_row = nullptr;
-      if (EPI == TC_EMBED) embed_feat_row = p.feat + (long)((e_mbase < p.M ? e_mbase : 0) / p.batch) * p.N;
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) + as * TBN;
-#pragma unroll 1
-      for (int c = chalf * HALF; c < (chalf + 1) * HALF && c < TBN; c += 32) {
-        const int n0 = nt * TBN + c;
-        // this chunk's feat / bias values are requested BEFORE the accumulator load: their latency overlaps the TMEM read
-        float ef = 0.f, eb = 0.f;
-        if (EPI == TC_EMBED && n0 + 32 <= p.N) {
-          eb = __ldg(p.bias + n0 + lane);
-          if (e_one_sample) ef = __ldg(embed_feat_row + n0 + lane);
-        }
-        uint32_t v[32];
-        tmem_ld32(trow + c, v);
-        if (m < p.M && n0 < p.N) {
-          if (EPI == TC_STORE || EPI == TC_BIAS_RELU) {
-            float* crow = p.C + (long)m * p.ldc + n0;
-            if (n0 + 32 <= p.N && (EPI == TC_STORE || (p.M & 1) == 0)) {
-              // handled below with the whole warp (coalesced row stores)
-            } else if (n0 + 32 <= p.N) {
+      const int n0 = nt * TBN + c;
+    // embedding epilogue: lane = row.  The 32 feat / bias values of a chunk are fetched by ONE coalesced load per warp
+    // (lane j loads column j) and broadcast through a 256-byte shared-memory patch; the finished 16-bit tiles are staged
+    // in the TMA 64-byte-swizzle layout and leave through cp.async.bulk.tensor stores -- no per-thread global stores and
+    // no read-back of the staging tile
+    const int e_mbase = mt * TBM + quarter * 32;
+    const bool e_one_sample = (p.batch & 31) == 0;          // sample-major rows: a warp's 32 rows share one feature row
+    const float* embed_feat_row = nullptr;
+    if (EPI == TC_EMBED) embed_feat_row = p.feat + (long)((e_mbase < p.M ? e_mbase : 0) / p.batch) * p.N;
+      // this chunk's feat / bias values
+      float ef = 0.f, eb = 0.f;
+      if (EPI == TC_EMBED && n0 + 32 <= p.N) {
+        eb = __ldg(p.bias + n0 + lane);
+        if (e_one_sample) ef = __ldg(embed_feat_row + n0 + lane);
+      }
+      if (m < p.M && n0 < p.N) {
+        if (EPI == TC_STORE || EPI == TC_BIAS_RELU) {
+          float* crow = p.C + ks * p.part_stride + (long)m * p.ldc + n0;
+          if (n0 + 32 <= p.N && (EPI == TC_STORE || (p.M & 1) == 0)) {
+            // handled below with the whole warp (coalesced row stores)
+          } else if (n0 + 32 <= p.N) {
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                       __uint_as_float(v[j + 3]));
-                if (EPI == TC_BIAS_RELU) {
-                  const float4 b = *reinterpret_cast<const float4*>(p.bias + n0 + j);
-                  o.x = fmaxf(o.x + b.x, 0.f); o.y = fmaxf(o.y + b.y, 0.f);
-                  o.z = fmaxf(o.z + b.z, 0.f); o.w = fmaxf(o.w + b.w, 0.f);
-                }
-                *reinterpret_cast<float4*>(crow + j) = o;
-                if (EPI == TC_BIAS_RELU && p.o_hiT) {   // bf16 (N, M) image: lanes = consecutive m -> coalesced
-                  p.o_hiT[(long)(n0 + j) * p.M + m] = __float2bfloat16_rn(o.x);
-                  p.o_hiT[(long)(n0 + j + 1) * p.M + m] = __float2bfloat16_rn(o.y);
-                  p.o_hiT[(long)(n0 + j + 2) * p.M + m] = __float2bfloat16_rn(o.z);
-                  p.o_hiT[(long)(n0 + j + 3) * p.M + m] = __float2bfloat16_rn(o.w);
-                }
+            for (int j = 0; j < 32; j += 4) {
+              float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
+                                     __uint_as_float(v[j + 3]));
+              if (EPI == TC_BIAS_RELU) {
+                const float4 b = *reinterpret_cast<const float4*>(p.bias + n0 + j);
+                o.x = fmaxf(o.x + b.x, 0.f); o.y = fmaxf(o.y + b.y, 0.f);
+                o.z = fmaxf(o.z + b.z, 0.f); o.w = fmaxf(o.w + b.w, 0.f);
               }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                if (n0 + j < p.N) {
-                  float o = __uint_as_float(v[j]);
-                  if (EPI == TC_BIAS_RELU) o = fmaxf(o + p.bias[n0 + j], 0.f);
-                  crow[j] = o;
-                  if (EPI == TC_BIAS_RELU && p.o_hiT) p.o_hiT[(long)(n0 + j) * p.M + m] = __float2bfloat16_rn(o);
-                }
+              *reinterpret_cast<float4*>(crow + j) = o;
+              if (EPI == TC_BIAS_RELU && p.o_hiT) {   // bf16 (N, M) image: lanes = consecutive m -> coalesced
+                p.o_hiT[(long)(n0 + j) * p.M + m] = __float2bfloat16_rn(o.x);
+                p.o_hiT[(long)(n0 + j + 1) * p.M + m] = __float2bfloat16_rn(o.y);
+                p.o_hiT[(long)(n0 + j + 2) * p.M + m] = __float2bfloat16_rn(o.z);
+                p.o_hiT[(long)(n0 + j + 3) * p.M + m] = __float2bfloat16_rn(o.w);
               }
             }
-          } else if (EPI == TC_BIAS_RELU_NCHW) {
-            const int b = m / p.ohw, pp = m - b * p.ohw;
-            float* cb = p.C + ((long)b * p.N + n0) * p.ohw + pp;   // lanes = consecutive pp: coalesced per n
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (n0 + j < p.N) cb[(long)j * p.ohw] = fmaxf(__uint_as_float(v[j]) + p.bias[n0 + j], 0.f);
-          } else if (EPI == TC_EMBED || EPI == TC_COL2IM || EPI == TC_CONV) {
-            // handled below with the whole warp
-          } else if (!(p.vec_acc && n0 + 32 <= p.N)) {
-            float* crow = p.C + (long)m * p.ldc + n0;
+          } else {
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
               if (n0 + j < p.N) {
-                const float o = __uint_as_float(v[j]) * (EPI == TC_ATOMIC ? p.alpha : 1.f);
-                if (p.k_splits == 1) {   // sole contributor: += without atomics
-                  crow[j] += o;
-                  if (EPI == TC_NOISY_WGRAD) p.out2[(long)m * p.ldc + n0 + j] += o * p.eps[(long)m * p.ldc + n0 + j];
-                } else {
-                  atomicAdd(crow + j, o);
-                  if (EPI == TC_NOISY_WGRAD)
-                    atomicAdd(p.out2 + (long)m * p.ldc + n0 + j, o * p.eps[(long)m * p.ldc + n0 + j]);
-                }
+                float o = __uint_as_float(v[j]);
+                if (EPI == TC_BIAS_RELU) o = fmaxf(o + p.bias[n0 + j], 0.f);
+                crow[j] = o;
+                if (EPI == TC_BIAS_RELU && p.o_hiT) p.o_hiT[(long)(n0 + j) * p.M + m] = __float2bfloat16_rn(o);
               }
             }
           }
-        }
-        if (EPI == TC_CONV && n0 < p.N) {
-          // strip convolution: relu(acc + bias) -> (optional) fp32 NCHW output + the NEXT layer's space-to-depth images.
-          // The bias of this warp's 32 columns sits in registers for the whole kernel (N <= 64 = one n-tile); the image
-          // rows go through the staging transpose so that a quarter-warp writes one pixel's 64-byte channel run.
-          const int gg = p.strip_G * p.strip_G;
-          const int mm = m < p.M ? m : 0;
-          const int b = mm / gg, rem = mm - b * gg;
-          const int gy = rem / p.strip_G, gx = rem - gy * p.strip_G;
-          const bool valid = m < p.M && gy < p.cv_oh && gx < p.cv_ow;
-          float x[32];
+        } else if (EPI == TC_BIAS_RELU_NCHW) {
+          const int b = m / p.ohw, pp = m - b * p.ohw;
+          float* cb = p.C + ((long)b * p.N + n0) * p.ohw + pp;   // lanes = consecutive pp: coalesced per n
 #pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = n0 + j < p.N ? fmaxf(__uint_as_float(v[j]) + conv_bias[j], 0.f) : 0.f;
-          if (p.C != nullptr && valid) {
-            const int plane = p.cv_oh * p.cv_ow;
-            float* cb = p.C + ((long)b * p.N + n0) * plane + gy * p.cv_ow + gx;     // lanes = consecutive gx
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (n0 + j < p.N) cb[(long)j * plane] = x[j];
-          }
-          if (p.nx_hi != nullptr && n0 + 32 <= p.N) {          // warp-uniform
-            // this pixel's channels are contiguous in the next layer's space-to-depth row
-            long o = -1;
-            if (valid) {
-              const int sn = p.nx_s, by = gy / sn, bx = gx / sn;
-              const long r = ((long)b * p.nx_G + by) * p.nx_G + bx;
-              o = r * ((long)sn * sn * p.N) + (long)((gy - by * sn) * sn + (gx - bx * sn)) * p.N + n0;
-            }
-            uint32_t hw[32];      // [0..15] hi pairs, [16..31] lo pairs
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) {
-              const uint32_t hwj = pack16x2(x[j], x[j + 1], false);
-              hw[j / 2] = hwj;
-              hw[16 + j / 2] = pack16x2(x[j] - __uint_as_float(hwj << 16), x[j + 1] - __uint_as_float(hwj & 0xffff0000u), false);
-            }
-            const uint32_t st = epi_stage + (warp - 2) * (32 * kStRow * 4);
-            stage_row(st, hw, lane);
-            const int sub = lane >> 3, piece = lane & 7;
-            bf16* dstb = piece < 4 ? p.nx_hi : p.nx_lo;
-            uint4 pc[8];                      // all pieces in flight before the first store (one shared-memory latency)
-            long orow[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              pc[i] = staged_piece(st, 4 * i + sub, piece);
-              orow[i] = __shfl_sync(0xffffffffu, o, 4 * i + sub);
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              if (orow[i] >= 0 && dstb != nullptr) *reinterpret_cast<uint4*>(dstb + orow[i] + (piece & 3) * 8) = pc[i];
-          }
-        }
-        if (EPI == TC_COL2IM && n0 < p.N) {
-          // din[b, c, oh*s + kh, ow*s + kw] += dcol[m, (c, kh, kw)]: lane j decodes column n0 + j once, the offsets are
-          // broadcast by shuffle; lanes = consecutive output pixels, so one red instruction touches a few lines
-          const int khw = p.ci_kh * p.ci_kw;
-          const int kcol = n0 + lane;
-          int coff = -1;
-          if (kcol < p.N) {
-            const int c = kcol / khw, r = kcol - c * khw;
-            const int kh = r / p.ci_kw, kw = r - kh * p.ci_kw;
-            coff = (c * p.ci_h + kh) * p.ci_w + kw;
-          }
-          bool row_ok = m < p.M;
-          const int mm = row_ok ? m : 0;
-          const int b = mm / p.ohw, pp = mm - b * p.ohw;                 // ohw = G*G on the strip grid
-          const int rw = p.ci_G ? p.ci_G : p.ci_ow;
-          const int oh = pp / rw, ow = pp - oh * rw;
-          if (p.ci_G) row_ok = row_ok && oh < p.ci_oh && ow < p.ci_ow;   // grid rows beyond the real outputs carry zeros
-          float* base = p.C + ((long)b * p.ci_cin * p.ci_h + oh * p.ci_stride) * p.ci_w + ow * p.ci_stride;
+          for (int j = 0; j < 32; ++j)
+            if (n0 + j < p.N) cb[(long)j * p.ohw] = fmaxf(__uint_as_float(v[j]) + p.bias[n0 + j], 0.f);
+        } else if (EPI == TC_EMBED || EPI == TC_COL2IM || EPI == TC_CONV) {
+          // handled below with the whole warp
+        } else if (!(p.vec_acc && n0 + 32 <= p.N)) {
+          float* crow = p.C + (long)m * p.ldc + n0;
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
-            const int off = __shfl_sync(0xffffffffu, coff, j);
-            if (row_ok && off >= 0)
-              asm volatile("red.global.add.f32 [%0], %1;" ::"l"(base + off), "f"(__uint_as_float(v[j])) : "memory");
-          }
-        }
-        if ((EPI == TC_STORE || EPI == TC_EMBED || (EPI == TC_BIAS_RELU && (p.M & 1) == 0) ||
-             ((EPI == TC_ATOMIC || EPI == TC_NOISY_WGRAD) && p.vec_acc)) && n0 + 32 <= p.N) {
-          const uint32_t st = epi_stage + (warp - 2) * (32 * kStRow * 4);
-          const int m_base = mt * TBM + quarter * 32;
-          const int rows_valid = min(32, p.M - m_base);            // warp-uniform
-          if (rows_valid > 0) {
-            if (EPI == TC_STORE) {
-              if (p.o_hi != nullptr) {                           // bf16 result (M, N) instead of fp32: 64-byte row pieces
-                uint32_t hw2[32];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                  const __nv_bfloat162 h2 = __floats2bfloat162_rn(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-                  hw2[j] = *reinterpret_cast<const uint32_t*>(&h2);
-                  hw2[16 + j] = 0u;
-                }
-                warp_store_rows_bf16(st, hw2, lane, p.o_hi + (long)m_base * p.N + n0, nullptr, p.N, rows_valid);
-              } else {
-                warp_store_rows_f32(st, v, lane, p.C + (long)m_base * p.ldc + n0, p.ldc, rows_valid);
-              }
-            } else if (EPI == TC_ATOMIC) {
-              warp_accum_rows_f32<false>(st, v, lane, p.C + (long)m_base * p.ldc + n0, nullptr, nullptr, p.ldc, rows_valid,
-                                         p.k_splits > 1, p.alpha);
-            } else if (EPI == TC_NOISY_WGRAD) {
-              const long o0 = (long)m_base * p.ldc + n0;
-              warp_accum_rows_f32<true>(st, v, lane, p.C + o0, p.out2 + o0, p.eps + o0, p.ldc, rows_valid, p.k_splits > 1,
-                                        1.f);
-            } else if (EPI == TC_BIAS_RELU) {
-              const float* br = p.bias + n0;
-              uint32_t hw[16];
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(br + j));
-                const float x0 = fmaxf(__uint_as_float(v[j]) + bb.x, 0.f), x1 = fmaxf(__uint_as_float(v[j + 1]) + bb.y, 0.f);
-                const float x2 = fmaxf(__uint_as_float(v[j + 2]) + bb.z, 0.f), x3 = fmaxf(__uint_as_float(v[j + 3]) + bb.w, 0.f);
-                const __nv_bfloat162 h01 = __floats2bfloat162_rn(x0, x1), h23 = __floats2bfloat162_rn(x2, x3);
-                hw[j / 2] = *reinterpret_cast<const uint32_t*>(&h01);
-                hw[j / 2 + 1] = *reinterpret_cast<const uint32_t*>(&h23);
-                v[j] = __float_as_uint(x0); v[j + 1] = __float_as_uint(x1);
-                v[j + 2] = __float_as_uint(x2); v[j + 3] = __float_as_uint(x3);
-              }
-              if (p.o_hiT) store_transposed_pairs(p.o_hiT, hw, n0, m, p.M, lane, m < p.M);
-              warp_store_rows_f32(st, v, lane, p.C + (long)m_base * p.ldc + n0, p.ldc, rows_valid);
-              if (p.o_hi) {                                     // bf16 row-major image (M, N): 64-byte row pieces
-                uint32_t hw2[32];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) { hw2[j] = hw[j]; hw2[16 + j] = 0u; }
-                warp_store_rows_bf16(st, hw2, lane, p.o_hi + (long)m_base * p.N + n0, nullptr, p.N, rows_valid);
-              }
-            } else {
-              // x = feat[b] * relu(acc + bias)   (model.py:146-151); N % 32 == 0 is required by the host wrapper.
-              const bool f16 = (p.fmt & 4) != 0;
-              const uint32_t fb = epi_fb + (warp - 2) * 256;
-              const bool row_ok = m < p.M;
-              const float* frow = p.feat + (long)((row_ok ? m : 0) / p.batch) * p.N + n0;   // per-row feat (several samples per warp)
-              // one image: the two 2 KB halves of the staging tile alternate, so only the store of TWO tiles ago must have
-              // read its half (the store of the previous tile stays in flight); two images use both halves every tile
-              const bool one_img = p.o_lo == nullptr;
-              const uint32_t st0 = one_img ? st + (local & 1) * 2048 : st;
-              if (lane == 0) { if (one_img) tma_store_wait_read1(); else tma_store_wait_read(); }
-              __syncwarp();
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(fb + lane * 4), "r"(__float_as_uint(ef)) : "memory");
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(fb + 128 + lane * 4), "r"(__float_as_uint(eb)) : "memory");
-              __syncwarp();
-              uint32_t w0[16], w1[16];                            // image 0 / image 1 column pairs of this lane's row
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const uint4 bu = lds128(fb + 128 + 16 * j);
-                uint4 fu;
-                if (e_one_sample) fu = lds128(fb + 16 * j);
-                else fu = __ldg(reinterpret_cast<const uint4*>(frow) + j);
-                const float x0 = __uint_as_float(fu.x) * fmaxf(__uint_as_float(v[4 * j]) + __uint_as_float(bu.x), 0.f);
-                const float x1 = __uint_as_float(fu.y) * fmaxf(__uint_as_float(v[4 * j + 1]) + __uint_as_float(bu.y), 0.f);
-                const float x2 = __uint_as_float(fu.z) * fmaxf(__uint_as_float(v[4 * j + 2]) + __uint_as_float(bu.z), 0.f);
-                const float x3 = __uint_as_float(fu.w) * fmaxf(__uint_as_float(v[4 * j + 3]) + __uint_as_float(bu.w), 0.f);
-                if (p.C && row_ok) *reinterpret_cast<float4*>(p.C + (long)m * p.N + n0 + 4 * j) = make_float4(x0, x1, x2, x3);
-                if (f16) {            // fp16(x) feeds the single-pass head forward, bf16(x) the backward products
-                  w0[2 * j] = pack16x2(x0, x1, true); w0[2 * j + 1] = pack16x2(x2, x3, true);
-                  w1[2 * j] = pack16x2(x0, x1, false); w1[2 * j + 1] = pack16x2(x2, x3, false);
-                } else {              // bf16 hi + residual lo (split-bf16 x3 head forward)
-                  const uint32_t h0 = pack16x2(x0, x1, false), h1 = pack16x2(x2, x3, false);
-                  w0[2 * j] = h0; w0[2 * j + 1] = h1;
-                  w1[2 * j] = pack16x2(x0 - __uint_as_float(h0 << 16), x1 - __uint_as_float(h0 & 0xffff0000u), false);
-                  w1[2 * j + 1] = pack16x2(x2 - __uint_as_float(h1 << 16), x3 - __uint_as_float(h1 & 0xffff0000u), false);
-                }
-              }
-              // 32 rows x 64 bytes per image in the TMA SWIZZLE_64B layout: 16-byte chunk c of row r sits at chunk c ^ ((r >> 1) & 3)
-              const uint32_t srow = st0 + lane * 64;
-              const int sw = (lane >> 1) & 3;
-#pragma unroll
-              for (int c = 0; c < 4; ++c) {
-                if (p.o_hi) sts128(srow + ((c ^ sw) << 4), w0[4 * c], w0[4 * c + 1], w0[4 * c + 2], w0[4 * c + 3]);
-                if (p.o_lo) sts128(srow + 2048 + ((c ^ sw) << 4), w1[4 * c], w1[4 * c + 1], w1[4 * c + 2], w1[4 * c + 3]);
-              }
-              fence_proxy_async();                                // generic-proxy writes -> visible to the TMA engine
-              __syncwarp();
-              if (lane == 0) {
-                if (p.o_hi) tma_store_2d(&p.mapO[0], st0, n0, m_base);
-                if (p.o_lo) tma_store_2d(&p.mapO[1], st0 + 2048, n0, m_base);
-                tma_store_commit();
-              }
+            if (n0 + j < p.N) {
+              const float o = __uint_as_float(v[j]) * (EPI == TC_ATOMIC ? p.alpha : 1.f);
+              crow[j] += o;              // the only writer of these rows (split-K: per-split partials)
+              if (EPI == TC_NOISY_WGRAD) p.out2[(long)m * p.ldc + n0 + j] += o * p.eps[(long)m * p.ldc + n0 + j];
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
+      if (EPI == TC_CONV && n0 < p.N) {
+        // strip convolution: relu(acc + bias) -> (optional) fp32 NCHW output + the NEXT layer's space-to-depth images.
+        // The bias of this warp's 32 columns sits in registers for the whole kernel (N <= 64 = one n-tile); the image
+        // rows go through the staging transpose so that a quarter-warp writes one pixel's 64-byte channel run.
+        const int gg = p.strip_G * p.strip_G;
+        const int mm = m < p.M ? m : 0;
+        const int b = mm / gg, rem = mm - b * gg;
+        const int gy = rem / p.strip_G, gx = rem - gy * p.strip_G;
+        const bool valid = m < p.M && gy < p.cv_oh && gx < p.cv_ow;
+        float x[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) x[j] = n0 + j < p.N ? fmaxf(__uint_as_float(v[j]) + conv_bias[j], 0.f) : 0.f;
+        if (p.C != nullptr && valid) {
+          const int plane = p.cv_oh * p.cv_ow;
+          float* cb = p.C + ((long)b * p.N + n0) * plane + gy * p.cv_ow + gx;     // lanes = consecutive gx
+#pragma unroll
+          for (int j = 0; j < 32; ++j)
+            if (n0 + j < p.N) cb[(long)j * plane] = x[j];
+        }
+        if (p.nx_hi != nullptr && n0 + 32 <= p.N) {          // warp-uniform
+          // this pixel's channels are contiguous in the next layer's space-to-depth row
+          long o = -1;
+          if (valid) {
+            const int sn = p.nx_s, by = gy / sn, bx = gx / sn;
+            const long r = ((long)b * p.nx_G + by) * p.nx_G + bx;
+            o = r * ((long)sn * sn * p.N) + (long)((gy - by * sn) * sn + (gx - bx * sn)) * p.N + n0;
+          }
+          uint32_t hw[32];      // [0..15] hi pairs, [16..31] lo pairs
+#pragma unroll
+          for (int j = 0; j < 32; j += 2) {
+            const uint32_t hwj = pack16x2(x[j], x[j + 1], false);
+            hw[j / 2] = hwj;
+            hw[16 + j / 2] = pack16x2(x[j] - __uint_as_float(hwj << 16), x[j + 1] - __uint_as_float(hwj & 0xffff0000u), false);
+          }
+          stage_row(st, hw, lane);
+          const int sub = lane >> 3, piece = lane & 7;
+          bf16* dstb = piece < 4 ? p.nx_hi : p.nx_lo;
+          uint4 pc[8];                      // all pieces in flight before the first store (one shared-memory latency)
+          long orow[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            pc[i] = staged_piece(st, 4 * i + sub, piece);
+            orow[i] = __shfl_sync(0xffffffffu, o, 4 * i + sub);
+          }
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (orow[i] >= 0 && dstb != nullptr) *reinterpret_cast<uint4*>(dstb + orow[i] + (piece & 3) * 8) = pc[i];
+        }
+      }
+      if (EPI == TC_COL2IM && n0 < p.N) {
+        // din[b, c, oh*s + kh, ow*s + kw] += dcol[m, (c, kh, kw)]: lane j decodes column n0 + j once, the offsets are
+        // broadcast by shuffle; lanes = consecutive output pixels, so one red instruction touches a few lines
+        const int khw = p.ci_kh * p.ci_kw;
+        const int kcol = n0 + lane;
+        int coff = -1;
+        if (kcol < p.N) {
+          const int c = kcol / khw, r = kcol - c * khw;
+          const int kh = r / p.ci_kw, kw = r - kh * p.ci_kw;
+          coff = (c * p.ci_h + kh) * p.ci_w + kw;
+        }
+        bool row_ok = m < p.M;
+        const int mm = row_ok ? m : 0;
+        const int b = mm / p.ohw, pp = mm - b * p.ohw;                 // ohw = G*G on the strip grid
+        const int rw = p.ci_G ? p.ci_G : p.ci_ow;
+        const int oh = pp / rw, ow = pp - oh * rw;
+        if (p.ci_G) row_ok = row_ok && oh < p.ci_oh && ow < p.ci_ow;   // grid rows beyond the real outputs carry zeros
+        float* base = p.C + ((long)b * p.ci_cin * p.ci_h + oh * p.ci_stride) * p.ci_w + ow * p.ci_stride;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int off = __shfl_sync(0xffffffffu, coff, j);
+          if (row_ok && off >= 0)
+            asm volatile("red.global.add.f32 [%0], %1;" ::"l"(base + off), "f"(__uint_as_float(v[j])) : "memory");
+        }
+      }
+      if ((EPI == TC_STORE || EPI == TC_EMBED || (EPI == TC_BIAS_RELU && (p.M & 1) == 0) ||
+           ((EPI == TC_ATOMIC || EPI == TC_NOISY_WGRAD) && p.vec_acc)) && n0 + 32 <= p.N) {
+        const int m_base = mt * TBM + quarter * 32;
+        const int rows_valid = min(32, p.M - m_base);            // warp-uniform
+        if (rows_valid > 0) {
+          if (EPI == TC_STORE) {
+            if (p.o_hi != nullptr) {                           // bf16 result (M, N) instead of fp32: 64-byte row pieces
+              uint32_t hw2[32];
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+                const __nv_bfloat162 h2 = __floats2bfloat162_rn(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
+                hw2[j] = *reinterpret_cast<const uint32_t*>(&h2);
+                hw2[16 + j] = 0u;
+              }
+              warp_store_rows_bf16(st, hw2, lane, p.o_hi + (long)m_base * p.N + n0, nullptr, p.N, rows_valid);
+            } else {
+              warp_store_rows_f32(st, v, lane, p.C + ks * p.part_stride + (long)m_base * p.ldc + n0, p.ldc, rows_valid);
+            }
+          } else if (EPI == TC_ATOMIC) {
+            warp_accum_rows_f32<false>(st, v, lane, p.C + (long)m_base * p.ldc + n0, nullptr, nullptr, p.ldc, rows_valid,
+                                       p.alpha);
+          } else if (EPI == TC_NOISY_WGRAD) {
+            const long o0 = (long)m_base * p.ldc + n0;
+            warp_accum_rows_f32<true>(st, v, lane, p.C + o0, p.out2 + o0, p.eps + o0, p.ldc, rows_valid, 1.f);
+          } else if (EPI == TC_BIAS_RELU) {
+            const float* br = p.bias + n0;
+            uint32_t hw[16];
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              const float4 bb = __ldg(reinterpret_cast<const float4*>(br + j));
+              const float x0 = fmaxf(__uint_as_float(v[j]) + bb.x, 0.f), x1 = fmaxf(__uint_as_float(v[j + 1]) + bb.y, 0.f);
+              const float x2 = fmaxf(__uint_as_float(v[j + 2]) + bb.z, 0.f), x3 = fmaxf(__uint_as_float(v[j + 3]) + bb.w, 0.f);
+              const __nv_bfloat162 h01 = __floats2bfloat162_rn(x0, x1), h23 = __floats2bfloat162_rn(x2, x3);
+              hw[j / 2] = *reinterpret_cast<const uint32_t*>(&h01);
+              hw[j / 2 + 1] = *reinterpret_cast<const uint32_t*>(&h23);
+              v[j] = __float_as_uint(x0); v[j + 1] = __float_as_uint(x1);
+              v[j + 2] = __float_as_uint(x2); v[j + 3] = __float_as_uint(x3);
+            }
+            if (p.o_hiT) store_transposed_pairs(p.o_hiT, hw, n0, m, p.M, lane, m < p.M);
+            warp_store_rows_f32(st, v, lane, p.C + ks * p.part_stride + (long)m_base * p.ldc + n0, p.ldc, rows_valid);
+            if (p.o_hi) {                                     // bf16 row-major image (M, N): 64-byte row pieces
+              uint32_t hw2[32];
+#pragma unroll
+              for (int j = 0; j < 16; ++j) { hw2[j] = hw[j]; hw2[16 + j] = 0u; }
+              warp_store_rows_bf16(st, hw2, lane, p.o_hi + (long)m_base * p.N + n0, nullptr, p.N, rows_valid);
+            }
+          } else {
+            // x = feat[b] * relu(acc + bias)   (model.py:146-151); N % 32 == 0 is required by the host wrapper.
+            const bool f16 = (p.fmt & 4) != 0;
+            const uint32_t fb = epi_fb + ew * 256;
+            const bool row_ok = m < p.M;
+            const float* frow = p.feat + (long)((row_ok ? m : 0) / p.batch) * p.N + n0;   // per-row feat (several samples per warp)
+            const uint32_t st0 = st;                            // o_hi in the first 2 KB, o_lo in the second
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(fb + lane * 4), "r"(__float_as_uint(ef)) : "memory");
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(fb + 128 + lane * 4), "r"(__float_as_uint(eb)) : "memory");
+            __syncwarp();
+            uint32_t w0[16], w1[16];                            // image 0 / image 1 column pairs of this lane's row
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const uint4 bu = lds128(fb + 128 + 16 * j);
+              uint4 fu;
+              if (e_one_sample) fu = lds128(fb + 16 * j);
+              else fu = __ldg(reinterpret_cast<const uint4*>(frow) + j);
+              const float x0 = __uint_as_float(fu.x) * fmaxf(__uint_as_float(v[4 * j]) + __uint_as_float(bu.x), 0.f);
+              const float x1 = __uint_as_float(fu.y) * fmaxf(__uint_as_float(v[4 * j + 1]) + __uint_as_float(bu.y), 0.f);
+              const float x2 = __uint_as_float(fu.z) * fmaxf(__uint_as_float(v[4 * j + 2]) + __uint_as_float(bu.z), 0.f);
+              const float x3 = __uint_as_float(fu.w) * fmaxf(__uint_as_float(v[4 * j + 3]) + __uint_as_float(bu.w), 0.f);
+              if (p.C && row_ok) *reinterpret_cast<float4*>(p.C + (long)m * p.N + n0 + 4 * j) = make_float4(x0, x1, x2, x3);
+              if (f16) {            // fp16(x) feeds the single-pass head forward, bf16(x) the backward products
+                w0[2 * j] = pack16x2(x0, x1, true); w0[2 * j + 1] = pack16x2(x2, x3, true);
+                w1[2 * j] = pack16x2(x0, x1, false); w1[2 * j + 1] = pack16x2(x2, x3, false);
+              } else {              // bf16 hi + residual lo (split-bf16 x3 head forward)
+                const uint32_t h0 = pack16x2(x0, x1, false), h1 = pack16x2(x2, x3, false);
+                w0[2 * j] = h0; w0[2 * j + 1] = h1;
+                w1[2 * j] = pack16x2(x0 - __uint_as_float(h0 << 16), x1 - __uint_as_float(h0 & 0xffff0000u), false);
+                w1[2 * j + 1] = pack16x2(x2 - __uint_as_float(h1 << 16), x3 - __uint_as_float(h1 & 0xffff0000u), false);
+              }
+            }
+            // 32 rows x 64 bytes per image in the TMA SWIZZLE_64B layout: 16-byte chunk c of row r sits at chunk c ^ ((r >> 1) & 3)
+            const uint32_t srow = st0 + lane * 64;
+            const int sw = (lane >> 1) & 3;
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              if (p.o_hi) sts128(srow + ((c ^ sw) << 4), w0[4 * c], w0[4 * c + 1], w0[4 * c + 2], w0[4 * c + 3]);
+              if (p.o_lo) sts128(srow + 2048 + ((c ^ sw) << 4), w1[4 * c], w1[4 * c + 1], w1[4 * c + 2], w1[4 * c + 3]);
+            }
+            fence_proxy_async();                                // generic-proxy writes -> visible to the TMA engine
+            __syncwarp();
+            if (lane == 0) {
+              if (p.o_hi) tma_store_2d(&p.mapO[0], st0, n0, m_base);
+              if (p.o_lo) tma_store_2d(&p.mapO[1], st0 + 2048, n0, m_base);
+              tma_store_commit();
+            }
+          }
+        }
+      }
     }
   }
-  if (EPI == TC_EMBED && warp >= 2 && lane == 0) tma_store_wait_all();   // bulk stores read this CTA's shared memory
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
-  }
+  if (EPI == TC_EMBED && lane == 0) tma_store_wait_all();   // bulk stores read this CTA's shared memory
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -806,8 +831,21 @@ static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUt
   }
   const int units = p.m_tiles * p.n_tiles * p.k_splits;
   const int grid = units < sms ? units : sms;
-  gemm_tc_kernel<NSPLIT, EPI, BN><<<grid, tc_threads(EPI), Cfg::kSmemBytes, s>>>(a_hi, a_lo, b_hi, b_lo, p);
+  gemm_tc_kernel<NSPLIT, EPI, BN><<<grid, kTcThreads, Cfg::kSmemBytes, s>>>(a_hi, a_lo, b_hi, b_lo, p);
   return (int)cudaGetLastError();
+}
+
+// C[m, n] += alpha * sum_k part[k][m, n] (k ascending); out2[m, n] += (sum_k part[k][m, n]) * eps[m, n] when out2 is set
+__global__ void split_k_reduce_kernel(int M, int N, int splits, long stride, long ldp, const float* __restrict__ part,
+                                      float* __restrict__ C, long ldc, float alpha, float* __restrict__ out2,
+                                      const float* __restrict__ eps) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)M * N) return;
+  const long m = i / N, n = i - m * N;
+  float acc = 0.f;
+  for (int k = 0; k < splits; ++k) acc += part[k * stride + m * ldp + n];
+  C[m * ldc + n] += alpha * acc;
+  if (out2 != nullptr) out2[m * ldc + n] += acc * eps[m * ldc + n];
 }
 
 // C (+)= A * B^T on the tensor cores.  A (M,K), B (N,K) bf16 row-major (K % 8 == 0); *_lo may be null (NSPLIT 1).
@@ -832,17 +870,9 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
         (((ex->mn_major & 3) != 3) && (K % 8)))
       return (int)cudaErrorInvalidValue;
   }
-  int bn = (ex != nullptr && ex->mn_major) ? ((narrow_ok && N <= 64) ? 64 : 256)
-                                           : (narrow_ok && N <= 32) ? 32 : (narrow_ok && N <= 64) ? 64 : 256;
-  if (epi == TC_BIAS_RELU && split3 && !(ex != nullptr && ex->mn_major) && N % 128 == 0) {
-    // head forward with few rows (K = 32 quantiles): 128-wide tiles when they fill the persistent grid's last round
-    // noticeably better (512 tiles = 3.46 rounds of 148 CTAs -> 1024 half tiles = 6.92 rounds)
-    const long mt = (M + TBM - 1) / TBM, t256 = mt * ((N + 255) / 256), t128 = mt * (N / 128);
-    auto eff = [](long t) { const long r = (t + 147) / 148; return (double)t / (double)(r * 148); };
-    if (eff(t128) > eff(t256) + 0.08) bn = 128;
-  }
-  if (epi == TC_EMBED) bn = 128;   // four epilogue warp sets x one 32-column chunk; 64 KB stages leave room for their staging
-  // (32-wide tiles for conv3's 324 strip tiles were tried: slower -- only four epilogue warps drain a 32-column tile)
+  // 128-wide tiles: the m64n128 accumulator of each consumer warpgroup is 64 registers per thread
+  const int bn = (ex != nullptr && ex->mn_major) ? ((narrow_ok && N <= 64) ? 64 : 128)
+                                                 : (narrow_ok && N <= 32) ? 32 : (narrow_ok && N <= 64) ? 64 : 128;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
   if (mn) {
@@ -873,11 +903,13 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
   p.n_tiles = (N + bn - 1) / bn;
   p.kb_total = (K + TBK - 1) / TBK;
   if (split_k < 1) split_k = 1;
+  // at most one round of CTAs: more splits would only multiply the partial sums written to scratch (gemm.h)
+  if (split_k > tc_max_split(p.m_tiles * p.n_tiles)) split_k = tc_max_split(p.m_tiles * p.n_tiles);
   if (split_k > p.kb_total) split_k = p.kb_total;
   p.kb_per_split = (p.kb_total + split_k - 1) / split_k;
   p.k_splits = (p.kb_total + p.kb_per_split - 1) / p.kb_per_split;
   if (p.k_splits > 1 && epi != TC_ATOMIC && epi != TC_NOISY_WGRAD) return (int)cudaErrorInvalidValue;
-  p.C = C; p.ldc = ldc; p.bias = bias; p.out2 = out2; p.eps = eps;
+  p.C = C; p.ldc = ldc; p.bias = bias; p.out2 = out2; p.eps = eps; p.part_stride = 0;
   p.alpha = ex ? ex->alpha : 1.f;
   p.vec_acc = (ldc % 4 == 0) && (reinterpret_cast<uintptr_t>(C) & 15) == 0 && (reinterpret_cast<uintptr_t>(out2) & 15) == 0 &&
               (reinterpret_cast<uintptr_t>(eps) & 15) == 0;
@@ -902,51 +934,67 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
     if (ex->b2_lo && (rc = make_map(&p.mapO[1], ex->b2_lo, N, K, bn))) return rc;
   }
   if ((p.fmt & 3) && (split3 || split2)) return (int)cudaErrorInvalidValue;      // fp16 images are single-pass operands
-  if ((p.fmt & 3) == 1 || (p.fmt & 3) == 2) return (int)cudaErrorInvalidValue;   // mixed fp16 x bf16: illegal instruction
+  if ((p.fmt & 3) == 1 || (p.fmt & 3) == 2) return (int)cudaErrorInvalidValue;   // wgmma takes one 16-bit format for A and B
   if ((p.fmt & 4) && epi != TC_EMBED) return (int)cudaErrorInvalidValue;
   if (epi == TC_EMBED && ((N % 32) || (M % 2) || p.o_hiT || p.o_loT)) return (int)cudaErrorInvalidValue;
   if (epi == TC_EMBED) {            // the 16-bit images leave through TMA stores
     if (p.o_hi && (rc = make_store_map(&p.mapO[0], p.o_hi, M, N))) return rc;
     if (p.o_lo && (rc = make_store_map(&p.mapO[1], p.o_lo, M, N))) return rc;
   }
-#define RIQN_TC_GO(NS, EP) return launch_tc<NS, EP, 256>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
+  const auto go = [&](int epi) -> int {
+#define RIQN_TC_GO(NS, EP) return launch_tc<NS, EP, 128>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
 #define RIQN_TC_NARROW(NS, EP)                                                                  \
-  if (bn == 32) return launch_tc<NS, EP, 32>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);                  \
-  if (bn == 64) return launch_tc<NS, EP, 64>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
-  if (split3) {
-    switch (epi) {
-      case TC_STORE: RIQN_TC_GO(3, TC_STORE);
-      case TC_BIAS_RELU:
-        if (bn == 128) return launch_tc<3, TC_BIAS_RELU, 128>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
-        RIQN_TC_GO(3, TC_BIAS_RELU);
-      case TC_ATOMIC: RIQN_TC_GO(3, TC_ATOMIC);
-      case TC_NOISY_WGRAD: RIQN_TC_GO(3, TC_NOISY_WGRAD);
-      case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(3, TC_BIAS_RELU_NCHW); RIQN_TC_GO(3, TC_BIAS_RELU_NCHW);
-      case TC_CONV: RIQN_TC_NARROW(3, TC_CONV); break;
-      case TC_EMBED: return launch_tc<3, TC_EMBED, 128>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
+    if (bn == 32) return launch_tc<NS, EP, 32>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);                  \
+    if (bn == 64) return launch_tc<NS, EP, 64>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
+    if (split3) {
+      switch (epi) {
+        case TC_STORE: RIQN_TC_GO(3, TC_STORE);
+        case TC_BIAS_RELU: RIQN_TC_GO(3, TC_BIAS_RELU);
+        case TC_ATOMIC: RIQN_TC_GO(3, TC_ATOMIC);
+        case TC_NOISY_WGRAD: RIQN_TC_GO(3, TC_NOISY_WGRAD);
+        case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(3, TC_BIAS_RELU_NCHW); RIQN_TC_GO(3, TC_BIAS_RELU_NCHW);
+        case TC_CONV: RIQN_TC_NARROW(3, TC_CONV); break;
+        case TC_EMBED: RIQN_TC_GO(3, TC_EMBED);
+      }
+    } else if (split2) {
+      switch (epi) {
+        case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(2, TC_BIAS_RELU_NCHW); RIQN_TC_GO(2, TC_BIAS_RELU_NCHW);
+        case TC_CONV: RIQN_TC_NARROW(2, TC_CONV); break;
+        case TC_STORE: RIQN_TC_GO(2, TC_STORE);
+        default: return (int)cudaErrorInvalidValue;
+      }
+    } else {
+      switch (epi) {
+        case TC_STORE: RIQN_TC_NARROW(1, TC_STORE); RIQN_TC_GO(1, TC_STORE);
+        case TC_COL2IM: RIQN_TC_GO(1, TC_COL2IM);
+        case TC_BIAS_RELU: RIQN_TC_GO(1, TC_BIAS_RELU);
+        case TC_ATOMIC: RIQN_TC_NARROW(1, TC_ATOMIC); RIQN_TC_GO(1, TC_ATOMIC);
+        case TC_NOISY_WGRAD: RIQN_TC_GO(1, TC_NOISY_WGRAD);
+        case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(1, TC_BIAS_RELU_NCHW); RIQN_TC_GO(1, TC_BIAS_RELU_NCHW);
+        case TC_CONV: RIQN_TC_NARROW(1, TC_CONV); break;
+        case TC_EMBED: RIQN_TC_GO(1, TC_EMBED);
+      }
     }
-  } else if (split2) {
-    switch (epi) {
-      case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(2, TC_BIAS_RELU_NCHW); RIQN_TC_GO(2, TC_BIAS_RELU_NCHW);
-      case TC_CONV: RIQN_TC_NARROW(2, TC_CONV); break;
-      case TC_STORE: RIQN_TC_GO(2, TC_STORE);
-      default: return (int)cudaErrorInvalidValue;
-    }
-  } else {
-    switch (epi) {
-      case TC_STORE: RIQN_TC_NARROW(1, TC_STORE); RIQN_TC_GO(1, TC_STORE);
-      case TC_COL2IM: RIQN_TC_GO(1, TC_COL2IM);
-      case TC_BIAS_RELU: RIQN_TC_GO(1, TC_BIAS_RELU);
-      case TC_ATOMIC: RIQN_TC_NARROW(1, TC_ATOMIC); RIQN_TC_GO(1, TC_ATOMIC);
-      case TC_NOISY_WGRAD: RIQN_TC_GO(1, TC_NOISY_WGRAD);
-      case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(1, TC_BIAS_RELU_NCHW); RIQN_TC_GO(1, TC_BIAS_RELU_NCHW);
-      case TC_CONV: RIQN_TC_NARROW(1, TC_CONV); break;
-      case TC_EMBED: return launch_tc<1, TC_EMBED, 128>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
-    }
-  }
 #undef RIQN_TC_NARROW
 #undef RIQN_TC_GO
-  return (int)cudaErrorInvalidValue;
+    return (int)cudaErrorInvalidValue;
+  };
+  if (p.k_splits == 1) return go(epi);
+  // split-K: every split stores its partial product in its own slab of scratch (plain stores), then one pass adds the
+  // slabs in split order into C (and out2), so the sum does not depend on which CTA finishes first
+  const long ldp = (N + 3) & ~3L;           // 16-byte aligned slab rows for the vectorised stores
+  StreamScratch part;
+  RIQN_CUDA(part.alloc((size_t)p.k_splits * M * ldp, s));
+  const float alpha = epi == TC_ATOMIC ? p.alpha : 1.f;
+  p.C = part.p;
+  p.ldc = ldp;
+  p.part_stride = (long)M * ldp;
+  p.o_hi = nullptr;
+  if ((rc = go(TC_STORE))) return rc;
+  const long n = (long)M * N;
+  split_k_reduce_kernel<<<riqn_cdiv(n, 256), 256, 0, s>>>(M, N, p.k_splits, p.part_stride, ldp, part.p, C, ldc, alpha,
+                                                          epi == TC_NOISY_WGRAD ? out2 : nullptr, eps);
+  return (int)cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------- operand producers

@@ -10,7 +10,7 @@
 #include "../../include/riqn_b200.h"
 
 namespace riqn {
-int colsum_atomic(long M, int N, const float* X, float* out, cudaStream_t s);
+int colsum_add(long M, int N, const float* X, float* out, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // RNG fills
@@ -76,13 +76,13 @@ __global__ void cos_embed_bf16_kernel(int B, int Nq, int E, const float* __restr
 
 // Backward through x = feat[b] (.) phi[r] on bf16 operand images:
 //   x = x_hi (+ x_lo);  dpre = dX * feat * 1{x>0}  -> dpre (R, F) bf16 row-major (MN-major operand of the dW_e product)
-//   dfeat[b,f] = (sum_q dX * x) / feat ;  dbe[f] += sum_r dpre
+//   dfeat[b,f] = (sum_q dX * x) / feat ;  dbe_part[b,f] = sum_q dpre (the caller sums over b in order)
 // Rows are sample-major, so one block = one sample x 32 features walks that sample's Nq contiguous rows.
 __global__ void embed_bwd_tile_kernel(int B, int Nq, int F, const __nv_bfloat16* __restrict__ x_hi,
                                       const __nv_bfloat16* __restrict__ x_lo, const float* __restrict__ feat,
                                       const float* __restrict__ dX, const __nv_bfloat16* __restrict__ dXb,
                                       __nv_bfloat16* __restrict__ dpre, float* __restrict__ dfeat,
-                                      float* __restrict__ dbe) {
+                                      float* __restrict__ dbe_part) {
   __shared__ float red[2][8][32];
   const int f0 = blockIdx.x * 32, b = blockIdx.y;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
@@ -109,7 +109,7 @@ __global__ void embed_bwd_tile_kernel(int B, int Nq, int F, const __nv_bfloat16*
 #pragma unroll
     for (int j = 0; j < 8; ++j) { fs += red[0][j][tx]; bs += red[1][j][tx]; }
     dfeat[(long)b * F + f] = ft > 0.f ? fs / ft : 0.f;
-    atomicAdd(&dbe[f], bs);
+    dbe_part[(long)b * F + f] = bs;
   }
 }
 
@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(256) embed_bwd_wide_kernel(int B, int Nq, int 
                                                              const float* __restrict__ feat, const float* __restrict__ dX,
                                                              const __nv_bfloat16* __restrict__ dXb,
                                                              __nv_bfloat16* __restrict__ dpre, float* __restrict__ dfeat,
-                                                             float* __restrict__ dbe) {
+                                                             float* __restrict__ dbe_part) {
   __shared__ float red[2][8][128];
   const int f0 = blockIdx.x * 128, b = blockIdx.y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(256) embed_bwd_wide_kernel(int B, int Nq, int 
     for (int j = 0; j < 8; ++j) { fs += red[0][j][t]; bs += red[1][j][t]; }
     const float fv = feat[(long)b * F + f0 + t];
     dfeat[(long)b * F + f0 + t] = fv > 0.f ? fs / fv : 0.f;
-    atomicAdd(&dbe[f0 + t], bs);
+    dbe_part[(long)b * F + f0 + t] = bs;
   }
 }
 
@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(256) embed_bwd_wide8_kernel(int B, int Nq, int
                                                               const float* __restrict__ feat,
                                                               const __nv_bfloat16* __restrict__ dXb,
                                                               __nv_bfloat16* __restrict__ dpre, float* __restrict__ dfeat,
-                                                              float* __restrict__ dbe) {
+                                                              float* __restrict__ dbe_part) {
   __shared__ float red[2][8][256];
   const int f0 = blockIdx.x * 256, b = blockIdx.y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -272,7 +272,7 @@ __global__ void __launch_bounds__(256) embed_bwd_wide8_kernel(int B, int Nq, int
     for (int j = 0; j < 8; ++j) { fs += red[0][j][t]; bs += red[1][j][t]; }
     const float ftv = feat[(long)b * F + f0 + t];
     dfeat[(long)b * F + f0 + t] = ftv > 0.f ? fs / ftv : 0.f;
-    atomicAdd(&dbe[f0 + t], bs);
+    dbe_part[(long)b * F + f0 + t] = bs;
   }
 }
 
@@ -792,7 +792,7 @@ __global__ void __launch_bounds__(256) z_dueling_bwd_bf16_kernel(long R, int B, 
                                                                  const int64_t* __restrict__ actions,
                                                                  __nv_bfloat16* __restrict__ dh_hi,
                                                                  __nv_bfloat16* __restrict__ dh_hiT,
-                                                                 float* __restrict__ colsum, float* __restrict__ dz,
+                                                                 float* __restrict__ colsum_part, float* __restrict__ dz,
                                                                  __nv_bfloat16* __restrict__ dz_bf) {
   extern __shared__ __align__(16) float sW[];          // (1+A)*HID weights | HID colmean | 2*HID column sums | tile
   float* wbar = sW + (1 + A) * HID;
@@ -904,12 +904,17 @@ __global__ void __launch_bounds__(256) z_dueling_bwd_bf16_kernel(long R, int B, 
   }
   __syncthreads();                                               // the tile is rewritten by the next row block
   }
+  // the warps' column sums are added in warp order, and the block's sums leave as partial blockIdx.x of colsum_part
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {
+    if ((int)(threadIdx.x >> 5) == w) {
 #pragma unroll
-  for (int it = 0; it < 4; ++it)
+      for (int it = 0; it < 4; ++it)
 #pragma unroll
-    for (int i = 0; i < 8; ++i) atomicAdd(&cs[(lane + 32 * it) * 8 + i], bs[it][i]);
-  __syncthreads();
-  for (int c = threadIdx.x; c < 2 * HID; c += blockDim.x) atomicAdd(&colsum[c], cs[c]);
+        for (int i = 0; i < 8; ++i) cs[(lane + 32 * it) * 8 + i] += bs[it][i];
+    }
+    __syncthreads();
+  }
+  for (int c = threadIdx.x; c < 2 * HID; c += blockDim.x) colsum_part[(long)blockIdx.x * 2 * HID + c] = cs[c];
 }
 
 // dWz (32, 2*HID) from dz^T * H  ->  parameter gradients of the two noisy z-layers.
@@ -993,7 +998,7 @@ __global__ void adam_kernel(long n, float* __restrict__ p, const float* __restri
 
 static inline int grid_for(long total, int per = 256) {
   long b = (total + per - 1) / per;
-  return (int)(b > 148L * 64 ? 148L * 64 : (b < 1 ? 1 : b));
+  return (int)(b > 64L * riqn_sms() ? 64L * riqn_sms() : (b < 1 ? 1 : b));
 }
 
 }  // namespace riqn
@@ -1078,7 +1083,7 @@ RIQN_API int riqn_quantile_embed_fwd(int batch, int num_quantiles, int embed_dim
   return gemm_f32((int)R, feat_dim, embed_dim, cosv, embed_dim, 1, iqn_w, embed_dim, 1, x, feat_dim, EPI_EMBED, e, 1, s);
 }
 
-// Tensor-core embedding: cos -> bf16 (hi, lo); x = feat (.) relu(cos W_e^T + b_e) computed by the tcgen05 GEMM whose
+// Tensor-core embedding: cos -> bf16 (hi, lo); x = feat (.) relu(cos W_e^T + b_e) computed by the wgmma GEMM whose
 // epilogue writes the bf16 operand images of x directly (x_hi/x_lo row-major for the head product, x_hiT/x_loT
 // transposed for its weight gradient) and, only if x32 != NULL, the fp32 matrix.
 RIQN_API int riqn_quantile_embed_fwd_tc(int batch, int num_quantiles, int embed_dim, int feat_dim, const float* tau,
@@ -1119,22 +1124,26 @@ RIQN_API int riqn_quantile_embed_bwd_tc(int batch, int num_quantiles, int embed_
   cudaStream_t s = (cudaStream_t)stream;
   const long R = (long)batch * num_quantiles;
   if (R % 8 || feat_dim % 8 || embed_dim % 8) return (int)cudaErrorInvalidValue;
+  // the bias gradient leaves as one partial per sample (dbe_part[b, f]), summed over b in order below
+  StreamScratch dbe_buf;
+  RIQN_CUDA(dbe_buf.alloc((size_t)batch * feat_dim, s));
+  float* dbe_part = dbe_buf.p;
   if (num_quantiles % 2 == 0 && feat_dim % 4 == 0) {
     dim3 grid((feat_dim + 127) / 128, batch);
 #define RIQN_EMB_BWD(DXB, XLO)                                                                                          \
   embed_bwd_wide_kernel<DXB, XLO><<<grid, 256, 0, s>>>(batch, num_quantiles, feat_dim, (const __nv_bfloat16*)x_hi,        \
                                                        (const __nv_bfloat16*)x_lo, feat, (const float*)dx,                \
-                                                       (const __nv_bfloat16*)dx, (__nv_bfloat16*)dpre, dfeat, grad_iqn_b)
+                                                       (const __nv_bfloat16*)dx, (__nv_bfloat16*)dpre, dfeat, dbe_part)
     if (dx_is_bf16 && feat_dim % 8 == 0) {
       dim3 grid8((feat_dim + 255) / 256, batch);
       if (x_lo)
         embed_bwd_wide8_kernel<true><<<grid8, 256, 0, s>>>(batch, num_quantiles, feat_dim, (const __nv_bfloat16*)x_hi,
                                                            (const __nv_bfloat16*)x_lo, feat, (const __nv_bfloat16*)dx,
-                                                           (__nv_bfloat16*)dpre, dfeat, grad_iqn_b);
+                                                           (__nv_bfloat16*)dpre, dfeat, dbe_part);
       else
         embed_bwd_wide8_kernel<false><<<grid8, 256, 0, s>>>(batch, num_quantiles, feat_dim, (const __nv_bfloat16*)x_hi,
                                                             nullptr, feat, (const __nv_bfloat16*)dx, (__nv_bfloat16*)dpre,
-                                                            dfeat, grad_iqn_b);
+                                                            dfeat, dbe_part);
     } else if (dx_is_bf16) { if (x_lo) RIQN_EMB_BWD(true, true); else RIQN_EMB_BWD(true, false); }
     else            { if (x_lo) RIQN_EMB_BWD(false, true); else RIQN_EMB_BWD(false, false); }
 #undef RIQN_EMB_BWD
@@ -1143,9 +1152,10 @@ RIQN_API int riqn_quantile_embed_bwd_tc(int batch, int num_quantiles, int embed_
     embed_bwd_tile_kernel<<<grid, 256, 0, s>>>(batch, num_quantiles, feat_dim, (const __nv_bfloat16*)x_hi,
                                                (const __nv_bfloat16*)x_lo, feat, dx_is_bf16 ? nullptr : (const float*)dx,
                                                dx_is_bf16 ? (const __nv_bfloat16*)dx : nullptr, (__nv_bfloat16*)dpre, dfeat,
-                                               grad_iqn_b);
+                                               dbe_part);
   }
   RIQN_LAUNCH_CHECK();
+  if (int rc = sum_slots_add(batch, feat_dim, dbe_part, grad_iqn_b, s)) return rc;
   const int m_tiles = (feat_dim + 127) / 128;
   const int split = tc_pick_split(m_tiles, (R + 63) / 64);
   // dWe[f, i] += sum_r dpre[r, f] * cos[r, i]: both operands row-major, reduction over the rows (MN-major operands)
@@ -1164,11 +1174,11 @@ RIQN_API int riqn_quantile_embed_bwd(int batch, int num_quantiles, int embed_dim
   embed_bwd_elem_kernel<<<riqn_cdiv((long)batch * feat_dim, 256), 256, 0, s>>>(batch, num_quantiles, feat_dim, x, feat,
                                                                              dx_inout, dfeat);
   RIQN_LAUNCH_CHECK();
-  int rc = colsum_atomic(R, feat_dim, dx_inout, grad_iqn_b, s);
+  int rc = colsum_add(R, feat_dim, dx_inout, grad_iqn_b, s);
   if (rc) return rc;
   EpiArgs e;
   const int tiles = (feat_dim + 127) / 128;
-  int split = (3 * 148 + tiles - 1) / tiles;
+  int split = (3 * riqn_sms() + tiles - 1) / tiles;
   if ((long)split * 64 > R) split = (int)((R + 63) / 64);
   // dWe[f, i] += sum_r dpre[r, f] * cos[r, i]
   return gemm_f32(feat_dim, embed_dim, (int)R, dx_inout, 1, feat_dim, cosv, 1, embed_dim, grad_iqn_w, embed_dim,
@@ -1205,7 +1215,7 @@ RIQN_API int riqn_noisy_linear_wgrad(long rows, int in_features, int out_feature
                     in_features, EPI_NOISY_WGRAD, e, 1, s);
   if (rc) return rc;
   RIQN_CUDA(cudaMemsetAsync(db_scratch, 0, sizeof(float) * out_features, s));
-  rc = colsum_atomic(rows, out_features, dh, db_scratch, s);
+  rc = colsum_add(rows, out_features, dh, db_scratch, s);
   if (rc) return rc;
   noisy_bias_grad_kernel<<<riqn_cdiv(out_features, 256), 256, 0, s>>>(out_features, db_scratch, bias_epsilon,
                                                                     grad_bias_mu, grad_bias_sigma);
@@ -1218,7 +1228,7 @@ RIQN_API int riqn_noisy_bias_grad(long rows, int out_features, const float* dh, 
   cudaStream_t s = (cudaStream_t)stream;
   if (dh) {            // dh == NULL: db_scratch already holds the column sums (riqn_dueling_bwd_bf16)
     RIQN_CUDA(cudaMemsetAsync(db_scratch, 0, sizeof(float) * out_features, s));
-    int rc = colsum_atomic(rows, out_features, dh, db_scratch, s);
+    int rc = colsum_add(rows, out_features, dh, db_scratch, s);
     if (rc) return rc;
   }
   noisy_bias_grad_kernel<<<riqn_cdiv(out_features, 256), 256, 0, s>>>(out_features, db_scratch, bias_epsilon,
@@ -1251,13 +1261,13 @@ RIQN_API int riqn_dueling_fwd(long rows, int batch, int hidden, int action_space
                                        (int)zs_smem_bytes<512>(24)));
         attrs_once.done[attr4_dev] = true;
       }
-      z_dueling_fwd4s_kernel<512><<<148, ZS_WARPS * 32, zs_smem_bytes<512>(action_space), (cudaStream_t)stream>>>(
+      z_dueling_fwd4s_kernel<512><<<riqn_sms(), ZS_WARPS * 32, zs_smem_bytes<512>(action_space), (cudaStream_t)stream>>>(
           rows, batch, action_space, h, wz, bz, q);
       return (int)cudaGetLastError();
     }
-    z_dueling_fwd4_kernel<512><<<148 * 2, 256, smem, (cudaStream_t)stream>>>(rows, batch, action_space, h, wz, bz, q);
+    z_dueling_fwd4_kernel<512><<<riqn_sms() * 2, 256, smem, (cudaStream_t)stream>>>(rows, batch, action_space, h, wz, bz, q);
   } else {
-    z_dueling_fwd_kernel<512><<<148 * 4, 256, smem, (cudaStream_t)stream>>>(rows, batch, action_space, h, wz, bz, q);
+    z_dueling_fwd_kernel<512><<<riqn_sms() * 4, 256, smem, (cudaStream_t)stream>>>(rows, batch, action_space, h, wz, bz, q);
   }
   return (int)cudaGetLastError();
 }
@@ -1274,7 +1284,7 @@ RIQN_API int riqn_dueling_bwd(long rows, int batch, int hidden, int action_space
     RIQN_CUDA(cudaFuncSetAttribute(z_dueling_bwd_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     attr_once.done[attr_dev] = true;
   }
-  z_dueling_bwd_kernel<512><<<148 * 4, 256, smem, (cudaStream_t)stream>>>(rows, batch, action_space, h, wz, dtheta, gscale, gscale_mul,
+  z_dueling_bwd_kernel<512><<<riqn_sms() * 4, 256, smem, (cudaStream_t)stream>>>(rows, batch, action_space, h, wz, dtheta, gscale, gscale_mul,
                                                                        (const int64_t*)actions, dh, dz, (__nv_bfloat16*)dz_bf16);
   return (int)cudaGetLastError();
 }
@@ -1295,11 +1305,16 @@ RIQN_API int riqn_dueling_bwd_bf16(long rows, int batch, int hidden, int action_
   }
   RIQN_CUDA(cudaMemsetAsync(dh_colsum, 0, sizeof(float) * 2 * hidden, s));
   const long n_blk = (rows + 31) / 32;
-  z_dueling_bwd_bf16_kernel<512><<<(unsigned)(n_blk < 148 * 2 ? n_blk : 148 * 2), 256, smem, s>>>(
+  const int grid = (int)(n_blk < 2L * riqn_sms() ? n_blk : 2L * riqn_sms());
+  StreamScratch colsum_buf;
+  RIQN_CUDA(colsum_buf.alloc((size_t)grid * 2 * hidden, s));
+  float* colsum_part = colsum_buf.p;
+  z_dueling_bwd_bf16_kernel<512><<<grid, 256, smem, s>>>(
       rows, batch, action_space, h, (const __nv_bfloat16*)h_bf16, wz, dtheta, gscale, gscale_mul, (const int64_t*)actions,
       (__nv_bfloat16*)dh_hi,
-      (__nv_bfloat16*)dh_hi_t, dh_colsum, dz, (__nv_bfloat16*)dz_bf16);
-  return (int)cudaGetLastError();
+      (__nv_bfloat16*)dh_hi_t, colsum_part, dz, (__nv_bfloat16*)dz_bf16);
+  RIQN_LAUNCH_CHECK();
+  return sum_slots_add(grid, 2 * hidden, colsum_part, dh_colsum, s);
 }
 
 RIQN_API int riqn_z_wgrad(long rows, int hidden, int action_space, const float* dz, const float* h, float* dwz_scratch,
@@ -1316,7 +1331,7 @@ RIQN_API int riqn_z_wgrad(long rows, int hidden, int action_space, const float* 
   if ((long)split * 64 > rows) split = (int)((rows + 63) / 64);
   int rc = gemm_f32(32, W, (int)rows, dz, 1, 32, h, 1, W, dwz_scratch, W, EPI_ATOMIC, e, split, s);
   if (rc) return rc;
-  rc = colsum_atomic(rows, 32, dz, dbz_scratch, s);
+  rc = colsum_add(rows, 32, dz, dbz_scratch, s);
   if (rc) return rc;
   z_wgrad_finish_kernel<<<riqn_cdiv((long)action_space * hidden, 256), 256, 0, s>>>(
       action_space, hidden, dwz_scratch, dbz_scratch, eps_w_zv, eps_b_zv, eps_w_za, eps_b_za, g_mu_zv, g_sig_zv, g_bmu_zv,
@@ -1343,7 +1358,7 @@ RIQN_API int riqn_z_wgrad_tc(long rows, int hidden, int action_space, const void
   int rc = gemm_bf16_tc(32, W, (int)rows, (const __nv_bfloat16*)dz_bf16, nullptr, (const __nv_bfloat16*)h_bf16, nullptr,
                         dwz_scratch, W, TC_ATOMIC, nullptr, nullptr, nullptr, split, s, &ex);
   if (rc) return rc;
-  rc = colsum_atomic(rows, 32, dz, dbz_scratch, s);
+  rc = colsum_add(rows, 32, dz, dbz_scratch, s);
   if (rc) return rc;
   z_wgrad_finish_kernel<<<riqn_cdiv((long)action_space * hidden, 256), 256, 0, s>>>(
       action_space, hidden, dwz_scratch, dbz_scratch, eps_w_zv, eps_b_zv, eps_w_za, eps_b_za, g_mu_zv, g_sig_zv, g_bmu_zv,

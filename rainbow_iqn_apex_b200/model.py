@@ -7,7 +7,7 @@ same constructor arguments, same parameter / buffer names and shapes
 same ``forward(x, num_quantiles)`` -> ``(q (Nq*B, A), quantiles (Nq*B, 1))`` row convention
 (row = quantile * B + sample) and same ``reset_noise()`` semantics.
 
-B200-native layout: all trainable parameters live in ONE flat fp32 arena in HBM (gradients and the
+Device-native layout: all trainable parameters live in ONE flat fp32 arena in HBM (gradients and the
 Adam moments in matching arenas), ordered so that fcnoisy_h_v|fcnoisy_h_a form a single
 (2*hidden, 3136) operand and fcnoisy_z_v|fcnoisy_z_a a single (1+A, hidden) operand.  The nn.Parameters
 are views of the arena, so torch's state_dict / load_state_dict / checkpoints keep working while the
@@ -32,9 +32,9 @@ _EAGER_STREAMS = 1 << 39
 _ALIGN = 64  # floats; arena groups start on 256-byte boundaries
 
 # Arithmetic of the hidden NoisyLinear products (x W^T, dh W, dh^T x -- 91% of the step's FLOPs):
-#   "bf16x3": tcgen05 tensor cores, every operand split into bf16 hi + lo, 3 MMAs per k-step (fp32-faithful)
-#   "bf16"  : tcgen05 tensor cores, operands rounded to bf16 once, fp32 accumulation in TMEM
-#   "fp16"  : (forward only) ONE tcgen05 pass on fp16 images of x and W (11-bit significands: the error of a tf32 product
+#   "bf16x3": wgmma tensor cores, every operand split into bf16 hi + lo, 3 MMAs per k-step (fp32-faithful)
+#   "bf16"  : wgmma tensor cores, operands rounded to bf16 once, fp32 accumulation in registers
+#   "fp16"  : (forward only) ONE wgmma pass on fp16 images of x and W (11-bit significands: the error of a tf32 product
 #             at the bf16 rate; activations / weights of this network sit far inside the fp16 range).  The small products
 #             (conv trunk, quantile embedding: 5% of the FLOPs) keep the split-bf16 x3 arithmetic.
 #   "fp32"  : CUDA-core fp32 GEMM (gemm_simt.cu), the cross-check path
@@ -172,7 +172,7 @@ class DQN(nn.Module):
         self.history = args.history_length
         self.hidden = args.hidden_size
         if self.hidden != 512:
-            raise ValueError("the sm_100a kernels are specialised for hidden_size == 512")
+            raise ValueError("the sm_90a kernels are specialised for hidden_size == 512")
         self.conv1 = nn.Conv2d(args.history_length, 32, 8, stride=4, padding=1)
         self.conv2 = nn.Conv2d(32, 64, 4, stride=2)
         self.conv3 = nn.Conv2d(64, 64, 3)
@@ -399,7 +399,7 @@ class DQN(nn.Module):
                 self._iqn_ops = (mk(FEAT, self.quantile_embedding_dim), mk(FEAT, self.quantile_embedding_dim))
 
     def _refresh_tc_operands(self, force=False, h_done=False):
-        """bf16 (hi, lo) images of the composed hidden-layer weights for the tcgen05 path: (2*hid, 3136) K-major for
+        """bf16 (hi, lo) images of the composed hidden-layer weights for the wgmma path: (2*hid, 3136) K-major for
         the forward product and the transposed (3136, 2*hid) copy the data-gradient product consumes.  The images of
         the noise-free weights (convolutions, iqn_fc) are only rebuilt when those weights may have changed: after an
         optimiser step (optim.Adam marks the owner), after compose_weights() (``force``), or on first use."""

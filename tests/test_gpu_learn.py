@@ -332,3 +332,35 @@ def test_c51_loss_api_vs_oracle(cuda_dev):
     a = actor.act(frames)
     p_eval = net.dqn_forward_c51(net.to_torch(params), torch.from_numpy(b["states"][:1]).float().div_(255), 18, 51, training=False)
     assert a == int((p_eval * torch.linspace(-10, 10, 51)).sum(2).argmax(1))
+
+
+@pytest.mark.parametrize("graph", [False, True])
+def test_learner_steps_are_bitwise_reproducible(cuda_dev, graph):
+    """Two learners built from the same seed draw the same prioritized samples and compute bit-identical losses and
+    parameters over several steps at the benchmarked size, eagerly and replayed from the step's CUDA graph.  The losses become the next steps' priorities, so any
+    order-dependent rounding (a float atomic in a cross-block sum) would change which transitions are drawn later."""
+    import bench
+    from rainbow_iqn_apex_b200 import Learner, ReplayMemory
+    cap = 1 << 14
+
+    def run():
+        torch.manual_seed(5)
+        a = bench.make_args(cuda_dev, cap)
+        learner = Learner(a, bench.ACTIONS, None)
+        learner.train()
+        mem = ReplayMemory(a, None)
+        bench.fill_replay(mem, cap, cuda_dev, 7)
+        if graph:
+            learner.enable_cuda_graph(mem)
+        steps = []
+        for _ in range(6):
+            idxs, loss = learner.learn_and_update(mem)
+            steps.append((idxs.clone(), loss.clone()))
+        torch.cuda.synchronize()
+        return steps, learner.online_net._flat.detach().clone()
+
+    (s1, p1), (s2, p2) = run(), run()
+    for k, ((i1, l1), (i2, l2)) in enumerate(zip(s1, s2)):
+        assert torch.equal(i1, i2), f"step {k}: sampled indices differ"
+        assert torch.equal(l1, l2), f"step {k}: losses differ"
+    assert torch.equal(p1, p2)

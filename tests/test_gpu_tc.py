@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMA GEMM (csrc/gemm_tc.cu) against float64 products computed on the host."""
+"""GPU: the wgmma/TMA GEMM (csrc/gemm_tc.cu) against float64 products computed on the host."""
 import numpy as np
 import pytest
 import torch
@@ -65,7 +65,7 @@ def test_tc_gemm_splitk_atomic(cuda_dev, split3):
 
 
 def test_tc_gemm_many_tiles_persistent(cuda_dev):
-    _run(cuda_dev, 4096, 2048, 1024, False, seed=6)           # 256 tiles > 148 SMs: accumulator ring wraps
+    _run(cuda_dev, 4096, 2048, 1024, False, seed=6)           # 512 tiles > 132 SMs: every CTA walks several tiles
     _run(cuda_dev, 8192, 1024, 512, True, epi=1, seed=7)
 
 
@@ -114,7 +114,7 @@ def test_tc_gemm_mn_major(cuda_dev):
 
 def test_tc_gemm_fp16_operands(cuda_dev):
     """fp16 x fp16 single-pass products (the head forward's arithmetic), K-major and MN-major; a product mixing fp16 and
-    bf16 images is refused (tcgen05 kind::f16 faults with an illegal instruction when the A / B formats differ)."""
+    bf16 images is refused (wgmma takes one 16-bit format for both operands)."""
     from rainbow_iqn_apex_b200._lib import RiqnError, call, ptr
     rs = np.random.RandomState(43)
     M, N, K = 300, 1024, 3136

@@ -1,6 +1,6 @@
-"""SASS evidence for profiles/: per kernel of libriqn_b200.so, how many tcgen05 / TMA / TMEM instructions it contains
-(`cuobjdump -sass`; the PTX names never appear in SASS: tcgen05.mma = UTC*MMA, tcgen05.ld = LDTM, TMA load / store =
-UTMALDG / UTMASTG, cp.async.bulk (non-tensor) = UBLKCP, tcgen05.commit = UTCBAR, TMEM alloc = UTCATOMSWS).  Usage: python tools/sass_summary.py > profiles/sass_summary.txt"""
+"""SASS evidence: per kernel of libriqn_b200.so, how many tensor-core / TMA instructions it contains (`cuobjdump -sass`;
+the PTX names never appear in SASS: wgmma.mma_async = HGMMA, TMA load / store = UTMALDG / UTMASTG, cp.async.bulk
+(non-tensor) = UBLKCP).  Usage: python tools/sass_summary.py"""
 import collections
 import os
 import re
@@ -10,7 +10,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "rainbow_iqn_apex_b200", "libriqn_b200.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], stdout=subprocess.PIPE, text=True, check=True).stdout
-MNEM = ("UTCHMMA", "UTMALDG", "UTMASTG", "UBLKCP", "LDTM", "UTCBAR", "UTCATOMSWS", "HMMA", "REDG", "ATOMG")
+MNEM = ("HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "HMMA", "REDG", "ATOMG")
 counts, cur = collections.OrderedDict(), None
 for line in out.splitlines():
     m = re.search(r"Function : (\S+)", line)
@@ -24,7 +24,7 @@ for line in out.splitlines():
         if re.search(r"\b%s\b|\b%s\." % (k, k), line):
             counts[cur][k] += 1
 demangled = subprocess.run(["c++filt"], input="\n".join(counts), stdout=subprocess.PIPE, text=True).stdout.splitlines()
-print("# cuobjdump -sass rainbow_iqn_apex_b200/libriqn_b200.so  (sm_100a); instruction counts per kernel")
+print("# cuobjdump -sass rainbow_iqn_apex_b200/libriqn_b200.so  (sm_90a); instruction counts per kernel")
 print("# %-78s %s" % ("kernel", " ".join("%10s" % k for k in MNEM)))
 tot = collections.Counter()
 for (name, c), d in zip(counts.items(), demangled):

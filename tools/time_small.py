@@ -1,4 +1,4 @@
-"""Fixed cost of one tcgen05 GEMM launch (tiny shapes) and of the narrow strip-convolution tiles."""
+"""Fixed cost of one wgmma GEMM launch (tiny shapes) and of the narrow strip-convolution tiles."""
 import sys, os, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rainbow_iqn_apex_b200._lib import call, ptr
@@ -21,4 +21,4 @@ def run(M, N, K, reps=50):
     g.replay(); torch.cuda.synchronize()
     e0.record(); g.replay(); e1.record(); torch.cuda.synchronize()
     print(f"M={M} N={N} K={K}: {e0.elapsed_time(e1) * 1e3 / reps:7.2f} us per launch (graph of {reps})")
-run(128, 64, 64); run(128, 256, 64); run(128 * 148, 256, 64); run(128 * 148, 256, 512); run(128 * 148 * 3, 64, 512); run(41472, 64, 576)
+run(128, 64, 64); run(128, 256, 64); run(128 * 132, 256, 64); run(128 * 132, 256, 512); run(128 * 132 * 3, 64, 512); run(41472, 64, 576)
