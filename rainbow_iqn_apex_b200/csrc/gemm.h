@@ -74,6 +74,20 @@ struct TcExtra {
 int gemm_bf16_tc(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, const __nv_bfloat16* B_hi,
                  const __nv_bfloat16* B_lo, float* C, long ldc, int epi, const float* bias, float* out2, const float* eps,
                  int split_k, cudaStream_t s, const TcExtra* ex);
+//
+// Tile choice.  Single-pass (fp16 or bf16) products take 128x256 tiles (one producer and two m64n256 consumer
+// warpgroups) when
+//   * the epilogue is TC_BIAS_RELU without a transposed image, TC_STORE, or TC_NOISY_WGRAD that the split rule below
+//     leaves unsplit (the wide tiles never change a product's split count, so every output element keeps its reduction
+//     order and the result is bitwise the one of 128-wide tiles),
+//   * the operands are K-major, or mn_major 2 / 3 without strip shifts,
+//   * N > 128 and K >= 1024 (16 k-blocks: with fewer the epilogue dominates and 128-wide tiles spread it over more SMs),
+//   * and the wide tiles fill the SMs (at least one per SM), or take at most half as many rounds of CTAs as the 128-wide
+//     ones (the 1024 x 3136 weight gradient: 104 wide tiles in one round against 200 narrow ones in two).
+// These are the NoisyLinear head's forward, data gradient and weight gradient.  Everything else runs 128x{128,64,32}
+// tiles: split-bf16 x3, the convolutions, the embedding, col2im, narrow outputs, split products and small products that
+// would leave SMs idle.
+//
 // Split-K over a persistent grid of one CTA per SM: every split writes its partial product to scratch and one pass adds
 // them in split order, so splits beyond one round of CTAs only add partial sums.  tc_max_split is the most splits that
 // still fit in one round for `tiles` output tiles; tc_pick_split takes that many, but no more than the `kb` reduction

@@ -18,6 +18,7 @@
 // fp32 reference instead of bf16's 1e-4.
 #include <cuda.h>
 #include <cudaTypedefs.h>
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <tuple>
@@ -171,6 +172,38 @@ struct Wgmma<128> {
   }
 };
 
+template <>
+struct Wgmma<256> {
+  template <int F16, int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t da, uint64_t db, uint32_t acc) {
+#define RIQN_WGMMA(TY) \
+    asm volatile( \
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n" \
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n}\n" \
+        : \
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), \
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), \
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), \
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), \
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), \
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), \
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127]) \
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB))
+    if constexpr (F16) RIQN_WGMMA("f16"); else RIQN_WGMMA("bf16");
+#undef RIQN_WGMMA
+  }
+};
+
 template <int N>
 __device__ __forceinline__ void wgmma_tile(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc, bool f16, int mn) {
   const bool ta = (mn & 1) != 0, tb = (mn & 2) != 0;   // bit 0: A MN-major, bit 1: B MN-major
@@ -303,6 +336,19 @@ __device__ __forceinline__ void store_transposed_pairs(bf16* tb, const uint32_t*
   }
 }
 
+// One k-block (four k16 steps) of a single-pass product.  mn: bit 0 A MN-major, bit 1 B MN-major.
+template <int TBN>
+__device__ __forceinline__ void mma_kblock(float (&d)[TBN / 2], uint32_t sa, uint32_t sb, bool first, bool f16, int mn) {
+#pragma unroll
+  for (int k = 0; k < TBK / MMA_K; ++k) {
+    const uint32_t koff_mn = k * (MMA_K / 8) * 1024;   // MN-major: 16 reduction rows = two 8-row swizzle atoms
+    const uint32_t koff_k = k * MMA_K * 2;             // K-major: bytes inside the 128 B swizzle row
+    const uint64_t da = (mn & 1) ? gmma_desc_mn128(sa + koff_mn) : gmma_desc_k128(sa + koff_k);
+    const uint64_t db = (mn & 2) ? gmma_desc_mn128(sb + koff_mn) : gmma_desc_k128(sb + koff_k);
+    wgmma_tile<TBN>(d, da, db, (!first || k > 0) ? 1u : 0u, f16, mn);
+  }
+}
+
 struct alignas(64) TcArgs {
   CUtensorMap mapO[2];   // TC_EMBED: TMA-store maps of o_hi / o_lo ((M, N) 16-bit row-major, box 32 x 32, 64-byte swizzle)
   int M, N, K;
@@ -329,7 +375,8 @@ struct alignas(64) TcArgs {
   long part_stride;      // TC_STORE of split-K partials: split ks writes C + ks * part_stride (0 otherwise)
 };
 
-template <int NSPLIT, int EPI, int BN>
+// MODE (128x256 tiles only; 0 otherwise): bits 0-1 = mn_major, bit 2 = fp16 operands
+template <int NSPLIT, int EPI, int BN, int MODE = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                const __grid_constant__ CUtensorMap mapB_hi, const __grid_constant__ CUtensorMap mapB_lo,
@@ -361,6 +408,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 
   if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer (one thread)
+    // 128x256 tiles: the producer warpgroup hands its registers to the consumers' 128 accumulators per thread
+    // (128 * 40 + 256 * 232 = the 64512 registers the launch gets at 168 per thread)
+    if constexpr (BN == 256) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -427,7 +477,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
   }
 
   // -------------------------------------------------------------------- consumer warpgroups (wgmma + epilogue)
-  const int g = (warp >> 2) - 1;                // this warpgroup's 64 tile rows start at 64 g
+  if constexpr (BN == 256) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int g = (warp >> 2) - 1;               // this warpgroup's 64 tile rows start at 64 g
   const int wq = warp & 3;                      // warp in the warpgroup: fragment rows [16 wq, +16)
   const int band = wq & 1, colhalf = wq >> 1;   // epilogue: 32-row band of the slab, 32-column half of each 64-column chunk
   const int quarter = 2 * g + band;             // the tile rows [32 quarter, +32) this warp's lanes hold in the epilogue
@@ -464,7 +515,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
       const uint32_t sa = s0 + g * 8192;        // this warpgroup's 64 rows (K-major) or 64-row MN slab (MN-major) of A
       const uint32_t sb = s0 + Cfg::kOps * Cfg::kABytes;
       wgmma_fence();
-      if (NSPLIT == 1 && p.mn_major) {
+      if constexpr (BN == 256) {
+        // operand modes fixed at compile time: run-time choices between wgmma variants make ptxas serialise them.  For
+        // the same reason the edge tile (N = 3136: 64 real columns in the last one) runs full-width on TMA's zero fill.
+        mma_kblock<TBN>(acc, sa, sb, kb == kb0, (MODE & 4) != 0, MODE & 3);
+      } else if (NSPLIT == 1 && p.mn_major) {
 #pragma unroll
         for (int k = 0; k < TBK / MMA_K; ++k) {
           const uint32_t koff_mn = k * (MMA_K / 8) * 1024;   // MN-major: 16 reduction rows = two 8-row swizzle atoms
@@ -499,6 +554,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
     // ---- epilogue, one 64-column chunk at a time: fragment -> slab -> (row per lane) v[32] -> fused epilogue
 #pragma unroll
     for (int h = 0; h < (TBN + 63) / 64; ++h) {
+      if (BN == 256 && nt * TBN + 64 * h >= p.N) break;         // edge tile: the remaining chunks hold no real column
       if (EPI == TC_EMBED && lane == 0) tma_store_wait_read();   // bulk stores of the previous chunk read the staging tiles
       wg_bar(1 + g);
       {
@@ -813,14 +869,14 @@ static int make_store_map(CUtensorMap* map, const bf16* base, long rows, long co
   return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
 }
 
-template <int NSPLIT, int EPI, int BN>
+template <int NSPLIT, int EPI, int BN, int MODE = 0>
 static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
                      const TcArgs& p, cudaStream_t s) {
   using Cfg = TcCfg<NSPLIT, BN, EPI>;
   static PerDeviceOnce attr_once;
   const int attr_dev = PerDeviceOnce::device();
   if (!attr_once.done[attr_dev]) {
-    RIQN_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<NSPLIT, EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    RIQN_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<NSPLIT, EPI, BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)Cfg::kSmemBytes));
     attr_once.done[attr_dev] = true;
   }
@@ -831,7 +887,7 @@ static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUt
   }
   const int units = p.m_tiles * p.n_tiles * p.k_splits;
   const int grid = units < sms ? units : sms;
-  gemm_tc_kernel<NSPLIT, EPI, BN><<<grid, kTcThreads, Cfg::kSmemBytes, s>>>(a_hi, a_lo, b_hi, b_lo, p);
+  gemm_tc_kernel<NSPLIT, EPI, BN, MODE><<<grid, kTcThreads, Cfg::kSmemBytes, s>>>(a_hi, a_lo, b_hi, b_lo, p);
   return (int)cudaGetLastError();
 }
 
@@ -870,9 +926,22 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
         (((ex->mn_major & 3) != 3) && (K % 8)))
       return (int)cudaErrorInvalidValue;
   }
+  // 128x256 tiles for the head products (rule in gemm.h).  The split count is the one the 128-wide tiles get, so that
+  // every output element keeps its reduction order; the NoisyLinear weight gradient goes wide only unsplit.
+  const long kb_all = (K + TBK - 1) / TBK;
+  bool wide = false;
+  if (!split3 && !split2 && N > 128 && kb_all >= 16 && (mn ? (ex->mn_major != 1 && ex->wg_t == 0) : !strip) &&
+      (epi == TC_STORE || epi == TC_NOISY_WGRAD ||
+       (epi == TC_BIAS_RELU && !mn && (ex == nullptr || ex->o_hiT == nullptr)))) {
+    const long sms = riqn_sms();
+    const long t128 = (long)((M + TBM - 1) / TBM) * ((N + 127) / 128), t256 = (long)((M + TBM - 1) / TBM) * ((N + 255) / 256);
+    const bool unsplit = std::min(std::max(split_k, 1), std::min<int>(tc_max_split(t128), (int)kb_all)) == 1;
+    wide = (epi != TC_NOISY_WGRAD || unsplit) && (t256 >= sms || 2 * ((t256 + sms - 1) / sms) <= (t128 + sms - 1) / sms);
+  }
   // 128-wide tiles: the m64n128 accumulator of each consumer warpgroup is 64 registers per thread
-  const int bn = (ex != nullptr && ex->mn_major) ? ((narrow_ok && N <= 64) ? 64 : 128)
-                                                 : (narrow_ok && N <= 32) ? 32 : (narrow_ok && N <= 64) ? 64 : 128;
+  const int bn = wide ? 256
+                      : (ex != nullptr && ex->mn_major) ? ((narrow_ok && N <= 64) ? 64 : 128)
+                                                        : (narrow_ok && N <= 32) ? 32 : (narrow_ok && N <= 64) ? 64 : 128;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
   if (mn) {
@@ -963,6 +1032,15 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
         case TC_STORE: RIQN_TC_GO(2, TC_STORE);
         default: return (int)cudaErrorInvalidValue;
       }
+    } else if (bn == 256) {
+      const int mode = p.mn_major | ((p.fmt & 3) ? 4 : 0);
+#define RIQN_TC_WIDE(EP, MD) if (epi == EP && mode == MD) return launch_tc<1, EP, 256, MD>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
+      RIQN_TC_WIDE(TC_BIAS_RELU, 0); RIQN_TC_WIDE(TC_BIAS_RELU, 4);
+      RIQN_TC_WIDE(TC_STORE, 0); RIQN_TC_WIDE(TC_STORE, 2); RIQN_TC_WIDE(TC_STORE, 3);
+      RIQN_TC_WIDE(TC_STORE, 4); RIQN_TC_WIDE(TC_STORE, 6); RIQN_TC_WIDE(TC_STORE, 7);
+      RIQN_TC_WIDE(TC_NOISY_WGRAD, 0); RIQN_TC_WIDE(TC_NOISY_WGRAD, 2); RIQN_TC_WIDE(TC_NOISY_WGRAD, 3);
+      RIQN_TC_WIDE(TC_NOISY_WGRAD, 4); RIQN_TC_WIDE(TC_NOISY_WGRAD, 6); RIQN_TC_WIDE(TC_NOISY_WGRAD, 7);
+#undef RIQN_TC_WIDE
     } else {
       switch (epi) {
         case TC_STORE: RIQN_TC_NARROW(1, TC_STORE); RIQN_TC_GO(1, TC_STORE);
