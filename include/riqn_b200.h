@@ -254,6 +254,14 @@ int riqn_dueling_bwd_bf16(long rows, int batch, int hidden, int action_space, co
                           const float* dtheta, const float* gscale, float gscale_mul, const long long* actions, void* dh_hi,
                           void* dh_hi_t,
                           float* dh_colsum, float* dz, void* dz_bf16, void* stream);
+/* The same two backwards for a dense upstream gradient grad_q = dL/dq (rows, A), fp32, quantile-major rows q*batch+b as
+ * riqn_dueling_fwd writes q:  dv = sum_a grad_q[a] ; da_k = grad_q[k] - dv/A ; dh_v = dv * w_zv ; dh_a = sum_k da_k w_za[k],
+ * both masked by h > 0.  Outputs and their layouts are those of riqn_dueling_bwd / riqn_dueling_bwd_bf16. */
+int riqn_dueling_bwd_dense(long rows, int batch, int hidden, int action_space, const float* h, const float* wz,
+                           const float* grad_q, float* dh, float* dz, void* dz_bf16, void* stream);
+int riqn_dueling_bwd_dense_bf16(long rows, int batch, int hidden, int action_space, const float* h, const void* h_bf16,
+                                const float* wz, const float* grad_q, void* dh_hi, void* dh_hi_t, float* dh_colsum,
+                                float* dz, void* dz_bf16, void* stream);
 /* Parameter gradients of the two z-layers (accumulated): dwz_scratch 32*2*hidden floats, dbz_scratch 32. */
 /* Same with the reduction dz^T h on the tensor cores, straight from the row-major bf16 images dz_bf16 (rows, 32) and
  * h_bf16 (rows, 2*hidden) (rows % 8 == 0). */
@@ -299,6 +307,12 @@ int riqn_c51_loss_fwd_bwd(int batch, int action_space, int atoms, const float* l
 /* dzv (batch, atoms), dza (batch, A*atoms) from dq scaled by gscale[b] (dueling backward). */
 int riqn_c51_head_bwd(int batch, int action_space, int atoms, const float* dq, const float* gscale, float gscale_mul,
                       const long long* actions, float* dzv, float* dza, void* stream);
+/* The same for a dense upstream gradient grad_out = dL/dout (batch, A, atoms) of the head's output out = p (is_log == 0)
+ * or log p (is_log != 0) as riqn_c51_head_fwd wrote it:  log: dq = grad_out - p * sum_atoms grad_out ;
+ * softmax: dq = p * (grad_out - sum_atoms p grad_out) ; then dzv[b,j] = sum_a dq[b,a,j], dza[b,a,j] = dq[b,a,j] - dzv[b,j]/A.
+ * atoms <= 64. */
+int riqn_c51_head_bwd_dense(int batch, int action_space, int atoms, const float* out, const float* grad_out, int is_log,
+                            float* dzv, float* dza, void* stream);
 /* n floats <- 0 (the gradient arena's zero_grad, learner.py:22): cudaMemsetAsync on the caller's stream. */
 int riqn_zero_f32(float* p, long n, void* stream);
 /* grad[i] = 0 where act[i] <= 0. */

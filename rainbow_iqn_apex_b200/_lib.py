@@ -65,6 +65,8 @@ SIGNATURES = {
     "riqn_dueling_fwd": [C.c_long, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P],
     "riqn_dueling_bwd": [C.c_long, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, C.c_float, _P, _P, _P, _P, _P],
     "riqn_dueling_bwd_bf16": [C.c_long, C.c_int, C.c_int, C.c_int] + [_P] * 5 + [C.c_float] + [_P] * 7,
+    "riqn_dueling_bwd_dense": [C.c_long, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
+    "riqn_dueling_bwd_dense_bf16": [C.c_long, C.c_int, C.c_int, C.c_int] + [_P] * 10,
     "riqn_z_wgrad": [C.c_long, C.c_int, C.c_int] + [_P] * 17,
     "riqn_z_wgrad_tc": [C.c_long, C.c_int, C.c_int] + [_P] * 18,
     "riqn_argmax_mean": [C.c_int, C.c_int, C.c_int, _P, _P, _P],
@@ -74,6 +76,7 @@ SIGNATURES = {
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,
                               C.c_float, _P, _P, _P, _P],
     "riqn_c51_head_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P, _P],
+    "riqn_c51_head_bwd_dense": [C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P],
     "riqn_zero_f32": [_P, C.c_long, _P],
     "riqn_relu_mask": [C.c_long, _P, _P, _P],
     "riqn_linear_fwd_ld": [C.c_long, C.c_int, C.c_int, _P, C.c_long, _P, _P, _P, C.c_long, C.c_int, _P],

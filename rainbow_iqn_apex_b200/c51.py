@@ -16,7 +16,7 @@ def forward(net, x, log=False, keep=None, fresh_weights=False, want_argmax=None,
     """Returns probabilities (or log-probabilities) (B, A, atoms).  model.py:120-129"""
     from .model import PRECISION
     if not fresh_weights:
-        net.compose_weights()
+        net._compose_weights()
     feat = net.trunk(x, keep)
     B = feat.shape[0]
     dev = feat.device
@@ -90,50 +90,67 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     def backward(gscale, gscale_mul=1.0):
         if getattr(on, "_noise_version", 0) != version:
             raise RuntimeError("the online network's noise was resampled between the C51 loss and its backward")
-        hid = on.hidden
-        gv = on.grad_view
-        hvL, haL, zvL, zaL = on.fcnoisy_h_v, on.fcnoisy_h_a, on.fcnoisy_z_v, on.fcnoisy_z_a
-        h = keep["h"]
         gscale = gscale.contiguous().float()
         dzv = torch.empty(B, atoms, device=dev)
         dza = torch.empty(B, A * atoms, device=dev)
         call("riqn_c51_head_bwd", B, A, atoms, ptr(dq), ptr(gscale), float(gscale_mul), ptr(actions), ptr(dzv), ptr(dza))
-        dh = torch.empty(B, 2 * hid, device=dev)
-        dhv, dha = dh[:, :hid], dh[:, hid:]
-        hv, ha = h[:, :hid], h[:, hid:]
-        w_z = on._w_eff_z
-        wzv, wza = w_z[:atoms], w_z[atoms:]
-        call("riqn_linear_dgrad_ld", B, hid, atoms, ptr(dzv), atoms, ptr(wzv), ptr(dhv), 2 * hid)
-        call("riqn_linear_dgrad_ld", B, hid, A * atoms, ptr(dza), A * atoms, ptr(wza), ptr(dha), 2 * hid)
-        call("riqn_relu_mask", dh.numel(), ptr(h), ptr(dh))
-        scratch = torch.empty(max(A * atoms, 2 * hid), device=dev)
-        for layer, d, xin in ((zvL, dzv, hv), (zaL, dza, ha)):
-            call("riqn_noisy_wgrad_ld", B, hid, layer.out_features, ptr(d), layer.out_features, ptr(xin), 2 * hid,
-                 ptr(layer.weight_epsilon), ptr(gv(layer.weight_mu)), ptr(gv(layer.weight_sigma)))
-            call("riqn_noisy_bias_grad", B, layer.out_features, ptr(d), ptr(layer.bias_epsilon), ptr(scratch),
-                 ptr(gv(layer.bias_mu)), ptr(gv(layer.bias_sigma)))
-        # hidden layers: [h_v | h_a] adjacent in every arena (parameters, gradients, epsilons)
-        dfeat = torch.empty(B, FEAT, device=dev)
-        if keep.get("x_bf") is not None:
-            # tensor cores: dW = dh^T x straight from the row-major bf16 images (MN-major operands), dx = dh W from W itself
-            from .model import PRECISION
-            dh_bf = torch.empty(B, 2 * hid, dtype=torch.bfloat16, device=dev)
-            call("riqn_split_bf16", B, 2 * hid, ptr(dh), ptr(dh_bf), None, None, None, 0)
-            w_bf = on._w_lo if PRECISION["fwd"] == "fp16" else on._w_hi
-            call("riqn_gemm_bf16_tc_mn", 2 * hid, FEAT, B, ptr(dh_bf), ptr(keep["x_bf"]), 1, ptr(gv(hvL.weight_mu)), FEAT, 3,
-                 ptr(gv(hvL.weight_sigma)), ptr(hvL.weight_epsilon), 1.0, 1, None, 0)
-            call("riqn_noisy_bias_grad", B, 2 * hid, ptr(dh), ptr(hvL.bias_epsilon), ptr(scratch), ptr(gv(hvL.bias_mu)),
-                 ptr(gv(hvL.bias_sigma)))
-            call("riqn_gemm_bf16_tc_mn", B, FEAT, 2 * hid, ptr(dh_bf), ptr(w_bf), 0, ptr(dfeat), FEAT, 0, None, None, 1.0, 1,
-                 None, 0)
-        else:
-            call("riqn_noisy_linear_wgrad", B, FEAT, 2 * hid, ptr(dh), ptr(keep["feat"]), ptr(hvL.weight_epsilon),
-                 ptr(hvL.bias_epsilon), ptr(scratch), ptr(gv(hvL.weight_mu)), ptr(gv(hvL.weight_sigma)), ptr(gv(hvL.bias_mu)),
-                 ptr(gv(hvL.bias_sigma)))
-            call("riqn_noisy_linear_dgrad", B, FEAT, 2 * hid, ptr(dh), ptr(on._w_eff_h), ptr(dfeat))
-        on.backward_trunk(keep, dfeat)
+        _backward_below_head(on, keep, dzv, dza, on.grad_view)
 
     return loss, backward
+
+
+def backward_dense(on, keep, out, grad_out, log, gv):
+    """Parameter gradients of a forward recorded in ``keep`` given the dense dL/dout ``grad_out`` (B, A, atoms) of its
+    output ``out`` (probabilities, or log-probabilities when ``log``); ``gv(param)`` is each parameter's gradient buffer."""
+    B, A, atoms = out.shape
+    dzv = torch.empty(B, atoms, device=out.device)
+    dza = torch.empty(B, A * atoms, device=out.device)
+    call("riqn_c51_head_bwd_dense", B, A, atoms, ptr(out), ptr(grad_out), 1 if log else 0, ptr(dzv), ptr(dza))
+    _backward_below_head(on, keep, dzv, dza, gv)
+
+
+def _backward_below_head(on, keep, dzv, dza, gv):
+    """From the z-layer data gradients dzv (B, atoms), dza (B, A*atoms) down to the trunk: z-layer and hidden-layer
+    NoisyLinear gradients, then the convolutions."""
+    B, dev = keep["B"], dzv.device
+    A, atoms = on.action_space, on.atoms
+    hid = on.hidden
+    hvL, haL, zvL, zaL = on.fcnoisy_h_v, on.fcnoisy_h_a, on.fcnoisy_z_v, on.fcnoisy_z_a
+    h = keep["h"]
+    dh = torch.empty(B, 2 * hid, device=dev)
+    dhv, dha = dh[:, :hid], dh[:, hid:]
+    hv, ha = h[:, :hid], h[:, hid:]
+    w_z = on._w_eff_z
+    wzv, wza = w_z[:atoms], w_z[atoms:]
+    call("riqn_linear_dgrad_ld", B, hid, atoms, ptr(dzv), atoms, ptr(wzv), ptr(dhv), 2 * hid)
+    call("riqn_linear_dgrad_ld", B, hid, A * atoms, ptr(dza), A * atoms, ptr(wza), ptr(dha), 2 * hid)
+    call("riqn_relu_mask", dh.numel(), ptr(h), ptr(dh))
+    scratch = torch.empty(max(A * atoms, 2 * hid), device=dev)
+    for layer, d, xin in ((zvL, dzv, hv), (zaL, dza, ha)):
+        call("riqn_noisy_wgrad_ld", B, hid, layer.out_features, ptr(d), layer.out_features, ptr(xin), 2 * hid,
+             ptr(layer.weight_epsilon), ptr(gv(layer.weight_mu)), ptr(gv(layer.weight_sigma)))
+        call("riqn_noisy_bias_grad", B, layer.out_features, ptr(d), ptr(layer.bias_epsilon), ptr(scratch),
+             ptr(gv(layer.bias_mu)), ptr(gv(layer.bias_sigma)))
+    # hidden layers: [h_v | h_a] adjacent in every arena (parameters, gradients, epsilons)
+    dfeat = torch.empty(B, FEAT, device=dev)
+    if keep.get("x_bf") is not None:
+        # tensor cores: dW = dh^T x straight from the row-major bf16 images (MN-major operands), dx = dh W from W itself
+        from .model import PRECISION
+        dh_bf = torch.empty(B, 2 * hid, dtype=torch.bfloat16, device=dev)
+        call("riqn_split_bf16", B, 2 * hid, ptr(dh), ptr(dh_bf), None, None, None, 0)
+        w_bf = on._w_lo if PRECISION["fwd"] == "fp16" else on._w_hi
+        call("riqn_gemm_bf16_tc_mn", 2 * hid, FEAT, B, ptr(dh_bf), ptr(keep["x_bf"]), 1, ptr(gv(hvL.weight_mu)), FEAT, 3,
+             ptr(gv(hvL.weight_sigma)), ptr(hvL.weight_epsilon), 1.0, 1, None, 0)
+        call("riqn_noisy_bias_grad", B, 2 * hid, ptr(dh), ptr(hvL.bias_epsilon), ptr(scratch), ptr(gv(hvL.bias_mu)),
+             ptr(gv(hvL.bias_sigma)))
+        call("riqn_gemm_bf16_tc_mn", B, FEAT, 2 * hid, ptr(dh_bf), ptr(w_bf), 0, ptr(dfeat), FEAT, 0, None, None, 1.0, 1,
+             None, 0)
+    else:
+        call("riqn_noisy_linear_wgrad", B, FEAT, 2 * hid, ptr(dh), ptr(keep["feat"]), ptr(hvL.weight_epsilon),
+             ptr(hvL.bias_epsilon), ptr(scratch), ptr(gv(hvL.weight_mu)), ptr(gv(hvL.weight_sigma)), ptr(gv(hvL.bias_mu)),
+             ptr(gv(hvL.bias_sigma)))
+        call("riqn_noisy_linear_dgrad", B, FEAT, 2 * hid, ptr(dh), ptr(on._w_eff_h), ptr(dfeat))
+    on.backward_trunk(keep, dfeat)
 
 
 class _C51Loss(torch.autograd.Function):

@@ -124,6 +124,46 @@ __global__ void c51_head_bwd_kernel(int B, int A, int atoms, const float* __rest
   if (a == 0) dzv[b * atoms + j] = g;
 }
 
+// Dense upstream gradient G (B, A, atoms) of the head's output, one block per sample, one warp per action (atoms <= 64:
+// lane owns j = lane and lane + 32).  out holds p (is_log == 0) or log p (is_log != 0):
+//   log-softmax: dq = G - p * sum_j G ;  softmax: dq = p * (G - sum_j p G)
+// then the dueling split over actions, per atom: dzv[j] = sum_a dq[a,j] (a ascending), dza[a,j] = dq[a,j] - dzv[j] / A.
+__global__ void c51_head_bwd_dense_kernel(int A, int atoms, const float* __restrict__ out, const float* __restrict__ G,
+                                          int is_log, float* __restrict__ dzv, float* __restrict__ dza) {
+  extern __shared__ float sdq[];     // dq[A * atoms] | dv[atoms]
+  float* dv = sdq + A * atoms;
+  const int b = blockIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int a = warp; a < A; a += nw) {
+    const long o = ((long)b * A + a) * atoms;
+    float p[2] = {0.f, 0.f}, g[2] = {0.f, 0.f};
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int j = lane + 32 * u;
+      if (j < atoms) {
+        p[u] = is_log ? expf(out[o + j]) : out[o + j];
+        g[u] = G[o + j];
+      }
+    }
+    const float s = is_log ? warp_sum(g[0] + g[1]) : warp_sum(p[0] * g[0] + p[1] * g[1]);
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int j = lane + 32 * u;
+      if (j < atoms) sdq[a * atoms + j] = is_log ? g[u] - p[u] * s : p[u] * (g[u] - s);
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < atoms; j += blockDim.x) {
+    float t = 0.f;
+    for (int a = 0; a < A; ++a) t += sdq[a * atoms + j];
+    dv[j] = t;
+    dzv[(long)b * atoms + j] = t;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < A * atoms; i += blockDim.x)
+    dza[(long)b * A * atoms + i] = sdq[i] - dv[i % atoms] / (float)A;
+}
+
 __global__ void relu_mask_kernel(long n, const float* __restrict__ act, float* __restrict__ grad) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && !(act[i] > 0.f)) grad[i] = 0.f;
@@ -159,6 +199,16 @@ RIQN_API int riqn_c51_head_bwd(int batch, int action_space, int atoms, const flo
   const long n = (long)batch * action_space * atoms;
   c51_head_bwd_kernel<<<riqn_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(batch, action_space, atoms, dq, gscale, gscale_mul,
                                                                           (const int64_t*)actions, dzv, dza);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_c51_head_bwd_dense(int batch, int action_space, int atoms, const float* out, const float* grad_out,
+                                     int is_log, float* dzv, float* dza, void* stream) {
+  riqn::note_launches(1);
+  if (atoms > 64) return (int)cudaErrorInvalidValue;
+  const size_t smem = sizeof(float) * ((size_t)action_space * atoms + atoms);
+  if (smem > 48 * 1024) return (int)cudaErrorInvalidValue;
+  c51_head_bwd_dense_kernel<<<batch, 256, smem, (cudaStream_t)stream>>>(action_space, atoms, out, grad_out, is_log, dzv, dza);
   return (int)cudaGetLastError();
 }
 

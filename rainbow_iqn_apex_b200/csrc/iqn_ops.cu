@@ -742,8 +742,19 @@ __global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __rest
 //   g = dtheta[r] * gscale[b];  dq[a] = g*1{a==act}  =>  dv = g ,  da_k = g*(1{k==act} - 1/A)
 //   dH_v = dv * w_zv ; dH_a = g*(W_za[act] - colmean(W_za)) ; masked by H > 0
 //   dz (R, 32): [g, da_0..da_{A-1}, 0...] feeds the z-layer weight-gradient reduction.
+// DENSE: dtheta is a dense upstream gradient G (R, A), quantile-major rows, in place of the one-hot dtheta*gscale:
+//   dv = sum_a G[a] ; da_k = G[k] - dv/A ; dH_v = dv * w_zv ; dH_a = sum_k da_k * W_za[k]  (k ascending), masked by H > 0
+// gscale, gmul and actions are unused.
 // ------------------------------------------------------------------------------------------------
-template <int HID>
+// One warp: lane 0 <- dv, lane 1+k <- da_k (k < A), other lanes 0, from G row g_row (a warp-uniform row).
+__device__ __forceinline__ float dense_dz_lane(const float* __restrict__ g_row, int A, int lane) {
+  const float gk = lane < A ? g_row[lane] : 0.f;
+  const float dv = warp_sum(gk);
+  const float g_prev = __shfl_up_sync(0xffffffffu, gk, 1);      // lane l holds G[l - 1]
+  return lane == 0 ? dv : (lane <= A ? g_prev - dv / (float)A : 0.f);
+}
+
+template <int HID, bool DENSE = false>
 __global__ void z_dueling_bwd_kernel(long R, int B, int A, const float* __restrict__ H, const float* __restrict__ Wz,
                                      const float* __restrict__ dtheta, const float* __restrict__ gscale, float gmul,
                                      const int64_t* __restrict__ actions, float* __restrict__ dH,
@@ -762,6 +773,31 @@ __global__ void z_dueling_bwd_kernel(long R, int B, int A, const float* __restri
   for (long r = (long)blockIdx.x * wpb + warp; r < R; r += (long)gridDim.x * wpb) {
     const int Nq = (int)(R / B);
     const int b = (int)(r / Nq);                            // sample-major rows; dtheta arrives quantile-major
+    if constexpr (DENSE) {
+      const float z = dense_dz_lane(dtheta + ((r - (long)b * Nq) * B + b) * A, A, lane);
+      const float dv = __shfl_sync(0xffffffffu, z, 0);
+      constexpr int T = HID / 32;
+      float da[T];
+#pragma unroll
+      for (int t = 0; t < T; ++t) da[t] = 0.f;
+      for (int k = 0; k < A; ++k) {
+        const float dk = __shfl_sync(0xffffffffu, z, 1 + k);
+        const float* wk = sW + (1 + k) * HID;
+#pragma unroll
+        for (int t = 0; t < T; ++t) da[t] = fmaf(dk, wk[lane + 32 * t], da[t]);
+      }
+      const float* h = H + r * (2 * HID);
+      float* o = dH + r * (2 * HID);
+#pragma unroll
+      for (int t = 0; t < T; ++t) {
+        const int j = lane + 32 * t;
+        o[j] = h[j] > 0.f ? dv * sW[j] : 0.f;
+        o[HID + j] = h[HID + j] > 0.f ? da[t] : 0.f;
+      }
+      dz[r * 32 + lane] = z;
+      if (dz_bf) dz_bf[r * 32 + lane] = __float2bfloat16_rn(z);
+      continue;
+    }
     const float g = dtheta[(r - (long)b * Nq) * B + b] * (gscale[b] * gmul);
     const int act = (int)actions[b];
     const float* h = H + r * (2 * HID);
@@ -783,7 +819,8 @@ __global__ void z_dueling_bwd_kernel(long R, int B, int A, const float* __restri
 // (dh_hi (R, 2*HID) for the dgrad, dh_hiT (2*HID, R) for the wgrad) plus its fp32 column sums (bias gradients); the fp32
 // dH matrix is never written.  One block = 32 consecutive rows; the transposed image goes through an XOR-swizzled
 // shared tile (16-byte chunk c/8 of row r sits in slot (c/8) ^ ((r >> 3) & 3)) and leaves as 64-byte column segments.
-template <int HID>
+// DENSE: as in z_dueling_bwd_kernel, dtheta is the dense upstream gradient G (R, A).
+template <int HID, bool DENSE = false>
 __global__ void __launch_bounds__(256) z_dueling_bwd_bf16_kernel(long R, int B, int A, const float* __restrict__ H,
                                                                  const __nv_bfloat16* __restrict__ Hb,
                                                                  const float* __restrict__ Wz,
@@ -824,9 +861,30 @@ __global__ void __launch_bounds__(256) z_dueling_bwd_bf16_kernel(long R, int B, 
     const bool ok = r < R;
     const long rc = ok ? r : 0;
     const int b = (int)(rc / Nq);                            // sample-major rows; dtheta arrives quantile-major
-    const float g = ok ? dtheta[(rc - (long)b * Nq) * B + b] * (gscale[b] * gmul) : 0.f;
-    const int act = (int)actions[b];
-    const float* wa = sW + (1 + act) * HID;
+    float g, zd = 0.f;                                       // DENSE: zd = this lane's dz entry, g = dv
+    float da[2][8];                                          // DENSE: advantage-stream gradient of chunks lane+64, lane+96
+    int act = 0;
+    const float* wa = sW;
+    if constexpr (DENSE) {
+      zd = ok ? dense_dz_lane(dtheta + ((rc - (long)b * Nq) * B + b) * A, A, lane) : 0.f;   // ok is warp-uniform
+      g = __shfl_sync(0xffffffffu, zd, 0);
+#pragma unroll
+      for (int c = 0; c < 2; ++c)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) da[c][i] = 0.f;
+      for (int k = 0; k < A; ++k) {
+        const float dk = __shfl_sync(0xffffffffu, zd, 1 + k);
+        const float* wk = sW + (1 + k) * HID + lane * 8;
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+#pragma unroll
+          for (int i = 0; i < 8; ++i) da[c][i] = fmaf(dk, wk[256 * c + i], da[c][i]);
+      }
+    } else {
+      g = ok ? dtheta[(rc - (long)b * Nq) * B + b] * (gscale[b] * gmul) : 0.f;
+      act = (int)actions[b];
+      wa = sW + (1 + act) * HID;
+    }
     // the ReLU mask only needs the SIGN of h: read the bf16 image when the forward left one (half the bytes); all of
     // a row's loads are issued before the first use
     float hrow[4][8];
@@ -860,6 +918,9 @@ __global__ void __launch_bounds__(256) z_dueling_bwd_bf16_kernel(long R, int B, 
       if (it < 2) {                                            // value stream: dv * w_zv
 #pragma unroll
         for (int i = 0; i < 8; ++i) val[i] = hv[i] > 0.f ? g * sW[j0 + i] : 0.f;
+      } else if constexpr (DENSE) {                            // advantage stream: sum_k da_k W_za[k]
+#pragma unroll
+        for (int i = 0; i < 8; ++i) val[i] = hv[i] > 0.f ? da[it - 2][i] : 0.f;
       } else {                                                 // advantage stream: g * (W_za[act] - colmean)
 #pragma unroll
         for (int i = 0; i < 8; ++i) val[i] = hv[i] > 0.f ? g * (wa[j0 + i] - wbar[j0 + i]) : 0.f;
@@ -878,7 +939,8 @@ __global__ void __launch_bounds__(256) z_dueling_bwd_bf16_kernel(long R, int B, 
     }
     if (ok) {
       float z = 0.f;
-      if (lane == 0) z = g;
+      if constexpr (DENSE) z = zd;
+      else if (lane == 0) z = g;
       else if (lane <= A) z = g * ((lane - 1 == act ? 1.f : 0.f) - 1.f / (float)A);
       dz[r * 32 + lane] = z;
       if (dz_bf) dz_bf[r * 32 + lane] = __float2bfloat16_rn(z);     // (R, 32) row-major: MN-major operand of dWz
@@ -1315,6 +1377,48 @@ RIQN_API int riqn_dueling_bwd_bf16(long rows, int batch, int hidden, int action_
       (__nv_bfloat16*)dh_hi_t, colsum_part, dz, (__nv_bfloat16*)dz_bf16);
   RIQN_LAUNCH_CHECK();
   return sum_slots_add(grid, 2 * hidden, colsum_part, dh_colsum, s);
+}
+
+RIQN_API int riqn_dueling_bwd_dense(long rows, int batch, int hidden, int action_space, const float* h, const float* wz,
+                                    const float* grad_q, float* dh, float* dz, void* dz_bf16, void* stream) {
+  riqn::note_launches(1);
+  if (hidden != 512 || action_space > 31) return (int)cudaErrorInvalidValue;
+  const size_t smem = sizeof(float) * ((1 + action_space) * hidden + hidden);
+  static PerDeviceOnce attr_once;
+  const int attr_dev = PerDeviceOnce::device();
+  if (!attr_once.done[attr_dev]) {
+    RIQN_CUDA(cudaFuncSetAttribute(z_dueling_bwd_kernel<512, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    attr_once.done[attr_dev] = true;
+  }
+  z_dueling_bwd_kernel<512, true><<<riqn_sms() * 4, 256, smem, (cudaStream_t)stream>>>(
+      rows, batch, action_space, h, wz, grad_q, nullptr, 0.f, nullptr, dh, dz, (__nv_bfloat16*)dz_bf16);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_dueling_bwd_dense_bf16(long rows, int batch, int hidden, int action_space, const float* h,
+                                         const void* h_bf16, const float* wz, const float* grad_q, void* dh_hi,
+                                         void* dh_hi_t, float* dh_colsum, float* dz, void* dz_bf16, void* stream) {
+  riqn::note_launches(1);
+  if (hidden != 512 || action_space > 31 || rows % 8) return (int)cudaErrorInvalidValue;
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t smem = sizeof(float) * ((1 + action_space) * hidden + hidden + 2 * hidden) + 32 * 128 * 16;
+  static PerDeviceOnce attr_once;
+  const int attr_dev = PerDeviceOnce::device();
+  if (!attr_once.done[attr_dev]) {
+    RIQN_CUDA(cudaFuncSetAttribute(z_dueling_bwd_bf16_kernel<512, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   160 * 1024));
+    attr_once.done[attr_dev] = true;
+  }
+  RIQN_CUDA(cudaMemsetAsync(dh_colsum, 0, sizeof(float) * 2 * hidden, s));
+  const long n_blk = (rows + 31) / 32;
+  const int grid = (int)(n_blk < 2L * riqn_sms() ? n_blk : 2L * riqn_sms());
+  StreamScratch colsum_buf;
+  RIQN_CUDA(colsum_buf.alloc((size_t)grid * 2 * hidden, s));
+  z_dueling_bwd_bf16_kernel<512, true><<<grid, 256, smem, s>>>(
+      rows, batch, action_space, h, (const __nv_bfloat16*)h_bf16, wz, grad_q, nullptr, 0.f, nullptr, (__nv_bfloat16*)dh_hi,
+      (__nv_bfloat16*)dh_hi_t, colsum_buf.p, dz, (__nv_bfloat16*)dz_bf16);
+  RIQN_LAUNCH_CHECK();
+  return sum_slots_add(grid, 2 * hidden, colsum_buf.p, dh_colsum, s);
 }
 
 RIQN_API int riqn_z_wgrad(long rows, int hidden, int action_space, const float* dz, const float* h, float* dwz_scratch,

@@ -129,7 +129,13 @@ class NoisyLinear(nn.Module):
              ptr(self.bias_epsilon), ptr(self._w_eff), ptr(self._b_eff), 1 if self.training else 0)
 
     def forward(self, input):
-        """model.py:45-53 (inference helper; the learner path goes through DQN's fused ops)."""
+        """model.py:45-53 (fp32 helper; the learner path goes through DQN's fused ops).  Differentiable with respect to
+        the input and the four parameters when grad mode is on (riqn_noisy_linear_dgrad / _wgrad)."""
+        if torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())):
+            return _NoisyLinearFn.apply(self, input, self.weight_mu, self.weight_sigma, self.bias_mu, self.bias_sigma)
+        return self._forward(input)
+
+    def _forward(self, input):
         self._compose()
         x = input.contiguous().float()
         out = torch.empty(x.shape[0], self.out_features, device=x.device)
@@ -197,9 +203,10 @@ class DQN(nn.Module):
         self._dyn = None
         self._tau_stream_offset = 0   # rank-private quantile stream under data parallelism
         self._rng_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        self._param_version = 0      # bumped by every parameter update; a pending autograd backward checks it
         self._flatten()
         # anything that rewrites the noise-free weights must invalidate their cached bf16 operand images
-        self.register_load_state_dict_post_hook(lambda module, _incompatible: setattr(module, "_static_ops_dirty", True))
+        self.register_load_state_dict_post_hook(lambda module, _incompatible: module._params_changed())
         if self._flat.is_cuda:
             self.reset_noise()
 
@@ -243,7 +250,7 @@ class DQN(nn.Module):
                 p._riqn_offset = off
                 i += 1
         self._flat, self._flat_grad = flat, flat_grad
-        self._static_ops_dirty = True
+        self._params_changed()
         # epsilon arena: [h_v.weight_epsilon | h_a.weight_epsilon], h bias eps, [z_v | z_a] weight eps, z bias eps
         hv, ha, zv, za = self.fcnoisy_h_v, self.fcnoisy_h_a, self.fcnoisy_z_v, self.fcnoisy_z_a
         eg = [[(hv, "weight_epsilon"), (ha, "weight_epsilon")], [(hv, "bias_epsilon"), (ha, "bias_epsilon")],
@@ -286,6 +293,12 @@ class DQN(nn.Module):
             self.reset_noise()  # NoisyLinear.__init__ resets noise in the reference (model.py:23)
         return out
 
+    def _params_changed(self):
+        """The parameters were rewritten (optimiser step, load_state_dict, new arenas): the cached operand images of the
+        noise-free weights are stale, and so is the saved state of any forward still waiting for its backward."""
+        self._static_ops_dirty = True
+        self._param_version += 1
+
     def zero_grad(self, set_to_none=False):
         """One memset over the gradient arena; the .grad views stay bound (learner.py:22)."""
         if self._flat_grad.is_cuda:
@@ -310,6 +323,7 @@ class DQN(nn.Module):
         """model.py:159-162.  ``noise``: optional {layer_name: (f(eps_in), f(eps_out))} injection.
         All NoisyLinear layers are redrawn and recomposed by ONE riqn_noisy_reset_net call (two launches)."""
         self._noise_version = getattr(self, "_noise_version", 0) + 1     # backward passes check it: they read the LIVE weights
+        self._composed_training = self.training
         layers = self.noisy_layers()
         if not self._flat.is_cuda or any(m.in_features % 4 for _, m in layers):
             for name, module in layers:
@@ -376,9 +390,18 @@ class DQN(nn.Module):
 
     def compose_weights(self):
         """Recompute the effective weights from the stored epsilons (after load_state_dict / optimiser steps)."""
+        self._param_version += 1
+        self._compose_weights()
+
+    def _compose_weights(self):
         for _, module in self.noisy_layers():
             module._compose()
         self._refresh_tc_operands(force=True)
+        self._composed_training = self.training
+
+    def _live_weights_key(self):
+        """What the composed weights a backward reads depend on: noise sample, parameter values, train / eval mode."""
+        return (getattr(self, "_noise_version", 0), self._param_version, getattr(self, "_composed_training", None))
 
     def _ensure_tc_buffers(self):
         """Allocate the bf16 operand images once per device."""
@@ -660,14 +683,28 @@ class DQN(nn.Module):
                         head_bwd_tc=bwd_tc, emb_bwd_tc=emb_tc)
         return q
 
+    def __call__(self, x, num_quantiles=None, log=False, tau=None, **internal):
+        """``net(x, N)`` / ``net(x, log=...)``, the reference's call.  With grad mode on, a parameter that requires grad and
+        none of forward()'s internal arguments, the call is one autograd node (_DQNForward): the output (q, or the C51
+        (log-)probabilities) has a grad_fn, and ``.backward()`` of any scalar built from it accumulates the parameter
+        gradients into ``param.grad``.  Otherwise it is forward() itself, which the learner's own passes call directly."""
+        if not internal and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            for name, t in (("x", x), ("tau", tau)):
+                if torch.is_tensor(t) and t.requires_grad:
+                    raise RuntimeError(f"DQN.forward computes gradients for the network's parameters only, not for its "
+                                       f"inputs: {name} requires grad (pass {name}.detach())")
+            params = [p for p in self.parameters() if p.requires_grad]
+            return _DQNForward.apply(self, x, num_quantiles, log, tau, *params)
+        return super().__call__(x, num_quantiles, log, tau, **internal)
+
     def forward(self, x, num_quantiles=None, log=False, tau=None, keep=None, fresh_weights=False, col_cache=None, feat=None):
         """model.py:112-157.  Returns (q, quantiles) in IQN mode.  ``feat`` (B, 3136): trunk output computed by the caller
-        (trunk_pair); only valid for no-grad passes."""
+        (trunk_pair); only valid for no-grad passes.  ``keep``: dict that receives the backward's operands."""
         if self.rainbow_only:
             from . import c51
             return c51.forward(self, x, log=log, keep=keep, fresh_weights=fresh_weights)
         if not fresh_weights:
-            self.compose_weights()
+            self._compose_weights()
         if feat is None or keep is not None:
             feat = self.trunk(x, keep, col_cache)
         if tau is None:
@@ -684,13 +721,42 @@ class DQN(nn.Module):
         if keep.get("noise_version", None) != getattr(self, "_noise_version", 0):
             raise RuntimeError("the network's noise was resampled between this forward pass and its backward: the composed "
                                "weights / epsilons of the gradient pass are gone (call backward before the next reset_noise)")
+        R, B, hid, A = keep["feat"].shape[0] * keep["num_quantiles"], keep["feat"].shape[0], self.hidden, self.action_space
+
+        def one_hot(fused_dh, dh, dh_hi, dbs, dz, dzT):
+            if fused_dh:
+                call("riqn_dueling_bwd_bf16", R, B, hid, A, ptr(keep["h"]), ptr(keep["tc"].get("h_hi")), ptr(self._w_eff_z),
+                     ptr(dtheta), ptr(gscale), float(gscale_mul), ptr(actions), ptr(dh_hi), None, ptr(dbs), ptr(dz), ptr(dzT))
+            else:
+                call("riqn_dueling_bwd", R, B, hid, A, ptr(keep["h"]), ptr(self._w_eff_z), ptr(dtheta), ptr(gscale),
+                     float(gscale_mul), ptr(actions), ptr(dh), ptr(dz), ptr(dzT))
+        self._backward_head(keep, one_hot, self.grad_view)
+
+    def backward_iqn_dense(self, keep, grad_q, gv=None):
+        """Accumulate dL/dparams for the forward recorded in ``keep`` given the dense dL/dq ``grad_q`` (Nq*B, A), fp32,
+        rows quantile-major like forward()'s q.  ``gv(param)`` names the gradient buffer of each parameter (default: its
+        view of the gradient arena).  The caller checks that the forward's weights are still live."""
+        R, B, hid, A = keep["feat"].shape[0] * keep["num_quantiles"], keep["feat"].shape[0], self.hidden, self.action_space
+
+        def dense(fused_dh, dh, dh_hi, dbs, dz, dzT):
+            if fused_dh:
+                call("riqn_dueling_bwd_dense_bf16", R, B, hid, A, ptr(keep["h"]), ptr(keep["tc"].get("h_hi")),
+                     ptr(self._w_eff_z), ptr(grad_q), ptr(dh_hi), None, ptr(dbs), ptr(dz), ptr(dzT))
+            else:
+                call("riqn_dueling_bwd_dense", R, B, hid, A, ptr(keep["h"]), ptr(self._w_eff_z), ptr(grad_q), ptr(dh),
+                     ptr(dz), ptr(dzT))
+        self._backward_head(keep, dense, gv or self.grad_view)
+
+    def _backward_head(self, keep, dueling_bwd, gv):
+        """Everything below dL/dq: ``dueling_bwd(fused_dh, dh, dh_hi, dbs, dz, dzT)`` fills the dueling / z-layer data
+        gradients (dh (R, 2*hid) fp32, or its bf16 image dh_hi plus column sums dbs when ``fused_dh``; dz (R, 32) and its
+        bf16 image dzT), then the z-layer weight gradient, the hidden NoisyLinear products, the embedding and the trunk."""
         B = keep["feat"].shape[0]
         Nq = keep["num_quantiles"]
         R = B * Nq
         dev = keep["feat"].device
         hid, A, E = self.hidden, self.action_space, self.quantile_embedding_dim
         hv, ha, zv, za = self.fcnoisy_h_v, self.fcnoisy_h_a, self.fcnoisy_z_v, self.fcnoisy_z_a
-        gv = self.grad_view
         dz = torch.empty(R, 32, device=dev)
         tc = keep.get("tc")
         f16 = bool(tc and tc.get("f16"))
@@ -705,12 +771,9 @@ class DQN(nn.Module):
             dh = None
             dh_hi = torch.empty(R, 2 * hid, dtype=torch.bfloat16, device=dev)
             dh_hiT = None                            # the wgrad reads dh_hi itself (MN-major operand)
-            call("riqn_dueling_bwd_bf16", R, B, hid, A, ptr(keep["h"]), ptr(tc.get("h_hi")), ptr(self._w_eff_z), ptr(dtheta), ptr(gscale),
-                 float(gscale_mul), ptr(actions), ptr(dh_hi), None, ptr(dbs), ptr(dz), ptr(dzT))
         else:
-            dh = torch.empty(R, 2 * hid, device=dev)
-            call("riqn_dueling_bwd", R, B, hid, A, ptr(keep["h"]), ptr(self._w_eff_z), ptr(dtheta), ptr(gscale),
-                 float(gscale_mul), ptr(actions), ptr(dh), ptr(dz), ptr(dzT))
+            dh, dh_hi = torch.empty(R, 2 * hid, device=dev), None
+        dueling_bwd(fused_dh, dh, dh_hi, dbs, dz, dzT)
         dwz = torch.empty(32, 2 * hid, device=dev)
         dbz = torch.empty(32, device=dev)
         zargs = (ptr(dwz), ptr(dbz), ptr(zv.weight_epsilon), ptr(zv.bias_epsilon), ptr(za.weight_epsilon),
@@ -805,3 +868,93 @@ class DQN(nn.Module):
                      ptr(gv(conv.weight)), ptr(gv(conv.bias)), ptr(din))
             if i > 0:
                 douts[i - 1] = din
+
+
+def _grad_views(net, training):
+    """Gradient buffer of each parameter for a backward: its view of the arena.  A forward in eval mode ran on the
+    mu-only weights (model.py:45-53), so sigma is not in its graph: the sigma gradients go to a discarded buffer."""
+    if training:
+        return net.grad_view
+    scratch = torch.empty_like(net._flat_grad)
+    sigmas = {id(p) for _, m in net.noisy_layers() for p in (m.weight_sigma, m.bias_sigma)}
+
+    def gv(p):
+        off = net._offsets[id(p)]
+        return (scratch if id(p) in sigmas else net._flat_grad)[off:off + p.numel()].view(p.shape)
+    return gv
+
+
+class _DQNForward(torch.autograd.Function):
+    """DQN.forward as one autograd node.  The forward keeps its own backward operands (activations, bf16 images); the
+    weights it ran on stay live in the network, so its backward must come before the next reset_noise() or parameter
+    update.  The backward accumulates straight into the gradient arena behind every param.grad."""
+
+    @staticmethod
+    def forward(ctx, net, x, num_quantiles, log, tau, *params):
+        keep = {}
+        out = net.forward(x, num_quantiles, log, tau, keep)
+        ctx.net, ctx.keep, ctx.log, ctx.n_params = net, keep, log, len(params)
+        ctx.live = net._live_weights_key()
+        if net.rainbow_only:
+            ctx.save_for_backward(out)
+            return out
+        keep.pop("q")                # the outputs are not kept in ctx (a reference cycle through the graph)
+        keep.pop("tau")
+        q, tau = out
+        ctx.mark_non_differentiable(tau)
+        return q, tau
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out, *_):
+        net, keep = ctx.net, ctx.keep
+        if keep is None:
+            raise RuntimeError("backward through this DQN forward already ran: its saved state is released after the first "
+                               "backward (run the forward again for a second backward)")
+        if net._live_weights_key() != ctx.live:
+            raise RuntimeError("the network's weights changed between this forward and its backward (reset_noise(), an "
+                               "optimiser step, load_state_dict(), compose_weights() or a train/eval switch with a new "
+                               "forward): the backward reads the live weights, so call it before such a change")
+        ctx.keep = None
+        gv = _grad_views(net, ctx.live[2])
+        g = grad_out.contiguous().float()
+        if net.rainbow_only:
+            from . import c51
+            out, = ctx.saved_tensors
+            c51.backward_dense(net, keep, out, g, ctx.log, gv)
+        else:
+            net.backward_iqn_dense(keep, g, gv)
+        return (None,) * (5 + ctx.n_params)
+
+
+class _NoisyLinearFn(torch.autograd.Function):
+    """NoisyLinear.forward as an autograd node.  It keeps its input and a copy of the weights and noise it ran on, so a
+    reset_noise() or parameter update between the forward and the backward does not change the gradients."""
+
+    @staticmethod
+    def forward(ctx, layer, input, weight_mu, weight_sigma, bias_mu, bias_sigma):
+        x = input.contiguous().float()
+        out = layer._forward(x)
+        ctx.save_for_backward(x, layer._w_eff.clone(), layer.weight_epsilon.clone(), layer.bias_epsilon.clone())
+        ctx.training, ctx.in_dtype = layer.training, input.dtype
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        x, w_eff, eps_w, eps_b = ctx.saved_tensors
+        dy = grad_out.contiguous().float()
+        rows, n_in, n_out = x.shape[0], w_eff.shape[1], w_eff.shape[0]
+        dx = None
+        if ctx.needs_input_grad[1]:
+            dx = torch.empty_like(x)
+            call("riqn_noisy_linear_dgrad", rows, n_in, n_out, ptr(dy), ptr(w_eff), ptr(dx))
+            dx = dx.to(ctx.in_dtype)
+        g_wmu, g_wsig = torch.zeros_like(w_eff), torch.zeros_like(w_eff)
+        g_bmu, g_bsig = torch.zeros(n_out, device=x.device), torch.zeros(n_out, device=x.device)
+        db = torch.empty(n_out, device=x.device)
+        call("riqn_noisy_linear_wgrad", rows, n_in, n_out, ptr(dy), ptr(x), ptr(eps_w), ptr(eps_b), ptr(db), ptr(g_wmu),
+             ptr(g_wsig), ptr(g_bmu), ptr(g_bsig))
+        if not ctx.training:        # eval mode ran on weight_mu / bias_mu alone: sigma is not in the graph
+            g_wsig = g_bsig = None
+        return None, dx, g_wmu, g_wsig, g_bmu, g_bsig

@@ -57,7 +57,7 @@ class Adam(torch.optim.Optimizer):
         call("riqn_adam_step", self._flat.numel(), ptr(self._flat), ptr(grad_flat), ptr(self._exp_avg),
              ptr(self._exp_avg_sq), self._step, float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]),
              float(g["eps"]), float(self.grad_scale), self._dyn.ptr() if self._dyn is not None else None)
-        self._net._static_ops_dirty = True      # conv / iqn_fc operand images are rebuilt by the next reset_noise()
+        self._net._params_changed()             # conv / iqn_fc operand images are rebuilt by the next reset_noise()
 
     def bias_corrections(self, step):
         """(-(lr / (1 - b1^t)), sqrt(1 - b2^t)) of step t, as torch.optim.Adam computes them."""
