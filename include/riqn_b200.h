@@ -135,6 +135,21 @@ int riqn_split_bf16_scaled(long rows, int cols, const float* src, float scale, v
 /* out[i] ~ U(0,1): the quantile fractions tau.  Philox4x32-10 keyed by (seed, stream_id). */
 int riqn_fill_uniform(long n, unsigned long long seed, unsigned long long stream_id, float* out,
                       const riqn_dyn_state* dyn, void* stream);
+
+/* Distortion risk measures beta of riqn_fill_tau_distorted (IQN paper, Dabney et al. 2018, section 3.1). */
+#define RIQN_RISK_NEUTRAL 0   /* beta(t) = t                                                          */
+#define RIQN_RISK_CVAR 1      /* beta(t) = eta t,                                      0 < eta <= 1   */
+#define RIQN_RISK_WANG 2      /* beta(t) = Phi(Phi^-1(t) + eta),                       eta finite     */
+#define RIQN_RISK_CPW 3       /* beta(t) = t^eta / (t^eta + (1-t)^eta)^(1/eta),        eta > 0        */
+#define RIQN_RISK_POW 4       /* beta(t) = t^(1/(1+|eta|)) for eta >= 0, 1-(1-t)^(1/(1+|eta|)) for eta < 0, eta finite */
+#define RIQN_RISK_NORM 5      /* mean of eta uniforms,                                 eta in {1..32} */
+/* out[i] = beta(u_i): the distorted quantile fractions of risk-sensitive action selection.  u is exactly what
+ * riqn_fill_uniform(n, seed, stream_id) writes (same Philox counters, same dyn->rng_offset), so out[i] applies beta to
+ * the plain draw's element i.  Norm: out[i] = (u'[i*eta] + ... + u'[i*eta + eta-1]) / eta, summed in that order, where
+ * u' is what riqn_fill_uniform(n * eta, seed, stream_id) writes.  beta is evaluated in double and rounded once to float.
+ * Returns cudaErrorInvalidValue (and writes nothing) for an unknown measure or an eta outside its domain. */
+int riqn_fill_tau_distorted(long n, unsigned long long seed, unsigned long long stream_id, int measure, float eta,
+                            float* out, const riqn_dyn_state* dyn, void* stream);
 /* out[i] = sign(x) sqrt|x|, x ~ N(0,1): NoisyLinear._scale_noise (model.py:32-37). */
 int riqn_noisy_sample(long n, unsigned long long seed, unsigned long long stream_id, float* out,
                       const riqn_dyn_state* dyn, void* stream);

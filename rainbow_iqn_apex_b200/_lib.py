@@ -51,6 +51,7 @@ SIGNATURES = {
     "riqn_im2col_bf16_t": [C.POINTER(ConvGeom), _P, C.c_int, _P, _P],
     "riqn_split_bf16_scaled": [C.c_long, C.c_int, _P, C.c_float, _P, _P, _P],
     "riqn_fill_uniform": [C.c_long, C.c_ulonglong, C.c_ulonglong, _P, _P, _P],
+    "riqn_fill_tau_distorted": [C.c_long, C.c_ulonglong, C.c_ulonglong, C.c_int, C.c_float, _P, _P, _P],
     "riqn_noisy_sample": [C.c_long, C.c_ulonglong, C.c_ulonglong, _P, _P, _P],
     "riqn_noisy_compose": [C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, _P],
     "riqn_noisy_reset_net": [C.c_int, C.POINTER(NoisyLayer), C.c_ulonglong, C.c_int, C.c_int, _P, _P],

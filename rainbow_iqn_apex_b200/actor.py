@@ -20,15 +20,16 @@ class Actor(Agent):
         return tau
 
     def act(self, state_buffer):
-        """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN) or the expected
-        value of the categorical distribution (C51).  Frames go to the device as uint8; the /255 of the
+        """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN; distorted by ``self.risk``) or the
+        expected value of the categorical distribution (C51).  Frames go to the device as uint8; the /255 of the
         reference happens inside the conv kernel."""
         state = torch.from_numpy(np.stack(state_buffer).astype(np.uint8)).to(self.online_net._flat.device)
         with torch.no_grad():
             if self.rainbow_only:
                 p = self.online_net(state.unsqueeze(0))
                 return (p * self.support).sum(2).argmax(1).item()
-            quantile_values, _ = self.online_net(state.unsqueeze(0), self.num_quantile_samples, tau=self._pop_tau())
+            quantile_values, _ = self.online_net(state.unsqueeze(0), self.num_quantile_samples, tau=self._pop_tau(),
+                                                  risk=self.risk)
             a = torch.empty(1, dtype=torch.int64, device=state.device)
             call("riqn_argmax_mean", 1, self.num_quantile_samples, self.action_space, ptr(quantile_values), ptr(a))
             return int(a.item())
@@ -39,16 +40,18 @@ class Actor(Agent):
             if self.rainbow_only:
                 return (self.online_net(states_u8) * self.support).sum(2).argmax(1)
             E = states_u8.shape[0]
-            q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=self._pop_tau())
+            q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=self._pop_tau(), risk=self.risk)
             a = torch.empty(E, dtype=torch.int64, device=q.device)
             call("riqn_argmax_mean", E, self.num_quantile_samples, self.action_space, ptr(q), ptr(a))
             return a
 
     def act_batch_values(self, states_u8, tau=None):
-        """(E, A) mean quantile values behind act_batch (the argmax input; parity tests and epsilon schedules)."""
+        """(E, A) mean quantile values behind act_batch (the argmax input; parity tests and epsilon schedules): Q_beta
+        under ``self.risk``, the mean over K fractions beta(tau) unless ``tau`` is given."""
         with torch.no_grad():
             E = states_u8.shape[0]
-            q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=tau if tau is not None else self._pop_tau())
+            q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=tau if tau is not None else self._pop_tau(),
+                                   risk=self.risk)
             # q rows are quantile-major (k*E + e), like the reference (model.py:149)
             return q.view(self.num_quantile_samples, E, self.action_space).mean(0)
 

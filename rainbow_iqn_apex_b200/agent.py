@@ -3,7 +3,7 @@
 Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``args`` fields, same public
 attributes (online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
-compute_loss_actor_or_learner, save, train, eval).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting.  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema
 {T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160).
 """
@@ -13,7 +13,7 @@ import torch
 
 from . import _lib
 from . import compute_loss_iqn
-from .model import DQN
+from .model import DQN, check_risk
 from .optim import Adam
 
 
@@ -55,6 +55,18 @@ class Agent:
             for field in self._IQN_FIELDS:
                 setattr(self, field, getattr(args, field))
         self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}
+        # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
+        self.risk = None
+        self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
+
+    def set_risk(self, measure, eta=None):
+        """Act, and pick the double-DQN target action a*, under a distortion risk measure (IQN paper, section 3.1):
+        ``measure`` is "neutral", "cvar", "wang", "cpw", "pow" or "norm" (model.RISK_MEASURES), ``eta`` its parameter.
+        The K quantile fractions of those passes become beta(tau); the N and N' fractions of the loss stay uniform."""
+        risk = check_risk((measure, eta))
+        if risk is not None and self.rainbow_only:
+            raise ValueError("risk measures distort the IQN quantile fractions; rainbow_only (C51) acts risk-neutrally")
+        self.risk = risk
 
     @staticmethod
     def _read_checkpoint(path):

@@ -7,6 +7,7 @@ the parameters' ``.grad`` (views of the gradient arena), exactly where the refer
 
 Three network passes, in the reference's order and with a fresh noise sample before each
 (:234, :255, :289): online(next_states, K) -> a*; target(next_states, N') -> targets; online(states, N).
+Under a risk measure (Agent.set_risk) only the K pass draws distorted fractions beta(tau).
 """
 import os
 
@@ -46,7 +47,9 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     # both no-grad passes read next_states: their conv trunks (noise-free weights) run as ONE stacked batch, three launches
     pair = on.trunk_pair(tg, next_states) if not (on.rainbow_only or os.environ.get("RIQN_NO_TRUNK_PAIR") == "1") else None
     f_on, f_tg = pair if pair is not None else (None, None)
-    q_sel, _ = on.forward(next_states, K, tau=taus[0], fresh_weights=True, col_cache=cache, feat=f_on)   # :235-237
+    # the action selection alone acts under the agent's risk measure (IQN paper, section 3.1): a* = argmax_a Q_beta(x', a)
+    q_sel, tau_sel = on.forward(next_states, K, tau=taus[0], fresh_weights=True, col_cache=cache, feat=f_on,
+                                risk=getattr(agent, "risk", None))                                        # :235-237
     a_star = torch.empty(B, dtype=torch.int64, device=dev)
     call("riqn_argmax_mean", B, K, A, ptr(q_sel), ptr(a_star))                      # :238-245
     tg.reset_noise(noises[1])                                                       # :255
@@ -66,7 +69,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
          ptr(dtheta), ptr(theta_out), ptr(target_out))                              # :262-357
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on, tau=tau,
-                     keep=keep)
+                     keep=keep, tau_sel=tau_sel)
     return loss, dtheta, keep, actions
 
 

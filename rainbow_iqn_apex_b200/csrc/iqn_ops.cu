@@ -26,6 +26,48 @@ __global__ void fill_uniform_kernel(long n, uint64_t seed, uint64_t stream, floa
     if (i4 * 4 + j < n) out[i4 * 4 + j] = v[j];
 }
 
+// Distorted quantile fractions beta(tau) for risk-sensitive action selection (Dabney et al. 2018, IQN, section 3.1).
+// Output i reads the uniforms riqn_fill_uniform(n * m, seed, stream) writes at positions i*m .. i*m+m-1 (m = eta for
+// Norm, else 1), so the draw shares the counter layout, the stream id and the dyn offset of the plain one.  beta is
+// evaluated in double and rounded once to float.
+__global__ void fill_tau_distorted_kernel(long n, uint64_t seed, uint64_t stream, int measure, double eta,
+                                          float* __restrict__ out, const riqn_dyn_state* __restrict__ dyn) {
+  if (dyn) stream += dyn->rng_offset;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int m = measure == RIQN_RISK_NORM ? (int)eta : 1;
+  double s = 0.0;
+  long blk = -1;
+  uint4 r = make_uint4(0u, 0u, 0u, 0u);
+  for (int j = 0; j < m; ++j) {
+    const long p = i * m + j;
+    if ((p >> 2) != blk) {
+      blk = p >> 2;
+      r = Philox::draw(seed, stream, (uint64_t)blk);
+    }
+    const uint32_t w = (p & 3) == 0 ? r.x : (p & 3) == 1 ? r.y : (p & 3) == 2 ? r.z : r.w;
+    s += (double)Philox::u01(w);                 // exact: at most 32 multiples of 2^-25 below 32
+  }
+  double b;
+  switch (measure) {
+    case RIQN_RISK_CVAR: b = eta * s; break;
+    case RIQN_RISK_WANG: b = normcdf(normcdfinv(s) + eta); break;
+    case RIQN_RISK_CPW: {
+      const double a = pow(s, eta);
+      b = a / pow(a + pow(1.0 - s, eta), 1.0 / eta);
+      break;
+    }
+    case RIQN_RISK_POW: {
+      const double e = 1.0 / (1.0 + fabs(eta));
+      b = eta >= 0.0 ? pow(s, e) : 1.0 - pow(1.0 - s, e);
+      break;
+    }
+    case RIQN_RISK_NORM: b = s / eta; break;
+    default: b = s; break;                       // RIQN_RISK_NEUTRAL
+  }
+  out[i] = __double2float_rn(b);
+}
+
 // f(x) = sign(x) sqrt|x| of x ~ N(0,1)            (NoisyLinear._scale_noise, model.py:32-37)
 __global__ void fill_scaled_normal_kernel(long n, uint64_t seed, uint64_t stream, float* __restrict__ out,
                                           const riqn_dyn_state* __restrict__ dyn) {
@@ -1072,6 +1114,26 @@ RIQN_API int riqn_fill_uniform(long n, unsigned long long seed, unsigned long lo
   riqn::note_launches(1);
   if (n <= 0) return 0;
   fill_uniform_kernel<<<riqn_cdiv((n + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(n, seed, stream_id, out, dyn);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_fill_tau_distorted(long n, unsigned long long seed, unsigned long long stream_id, int measure,
+                                     float eta, float* out, const riqn_dyn_state* dyn, void* stream) {
+  bool ok;
+  switch (measure) {
+    case RIQN_RISK_NEUTRAL: ok = true; break;
+    case RIQN_RISK_CVAR: ok = eta > 0.f && eta <= 1.f; break;
+    case RIQN_RISK_WANG:
+    case RIQN_RISK_POW: ok = isfinite(eta); break;
+    case RIQN_RISK_CPW: ok = eta > 0.f && isfinite(eta); break;
+    case RIQN_RISK_NORM: ok = eta >= 1.f && eta <= 32.f && eta == floorf(eta); break;
+    default: ok = false;
+  }
+  if (!ok) return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  if (n <= 0) return 0;
+  fill_tau_distorted_kernel<<<riqn_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(n, seed, stream_id, measure,
+                                                                                 (double)eta, out, dyn);
   return (int)cudaGetLastError();
 }
 

@@ -61,8 +61,9 @@ class Learner(Agent):
                 torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
         self.optimiser.step()
 
-    def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights):
-        """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena."""
+    def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
+        """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena.
+        ``debug``: dict that receives the IQN loss's intermediates (compute_loss_iqn.loss_core)."""
         on = self.online_net
         dev = on._flat.device
         weights = weights.to(dev, torch.float32)
@@ -73,7 +74,7 @@ class Learner(Agent):
             bw(weights, 1.0 / weights.shape[0])
         else:
             loss, dtheta, keep, actions = compute_loss_iqn.loss_core(
-                self, states, actions, returns, next_states, nonterminals, keep_graph=True)
+                self, states, actions, returns, next_states, nonterminals, keep_graph=True, debug=debug)
             if getattr(self, "_debug", None) is not None:                       # parity tests: the pass's activations
                 self._debug.update(keep=keep)
             on.zero_grad()                                                      # learner.py:22
@@ -325,6 +326,21 @@ class Learner(Agent):
             self._bgraph_post.replay()
         self.optimiser._step += 1
         return self._bg_out
+
+    def set_risk(self, measure, eta=None):
+        """Agent.set_risk.  A captured step graph holds the measure and eta as kernel arguments, so it refuses once one
+        is captured: release_graphs(), set the risk, then capture again."""
+        if any(getattr(self, g, None) is not None for g in ("_graph", "_bgraph", "_lgraph")):
+            raise RuntimeError("this learner's step is captured in a CUDA graph that holds the current risk measure: "
+                               "call release_graphs(), set the risk, then recapture (enable_cuda_graph / "
+                               "enable_batch_graph / enable_learn_graph)")
+        super().set_risk(measure, eta)
+
+    def release_graphs(self):
+        """Drop every captured step graph; learn_and_update runs eagerly again until the next capture."""
+        self._graph = self._graph_post = self._graph_mem = self._graph_out = None
+        self._bgraph = self._bgraph_post = self._bg_out = None
+        self._lgraph = self._lg_out = None
 
     # north_star spellings
     update_target = Agent.update_target_net

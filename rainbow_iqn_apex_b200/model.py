@@ -15,7 +15,9 @@ optimiser and the gradient all-reduce touch one contiguous buffer.
 
 There is no PyTorch fallback: every tensor operation below is a C-ABI call (include/riqn_b200.h).
 """
+import ctypes
 import math
+import numbers
 import os
 import weakref
 
@@ -51,6 +53,38 @@ def set_precision(fwd=None, bwd=None):
             PRECISION[k] = v
     if PRECISION["fwd"] == "fp16" and PRECISION["bwd"] != "bf16":
         raise ValueError("the fp16 forward pairs with the bf16 backward (it reads the bf16 images written beside the fp16 ones)")
+
+
+# Distortion risk measures of risk-sensitive action selection (Dabney et al. 2018, IQN, section 3.1) -> the RIQN_RISK_*
+# codes of riqn_fill_tau_distorted (include/riqn_b200.h, which states each beta and the domain of eta).
+RISK_MEASURES = {"neutral": 0, "cvar": 1, "wang": 2, "cpw": 3, "pow": 4, "norm": 5}
+
+
+def check_risk(risk):
+    """Validate ``risk``: None or a ``(measure, eta)`` pair.  Returns None for the risk-neutral draw (plain uniform
+    fractions), else ``(measure, eta)`` with the measure lower-cased and eta a float.  The domain is checked on eta as
+    the kernel receives it (float32)."""
+    if risk is None:
+        return None
+    try:
+        measure, eta = risk
+    except (TypeError, ValueError):
+        raise ValueError(f"risk must be None or a (measure, eta) pair, got {risk!r}") from None
+    name = measure.lower() if isinstance(measure, str) else None
+    if name not in RISK_MEASURES:
+        raise ValueError(f"unknown risk measure {measure!r} (one of {', '.join(RISK_MEASURES)})")
+    if name == "neutral":
+        return None
+    if isinstance(eta, bool) or not isinstance(eta, numbers.Real):
+        raise ValueError(f"the {name} risk measure needs a real eta, got {eta!r}")
+    e = ctypes.c_float(eta).value
+    ok = {"cvar": 0.0 < e <= 1.0, "wang": math.isfinite(e), "cpw": 0.0 < e < math.inf, "pow": math.isfinite(e),
+          "norm": 1.0 <= e <= 32.0 and e == int(e)}[name]
+    if not ok:
+        need = {"cvar": "0 < eta <= 1", "wang": "a finite eta", "cpw": "eta > 0", "pow": "a finite eta",
+                "norm": "an integer eta in [1, 32]"}[name]
+        raise ValueError(f"the {name} risk measure needs {need}, got eta={eta!r}")
+    return name, float(eta)
 
 
 def _small_x3():
@@ -482,12 +516,19 @@ class DQN(nn.Module):
             m._dyn = dyn
             m._calls_in_step = 0
 
-    def draw_quantiles(self, n):
+    def draw_quantiles(self, n, risk=None):
+        """n quantile fractions tau ~ U(0,1) on the device, or beta(tau) under the distortion risk measure ``risk`` =
+        (measure, eta) (riqn_fill_tau_distorted: beta applied to the very uniforms the plain draw would return)."""
+        risk = check_risk(risk)
         tau = torch.empty(n, 1, device=self._flat.device)
         dyn = getattr(self, "_dyn", None)
         idx = self._tau_in_step if dyn is not None else self._tau_calls
-        call("riqn_fill_uniform", n, self._rng_seed ^ 0x7A75, self._tau_stream_offset + idx + (0 if dyn is not None else _EAGER_STREAMS), ptr(tau),
-             dyn.ptr() if dyn else None)
+        stream_id = self._tau_stream_offset + idx + (0 if dyn is not None else _EAGER_STREAMS)
+        if risk is None:
+            call("riqn_fill_uniform", n, self._rng_seed ^ 0x7A75, stream_id, ptr(tau), dyn.ptr() if dyn else None)
+        else:
+            call("riqn_fill_tau_distorted", n, self._rng_seed ^ 0x7A75, stream_id, RISK_MEASURES[risk[0]], risk[1], ptr(tau),
+                 dyn.ptr() if dyn else None)
         self._tau_calls += 1
         self._tau_in_step += 1
         return tau
@@ -683,24 +724,34 @@ class DQN(nn.Module):
                         head_bwd_tc=bwd_tc, emb_bwd_tc=emb_tc)
         return q
 
-    def __call__(self, x, num_quantiles=None, log=False, tau=None, **internal):
+    def __call__(self, x, num_quantiles=None, log=False, tau=None, risk=None, **internal):
         """``net(x, N)`` / ``net(x, log=...)``, the reference's call.  With grad mode on, a parameter that requires grad and
         none of forward()'s internal arguments, the call is one autograd node (_DQNForward): the output (q, or the C51
         (log-)probabilities) has a grad_fn, and ``.backward()`` of any scalar built from it accumulates the parameter
-        gradients into ``param.grad``.  Otherwise it is forward() itself, which the learner's own passes call directly."""
+        gradients into ``param.grad``.  Otherwise it is forward() itself, which the learner's own passes call directly.
+        ``risk``: see forward()."""
         if not internal and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             for name, t in (("x", x), ("tau", tau)):
                 if torch.is_tensor(t) and t.requires_grad:
                     raise RuntimeError(f"DQN.forward computes gradients for the network's parameters only, not for its "
                                        f"inputs: {name} requires grad (pass {name}.detach())")
             params = [p for p in self.parameters() if p.requires_grad]
-            return _DQNForward.apply(self, x, num_quantiles, log, tau, *params)
+            return _DQNForward.apply(self, x, num_quantiles, log, tau, risk, *params)
+        if risk is not None:
+            internal["risk"] = risk
         return super().__call__(x, num_quantiles, log, tau, **internal)
 
-    def forward(self, x, num_quantiles=None, log=False, tau=None, keep=None, fresh_weights=False, col_cache=None, feat=None):
+    def forward(self, x, num_quantiles=None, log=False, tau=None, keep=None, fresh_weights=False, col_cache=None, feat=None,
+                risk=None):
         """model.py:112-157.  Returns (q, quantiles) in IQN mode.  ``feat`` (B, 3136): trunk output computed by the caller
-        (trunk_pair); only valid for no-grad passes.  ``keep``: dict that receives the backward's operands."""
+        (trunk_pair); only valid for no-grad passes.  ``keep``: dict that receives the backward's operands.  ``risk``:
+        None or (measure, eta), a distortion risk measure (RISK_MEASURES) under which the drawn fractions are beta(tau); the
+        returned quantiles are those distorted fractions.  An explicit ``tau`` is embedded as given and ``risk`` then
+        draws nothing."""
+        risk = check_risk(risk)
         if self.rainbow_only:
+            if risk is not None:
+                raise ValueError("risk measures distort the IQN quantile fractions; the C51 network acts risk-neutrally")
             from . import c51
             return c51.forward(self, x, log=log, keep=keep, fresh_weights=fresh_weights)
         if not fresh_weights:
@@ -708,7 +759,7 @@ class DQN(nn.Module):
         if feat is None or keep is not None:
             feat = self.trunk(x, keep, col_cache)
         if tau is None:
-            tau = self.draw_quantiles(num_quantiles * x.shape[0])
+            tau = self.draw_quantiles(num_quantiles * x.shape[0], risk)
         else:
             tau = tau.to(feat.device, torch.float32).reshape(-1, 1).contiguous()
         q = self.iqn_head(feat, num_quantiles, tau, keep)
@@ -890,9 +941,9 @@ class _DQNForward(torch.autograd.Function):
     update.  The backward accumulates straight into the gradient arena behind every param.grad."""
 
     @staticmethod
-    def forward(ctx, net, x, num_quantiles, log, tau, *params):
+    def forward(ctx, net, x, num_quantiles, log, tau, risk, *params):
         keep = {}
-        out = net.forward(x, num_quantiles, log, tau, keep)
+        out = net.forward(x, num_quantiles, log, tau, keep, risk=risk)
         ctx.net, ctx.keep, ctx.log, ctx.n_params = net, keep, log, len(params)
         ctx.live = net._live_weights_key()
         if net.rainbow_only:
@@ -924,7 +975,7 @@ class _DQNForward(torch.autograd.Function):
             c51.backward_dense(net, keep, out, g, ctx.log, gv)
         else:
             net.backward_iqn_dense(keep, g, gv)
-        return (None,) * (5 + ctx.n_params)
+        return (None,) * (6 + ctx.n_params)
 
 
 class _NoisyLinearFn(torch.autograd.Function):
