@@ -63,6 +63,15 @@ typedef struct riqn_conv_geom {
                                 (B, history+n, 84, 84) replay window                             */
 } riqn_conv_geom;
 
+/* The trunk takes one of three paths:
+ *   - strip convolution (riqn_s2d_u8, riqn_conv_fwd_strip, riqn_conv_bwd_strip): uint8 frames with 16-byte aligned
+ *     samples and history 4, in every tensor-core precision mode;
+ *   - explicit im2col on the tensor cores (riqn_conv_fwd_tc, riqn_conv_bwd_tc): every other input (fp32 frames, uint8
+ *     frames that are unaligned or of another history);
+ *   - fp32 on the CUDA cores (riqn_conv_fwd, riqn_conv_bwd), the cross-check path.  riqn_conv_bwd on the operands of
+ *     riqn_im2col_f32 is also the backward of the other two when the backward is not bf16 or an im2col row count
+ *     (B*OH*OW) is not a multiple of 8. */
+
 /* out = relu(conv(in) + bias).  `in` is uint8 frames (x/255 applied on the fly, reproducing
  * redis_memory.py:527-536) when in_is_u8 != 0, else fp32.  `col` (B*OH*OW, Cin*KH*KW) is workspace
  * that riqn_conv_bwd re-uses. */
@@ -94,8 +103,7 @@ int riqn_conv_fwd_tc(const riqn_conv_geom* g, const void* in, int in_is_u8, cons
  *                ordered (dy, dx, within-block); out (B, Cout, OH, OW) fp32 = relu(conv + bias), or NULL when only the
  *                next layer's images are wanted (no-grad passes); next_hi / next_lo (may be
  *                NULL) receive the result as the NEXT layer's block matrix (block edge next_stride, grid next_grid,
- *                within-block order (iy, ix, c)).
- *   riqn_im2col_bf16_t: the transposed bf16 im2col (K, M) alone, the wgrad operand of riqn_conv_bwd_tc. */
+ *                within-block order (iy, ix, c)). */
 int riqn_s2d_u8(const riqn_conv_geom* g, const unsigned char* in, void* a_px, void* stream);
 int riqn_conv_fwd_strip(const riqn_conv_geom* g, const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,
                         const float* bias, float* out, void* next_hi, void* next_lo, int next_stride, int next_grid,
@@ -104,7 +112,6 @@ int riqn_conv_fwd_strip(const riqn_conv_geom* g, const void* a_hi, const void* a
  * halves of a stacked batch, samples [0, B/2) use w_hi / w_lo / bias, samples [B/2, B) use w2_hi / w2_lo / bias2; outputs and
  * next-layer images are the stacked (B, ...) tensors.  share_a != 0: the A image holds B/2 samples read by both halves (first
  * layer: the pixel block matrix).  Needs (B/2)*G*G % 128 == 0. */
-int riqn_im2col_bf16_t(const riqn_conv_geom* g, const void* in, int in_is_u8, void* colT_hi, void* stream);
 /* Backward of a strip convolution on the tensor cores, again without im2col matrices: a_hi is the block matrix the
  * forward read (riqn_s2d_u8 / the previous layer's next_hi); w_hi (Cout, K) bf16 weight in the ORIGINAL k order (data
  * gradient, read as an MN-major operand); perm (K ints): strip k order -> original k; dYg (B*G*G, Cout) bf16 and dwp_scratch (Cout*K floats)
@@ -114,18 +121,12 @@ int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, const float*
                         const int* perm, void* dYg, float* dwp_scratch, float* dw, float* dbias, float* din,
                         float wgrad_scale, void* stream);
 
-/* Backward on the tensor cores (bf16 operands, fp32 accumulate): wT_hi (K, Cout) bf16; dY_hi (M, Cout) and dYT_hi
- * (Cout, M) bf16 workspaces; dcol fp32 (M, K) workspace; dw/dbias accumulated; din may be NULL. */
+/* Backward of riqn_conv_fwd_tc on the tensor cores (bf16 operands, fp32 accumulate): colT_hi as that forward wrote it;
+ * wT_hi (K, Cout) bf16; dY_hi (M, Cout) and dYT_hi (Cout, M) bf16 workspaces; dcol fp32 (M, K) workspace; dw/dbias
+ * accumulated, dw += wgrad_scale * (dY^T col) (the trunk passes 1); din may be NULL. */
 int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const float* out, const void* colT_hi, const void* wT_hi,
                      void* dY_hi, void* dYT_hi, float* dcol, float* dw, float* dbias, float* din, float wgrad_scale,
                      void* stream);
-/* First layer on raw uint8 frames: pixel values 0..255 are exact in bf16, so the im2col operand has no lo image and the
- * reference's /255 (redis_memory.py:527-536) is folded into the weights: ws_hi / ws_lo = bf16 images of weight/255
- * (ws_lo == NULL: single-bf16 product).  col_px (M, K) and colT_px (K, M; may be NULL) hold pixel values; pass
- * wgrad_scale = 1/255 to riqn_conv_bwd_tc when it consumes colT_px.  in: 16-byte aligned, in_bstride % 16 == 0.
- * reuse_col != 0: col_px already holds the im2col of `in` (the online and target passes over next_states share it). */
-int riqn_conv_fwd_tc_u8(const riqn_conv_geom* g, const unsigned char* in, const void* ws_hi, const void* ws_lo,
-                        const float* bias, void* col_px, void* colT_px, float* out, int reuse_col, void* stream);
 /* split of (src * scale): bf16 hi / lo images of a scaled matrix (e.g. weight/255). */
 int riqn_split_bf16_scaled(long rows, int cols, const float* src, float scale, void* hi, void* lo, void* stream);
 

@@ -44,11 +44,9 @@ SIGNATURES = {
     "riqn_im2col_f32": [C.POINTER(ConvGeom), _P, C.c_int, _P, _P],
     "riqn_conv_fwd_tc": [C.POINTER(ConvGeom), _P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P],
     "riqn_conv_bwd_tc": [C.POINTER(ConvGeom), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_float, _P],
-    "riqn_conv_fwd_tc_u8": [C.POINTER(ConvGeom), _P, _P, _P, _P, _P, _P, _P, C.c_int, _P],
     "riqn_s2d_u8": [C.POINTER(ConvGeom), _P, _P, _P],
     "riqn_conv_fwd_strip": [C.POINTER(ConvGeom), _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, _P],
     "riqn_conv_bwd_strip": [C.POINTER(ConvGeom), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_float, _P],
-    "riqn_im2col_bf16_t": [C.POINTER(ConvGeom), _P, C.c_int, _P, _P],
     "riqn_split_bf16_scaled": [C.c_long, C.c_int, _P, C.c_float, _P, _P, _P],
     "riqn_fill_uniform": [C.c_long, C.c_ulonglong, C.c_ulonglong, _P, _P, _P],
     "riqn_fill_tau_distorted": [C.c_long, C.c_ulonglong, C.c_ulonglong, C.c_int, C.c_float, _P, _P, _P],

@@ -9,8 +9,6 @@ Three network passes, in the reference's order and with a fresh noise sample bef
 (:234, :255, :289): online(next_states, K) -> a*; target(next_states, N') -> targets; online(states, N).
 Under a risk measure (Agent.set_risk) only the K pass draws distorted fractions beta(tau).
 """
-import os
-
 import torch
 
 from ._lib import call, ptr
@@ -43,9 +41,9 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     dev = states.device
 
     on.reset_noise(noises[0])                                                       # :234
-    cache = {}   # conv1's pixel im2col of next_states is shared by the online and the target pass
+    cache = {}   # conv1's pixel block matrix of next_states is shared by the online and the target pass
     # both no-grad passes read next_states: their conv trunks (noise-free weights) run as ONE stacked batch, three launches
-    pair = on.trunk_pair(tg, next_states) if not (on.rainbow_only or os.environ.get("RIQN_NO_TRUNK_PAIR") == "1") else None
+    pair = on.trunk_pair(tg, next_states) if not on.rainbow_only else None
     f_on, f_tg = pair if pair is not None else (None, None)
     # the action selection alone acts under the agent's risk measure (IQN paper, section 3.1): a* = argmax_a Q_beta(x', a)
     q_sel, tau_sel = on.forward(next_states, K, tau=taus[0], fresh_weights=True, col_cache=cache, feat=f_on,

@@ -235,86 +235,6 @@ __global__ void im2col_bf16_u8_kernel(riqn_conv_geom g, const uint8_t* __restric
   }
 }
 
-// Raw-pixel im2col for the first layer: one block per sample stages the uint8 frame stack in shared memory (coalesced
-// 16-byte loads), then writes col (M, K) -- and colT (K, M) for the backward -- with the pixel VALUES 0..255 as bf16
-// (exact); the 1/255 of the reference (redis_memory.py:527-536) is folded into the weights / the gradient scale.
-__global__ void im2col_u8_staged_kernel(riqn_conv_geom g, const uint8_t* __restrict__ in, bf16* __restrict__ col,
-                                        bf16* __restrict__ colT) {
-  extern __shared__ __align__(16) uint8_t img[];
-  const int chw = g.Cin * g.H * g.W, K = g.Cin * g.KH * g.KW, K8 = K / 8, ohw = g.OH * g.OW;
-  const long b = blockIdx.x;
-  const int part = blockIdx.y, parts = gridDim.y;            // several blocks share a sample: more CTAs than SMs
-  const uint4* src = reinterpret_cast<const uint4*>(in + b * g.in_bstride);
-  for (int i = threadIdx.x; i < chw / 16; i += blockDim.x) reinterpret_cast<uint4*>(img)[i] = src[i];
-  __syncthreads();
-  auto px = [&](int c, int ih, int iw) -> uint32_t {
-    if (ih < 0 || ih >= g.H || iw < 0 || iw >= g.W) return 0u;
-    return __float_as_uint((float)img[(c * g.H + ih) * g.W + iw]) >> 16;     // exact bf16 bits of 0..255
-  };
-  // Fast path (the Atari first layer: 8-wide rows, stride 4, pad 1, nothing hangs over the right / bottom edge): a
-  // kernel row is bytes 4*ow-1 .. 4*ow+6 of an image row = byte 3 of word ow-1, word ow, bytes 0..2 of word ow+1.
-  const bool fast = g.KW == 8 && g.stride == 4 && g.pad == 1 && (g.W & 3) == 0 && (g.OW - 1) * 4 + 6 < g.W &&
-                    (g.OH - 1) * 4 - 1 + g.KH - 1 < g.H;
-  auto cvt2 = [](uint32_t w, uint32_t sa, uint32_t sb) -> uint32_t {      // two bytes of w -> two bf16 (exact)
-    const float fa = __uint_as_float(__byte_perm(w, 0x4B000000u, sa)) - 8388608.0f;
-    const float fb = __uint_as_float(__byte_perm(w, 0x4B000000u, sb)) - 8388608.0f;
-    return __byte_perm(__float_as_uint(fa), __float_as_uint(fb), 0x7632);
-  };
-  if (col && fast) {
-    const uint32_t* img32 = reinterpret_cast<const uint32_t*>(img);
-    const int wpr = g.W >> 2;                                   // words per image row
-    for (int item = part * blockDim.x + threadIdx.x; item < ohw * K8; item += parts * blockDim.x) {
-      const int m = item / K8, kr = item - m * K8;              // kr = c * KH + kh
-      const int oh = m / g.OW, ow = m - oh * g.OW;
-      const int c = kr / g.KH, kh = kr - c * g.KH;
-      const int ih = oh * 4 - 1 + kh;
-      uint4 o = make_uint4(0u, 0u, 0u, 0u);
-      if (ih >= 0) {
-        const uint32_t* rowp = img32 + (c * g.H + ih) * wpr + ow;
-        const uint32_t w0 = ow > 0 ? rowp[-1] : 0u, w1 = rowp[0], w2 = rowp[1];
-        const uint32_t a = __byte_perm(w0, w1, 0x0043);          // bytes: w0.3, w1.0   (upper two unused)
-        o.x = cvt2(a, 0x7650, 0x7651);
-        o.y = cvt2(w1, 0x7651, 0x7652);
-        o.z = cvt2(__byte_perm(w1, w2, 0x0043), 0x7650, 0x7651);
-        o.w = cvt2(w2, 0x7651, 0x7652);
-      }
-      *reinterpret_cast<uint4*>(col + (b * ohw + m) * K + kr * 8) = o;
-    }
-  } else if (col) {
-    for (int item = part * blockDim.x + threadIdx.x; item < ohw * K8; item += parts * blockDim.x) {
-      const int m = item / K8, k0 = (item - m * K8) * 8;
-      const int oh = m / g.OW, ow = m - oh * g.OW;
-      int kw = k0 % g.KW, kh = (k0 / g.KW) % g.KH, c = k0 / (g.KW * g.KH);
-      const int ih0 = oh * g.stride - g.pad, iw0 = ow * g.stride - g.pad;
-      uint32_t e[8];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        e[t] = px(c, ih0 + kh, iw0 + kw);
-        if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++c; } }
-      }
-      *reinterpret_cast<uint4*>(col + (b * ohw + m) * K + k0) =
-          make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16));
-    }
-  }
-  if (colT) {
-    const long M = (long)g.B * ohw;
-    const int M8 = ohw / 8;
-    for (int item = part * blockDim.x + threadIdx.x; item < K * M8; item += parts * blockDim.x) {
-      const int k = item / M8, m0 = (item - k * M8) * 8;
-      const int kw = k % g.KW, kh = (k / g.KW) % g.KH, c = k / (g.KW * g.KH);
-      int oh = m0 / g.OW, ow = m0 - oh * g.OW;
-      uint32_t e[8];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        e[t] = px(c, oh * g.stride + kh - g.pad, ow * g.stride + kw - g.pad);
-        if (++ow == g.OW) { ow = 0; ++oh; }
-      }
-      *reinterpret_cast<uint4*>(colT + (long)k * M + b * ohw + m0) =
-          make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16));
-    }
-  }
-}
-
 // fp32 NCHW input, staged: one block per sample converts its input ONCE into packed (hi | lo << 16) words in shared
 // memory (coalesced 16-byte loads; the plain kernel converts every pixel KH*KW/stride^2 times), then assembles the
 // (M, K) hi / lo rows from shared memory with 32-bit index arithmetic.  Bit-identical to im2col_bf16_kernel.
@@ -633,31 +553,6 @@ RIQN_API int riqn_conv_fwd_tc(const riqn_conv_geom* g, const void* in, int in_is
                       col_lo ? (const bf16*)w_lo : nullptr, out, g->Cout, TC_BIAS_RELU_NCHW, bias, nullptr, nullptr, 1, s, &ex);
 }
 
-// First layer on raw uint8 pixels: A = pixel values (exact in bf16, no lo image), B = bf16 hi (+lo) of weight/255.
-RIQN_API int riqn_conv_fwd_tc_u8(const riqn_conv_geom* g, const unsigned char* in, const void* ws_hi, const void* ws_lo,
-                                 const float* bias, void* col_px, void* colT_px, float* out, int reuse_col, void* stream) {
-  riqn::note_launches(reuse_col ? 1 : 2);
-  cudaStream_t s = (cudaStream_t)stream;
-  const long M = (long)g->B * g->OH * g->OW;
-  const int K = g->Cin * g->KH * g->KW, chw = g->Cin * g->H * g->W, ohw = g->OH * g->OW;
-  if (K % 8 || chw % 16 || g->in_bstride % 16 || (reinterpret_cast<uintptr_t>(in) & 15) || (colT_px && ohw % 8) || chw > 96 * 1024)
-    return (int)cudaErrorInvalidValue;
-  static PerDeviceOnce attr_once;
-  const int attr_dev = PerDeviceOnce::device();
-  if (!attr_once.done[attr_dev]) {
-    RIQN_CUDA(cudaFuncSetAttribute(im2col_u8_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    attr_once.done[attr_dev] = true;
-  }
-  if (!reuse_col) {      // reuse_col: col_px already holds this input's im2col (another network's pass over it)
-    im2col_u8_staged_kernel<<<dim3(g->B, 4), 256, chw, s>>>(*g, in, (bf16*)col_px, (bf16*)colT_px);
-    RIQN_LAUNCH_CHECK();
-  }
-  TcExtra ex;
-  ex.ohw = ohw;
-  return gemm_bf16_tc((int)M, g->Cout, K, (const bf16*)col_px, nullptr, (const bf16*)ws_hi, (const bf16*)ws_lo, out, g->Cout,
-                      TC_BIAS_RELU_NCHW, bias, nullptr, nullptr, 1, s, &ex);
-}
-
 // dY on the strip grid: row m' = (b, gy, gx) of dYg (B*G*G, Cout) bf16 holds dout * (out > 0) for real outputs
 // (gy < OH, gx < OW) and zeros elsewhere; dbias accumulated.  One block = 64 grid rows x all channels (Cout <= 64).
 __global__ void __launch_bounds__(256) conv_dy_grid_kernel(int B, int Cout, int OH, int OW, int G,
@@ -860,30 +755,6 @@ RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, con
   return 0;
 }
 
-// bf16 transposed im2col (K, M) alone -- the wgrad operand of riqn_conv_bwd_tc when the forward ran as a strip
-// convolution.  in_is_u8: raw pixel VALUES are written (pass wgrad_scale = 1/255 to riqn_conv_bwd_tc).
-RIQN_API int riqn_im2col_bf16_t(const riqn_conv_geom* g, const void* in, int in_is_u8, void* colT_hi, void* stream) {
-  riqn::note_launches(1);
-  cudaStream_t s = (cudaStream_t)stream;
-  const long M = (long)g->B * g->OH * g->OW;
-  const int K = g->Cin * g->KH * g->KW, chw = g->Cin * g->H * g->W, ohw = g->OH * g->OW;
-  if (K % 8 || M % 8) return (int)cudaErrorInvalidValue;
-  if (in_is_u8) {
-    if (chw % 16 || g->in_bstride % 16 || (reinterpret_cast<uintptr_t>(in) & 15) || ohw % 8 || chw > 96 * 1024)
-      return (int)cudaErrorInvalidValue;
-    static PerDeviceOnce attr_once;
-    const int attr_dev = PerDeviceOnce::device();
-    if (!attr_once.done[attr_dev]) {
-      RIQN_CUDA(cudaFuncSetAttribute(im2col_u8_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-      attr_once.done[attr_dev] = true;
-    }
-    im2col_u8_staged_kernel<<<dim3(g->B, 4), 256, chw, s>>>(*g, (const unsigned char*)in, nullptr, (bf16*)colT_hi);
-  } else {
-    im2col_bf16_t_kernel<float><<<grid_for(M * K / 8), 256, 0, s>>>(*g, (const float*)in, (bf16*)colT_hi);
-  }
-  return (int)cudaGetLastError();
-}
-
 RIQN_API int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const float* out, const void* colT_hi,
                               const void* wT_hi, void* dY_hi, void* dYT_hi, float* dcol, float* dw, float* dbias, float* din,
                               float wgrad_scale, void* stream) {
@@ -907,11 +778,11 @@ RIQN_API int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const 
   }
   RIQN_LAUNCH_CHECK();
   if (int rc_ = sum_slots_add(slots, g->Cout, dbias_part.p, dbias, s)) return rc_;
-  // dW[c, k] += sum_m dY[m, c] * col[m, k]      (K' = M is long: split it over every SM)
+  // dW[c, k] += wgrad_scale * sum_m dY[m, c] * col[m, k]      (K' = M is long: split it over every SM)
   const int n_tiles = (K + 127) / 128;
   int split = (riqn_sms() + n_tiles - 1) / n_tiles;
   TcExtra ex;
-  ex.alpha = wgrad_scale;          // 1/255 when colT holds raw pixel values
+  ex.alpha = wgrad_scale;
   int rc = gemm_bf16_tc(g->Cout, K, (int)M, (const bf16*)dYT_hi, nullptr, (const bf16*)colT_hi, nullptr, dw, K, TC_ATOMIC,
                         nullptr, nullptr, nullptr, split, s, &ex);
   if (rc) return rc;

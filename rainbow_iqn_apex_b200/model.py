@@ -42,7 +42,6 @@ _ALIGN = 64  # floats; arena groups start on 256-byte boundaries
 #   "fp32"  : CUDA-core fp32 GEMM (gemm_simt.cu), the cross-check path
 PRECISION = {"fwd": os.environ.get("RIQN_FWD_PRECISION", "fp16"), "bwd": os.environ.get("RIQN_BWD_PRECISION", "bf16")}
 WGRAD_SPLIT_K = int(os.environ.get("RIQN_WGRAD_SPLIT_K", "4"))
-_NO_STRIP = os.environ.get("RIQN_NO_STRIP_CONV", "0") == "1"      # fall back to the explicit-im2col forward
 
 
 def set_precision(fwd=None, bwd=None):
@@ -198,6 +197,13 @@ def _strip_perm(cin, k, stride, first):
 def _geom(batch, cin, h, cout, k, stride, pad, in_bstride=None):
     oh = (h + 2 * pad - k) // stride + 1
     return ConvGeom(batch, cin, h, h, cout, k, k, stride, pad, oh, oh, in_bstride if in_bstride else cin * h * h)
+
+
+def _strip_block(g):
+    """Block matrix of a strip convolution with geometry ``g`` (riqn_conv_fwd_strip): the padded input cut into
+    stride x stride blocks on a G x G grid, G = OH + k/stride - 1 (21, 10, 9 for conv1-3), each block a row of
+    stride^2 * Cin values.  Returns (G, row width)."""
+    return g.OH + g.KH // g.stride - 1, g.stride * g.stride * g.Cin
 
 
 class DQN(nn.Module):
@@ -450,8 +456,6 @@ class DQN(nn.Module):
             for name, conv in (("conv1", self.conv1), ("conv2", self.conv2), ("conv3", self.conv3)):
                 co, k = conv.weight.shape[0], conv.weight[0].numel()
                 self._conv_ops[name] = (mk(co, k), mk(co, k), mk(k, co))
-            k1 = self.conv1.weight[0].numel()
-            self._conv1_px_ops = (mk(32, k1), mk(32, k1))      # bf16 hi / lo of conv1.weight / 255 (uint8 ingest)
             if not self.rainbow_only:
                 self._iqn_ops = (mk(FEAT, self.quantile_embedding_dim), mk(FEAT, self.quantile_embedding_dim))
 
@@ -491,7 +495,6 @@ class DQN(nn.Module):
                 specs.append((conv.weight, None, 1.0, hi, lo, hiT))                       # original k order (+ transpose)
                 shi, slo = self._strip_ops[name]
                 specs.append((conv.weight, self._strip_perm32[name], 255.0 if name == "conv1" else 1.0, shi, slo, None))
-            specs.append((self.conv1.weight, None, 255.0, self._conv1_px_ops[0], self._conv1_px_ops[1], None))
             if not self.rainbow_only:
                 specs.append((self.iqn_fc.weight, None, 1.0, self._iqn_ops[0], self._iqn_ops[1], None))
             arr = (SplitJob * len(specs))()
@@ -536,7 +539,9 @@ class DQN(nn.Module):
     # ------------------------------------------------------------------ forward pieces
     def trunk(self, x, keep=None, col_cache=None):
         """conv1-3 + ReLU -> (B, 3136).  x: (B, history, 84, 84) uint8 (scaled by 1/255 on the fly) or
-        fp32; may be a view with a larger batch stride (the replay window).  model.py:115-118"""
+        fp32; may be a view with a larger batch stride (the replay window).  model.py:115-118.  Three paths: the strip
+        convolution (_strip_trunk) where _strip_ok allows it, else the explicit im2col on the tensor cores, or the fp32
+        CUDA-core convolution in the fp32 forward mode.  ``col_cache``: see _strip_trunk."""
         _lib.require_device()
         B = x.shape[0]
         if x.dtype not in (torch.uint8, torch.float32):
@@ -545,94 +550,97 @@ class DQN(nn.Module):
             x = x.contiguous()
         is_u8 = 1 if x.dtype == torch.uint8 else 0
         dev = x.device
-        g1 = _geom(B, self.history, 84, 32, 8, 4, 1, in_bstride=x.stride(0))
-        g2 = _geom(B, 32, 20, 64, 4, 2, 0)
-        g3 = _geom(B, 64, 9, 64, 3, 1, 0)
-        geoms, convs = (g1, g2, g3), (self.conv1, self.conv2, self.conv3)
+        geoms, convs = self._trunk_geoms(B, x.stride(0)), (self.conv1, self.conv2, self.conv3)
         outs = (torch.empty(B, 32, 20, 20, device=dev), torch.empty(B, 64, 9, 9, device=dev),
                 torch.empty(B, 64, 7, 7, device=dev))
         ins = (x, outs[0], outs[1])
         fwd = PRECISION["fwd"]
         # the backward runs on the tensor cores when it is bf16 and every im2col row count is a multiple of 8
         bwd_tc = keep is not None and PRECISION["bwd"] == "bf16" and fwd != "fp32" and all((g.B * g.OH * g.OW) % 8 == 0 for g in geoms)
-        need_col32 = keep is not None and not bwd_tc
         cols, colTs = [None] * 3, [None] * 3
-        px_scale = 1.0
-        strip = (fwd != "fp32" and is_u8 and x.stride(0) % 16 == 0 and x.data_ptr() % 16 == 0 and self.history * 16 == 64
-                 and not _NO_STRIP)
-        if strip:
-            # strip convolution (riqn_conv_fwd_strip): no im2col matrices in the forward; each layer's epilogue writes
-            # the next layer's block matrix.  Block grids: G = OH + k/stride - 1 = 21, 10, 9.
+        strip_bwd = None
+        if self._strip_ok(x):
+            # the fp32 activations of conv1 / conv2 are only read by the backward (ReLU masks): no-grad passes skip them
+            _, blocks = self._strip_trunk(x, outs if keep is not None else (None, None, outs[2]), col_cache=col_cache)
+            if bwd_tc:
+                strip_bwd = blocks                   # the strip backward reads the forward's block matrices
+        elif fwd == "fp32":
+            for i, (g, conv, inp, out) in enumerate(zip(geoms, convs, ins, outs)):
+                cols[i] = torch.empty(g.B * g.OH * g.OW, g.Cin * g.KH * g.KW, device=dev)
+                call("riqn_conv_fwd", g, ptr(inp), is_u8 if i == 0 else 0, ptr(conv.weight), ptr(conv.bias), ptr(cols[i]),
+                     ptr(out))
+        else:
             x3 = _small_x3()
-            bf = lambda *sh: torch.empty(*sh, dtype=torch.bfloat16, device=dev)
-            ckey = ("s2d", x.data_ptr(), tuple(x.shape), tuple(x.stride()))
-            if col_cache is not None and ckey in col_cache:
-                a1 = col_cache[ckey]                 # the pixel block matrix does not depend on the network's weights
-            else:
-                a1 = bf(B * 21 * 21, 16 * self.history)
-                call("riqn_s2d_u8", g1, ptr(x), ptr(a1))
-                if col_cache is not None:
-                    col_cache[ckey] = a1
-            a2_hi, a2_lo = bf(B * 100, 128), (bf(B * 100, 128) if x3 else None)
-            a3_hi, a3_lo = bf(B * 81, 64), (bf(B * 81, 64) if x3 else None)
-            ops = self._strip_ops
-            # the fp32 NCHW activations of conv1 / conv2 are only read by the backward (ReLU masks): no-grad passes skip them
-            o1, o2 = (ptr(outs[0]), ptr(outs[1])) if keep is not None else (None, None)
-            call("riqn_conv_fwd_strip", g1, ptr(a1), None, ptr(ops["conv1"][0]), ptr(ops["conv1"][1]) if x3 else None,
-                 ptr(self.conv1.bias), o1, ptr(a2_hi), ptr(a2_lo), 2, 10, None, None, None, 0)
-            call("riqn_conv_fwd_strip", g2, ptr(a2_hi), ptr(a2_lo), ptr(ops["conv2"][0]), ptr(ops["conv2"][1]) if x3 else None,
-                 ptr(self.conv2.bias), o2, ptr(a3_hi), ptr(a3_lo), 1, 9, None, None, None, 0)
-            call("riqn_conv_fwd_strip", g3, ptr(a3_hi), ptr(a3_lo), ptr(ops["conv3"][0]), ptr(ops["conv3"][1]) if x3 else None,
-                 ptr(self.conv3.bias), ptr(outs[2]), None, None, 0, 0, None, None, None, 0)
-            if keep is not None:                     # operands of the backward products
-                strip_bwd = None
-                if bwd_tc:                           # the strip backward reads the forward's block matrices
-                    strip_bwd = (a1, a2_hi, a3_hi)
-                    px_scale = 1.0 / 255.0
-                else:
-                    for i, (g, inp) in enumerate(zip(geoms, ins)):
-                        M, K = g.B * g.OH * g.OW, g.Cin * g.KH * g.KW
-                        cols[i] = torch.empty(M, K, device=dev)
-                        call("riqn_im2col_f32", g, ptr(inp), 1 if i == 0 else 0, ptr(cols[i]))
-                keep.update(x=x, g=geoms, col=tuple(cols), colT=tuple(colTs), out=outs, bwd_tc=bwd_tc, px_scale=px_scale,
-                            strip_bwd=strip_bwd)
-            return outs[2].view(B, FEAT)
-        for i, (g, conv, inp, out) in enumerate(zip(geoms, convs, ins, outs)):
-            M, K = g.B * g.OH * g.OW, g.Cin * g.KH * g.KW
-            u8 = is_u8 if i == 0 else 0
-            if fwd == "fp32":
-                cols[i] = torch.empty(M, K, device=dev)
-                call("riqn_conv_fwd", g, ptr(inp), u8, ptr(conv.weight), ptr(conv.bias), ptr(cols[i]), ptr(out))
-            elif i == 0 and u8 and x.stride(0) % 16 == 0 and x.data_ptr() % 16 == 0:
-                # raw-pixel path: pixel values are exact in bf16, /255 folded into the weights
-                ws_hi, ws_lo = self._conv1_px_ops
-                ckey = (x.data_ptr(), tuple(x.shape), tuple(x.stride()))
-                reuse = col_cache is not None and ckey in col_cache and not bwd_tc
-                col_px = col_cache[ckey] if reuse else torch.empty(M, K, dtype=torch.bfloat16, device=dev)
-                if col_cache is not None:
-                    col_cache[ckey] = col_px          # the pixel im2col does not depend on the network's weights
-                if bwd_tc:
-                    colTs[i] = torch.empty(K, M, dtype=torch.bfloat16, device=dev)
-                    px_scale = 1.0 / 255.0
-                call("riqn_conv_fwd_tc_u8", g, ptr(inp), ptr(ws_hi), ptr(ws_lo) if _small_x3() else None, ptr(conv.bias),
-                     ptr(col_px), ptr(colTs[i]), ptr(out), 1 if reuse else 0)
-                if need_col32:
-                    cols[i] = torch.empty(M, K, device=dev)
-                    call("riqn_im2col_f32", g, ptr(inp), u8, ptr(cols[i]))
-            else:
+            for i, (g, conv, inp, out) in enumerate(zip(geoms, convs, ins, outs)):
+                M, K = g.B * g.OH * g.OW, g.Cin * g.KH * g.KW
                 w_hi, w_lo, _ = self._conv_ops["conv%d" % (i + 1)]
                 col_hi = torch.empty(M, K, dtype=torch.bfloat16, device=dev)
-                col_lo = torch.empty(M, K, dtype=torch.bfloat16, device=dev) if _small_x3() else None
+                col_lo = torch.empty(M, K, dtype=torch.bfloat16, device=dev) if x3 else None
                 if bwd_tc:
                     colTs[i] = torch.empty(K, M, dtype=torch.bfloat16, device=dev)
-                call("riqn_conv_fwd_tc", g, ptr(inp), u8, ptr(w_hi), ptr(w_lo), ptr(conv.bias), ptr(col_hi), ptr(col_lo),
-                     ptr(colTs[i]), ptr(out))
-                if need_col32:
-                    cols[i] = torch.empty(M, K, device=dev)
-                    call("riqn_im2col_f32", g, ptr(inp), u8, ptr(cols[i]))
+                call("riqn_conv_fwd_tc", g, ptr(inp), is_u8 if i == 0 else 0, ptr(w_hi), ptr(w_lo), ptr(conv.bias),
+                     ptr(col_hi), ptr(col_lo), ptr(colTs[i]), ptr(out))
         if keep is not None:
-            keep.update(x=x, g=geoms, col=tuple(cols), colT=tuple(colTs), out=outs, bwd_tc=bwd_tc, px_scale=px_scale)
+            if not bwd_tc and fwd != "fp32":         # operands of the fp32 backward (riqn_conv_fwd wrote its own)
+                for i, (g, inp) in enumerate(zip(geoms, ins)):
+                    cols[i] = torch.empty(g.B * g.OH * g.OW, g.Cin * g.KH * g.KW, device=dev)
+                    call("riqn_im2col_f32", g, ptr(inp), is_u8 if i == 0 else 0, ptr(cols[i]))
+            keep.update(x=x, g=geoms, col=tuple(cols), colT=tuple(colTs), out=outs, bwd_tc=bwd_tc, strip_bwd=strip_bwd)
         return outs[2].view(B, FEAT)
+
+    def _trunk_geoms(self, B, in_bstride=None):
+        """Geometries of conv1-3 (model.py:65-67) over B samples; ``in_bstride``: batch stride of the frames."""
+        return (_geom(B, self.history, 84, 32, 8, 4, 1, in_bstride), _geom(B, 32, 20, 64, 4, 2, 0),
+                _geom(B, 64, 9, 64, 3, 1, 0))
+
+    def _strip_ok(self, x):
+        """Whether the trunk over the frames ``x`` runs as strip convolutions: a tensor-core forward, uint8 frames in the
+        (84*84, 84, 1) layout with 16-byte aligned samples (riqn_s2d_u8), and history 4 (conv1's block width
+        16 * history must be a multiple of 64)."""
+        return (PRECISION["fwd"] != "fp32" and x.dtype == torch.uint8 and x.stride()[1:] == (84 * 84, 84, 1)
+                and x.stride(0) % 16 == 0 and x.data_ptr() % 16 == 0 and self.history == 4)
+
+    def _strip_trunk(self, x, outs=None, other=None, col_cache=None):
+        """conv1-3 + ReLU over the uint8 frames ``x`` (see _strip_ok) with no im2col matrix: riqn_s2d_u8 writes conv1's
+        block matrix of raw pixel values, then three riqn_conv_fwd_strip launches each write the next layer's block
+        matrix from their epilogue.  ``outs``: the fp32 (B, C, OH, OW) outputs of conv1-3, conv1's and conv2's may be None;
+        by default only the features are written, to a new tensor.  ``other``: a second network over the same frames in the
+        same launches, as one stacked batch (samples [0, B) with self's weights, [B, 2B) with other's, both reading one pixel
+        block matrix); ``outs`` then hold 2B samples.  ``col_cache``: a dict that shares the pixel block matrix, which does
+        not depend on the weights, between passes over the same frames.  Returns the features (B or 2B, 3136) and the block
+        matrices the three layers read, the operands of riqn_conv_bwd_strip."""
+        B, dev, x3 = x.shape[0], x.device, _small_x3()
+        bf = lambda rows, cols: torch.empty(rows, cols, dtype=torch.bfloat16, device=dev)
+        key = (x.data_ptr(), tuple(x.shape), tuple(x.stride()))
+        a1 = col_cache.get(key) if col_cache is not None else None
+        if a1 is None:
+            g1 = self._trunk_geoms(B, x.stride(0))[0]
+            G, width = _strip_block(g1)
+            a1 = bf(B * G * G, width)
+            call("riqn_s2d_u8", g1, ptr(x), ptr(a1))
+            if col_cache is not None:
+                col_cache[key] = a1
+
+        def weights(net, name):                  # strip-ordered bf16 hi / lo images and bias of one layer
+            hi, lo = net._strip_ops[name]
+            return ptr(hi), ptr(lo) if x3 else None, ptr(getattr(net, name).bias)
+
+        geoms = self._trunk_geoms(B if other is None else 2 * B)
+        # (hi, lo) block matrix that each layer reads and (stride, grid) of its layout; conv3 writes none
+        blocks, layouts = [(a1, None)], []
+        for g in geoms[1:]:
+            G, width = _strip_block(g)
+            blocks.append((bf(g.B * G * G, width), bf(g.B * G * G, width) if x3 else None))
+            layouts.append((g.stride, G))
+        blocks.append((None, None))
+        layouts.append((0, 0))
+        if outs is None:
+            outs = (None, None, torch.empty(geoms[2].B, FEAT, device=dev))
+        for i, (name, g, out) in enumerate(zip(("conv1", "conv2", "conv3"), geoms, outs)):
+            w2 = weights(other, name) if other is not None else (None, None, None)
+            call("riqn_conv_fwd_strip", g, ptr(blocks[i][0]), ptr(blocks[i][1]), *weights(self, name), ptr(out),
+                 ptr(blocks[i + 1][0]), ptr(blocks[i + 1][1]), *layouts[i], *w2, 1 if other is not None and i == 0 else 0)
+        return outs[2].view(-1, FEAT), tuple(hi for hi, _ in blocks[:3])
 
     def trunk_pair(self, other, x):
         """conv1-3 of TWO networks (self = online, other = target) over the same uint8 frames in three launches instead of
@@ -640,30 +648,12 @@ class DQN(nn.Module):
         self's weights, [B, 2B) with other's -- the pixel block matrix is shared by both halves.  Returns (feat_self,
         feat_other), each (B, 3136); None when the fast path does not apply (the caller then runs the trunks one by one)."""
         B = x.shape[0]
-        if (PRECISION["fwd"] == "fp32" or _NO_STRIP or x.dtype != torch.uint8 or x.stride()[1:] != (84 * 84, 84, 1)
-                or x.stride(0) % 16 or x.data_ptr() % 16 or self.history != 4 or other.history != 4 or B % 128):
+        if B % 128 or not (self._strip_ok(x) and other._strip_ok(x)):     # each network's rows fill whole 128-row tiles
             return None
         for net in (self, other):                      # operand images of the noise-free weights (rebuilt only when dirty)
             if getattr(net, "_strip_ops", None) is None or getattr(net, "_static_ops_dirty", True):
                 net._refresh_tc_operands(h_done=True)
-        dev = x.device
-        x3 = _small_x3()
-        bf = lambda *sh: torch.empty(*sh, dtype=torch.bfloat16, device=dev)
-        g1 = _geom(B, self.history, 84, 32, 8, 4, 1, in_bstride=x.stride(0))
-        a1 = bf(B * 21 * 21, 16 * self.history)
-        call("riqn_s2d_u8", g1, ptr(x), ptr(a1))
-        g1p, g2p, g3p = _geom(2 * B, self.history, 84, 32, 8, 4, 1), _geom(2 * B, 32, 20, 64, 4, 2, 0), _geom(2 * B, 64, 9, 64, 3, 1, 0)
-        a2_hi, a2_lo = bf(2 * B * 100, 128), (bf(2 * B * 100, 128) if x3 else None)
-        a3_hi, a3_lo = bf(2 * B * 81, 64), (bf(2 * B * 81, 64) if x3 else None)
-        feat = torch.empty(2 * B, FEAT, device=dev)
-        so, oo = self._strip_ops, other._strip_ops
-        lo = lambda t: ptr(t) if x3 else None
-        call("riqn_conv_fwd_strip", g1p, ptr(a1), None, ptr(so["conv1"][0]), lo(so["conv1"][1]), ptr(self.conv1.bias), None,
-             ptr(a2_hi), ptr(a2_lo), 2, 10, ptr(oo["conv1"][0]), lo(oo["conv1"][1]), ptr(other.conv1.bias), 1)
-        call("riqn_conv_fwd_strip", g2p, ptr(a2_hi), ptr(a2_lo), ptr(so["conv2"][0]), lo(so["conv2"][1]), ptr(self.conv2.bias), None,
-             ptr(a3_hi), ptr(a3_lo), 1, 9, ptr(oo["conv2"][0]), lo(oo["conv2"][1]), ptr(other.conv2.bias), 0)
-        call("riqn_conv_fwd_strip", g3p, ptr(a3_hi), ptr(a3_lo), ptr(so["conv3"][0]), lo(so["conv3"][1]), ptr(self.conv3.bias),
-             ptr(feat), None, None, 0, 0, ptr(oo["conv3"][0]), lo(oo["conv3"][1]), ptr(other.conv3.bias), 0)
+        feat, _ = self._strip_trunk(x, other=other)
         return feat[:B], feat[B:]
 
     def iqn_head(self, feat, num_quantiles, tau, keep=None):
@@ -899,19 +889,20 @@ class DQN(nn.Module):
             if keep["bwd_tc"] and keep.get("strip_bwd") is not None:
                 name = "conv%d" % (i + 1)
                 w_hi = self._conv_ops[name][0]                 # (Cout, K) in the original k order
-                G = g.OH + g.KH // g.stride - 1
+                G, _ = _strip_block(g)
                 dYg = torch.empty(g.B * G * G, g.Cout, dtype=torch.bfloat16, device=dev)
                 dwp = torch.empty(g.Cout, K, device=dev)
+                # conv1's block matrix holds raw pixel values: the weight gradient takes the reference's 1/255 here
                 call("riqn_conv_bwd_strip", g, ptr(douts[i]), ptr(out), ptr(keep["strip_bwd"][i]), ptr(w_hi),
                      ptr(self._strip_perm32[name]), ptr(dYg), ptr(dwp), ptr(gv(conv.weight)), ptr(gv(conv.bias)), ptr(din),
-                     keep["px_scale"] if i == 0 else 1.0)
+                     1.0 / 255.0 if i == 0 else 1.0)
             elif keep["bwd_tc"]:
                 _, _, wT_hi = self._conv_ops["conv%d" % (i + 1)]
                 dY = torch.empty(M, g.Cout, dtype=torch.bfloat16, device=dev) if i > 0 else None
                 dYT = torch.empty(g.Cout, M, dtype=torch.bfloat16, device=dev)
                 dcol = torch.empty(M, K, device=dev) if i > 0 else None
                 call("riqn_conv_bwd_tc", g, ptr(douts[i]), ptr(out), ptr(keep["colT"][i]), ptr(wT_hi), ptr(dY), ptr(dYT),
-                     ptr(dcol), ptr(gv(conv.weight)), ptr(gv(conv.bias)), ptr(din), keep["px_scale"] if i == 0 else 1.0)
+                     ptr(dcol), ptr(gv(conv.weight)), ptr(gv(conv.bias)), ptr(din), 1.0)
             else:
                 dY = torch.empty(M, g.Cout, device=dev)
                 dcol = torch.empty(M, K, device=dev) if i > 0 else None

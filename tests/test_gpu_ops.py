@@ -57,6 +57,40 @@ def test_trunk_u8_and_f32(cuda_dev, nets):
     assert rel_err(got_view, ref2) < 3e-5
 
 
+def test_trunk_u8_im2col_fallback(cuda_dev):
+    """uint8 frames the strip convolution does not take (history 3: conv1's block width 16*3 is not a multiple of 64) run
+    the explicit im2col on the tensor cores: riqn_conv_fwd_tc forward, riqn_conv_bwd_tc backward."""
+    from rainbow_iqn_apex_b200 import DQN
+    B = 8                        # im2col row counts B*400, B*81, B*49 are multiples of 8: the backward stays on the tensor cores
+    args = make_args(cuda_dev)
+    args.history_length = 3
+    d = DQN(args, 18).to(cuda_dev)
+    params = net.make_params(17, history=3)
+    load_params(d, params)
+    rs = np.random.RandomState(8)
+    frames = rs.randint(0, 256, (B, 3, 84, 84)).astype(np.uint8)
+    x = torch.from_numpy(frames).to(cuda_dev)
+    xf = torch.from_numpy(frames.astype(np.float32) / np.float32(255))      # correctly rounded x / 255, as the kernels do
+    p = net.to_torch(params, requires_grad=True)
+    ref = net.conv_trunk(p, xf)
+    got = d.trunk(x)
+    assert rel_err(got.cpu().numpy(), ref.detach().numpy()) < 3e-5
+    # the uint8 im2col splits x / 255 into the same bf16 hi / lo operands as the fp32 im2col of x / 255
+    assert torch.equal(got, d.trunk(xf.to(cuda_dev)))
+    keep = {}
+    d.zero_grad()
+    d.trunk(x, keep)
+    assert keep["bwd_tc"] and keep["strip_bwd"] is None
+    dfeat = torch.from_numpy(rs.standard_normal((B, 3136)).astype(np.float32))
+    d.backward_trunk(keep, dfeat.to(cuda_dev))
+    ref.backward(dfeat)
+    for name in ("conv1", "conv2", "conv3"):
+        for part in ("weight", "bias"):
+            g_ref = p[f"{name}.{part}"].grad
+            g = d.grad_view(getattr(getattr(d, name), part)).cpu()
+            assert float((g - g_ref).norm() / g_ref.norm()) < 1e-2, (name, part)   # bf16 backward
+
+
 def test_forward_injected(cuda_dev, nets):
     d, params = nets
     B, Nq = 5, 8
