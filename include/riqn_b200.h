@@ -9,7 +9,8 @@
  * Conventions
  *   - every function returns 0 on success or a cudaError_t value; all buffers are caller-owned DEVICE pointers
  *     unless stated; work is enqueued on `stream` (a cudaStream_t passed as void*) and is stream-ordered,
- *     re-entrant per stream.  The only memory a call takes itself is temporary scratch for partial sums, allocated
+ *     re-entrant per stream.  The only memory a call takes itself is temporary scratch for partial sums (and the
+ *     strip-ordered weight copy of riqn_conv_bwd_strip), allocated
  *     from the device's stream-ordered pool on `stream` and released on `stream` before the call returns
  *     (cudaMallocAsync / cudaFreeAsync): no host synchronisation, no state shared between calls or streams, and
  *     inside a CUDA graph capture it becomes part of the graph;
@@ -113,10 +114,11 @@ int riqn_conv_fwd_strip(const riqn_conv_geom* g, const void* a_hi, const void* a
  * next-layer images are the stacked (B, ...) tensors.  share_a != 0: the A image holds B/2 samples read by both halves (first
  * layer: the pixel block matrix).  Needs (B/2)*G*G % 128 == 0. */
 /* Backward of a strip convolution on the tensor cores, again without im2col matrices: a_hi is the block matrix the
- * forward read (riqn_s2d_u8 / the previous layer's next_hi); w_hi (Cout, K) bf16 weight in the ORIGINAL k order (data
- * gradient, read as an MN-major operand); perm (K ints): strip k order -> original k; dYg (B*G*G, Cout) bf16 and dwp_scratch (Cout*K floats)
- * workspaces; dw / dbias accumulated; din (may be NULL; pad == 0 only) overwritten.  wgrad_scale = 1/255 when a_hi
- * holds raw pixel values. */
+ * forward read (riqn_s2d_u8 / the previous layer's next_hi); w_hi (Cout, K) bf16 weight in the ORIGINAL k order (the
+ * data gradient reads a strip-ordered copy the call makes in its scratch); perm (K ints): strip k order -> original k;
+ * dYg (B*G*G, Cout) bf16 and dwp_scratch (Cout*K floats) workspaces; dw / dbias accumulated; din (may be NULL; pad == 0
+ * and H == W == G*stride only) overwritten, every element once, as the transposed strip convolution of dYg.
+ * wgrad_scale = 1/255 when a_hi holds raw pixel values. */
 int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, const float* out, const void* a_hi, const void* w_hi,
                         const int* perm, void* dYg, float* dwp_scratch, float* dw, float* dbias, float* din,
                         float wgrad_scale, void* stream);

@@ -619,13 +619,16 @@ __global__ void __launch_bounds__(256) conv_dy_grid_kernel(int B, int Cout, int 
   if (threadIdx.x < Cout) dbias_part[(long)blockIdx.x * Cout + threadIdx.x] = bsum[threadIdx.x];   // summed in block order
 }
 
-// dw[c, perm[k']] += dwp[c, k']: the strip weight gradient back into the (Cout, Cin*KH*KW) parameter order
+// dw[c, perm[k']] += dwp[c, k']: the strip weight gradient back into the (Cout, Cin*KH*KW) parameter order.  With w_s
+// set, also w_s[c, k'] = w_hi[c, perm[k']]: the weight in strip order, the B operand of the data gradient.
 __global__ void unpermute_add_kernel(int Cout, int K, const float* __restrict__ dwp, const int* __restrict__ perm,
-                                     float* __restrict__ dw) {
+                                     float* __restrict__ dw, const bf16* __restrict__ w_hi, bf16* __restrict__ w_s) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= Cout * K) return;
   const int c = idx / K, kp = idx - c * K;
-  dw[(long)c * K + perm[kp]] += dwp[idx];
+  const long o = (long)c * K + perm[kp];
+  dw[o] += dwp[idx];
+  if (w_s) w_s[idx] = w_hi[o];
 }
 
 static int strip_params(const riqn_conv_geom* g, int* t, int* G, int* kc) {
@@ -682,41 +685,20 @@ RIQN_API int riqn_conv_fwd_strip(const riqn_conv_geom* g, const void* a_hi, cons
 //   dYg (B*G*G, Cout) = dout * (out > 0) on the strip grid;   dbias += column sums
 //   dW'[c, (shift, within)] = sum_m' dYg[m', c] * a_hi[m' + shift offset, within]   (MN-major operands, shifted rows)
 //   dw[c, perm[k']] += wgrad_scale * dW'[c, k']
-//   din += col2im(dYg * W)   (W (Cout, K) as MN-major operand; fused epilogue, pad == 0 only; din may be NULL)
-// din[b, c, ih, iw] = sum over (kh, kw) of dcol[(b, oh, ow) on the G x G strip grid, (c, kh, kw)] with
-// ih = oh * stride + kh, iw = ow * stride + kw (pad == 0), kh and kw ascending.  Threads run channel-fastest, so a warp
-// reads neighbouring columns of the same dcol rows.
-__global__ void col2im_gather_kernel(riqn_conv_geom g, int G, const float* __restrict__ dcol, float* __restrict__ din) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long n = (long)g.B * g.Cin * g.H * g.W;
-  if (i >= n) return;
-  const int c = (int)(i % g.Cin), iw = (int)((i / g.Cin) % g.W), ih = (int)((i / ((long)g.Cin * g.W)) % g.H);
-  const long b = i / ((long)g.Cin * g.W * g.H);
-  const int K = g.Cin * g.KH * g.KW;
-  float acc = 0.f;
-  for (int kh = 0; kh < g.KH; ++kh) {
-    const int oy = ih - kh;
-    if (oy < 0 || oy % g.stride) continue;
-    const int oh = oy / g.stride;
-    if (oh >= g.OH) continue;
-    for (int kw = 0; kw < g.KW; ++kw) {
-      const int ox = iw - kw;
-      if (ox < 0 || ox % g.stride) continue;
-      const int ow = ox / g.stride;
-      if (ow >= g.OW) continue;
-      acc += dcol[((b * G + oh) * G + ow) * K + (c * g.KH + kh) * g.KW + kw];
-    }
-  }
-  din[((b * g.Cin + c) * g.H + ih) * g.W + iw] = acc;
-}
-
+//   din = the transposed strip convolution of dYg (TC_CONV_DGRAD, pad == 0 only; din may be NULL): input block
+//         (b, gy, gx) adds, over the shifts (dy, dx) in ascending order, the product of dYg row (b, gy - dy, gx - dx)
+//         with that shift's (Cout, stride^2 * Cin) slab of the strip-ordered weight, each product formed in a fresh fp32
+//         accumulator.  Per input pixel that is the sum over (kh, kw), kh then kw ascending, of dY[(b, oh, ow), :] .
+//         W[:, (c, kh, kw)] with ih = oh * stride + kh, iw = ow * stride + kw.
 RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, const float* out, const void* a_hi,
                                  const void* w_hi, const int* perm, void* dYg, float* dwp_scratch, float* dw, float* dbias,
                                  float* din, float wgrad_scale, void* stream) {
-  riqn::note_launches(din ? 6 : 4);
+  riqn::note_launches(din ? 5 : 4);
   cudaStream_t s = (cudaStream_t)stream;
   int t, G, kc;
-  if (strip_params(g, &t, &G, &kc) || g->Cout > 64 || g->Cout % 8 || (din && g->pad != 0)) return (int)cudaErrorInvalidValue;
+  if (strip_params(g, &t, &G, &kc) || g->Cout > 64 || g->Cout % 8 ||
+      (din && (g->pad != 0 || g->H != g->W || G * g->stride != g->H)))
+    return (int)cudaErrorInvalidValue;
   const long Mg = (long)g->B * G * G;
   const int K = g->Cin * g->KH * g->KW;
   const long tiles = (Mg + 63) / 64;
@@ -736,21 +718,18 @@ RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, con
   int rc = gemm_bf16_tc(g->Cout, K, (int)Mg, (const bf16*)dYg, nullptr, (const bf16*)a_hi, nullptr, dwp_scratch, K, TC_ATOMIC,
                         nullptr, nullptr, nullptr, split, s, &ex);
   if (rc) return rc;
-  unpermute_add_kernel<<<(g->Cout * K + 255) / 256, 256, 0, s>>>(g->Cout, K, dwp_scratch, perm, dw);
+  StreamScratch w_s;               // the weight in strip order (Cout, K) bf16, written by the unpermute pass
+  if (din) RIQN_CUDA(w_s.alloc(((size_t)g->Cout * K + 1) / 2, s));
+  unpermute_add_kernel<<<(g->Cout * K + 255) / 256, 256, 0, s>>>(g->Cout, K, dwp_scratch, perm, dw, (const bf16*)w_hi,
+                                                                 (bf16*)w_s.p);
   RIQN_LAUNCH_CHECK();
   if (din) {
-    // dcol = dYg W on the strip grid, then every input pixel gathers its (kh, kw) contributions in a fixed order
-    StreamScratch dcol_buf;
-    RIQN_CUDA(dcol_buf.alloc((size_t)Mg * K, s));
-    float* dcol = dcol_buf.p;
-    TcExtra ci;
-    ci.mn_major = 2;               // B = the (Cout, K) weight itself, read as an MN-major operand (no transposed copy)
-    rc = gemm_bf16_tc((int)Mg, K, g->Cout, (const bf16*)dYg, nullptr, (const bf16*)w_hi, nullptr, dcol, K, TC_STORE, nullptr,
-                      nullptr, nullptr, 1, s, &ci);
+    TcExtra dg;
+    dg.strip_t = t; dg.strip_G = G;
+    dg.ci_cin = g->Cin; dg.ci_h = g->H; dg.ci_w = g->W; dg.ci_stride = g->stride;
+    rc = gemm_bf16_tc((int)Mg, kc * 64, g->Cout, (const bf16*)dYg, nullptr, (const bf16*)w_s.p, nullptr, din, 0,
+                      TC_CONV_DGRAD, nullptr, nullptr, nullptr, 1, s, &dg);
     if (rc) return rc;
-    const long n_in = (long)g->B * g->Cin * g->H * g->W;
-    col2im_gather_kernel<<<riqn_cdiv(n_in, 256), 256, 0, s>>>(*g, G, dcol, din);
-    RIQN_LAUNCH_CHECK();
   }
   return 0;
 }

@@ -34,7 +34,7 @@ int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const floa
 
 // ---- wgmma / TMA path (gemm_tc.cu) ---------------------------------------------------------------------------
 enum TcEpi { TC_STORE = 0, TC_BIAS_RELU = 1, TC_ATOMIC = 2, TC_NOISY_WGRAD = 3, TC_BIAS_RELU_NCHW = 4, TC_EMBED = 5,
-             TC_COL2IM = 6, TC_CONV = 7 };
+             TC_COL2IM = 6, TC_CONV = 7, TC_CONV_DGRAD = 8 };
 
 struct TcExtra {
   int ohw = 1;
@@ -51,6 +51,14 @@ struct TcExtra {
   // (may be null) receive the bf16 images in the NEXT layer's space-to-depth layout (block edge nx_s, grid nx_G).
   int strip_t = 0, strip_G = 0, strip_kc = 0, cv_oh = 0, cv_ow = 0, nx_s = 0, nx_G = 0;
   __nv_bfloat16 *nx_hi = nullptr, *nx_lo = nullptr;
+  // Data gradient of a strip convolution (TC_CONV_DGRAD), the same block grid read the other way: row m = (b, gy, gx) is
+  // one input block, column n = (iy, ix, c) one of its N = stride^2 * Cin values.  A = dYg (M, K = Cout <= 64) and
+  // k-block (dy, dx) (kb = dy*strip_t + dx, strip_t^2 of them) reads its rows m0 - (dy*strip_G + dx): the outputs that
+  // block (gy, gx) fed through that shift.  Rows off the real outputs are zeros in dYg, and rows before the start come
+  // from TMA's zero fill at negative coordinates, so no term crosses a row or a sample.  B = the strip-ordered weight
+  // (K, strip_t^2 * N), k-block kb reading its columns [kb*N, (kb+1)*N) as an MN-major operand.  Each shift's product is
+  // formed in a fresh accumulator and added to the fp32 sum in kb order (the order of kh, then kw, ascending);
+  // C = din, NCHW (ci_cin, ci_h, ci_w, ci_stride; ci_h == strip_G * ci_stride), written once.
   // MN-major operands (mn_major bit 0: A is (K, M) row-major, bit 1: B is (K, N) row-major): the reduction index is the
   // ROW, as in a weight gradient dW = dY^T X taken straight from the row-major activations, or a data gradient
   // dX = dY W read from the untransposed weight (mn_major = 2).  NSPLIT 1 only.
@@ -70,7 +78,7 @@ struct TcExtra {
 };
 
 // C (+)= A B^T, A (M,K) / B (N,K) row-major bf16 (K % 8 == 0); *_lo non-null selects the split-bf16 x3 product.
-// (TC_CONV: M = B*G*G grid rows, K = strip_t^2 * strip_kc * 64.)
+// (TC_CONV: M = B*G*G grid rows, K = strip_t^2 * strip_kc * 64.  TC_CONV_DGRAD: K = Cout, the reduction of one shift.)
 int gemm_bf16_tc(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, const __nv_bfloat16* B_hi,
                  const __nv_bfloat16* B_lo, float* C, long ldc, int epi, const float* bias, float* out2, const float* eps,
                  int split_k, cudaStream_t s, const TcExtra* ex);

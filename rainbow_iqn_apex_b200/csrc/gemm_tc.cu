@@ -425,6 +425,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* s = smem + stage * Cfg::kStageBytes;
           mbar_expect_tx(&full[stage], Cfg::kStageBytes);
+          if constexpr (EPI == TC_CONV_DGRAD) {
+            // shift (dy, dx): dYg rows m0 - (dy*G + dx) (negative ones arrive as zeros), and that shift's (K, N) weight slab
+            const int dy = kb / p.strip_t, dx = kb - dy * p.strip_t;
+            tma_load_2d(s, &mapA_hi, 0, mt * TBM - (dy * p.strip_G + dx), &full[stage]);
+#pragma unroll
+            for (int i = 0; i < TBN / 64; ++i)
+              tma_load_2d(s + Cfg::kABytes + i * 8192, &mapB_hi, kb * p.N + nt * TBN + 64 * i, 0, &full[stage]);
+            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            continue;
+          }
           if (NSPLIT == 1 && p.mn_major) {
             // MN-major operand ((K, MN) row-major): 64 x 64 boxes, inner coordinate = MN offset, outer = reduction row.
             // bit 0: A, bit 1: B; the other operand (if any) stays K-major.
@@ -508,6 +518,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
     // ---- mainloop: the wgmma groups of one k-block stay in flight while the next k-block's operands are awaited; a
     // ring slot is released once the groups that read it have retired
     float acc[TBN / 2];
+    float dg_sum[TBN / 2];                      // TC_CONV_DGRAD: the sum over the shifts so far
+    if constexpr (EPI == TC_CONV_DGRAD) {
+#pragma unroll
+      for (int i = 0; i < TBN / 2; ++i) dg_sum[i] = 0.f;
+    }
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&full[stage], phase);
@@ -515,7 +530,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
       const uint32_t sa = s0 + g * 8192;        // this warpgroup's 64 rows (K-major) or 64-row MN slab (MN-major) of A
       const uint32_t sb = s0 + Cfg::kOps * Cfg::kABytes;
       wgmma_fence();
-      if constexpr (BN == 256) {
+      if constexpr (EPI == TC_CONV_DGRAD) {
+        mma_kblock<TBN>(acc, sa, sb, true, false, 2);   // every shift starts from a zeroed accumulator
+      } else if constexpr (BN == 256) {
         // operand modes fixed at compile time: run-time choices between wgmma variants make ptxas serialise them.  For
         // the same reason the edge tile (N = 3136: 64 real columns in the last one) runs full-width on TMA's zero fill.
         mma_kblock<TBN>(acc, sa, sb, kb == kb0, (MODE & 4) != 0, MODE & 3);
@@ -546,10 +563,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
       }
       prev = stage;
       if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      if constexpr (EPI == TC_CONV_DGRAD) {
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < TBN / 2; ++i) dg_sum[i] += acc[i];
+      }
     }
     wgmma_wait<0>();
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
+    if constexpr (EPI == TC_CONV_DGRAD) {
+#pragma unroll
+      for (int i = 0; i < TBN / 2; ++i) acc[i] = dg_sum[i];
+    }
 
     // ---- epilogue, one 64-column chunk at a time: fragment -> slab -> (row per lane) v[32] -> fused epilogue
 #pragma unroll
@@ -638,7 +664,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 #pragma unroll
           for (int j = 0; j < 32; ++j)
             if (n0 + j < p.N) cb[(long)j * p.ohw] = fmaxf(__uint_as_float(v[j]) + p.bias[n0 + j], 0.f);
-        } else if (EPI == TC_EMBED || EPI == TC_COL2IM || EPI == TC_CONV) {
+        } else if (EPI == TC_EMBED || EPI == TC_COL2IM || EPI == TC_CONV || EPI == TC_CONV_DGRAD) {
           // handled below with the whole warp
         } else if (!(p.vec_acc && n0 + 32 <= p.N)) {
           float* crow = p.C + (long)m * p.ldc + n0;
@@ -724,6 +750,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
           const int off = __shfl_sync(0xffffffffu, coff, j);
           if (row_ok && off >= 0)
             asm volatile("red.global.add.f32 [%0], %1;" ::"l"(base + off), "f"(__uint_as_float(v[j])) : "memory");
+        }
+      }
+      if (EPI == TC_CONV_DGRAD && n0 < p.N) {
+        // din[b, c, gy*s + iy, gx*s + ix] = sum[(b, gy, gx), (iy, ix, c)]: lane j decodes column n0 + j once and the
+        // offsets are broadcast by shuffle; lanes = consecutive gx, so a store instruction covers a few image row runs
+        const int kcol = n0 + lane, s = p.ci_stride;
+        int coff = -1;
+        if (kcol < p.N) {
+          const int blk = kcol / p.ci_cin, c = kcol - blk * p.ci_cin, iy = blk / s, ix = blk - iy * s;
+          coff = (c * p.ci_h + iy) * p.ci_w + ix;
+        }
+        const bool row_ok = m < p.M;
+        const int gg = p.strip_G * p.strip_G, mm = row_ok ? m : 0;
+        const int b = mm / gg, rem = mm - b * gg, gy = rem / p.strip_G, gx = rem - gy * p.strip_G;
+        float* base = p.C + ((long)b * p.ci_cin * p.ci_h + gy * s) * p.ci_w + gx * s;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int off = __shfl_sync(0xffffffffu, coff, j);
+          if (row_ok && off >= 0) base[off] = __uint_as_float(v[j]);
         }
       }
       if ((EPI == TC_STORE || EPI == TC_EMBED || (EPI == TC_BIAS_RELU && (p.M & 1) == 0) ||
@@ -919,6 +964,11 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
                 K != ex->strip_t * ex->strip_t * ex->strip_kc * TBK || (ex->nx_hi && (N % 32))))
     return (int)cudaErrorInvalidValue;
   const long a_k = strip ? (long)ex->strip_kc * TBK : K;       // row length of the A image
+  const bool dgrad = epi == TC_CONV_DGRAD;
+  if (dgrad && (ex == nullptr || split3 || split2 || ex->mn_major || ex->strip_t < 1 || ex->strip_G < 1 || K > TBK ||
+                N % 64 || split_k > 1 || ex->ci_cin < 1 || ex->ci_stride < 1 || N != ex->ci_stride * ex->ci_stride * ex->ci_cin ||
+                ex->ci_h != ex->strip_G * ex->ci_stride || ex->ci_w != ex->ci_h))
+    return (int)cudaErrorInvalidValue;
   const bool mn = ex != nullptr && ex->mn_major != 0;
   if (mn) {
     // A (K, M), B (K, N) row-major; only the plain single-bf16 product with full-width (or 64-wide) N tiles
@@ -940,11 +990,17 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
   }
   // 128-wide tiles: the m64n128 accumulator of each consumer warpgroup is 64 registers per thread
   const int bn = wide ? 256
-                      : (ex != nullptr && ex->mn_major) ? ((narrow_ok && N <= 64) ? 64 : 128)
-                                                        : (narrow_ok && N <= 32) ? 32 : (narrow_ok && N <= 64) ? 64 : 128;
+                      : (dgrad || (ex != nullptr && ex->mn_major)) ? ((dgrad || narrow_ok) && N <= 64 ? 64 : 128)
+                                                                   : (narrow_ok && N <= 32) ? 32 : (narrow_ok && N <= 64) ? 64 : 128;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
-  if (mn) {
+  if (dgrad) {
+    // A = dYg (M, K), B = the strip-ordered weight (K, strip_t^2 * N) read in 64 x 64 MN-major boxes
+    rc = make_map(&ma_hi, A_hi, M, K, TBM);
+    if (rc) return rc;
+    rc = make_map(&mb_hi, B_hi, K, (long)ex->strip_t * ex->strip_t * N, 64);
+    if (rc) return rc;
+  } else if (mn) {
     const long b_cols = ex->wg_t ? (long)ex->wg_kc * TBK : N;      // strip weight gradient: B is the block matrix
     rc = (ex->mn_major & 1) ? make_map(&ma_hi, A_hi, K, M, 64) : make_map(&ma_hi, A_hi, M, K, TBM);
     if (rc) return rc;
@@ -970,7 +1026,7 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
   p.M = M; p.N = N; p.K = K;
   p.m_tiles = (M + TBM - 1) / TBM;
   p.n_tiles = (N + bn - 1) / bn;
-  p.kb_total = (K + TBK - 1) / TBK;
+  p.kb_total = dgrad ? ex->strip_t * ex->strip_t : (K + TBK - 1) / TBK;   // strip data gradient: one k-block per shift
   if (split_k < 1) split_k = 1;
   // at most one round of CTAs: more splits would only multiply the partial sums written to scratch (gemm.h)
   if (split_k > tc_max_split(p.m_tiles * p.n_tiles)) split_k = tc_max_split(p.m_tiles * p.n_tiles);
@@ -1045,6 +1101,9 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
       switch (epi) {
         case TC_STORE: RIQN_TC_NARROW(1, TC_STORE); RIQN_TC_GO(1, TC_STORE);
         case TC_COL2IM: RIQN_TC_GO(1, TC_COL2IM);
+        case TC_CONV_DGRAD:
+          if (bn == 64) return launch_tc<1, TC_CONV_DGRAD, 64>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
+          RIQN_TC_GO(1, TC_CONV_DGRAD);
         case TC_BIAS_RELU: RIQN_TC_GO(1, TC_BIAS_RELU);
         case TC_ATOMIC: RIQN_TC_NARROW(1, TC_ATOMIC); RIQN_TC_GO(1, TC_ATOMIC);
         case TC_NOISY_WGRAD: RIQN_TC_GO(1, TC_NOISY_WGRAD);
