@@ -307,6 +307,24 @@ int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_spac
                           const float* q_target, const float* tau, const long long* actions, const long long* a_star,
                           const float* returns, const float* nonterminals, float gamma_n, float kappa, float* loss,
                           float* dtheta, float* theta_out, float* target_out, void* stream);
+/* Munchausen-IQN (Vieillard, Pietquin & Geist 2020): the same loss and gradient against a soft, entropy-regularised target
+ * with a clipped log-policy bonus, in place of the double-DQN one.  q_target is ONE target-network pass over the stacked
+ * frames [next_states; states] with n_tau_prime * 2 * batch rows: row j*2*batch + b is s_{t+n}, row j*2*batch + batch + b
+ * is s_t of transition b.  With te = entropy_tau:
+ *   qbar'(a) = mean_j q_target[j*2*batch+b, a] ,  qbar(a) = mean_j q_target[j*2*batch+batch+b, a]     (j ascending)
+ *   l'(a)    = qbar'(a) - max qbar' - te * ln sum_a exp((qbar'(a) - max qbar') / te)   (a ascending; l from qbar likewise)
+ *   pi'(a)   = exp((qbar'(a) - max qbar') / te) / sum_a exp((qbar'(a) - max qbar') / te)
+ *   bonus[b] = alpha * min(max(l(actions[b]), l0), 0)
+ *   target[b,j] = returns[b] + bonus[b] + gamma_n*nonterminals[b] * sum_a pi'(a) (q_target[j*2*batch+b, a] - l'(a))
+ *   theta, loss, dtheta as in riqn_iqn_loss_fwd_bwd.
+ * The bonus also enters on terminal transitions.  The log-policy is never formed as log(pi): an underflowing pi gives a
+ * finite, very negative l, which the clip takes to l0.  bonus_out (batch), like theta_out / target_out, may be NULL.
+ * Returns cudaErrorInvalidValue (and writes nothing) for action_space > 32, entropy_tau <= 0, l0 > 0, alpha < 0, or any of
+ * the three non-finite. */
+int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                           const float* q_target, const float* tau, const long long* actions, const float* returns,
+                           const float* nonterminals, float gamma_n, float kappa, float alpha, float entropy_tau, float l0,
+                           float* loss, float* dtheta, float* theta_out, float* target_out, float* bonus_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Rainbow-only (C51) head and loss            replaces rainbowiqn/model.py:120-129, rainbowiqn/agent.py:77-141

@@ -71,6 +71,7 @@ SIGNATURES = {
     "riqn_argmax_mean": [C.c_int, C.c_int, C.c_int, _P, _P, _P],
     "riqn_iqn_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float,
                               _P, _P, _P, _P, _P],
+    "riqn_miqn_loss_fwd_bwd": [C.c_int] * 4 + [_P] * 6 + [C.c_float] * 5 + [_P] * 6,
     "riqn_c51_head_fwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,
                               C.c_float, _P, _P, _P, _P],

@@ -3,7 +3,8 @@
 Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``args`` fields, same public
 attributes (online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
-compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting.  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
+``munchausen`` for Munchausen-IQN targets.  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema
 {T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160).
 """
@@ -54,7 +55,12 @@ class Agent:
         else:                                            # IQN sampling sizes (agent.py:58-63)
             for field in self._IQN_FIELDS:
                 setattr(self, field, getattr(args, field))
-        self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}
+        self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each
+        # Munchausen-IQN targets: optional args fields (absent from the reference's namespace: plain IQN).
+        # None, or (alpha, entropy_tau, l0) of compute_loss_iqn.check_munchausen
+        self.munchausen = compute_loss_iqn.check_munchausen(
+            getattr(args, "munchausen", 0),
+            *(getattr(args, f, v) for f, v in compute_loss_iqn.MUNCHAUSEN_DEFAULTS.items()), rainbow_only=self.rainbow_only)
         # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
         self.risk = None
         self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
@@ -66,6 +72,8 @@ class Agent:
         risk = check_risk((measure, eta))
         if risk is not None and self.rainbow_only:
             raise ValueError("risk measures distort the IQN quantile fractions; rainbow_only (C51) acts risk-neutrally")
+        if self.munchausen is not None:
+            compute_loss_iqn.check_munchausen(1, *self.munchausen, risk=risk)
         self.risk = risk
 
     @staticmethod

@@ -734,23 +734,12 @@ __global__ void argmax_mean_kernel(int B, int K, int A, const float* __restrict_
 //   dth[i*B+b] = dloss[b]/dth_i  (indicator detached, :344-346)
 // One CTA per transition; thread i owns th_i and walks the N' targets staged in shared memory.
 // ------------------------------------------------------------------------------------------------
-__global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
-                                const float* __restrict__ q_tgt, const float* __restrict__ tau,
-                                const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
-                                const float* __restrict__ returns, const float* __restrict__ nonterminals,
-                                float gamma_n, float kappa, float* __restrict__ loss, float* __restrict__ dtheta,
-                                float* __restrict__ theta_out, float* __restrict__ target_out) {
-  extern __shared__ float sT[];  // Np targets + 32 reduction slots
-  float* red = sT + Np;
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int as = (int)a_star[b], ac = (int)actions[b];
-  const float g = __fmul_rn(gamma_n, nonterminals[b]);
-  for (int j = tid; j < Np; j += blockDim.x) {
-    const float t = __fadd_rn(returns[b], __fmul_rn(g, q_tgt[((long)j * B + b) * A + as]));
-    sT[j] = t;
-    if (target_out) target_out[(long)b * Np + j] = t;
-  }
-  __syncthreads();
+// The quantile-Huber part, shared with miqn_loss_kernel: the targets of transition b sit in sT[0..Np), red holds 32 slots.
+__device__ __forceinline__ void quantile_huber_loss(int B, int N, int Np, int A, int b, int ac,
+                                                    const float* __restrict__ q_on, const float* __restrict__ tau,
+                                                    float kappa, const float* sT, float* red, float* __restrict__ loss,
+                                                    float* __restrict__ dtheta, float* __restrict__ theta_out) {
+  const int tid = threadIdx.x;
   float part = 0.f;
   for (int i = tid; i < N; i += blockDim.x) {
     const float th = q_on[((long)i * B + b) * A + ac];
@@ -777,6 +766,98 @@ __global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __rest
     v = warp_sum(v);
     if (tid == 0) loss[b] = v / (float)Np;
   }
+}
+
+__global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
+                                const float* __restrict__ q_tgt, const float* __restrict__ tau,
+                                const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
+                                const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                                float gamma_n, float kappa, float* __restrict__ loss, float* __restrict__ dtheta,
+                                float* __restrict__ theta_out, float* __restrict__ target_out) {
+  extern __shared__ float sT[];  // Np targets + 32 reduction slots
+  float* red = sT + Np;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int as = (int)a_star[b], ac = (int)actions[b];
+  const float g = __fmul_rn(gamma_n, nonterminals[b]);
+  for (int j = tid; j < Np; j += blockDim.x) {
+    const float t = __fadd_rn(returns[b], __fmul_rn(g, q_tgt[((long)j * B + b) * A + as]));
+    sT[j] = t;
+    if (target_out) target_out[(long)b * Np + j] = t;
+  }
+  __syncthreads();
+  quantile_huber_loss(B, N, Np, A, b, ac, q_on, tau, kappa, sT, red, loss, dtheta, theta_out);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Munchausen-IQN loss (Vieillard, Pietquin & Geist 2020), forward + dloss/dtheta.  q_tgt is ONE target-network pass over
+// the stacked frames [next_states; states]: row j*2B + b is s_{t+n}, row j*2B + B + b is s_t of transition b.
+//   qbar'(a) = mean_j q_tgt[j*2B+b, a] ,  qbar(a) = mean_j q_tgt[j*2B+B+b, a]        (j ascending)
+//   l'(a) = qbar'(a) - max qbar' - te * ln sum_a exp((qbar'(a) - max qbar') / te)    (a ascending; l from qbar likewise)
+//   pi'(a) = exp((qbar'(a) - max qbar') / te) / sum_a exp(...)
+//   m = alpha * min(max(l(act[b]), l0), 0)
+//   T[b,j] = (R[b] + m) + fl(gamma^n)*nt[b] * sum_a pi'(a) (q_tgt[j*2B+b, a] - l'(a))   (a ascending)
+// then the quantile-Huber loss of iqn_loss_kernel.  The log-policy is only ever formed in this shifted form, so an
+// underflowing pi gives a finite, very negative l.  One CTA per transition, fixed summation orders, no atomics.
+// ------------------------------------------------------------------------------------------------
+__global__ void miqn_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
+                                 const float* __restrict__ q_tgt, const float* __restrict__ tau,
+                                 const int64_t* __restrict__ actions, const float* __restrict__ returns,
+                                 const float* __restrict__ nonterminals, float gamma_n, float kappa, float alpha,
+                                 float te, float l0, float* __restrict__ loss, float* __restrict__ dtheta,
+                                 float* __restrict__ theta_out, float* __restrict__ target_out,
+                                 float* __restrict__ bonus_out) {
+  extern __shared__ float sT[];  // Np targets + 32 reduction slots
+  float* red = sT + Np;
+  __shared__ float s_mean[2][32], s_pi[32], s_lp[32], s_m;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int ac = (int)actions[b];
+  const long rstride = 2L * B * A;                 // between consecutive fractions j of one frame
+  // 1. the two target-net means: set 0 over s_{t+n}, set 1 over s_t; one thread per (set, action), j ascending
+  for (int s = tid; s < 64; s += blockDim.x) {
+    const int set = s >> 5, a = s & 31;
+    if (a < A) {
+      const float* z = q_tgt + ((long)set * B + b) * A + a;
+      float acc = 0.f;
+#pragma unroll 8
+      for (int j = 0; j < Np; ++j) acc += z[j * rstride];
+      s_mean[set][a] = acc / (float)Np;
+    }
+  }
+  __syncthreads();
+  // 2. both log-softmaxes (every lane of warp 0 runs the same a-ascending sums) and the clipped log-policy bonus
+  if (tid < 32) {
+    for (int set = 0; set < 2; ++set) {
+      const float* qm = s_mean[set];
+      float mx = qm[0];
+      for (int a = 1; a < A; ++a) mx = fmaxf(mx, qm[a]);
+      float sum = 0.f;
+      for (int a = 0; a < A; ++a) sum += expf((qm[a] - mx) / te);
+      const float lse = te * logf(sum);
+      if (set == 0 && tid < A) {
+        const float d = qm[tid] - mx;
+        s_pi[tid] = expf(d / te) / sum;
+        s_lp[tid] = d - lse;
+      } else if (set == 1 && tid == 0) {
+        const float m = alpha * fminf(fmaxf((qm[ac] - mx) - lse, l0), 0.f);
+        s_m = m;
+        if (bonus_out) bonus_out[b] = m;
+      }
+    }
+  }
+  __syncthreads();
+  // 3. the N' soft double-expectation targets
+  const float g = __fmul_rn(gamma_n, nonterminals[b]);
+  const float rm = __fadd_rn(returns[b], s_m);
+  for (int j = tid; j < Np; j += blockDim.x) {
+    const float* z = q_tgt + ((long)j * 2 * B + b) * A;
+    float e = 0.f;
+    for (int a = 0; a < A; ++a) e = fmaf(s_pi[a], __fsub_rn(z[a], s_lp[a]), e);
+    const float t = __fadd_rn(rm, __fmul_rn(g, e));
+    sT[j] = t;
+    if (target_out) target_out[(long)b * Np + j] = t;
+  }
+  __syncthreads();
+  quantile_huber_loss(B, N, Np, A, b, ac, q_on, tau, kappa, sT, red, loss, dtheta, theta_out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1554,6 +1635,25 @@ RIQN_API int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int ac
   iqn_loss_kernel<<<batch, threads, smem, (cudaStream_t)stream>>>(
       batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, (const int64_t*)a_star,
       returns, nonterminals, gamma_n, kappa, loss, dtheta, theta_out, target_out);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                                    const float* q_target, const float* tau, const long long* actions,
+                                    const float* returns, const float* nonterminals, float gamma_n, float kappa,
+                                    float alpha, float entropy_tau, float l0, float* loss, float* dtheta,
+                                    float* theta_out, float* target_out, float* bonus_out, void* stream) {
+  if (action_space > 32 || !(entropy_tau > 0.f) || !isfinite(entropy_tau) || !(l0 <= 0.f) || !isfinite(l0) ||
+      !(alpha >= 0.f) || !isfinite(alpha))
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;
+  if (threads > 1024) threads = 1024;
+  if (threads < 32) threads = 32;
+  const size_t smem = sizeof(float) * (n_tau_prime + 32);
+  miqn_loss_kernel<<<batch, threads, smem, (cudaStream_t)stream>>>(
+      batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, returns, nonterminals,
+      gamma_n, kappa, alpha, entropy_tau, l0, loss, dtheta, theta_out, target_out, bonus_out);
   return (int)cudaGetLastError();
 }
 
