@@ -233,7 +233,9 @@ int riqn_quantile_embed_bwd(int batch, int num_quantiles, int embed_dim, int fea
  * (feat_dim, rows) for its weight gradient in the cross-check arithmetic modes (each may be NULL; the transposed images
  * are split from x32 by a second launch and therefore need x32 != NULL); x32 (may be NULL) is the fp32 matrix.  cos_hi / cos_lo
  * (rows, embed_dim) and cos_t_hi (embed_dim, rows; may be NULL) are outputs too.  cos_lo == NULL selects the
- * single-bf16 product.  iqn_w_hi / iqn_w_lo: bf16 images of iqn_fc.weight (riqn_split_bf16). */
+ * single-bf16 product.  iqn_w_hi / iqn_w_lo: bf16 images of iqn_fc.weight (riqn_split_bf16).  rows % 2, feat_dim % 32
+ * and embed_dim % 8 must be 0, and cos_hi, cos_lo, iqn_w_hi, iqn_w_lo, x32, x_hi, x_lo 16-byte aligned; a call rejected
+ * for its shapes or alignment (cudaErrorInvalidValue) writes nothing. */
 int riqn_quantile_embed_fwd_tc(int batch, int num_quantiles, int embed_dim, int feat_dim, const float* tau,
                                const float* feat, const void* iqn_w_hi, const void* iqn_w_lo, const float* iqn_b,
                                void* cos_hi, void* cos_lo, void* cos_t_hi, float* x32, void* x_hi, void* x_lo, void* x_hi_t,
@@ -280,7 +282,8 @@ int riqn_dueling_bwd_dense(long rows, int batch, int hidden, int action_space, c
 int riqn_dueling_bwd_dense_bf16(long rows, int batch, int hidden, int action_space, const float* h, const void* h_bf16,
                                 const float* wz, const float* grad_q, void* dh_hi, void* dh_hi_t, float* dh_colsum,
                                 float* dz, void* dz_bf16, void* stream);
-/* Parameter gradients of the two z-layers (accumulated): dwz_scratch 32*2*hidden floats, dbz_scratch 32. */
+/* Parameter gradients of the two z-layers (accumulated): dwz_scratch 32*2*hidden floats, dbz_scratch 32.
+ * 1 <= action_space <= 31, else cudaErrorInvalidValue and nothing is written. */
 /* Same with the reduction dz^T h on the tensor cores, straight from the row-major bf16 images dz_bf16 (rows, 32) and
  * h_bf16 (rows, 2*hidden) (rows % 8 == 0). */
 int riqn_z_wgrad_tc(long rows, int hidden, int action_space, const void* dz_bf16, const void* h_bf16, const float* dz,

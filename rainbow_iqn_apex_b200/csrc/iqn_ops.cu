@@ -1295,9 +1295,16 @@ RIQN_API int riqn_quantile_embed_fwd_tc(int batch, int num_quantiles, int embed_
                                         const float* feat, const void* iqn_w_hi, const void* iqn_w_lo, const float* iqn_b,
                                         void* cos_hi, void* cos_lo, void* cosT_hi, float* x32, void* x_hi, void* x_lo,
                                         void* x_hiT, void* x_loT, int x_fp16, void* stream) {
+  const long R = (long)batch * num_quantiles;
+  // every shape and operand alignment the product rejects (TMA needs 16-byte aligned bases; the epilogue's x32 stores are
+  // 16 bytes wide) is rejected here, before the cos images are written
+  const bool want_t = x_hiT != nullptr || x_loT != nullptr;    // transposed images (cross-check arithmetic modes only)
+  const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  if (R % 2 || feat_dim % 32 || embed_dim % 8 || (want_t && (x32 == nullptr || x_fp16)) || !a16(cos_hi) || !a16(cos_lo) ||
+      !a16(iqn_w_hi) || !a16(iqn_w_lo) || !a16(x32) || !a16(x_hi) || !a16(x_lo))
+    return (int)cudaErrorInvalidValue;
   riqn::note_launches(2);
   cudaStream_t s = (cudaStream_t)stream;
-  const long R = (long)batch * num_quantiles;
   cos_embed_bf16_kernel<<<riqn_cdiv(R * embed_dim, 256), 256, 0, s>>>(batch, num_quantiles, embed_dim, tau, (__nv_bfloat16*)cos_hi,
                                                                      (__nv_bfloat16*)cos_lo, (__nv_bfloat16*)cosT_hi);
   RIQN_LAUNCH_CHECK();
@@ -1307,8 +1314,6 @@ RIQN_API int riqn_quantile_embed_fwd_tc(int batch, int num_quantiles, int embed_
   ex.o_hi = (__nv_bfloat16*)x_hi;
   ex.o_lo = (__nv_bfloat16*)x_lo;
   ex.fmt = x_fp16 ? 4 : 0;       // x_hi = fp16(x) (head forward operand), x_lo (optional) = bf16(x) (backward operand)
-  const bool want_t = x_hiT != nullptr || x_loT != nullptr;    // transposed images (cross-check arithmetic modes only)
-  if (want_t && (x32 == nullptr || x_fp16)) return (int)cudaErrorInvalidValue;
   int rc = gemm_bf16_tc((int)R, feat_dim, embed_dim, (const __nv_bfloat16*)cos_hi, (const __nv_bfloat16*)cos_lo,
                         (const __nv_bfloat16*)iqn_w_hi, cos_lo ? (const __nv_bfloat16*)iqn_w_lo : nullptr, x32, feat_dim,
                         TC_EMBED, iqn_b, nullptr, nullptr, 1, s, &ex);
@@ -1568,6 +1573,7 @@ RIQN_API int riqn_z_wgrad(long rows, int hidden, int action_space, const float* 
                           float* dbz_scratch, const float* eps_w_zv, const float* eps_b_zv, const float* eps_w_za,
                           const float* eps_b_za, float* g_mu_zv, float* g_sig_zv, float* g_bmu_zv, float* g_bsig_zv,
                           float* g_mu_za, float* g_sig_za, float* g_bmu_za, float* g_bsig_za, void* stream) {
+  if (action_space < 1 || action_space > 31) return (int)cudaErrorInvalidValue;   // dwz_scratch has 32 rows
   riqn::note_launches(3);
   cudaStream_t s = (cudaStream_t)stream;
   const int W = 2 * hidden;
@@ -1591,10 +1597,10 @@ RIQN_API int riqn_z_wgrad_tc(long rows, int hidden, int action_space, const void
                              const float* eps_w_za, const float* eps_b_za, float* g_mu_zv, float* g_sig_zv, float* g_bmu_zv,
                              float* g_bsig_zv, float* g_mu_za, float* g_sig_za, float* g_bmu_za, float* g_bsig_za,
                              void* stream) {
+  if (rows % 8 || action_space < 1 || action_space > 31) return (int)cudaErrorInvalidValue;   // dwz_scratch has 32 rows
   riqn::note_launches(3);
   cudaStream_t s = (cudaStream_t)stream;
   const int W = 2 * hidden;
-  if (rows % 8) return (int)cudaErrorInvalidValue;
   RIQN_CUDA(cudaMemsetAsync(dwz_scratch, 0, sizeof(float) * 32 * W, s));
   RIQN_CUDA(cudaMemsetAsync(dbz_scratch, 0, sizeof(float) * 32, s));
   const int n_tiles = (W + 255) / 256;
