@@ -330,7 +330,42 @@ int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_spa
                            float* loss, float* dtheta, float* theta_out, float* target_out, float* bonus_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Rainbow-only (C51) head and loss            replaces rainbowiqn/model.py:120-129, rainbowiqn/agent.py:77-141
+ * FQF: fraction proposal network (Yang et al., NeurIPS 2019; no counterpart in the reference)
+ * The proposal's logits (batch, n) = feat W_f^T + b_f come from riqn_linear_fwd_ld (split-1 fp32 store, deterministic).
+ * Every entry point below takes 2 <= n <= 256 (and 1 <= action_space <= 32, batch >= 1) and returns
+ * cudaErrorInvalidValue, writing nothing, for anything else.
+ * ---------------------------------------------------------------------------------------------- */
+/* P = softmax(logits[b, :]), max-shifted, e_k = exp(l_k - max l) in double.  The cumulative sums c_i = sum_{k<i} e_k are
+ * formed in double with k ascending (one sequential sum per sample) and rounded once:
+ *   tau[b, 0] = 0, tau[b, i] = fl(c_i / c_n) (i = 1..n-1), tau[b, n] = 1 exactly      (batch, n+1), non-decreasing
+ *   tau_hat[i*batch + b] = (tau[b,i] + tau[b,i+1]) / 2, dtau[i*batch + b] = tau[b,i+1] - tau[b,i]   (quantile-major, fp32)
+ *   entropy[b] (may be NULL) = -sum_k P_k log P_k, formed as log c_n - sum_k (e_k / c_n)(l_k - max l) in double.
+ * A P_k that underflows float gives dtau == 0, never NaN. */
+int riqn_fqf_fractions(int batch, int n, const float* logits, float* tau, float* tau_hat, float* dtau, float* entropy,
+                       void* stream);
+/* Backward of the fraction loss with the quantile values detached.  q_hat (n*batch, A) is the pass at tau_hat, q_bnd
+ * ((n-1)*batch, A; more rows are allowed and ignored) the pass at the inner boundaries tau_1..tau_{n-1}, both
+ * quantile-major; with F(.) the value of action a = actions[b] and w = gscale[b] * gscale_mul (gscale may be NULL: 1):
+ *   g_i       = 2 F(tau_i) - F(tau_hat_i) - F(tau_hat_{i-1})             i = 1..n-1 (dW1/dtau_i, FQF Proposition 1)
+ *   loss[b]   = sum_i g_i tau_i - entropy_coef * H(P)                    (loss_out, unweighted; may be NULL)
+ *   G_k       = sum_{i>k} g_i                                            (dL/dP_k, k descending)
+ *   dlogits[b, k] = w * (P_k (G_k - sum_m P_m G_m) + entropy_coef * P_k (log P_k + H))
+ * All sums in double in the stated order, P recomputed from logits exactly as riqn_fqf_fractions does.  entropy_coef must
+ * be finite and >= 0, gscale_mul finite. */
+int riqn_fqf_fraction_bwd(int batch, int n, int action_space, const float* logits, const float* tau, const float* q_hat,
+                          const float* q_bnd, const long long* actions, const float* gscale, float gscale_mul,
+                          float entropy_coef, float* dlogits, float* loss_out, void* stream);
+/* grad_w (n, feat_dim) += dlogits^T feat, grad_b (n) += sum_b dlogits[b, :]: each element is one fp32 fmaf chain over b
+ * ascending, then added once.  No atomics. */
+int riqn_fqf_fraction_wgrad(int batch, int n, int feat_dim, const float* dlogits, const float* feat, float* grad_w,
+                            float* grad_b, void* stream);
+/* a_star[b] = argmax_a sum_k w[k*batch+b] * q[k*batch+b, a]: fp32 fmaf chain over k ascending, the first maximal index
+ * winning (as riqn_argmax_mean).  FQF's Q(s, a) = sum_i dtau_i F(s, tau_hat_i, a). */
+int riqn_argmax_weighted(int batch, int n, int action_space, const float* q, const float* w, long long* a_star,
+                         void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Rainbow-only (C51) head and loss           replaces rainbowiqn/model.py:120-129, rainbowiqn/agent.py:77-141
  * ---------------------------------------------------------------------------------------------- */
 /* zv (batch, atoms), za (batch, A*atoms) -> q = v + a - mean_a a; p / logp (batch, A, atoms) = (log_)softmax over
  * atoms (either may be NULL); a_star (may be NULL) = argmax_a sum_j support[j] p[b,a,j]  (agent.py:92-99). */

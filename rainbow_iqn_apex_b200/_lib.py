@@ -72,7 +72,11 @@ SIGNATURES = {
     "riqn_iqn_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float,
                               _P, _P, _P, _P, _P],
     "riqn_miqn_loss_fwd_bwd": [C.c_int] * 4 + [_P] * 6 + [C.c_float] * 5 + [_P] * 6,
-    "riqn_c51_head_fwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
+    "riqn_fqf_fractions": [C.c_int, C.c_int] + [_P] * 6,
+    "riqn_fqf_fraction_bwd": [C.c_int] * 3 + [_P] * 6 + [C.c_float] * 2 + [_P] * 3,
+    "riqn_fqf_fraction_wgrad": [C.c_int] * 3 + [_P] * 5,
+    "riqn_argmax_weighted": [C.c_int] * 3 + [_P] * 4,
+    "riqn_c51_head_fwd":[C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,
                               C.c_float, _P, _P, _P, _P],
     "riqn_c51_head_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P, _P],

@@ -7,6 +7,7 @@ import random
 import numpy as np
 import torch
 
+from . import fqf
 from ._lib import call, ptr
 from .agent import Agent
 from .learner import MODEL_WEIGHT_STR
@@ -19,15 +20,33 @@ class Actor(Agent):
         tau, self._inject_act_tau = self._inject_act_tau, None
         return tau
 
+    def _fqf_pass(self, states_u8):
+        """FQF acting: fractions proposed on the trunk features, one head pass at their tau_hat.  Returns (q (N*E, A),
+        dtau (N*E,)); Q = sum_i dtau_i q_i.  num_quantile_samples is not read."""
+        on = self.online_net
+        on._compose_weights()                  # what forward() does first; the trunk reads the refreshed images
+        feat = on.trunk(states_u8)
+        fr = self.fraction_net.propose(feat)
+        q, _ = on.forward(states_u8, self.num_tau_samples, tau=fr["tau_hat"], fresh_weights=True, feat=feat)
+        return q, fr["dtau"]
+
+    def _fqf_argmax(self, states_u8):
+        q, dtau = self._fqf_pass(states_u8)
+        a = torch.empty(states_u8.shape[0], dtype=torch.int64, device=q.device)
+        call("riqn_argmax_weighted", states_u8.shape[0], self.num_tau_samples, self.action_space, ptr(q), ptr(dtau), ptr(a))
+        return a
+
     def act(self, state_buffer):
-        """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN; distorted by ``self.risk``) or the
-        expected value of the categorical distribution (C51).  Frames go to the device as uint8; the /255 of the
-        reference happens inside the conv kernel."""
+        """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN; distorted by ``self.risk``), the
+        dtau-weighted mean over the proposed fractions (FQF) or the expected value of the categorical distribution (C51).
+        Frames go to the device as uint8; the /255 of the reference happens inside the conv kernel."""
         state = torch.from_numpy(np.stack(state_buffer).astype(np.uint8)).to(self.online_net._flat.device)
         with torch.no_grad():
             if self.rainbow_only:
                 p = self.online_net(state.unsqueeze(0))
                 return (p * self.support).sum(2).argmax(1).item()
+            if self.fqf is not None:
+                return int(self._fqf_argmax(state.unsqueeze(0)).item())
             quantile_values, _ = self.online_net(state.unsqueeze(0), self.num_quantile_samples, tau=self._pop_tau(),
                                                   risk=self.risk)
             a = torch.empty(1, dtype=torch.int64, device=state.device)
@@ -39,6 +58,8 @@ class Actor(Agent):
         with torch.no_grad():
             if self.rainbow_only:
                 return (self.online_net(states_u8) * self.support).sum(2).argmax(1)
+            if self.fqf is not None:
+                return self._fqf_argmax(states_u8)
             E = states_u8.shape[0]
             q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=self._pop_tau(), risk=self.risk)
             a = torch.empty(E, dtype=torch.int64, device=q.device)
@@ -47,9 +68,15 @@ class Actor(Agent):
 
     def act_batch_values(self, states_u8, tau=None):
         """(E, A) mean quantile values behind act_batch (the argmax input; parity tests and epsilon schedules): Q_beta
-        under ``self.risk``, the mean over K fractions beta(tau) unless ``tau`` is given."""
+        under ``self.risk``, the mean over K fractions beta(tau) unless ``tau`` is given.  FQF: sum_i dtau_i F(s, tau_hat_i, a)
+        over the proposed fractions (``tau`` is not taken)."""
         with torch.no_grad():
             E = states_u8.shape[0]
+            if self.fqf is not None:
+                if tau is not None:
+                    raise ValueError("FQF acts on its proposed fractions: act_batch_values takes no tau")
+                q, dtau = self._fqf_pass(states_u8)
+                return fqf.q_values(q, dtau, E, self.num_tau_samples, self.action_space)
             q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=tau if tau is not None else self._pop_tau(),
                                    risk=self.risk)
             # q rows are quantile-major (k*E + e), like the reference (model.py:149)

@@ -4,16 +4,17 @@ Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``
 attributes (online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
 compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
-``munchausen`` for Munchausen-IQN targets.  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
-optimiser is the arena Adam; checkpoints keep the reference schema
-{T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160).
+``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions.  The
+networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference
+schema {T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus the fraction network's two
+entries under FQF.
 """
 import os
 
 import torch
 
 from . import _lib
-from . import compute_loss_iqn
+from . import compute_loss_iqn, fqf
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -55,12 +56,26 @@ class Agent:
         else:                                            # IQN sampling sizes (agent.py:58-63)
             for field in self._IQN_FIELDS:
                 setattr(self, field, getattr(args, field))
-        self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each
+        self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each;
+        #                      FQF: {"noises": (n0, n1, n2)}
         # Munchausen-IQN targets: optional args fields (absent from the reference's namespace: plain IQN).
         # None, or (alpha, entropy_tau, l0) of compute_loss_iqn.check_munchausen
         self.munchausen = compute_loss_iqn.check_munchausen(
             getattr(args, "munchausen", 0),
             *(getattr(args, f, v) for f, v in compute_loss_iqn.MUNCHAUSEN_DEFAULTS.items()), rainbow_only=self.rainbow_only)
+        # FQF fraction proposal: optional args fields (absent from the reference's namespace: plain IQN).
+        # None, or (fraction_lr, entropy_coef) of fqf.check_fqf
+        self.fqf = fqf.check_fqf(getattr(args, "fqf", 0), *(getattr(args, f, v) for f, v in fqf.FQF_DEFAULTS.items()),
+                                 rainbow_only=self.rainbow_only, munchausen=self.munchausen,
+                                 num_tau_samples=getattr(args, "num_tau_samples", None))
+        self.fraction_net = self.fraction_optimiser = None
+        if self.fqf is not None:
+            # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed
+            self.fraction_net = fqf.FractionProposal(self.num_tau_samples, args.device)
+            self.fraction_optimiser = Adam(self.fraction_net.parameters(), lr=self.fqf[0], eps=args.adam_eps)
+            if checkpoint is not None and "fraction_net_state_dict" in checkpoint:
+                self.fraction_net.load_state_dict(checkpoint["fraction_net_state_dict"])
+                self.fraction_optimiser.load_state_dict(checkpoint["fraction_optimiser_state_dict"])
         # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
         self.risk = None
         self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
@@ -74,6 +89,8 @@ class Agent:
             raise ValueError("risk measures distort the IQN quantile fractions; rainbow_only (C51) acts risk-neutrally")
         if self.munchausen is not None:
             compute_loss_iqn.check_munchausen(1, *self.munchausen, risk=risk)
+        if getattr(self, "fqf", None) is not None:
+            fqf.check_fqf(1, *self.fqf, risk=risk)
         self.risk = risk
 
     @staticmethod
@@ -107,16 +124,18 @@ class Agent:
             self, states, actions, returns, next_states, nonterminals, debug=debug)
 
     def save(self, path, T_actors, T_learner, name):
-        """agent.py:150-160"""
-        torch.save(
-            {
-                "T_actors": T_actors,
-                "T_learner": T_learner,
-                "model_state_dict": self.online_net.state_dict(),
-                "optimiser_state_dict": self.optimiser.state_dict(),
-            },
-            os.path.join(path, name),
-        )
+        """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
+        fraction_optimiser_state_dict; model_state_dict keeps the reference schema either way."""
+        ckpt = {
+            "T_actors": T_actors,
+            "T_learner": T_learner,
+            "model_state_dict": self.online_net.state_dict(),
+            "optimiser_state_dict": self.optimiser.state_dict(),
+        }
+        if self.fqf is not None:
+            ckpt["fraction_net_state_dict"] = self.fraction_net.state_dict()
+            ckpt["fraction_optimiser_state_dict"] = self.fraction_optimiser.state_dict()
+        torch.save(ckpt, os.path.join(path, name))
 
     def train(self):
         self.online_net.train()

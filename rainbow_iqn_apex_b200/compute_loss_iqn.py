@@ -12,6 +12,11 @@ Under a risk measure (Agent.set_risk) only the K pass draws distorted fractions 
 Munchausen-IQN (Agent.munchausen, Vieillard, Pietquin & Geist 2020) replaces the double-DQN target by a soft one with a
 clipped log-policy bonus (riqn_miqn_loss_fwd_bwd).  It needs no a*, so it runs two passes: target([next_states; states], N')
 as one stacked batch, then online(states, N).
+
+FQF (Agent.fqf, Yang et al. 2019; see fqf.py) takes every fraction from the online fraction proposal instead of drawing
+them: online(next_states, N at the proposed tau_hat') -> a* by the dtau'-weighted mean; target(next_states, N at the
+tau_hat of states); online(states, N at tau_hat) and, without a reset, online(states, at tau_1..tau_{N-1}) for the fraction
+loss (_fqf_core, fraction_backward).  num_quantile_samples and num_tau_prime_samples are not read under FQF.
 """
 import ctypes
 import math
@@ -74,10 +79,12 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     if isinstance(inj, list):            # a queue of injections: one per call (Actor.compute_priorities chunks)
         inj = inj.pop(0) if inj else None
     noises = inj["noises"] if inj else (None, None, None)
-    taus = inj["taus"] if inj else (None, None, None)
+    taus = inj.get("taus", (None, None, None)) if inj else (None, None, None)     # FQF's hook has no fractions
     dev = states.device
     if getattr(agent, "munchausen", None) is not None:
         return _munchausen_core(agent, states, actions, returns, next_states, nonterminals, noises, taus, keep_graph, debug)
+    if getattr(agent, "fqf", None) is not None:
+        return _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises, keep_graph, debug)
 
     on.reset_noise(noises[0])                                                       # :234
     cache = {}   # conv1's pixel block matrix of next_states is shared by the online and the target pass
@@ -140,6 +147,70 @@ def _munchausen_core(agent, states, actions, returns, next_states, nonterminals,
     return loss, dtheta, keep, actions
 
 
+def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises, keep_graph, debug):
+    """loss_core under FQF (agent.fqf, the fraction proposal agent.fraction_net).  Injection hook: ``agent._inject =
+    {"noises": (n0, n1, n2)}``; FQF draws no random fractions.
+
+    The double-DQN step of the FQF paper's Algorithm 1, as its public implementations read it: fractions of s' from the
+    online proposal select a* = argmax_a sum_i dtau'_i F(s', tau_hat'_i, a); the target network is evaluated on s' at the
+    tau_hat of s; the online network at tau_hat (gradient pass) and, with the same composed weights, at the inner
+    boundaries tau_1..tau_{N-1} (no-grad) for the fraction loss's W1 gradient.  With ``keep_graph`` the fraction state
+    goes into ``keep["fqf"]`` for fraction_backward."""
+    on, tg, fnet = agent.online_net, agent.target_net, agent.fraction_net
+    B, A, N = states.shape[0], agent.action_space, agent.num_tau_samples
+    dev = states.device
+    on.reset_noise(noises[0])
+    cache = {}
+    pair = on.trunk_pair(tg, next_states)
+    f_on, f_tg = pair if pair is not None else (on.trunk(next_states, col_cache=cache), None)
+    fr_n = fnet.propose(f_on)                                                         # fractions of s'
+    q_sel, _ = on.forward(next_states, N, tau=fr_n["tau_hat"], fresh_weights=True, col_cache=cache, feat=f_on)
+    a_star = torch.empty(B, dtype=torch.int64, device=dev)
+    call("riqn_argmax_weighted", B, N, A, ptr(q_sel), ptr(fr_n["dtau"]), ptr(a_star))
+    # the conv trunk is noise-free: the gradient pass's trunk runs here, once, and its features propose the fractions of s
+    keep = {} if keep_graph else None
+    feat = on.trunk(states, keep)
+    fr = fnet.propose(feat)
+    tg.reset_noise(noises[1])
+    q_tgt, _ = tg.forward(next_states, N, tau=fr["tau_hat"], fresh_weights=True, col_cache=cache, feat=f_tg)
+    on.reset_noise(noises[2])
+    q_on, tau_hat = on.forward(states, N, tau=fr["tau_hat"], keep=keep, fresh_weights=True, feat=feat)
+    # the inner boundaries tau_1..tau_{N-1}, quantile-major; one more row block (tau_N = 1) keeps the row count even where
+    # the tensor-core embedding needs it
+    nb = N - 1 if (N - 1) * B % 2 == 0 else N
+    q_bnd, _ = on.forward(states, nb, tau=fr["tau"][:, 1:nb + 1].t().contiguous(), fresh_weights=True, feat=feat)
+
+    loss = torch.empty(B, device=dev)
+    dtheta = torch.empty(N * B, device=dev)
+    theta_out = target_out = None
+    if debug is not None:
+        theta_out = torch.empty(B, N, device=dev)
+        target_out = torch.empty(B, N, device=dev)
+    call("riqn_iqn_loss_fwd_bwd", B, N, N, A, ptr(q_on), ptr(q_tgt), ptr(tau_hat), ptr(actions), ptr(a_star),
+         ptr(returns), ptr(nonterminals), float(agent.discount ** agent.n), float(agent.kappa), ptr(loss),
+         ptr(dtheta), ptr(theta_out), ptr(target_out))
+    if keep is not None:
+        keep["fqf"] = dict(fr=fr, q_hat=q_on, q_bnd=q_bnd, actions=actions, debug=debug)
+    if debug is not None:
+        debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on, q_bnd=q_bnd,
+                     tau=fr["tau"], tau_hat=fr["tau_hat"], dtau=fr["dtau"], logits=fr["logits"], entropy=fr["entropy"],
+                     tau_next=fr_n["tau"], dtau_next=fr_n["dtau"], keep=keep)
+    return loss, dtheta, keep, actions
+
+
+def fraction_backward(agent, keep, gscale, gscale_mul=1.0):
+    """The FQF fraction loss's gradient, accumulated into agent.fraction_net's arena, for a loss_core call whose ``keep``
+    it reads; the surrogate of transition b is weighted by gscale[b] * gscale_mul like the quantile loss.  No-op
+    without FQF.  ``debug`` (loss_core's) receives dlogits and fraction_loss."""
+    fk = keep.get("fqf") if keep is not None else None
+    if fk is None:
+        return
+    dlogits, floss = agent.fraction_net.backward(fk["fr"], fk["q_hat"], fk["q_bnd"], fk["actions"], gscale, gscale_mul,
+                                                 agent.fqf[1])
+    if fk["debug"] is not None:
+        fk["debug"].update(dlogits=dlogits, fraction_loss=floss)
+
+
 class _IQNLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, agent, states, actions, returns, next_states, nonterminals, debug, *params):
@@ -151,7 +222,9 @@ class _IQNLoss(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_loss):
-        ctx.agent.online_net.backward_iqn(ctx.keep, ctx.dtheta, grad_loss.contiguous().float(), ctx.actions)
+        g = grad_loss.contiguous().float()
+        ctx.agent.online_net.backward_iqn(ctx.keep, ctx.dtheta, g, ctx.actions)
+        fraction_backward(ctx.agent, ctx.keep, g)          # FQF: into agent.fraction_net's arena (fraction_optimiser)
         ctx.keep = None
         # gradients were accumulated straight into the arena behind every parameter's .grad
         return (None,) * (7 + ctx.n_params)

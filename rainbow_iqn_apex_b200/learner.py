@@ -4,6 +4,10 @@
 sample -> loss -> zero_grad -> (weights*loss).mean().backward() -> Adam.step (learner.py:14-26) with the
 backward driven directly (no autograd graph) and the IS weights folded into the upstream gradient
 gscale[b] = weights[b] / B.  ``north_star`` spellings Agent.learn / Agent.update_target are aliased.
+
+Under FQF every step also zeroes, fills, (all-reduces) and steps the fraction proposal's own arena
+(agent.fraction_net, agent.fraction_optimiser).  A user's own loop around ``loss.backward()`` gets the fraction gradients
+from that backward too, and must zero them (fraction_net.zero_grad()) and call fraction_optimiser.step() itself.
 """
 import io
 
@@ -59,7 +63,40 @@ class Learner(Agent):
                 self._dp_tail = None
             else:
                 torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
-        self.optimiser.step()
+            if self.fraction_net is not None:   # FQF: the fraction arena (0.8 MB at N = 64) after the DQN's buckets
+                torch.distributed.all_reduce(self.fraction_net._flat_grad, group=self.process_group)
+        self._step_optimisers()
+
+    def _allreduce_all_grads(self):
+        """Data parallel with the collective outside the captured graphs: every gradient arena, one all-reduce each."""
+        torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
+        if self.fraction_net is not None:
+            torch.distributed.all_reduce(self.fraction_net._flat_grad, group=self.process_group)
+
+    def _optimisers(self):
+        return (self.optimiser,) if self.fraction_optimiser is None else (self.optimiser, self.fraction_optimiser)
+
+    def _step_optimisers(self):
+        for o in self._optimisers():
+            o.step()
+
+    def _advance_steps(self):
+        """A captured step was replayed: advance the host step counters its Adam launches stand for."""
+        for o in self._optimisers():
+            o._step += 1
+
+    def _new_dyn(self, dev):
+        """The step's riqn_dyn_state; under FQF with a second struct for the fraction optimiser's Adam."""
+        from .dynstate import DynState
+        return DynState(dev, slots=1 if self.fraction_optimiser is None else 2)
+
+    def _write_dyn(self, capacity, beta):
+        """Stage the next step's device scalars: the Adam bias corrections of every optimiser, capacity and beta."""
+        nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
+        more = ()
+        if self.fraction_optimiser is not None:
+            more = (self.fraction_optimiser.bias_corrections(self.fraction_optimiser._step + 1),)
+        self._dyn.write(nss, sbc, capacity, beta, *more)
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena.
@@ -78,9 +115,12 @@ class Learner(Agent):
             if getattr(self, "_debug", None) is not None:                       # parity tests: the pass's activations
                 self._debug.update(keep=keep)
             on.zero_grad()                                                      # learner.py:22
+            if self.fraction_net is not None:
+                self.fraction_net.zero_grad()
             on._grads_ready_hook = self._start_tail_allreduce if (self.process_group is not None and self.overlap_allreduce) else None
             on.backward_iqn(keep, dtheta, weights.contiguous(), actions, 1.0 / weights.shape[0])  # learner.py:23 (.mean())
             on._grads_ready_hook = None
+            compute_loss_iqn.fraction_backward(self, keep, weights.contiguous(), 1.0 / weights.shape[0])   # FQF only
         return loss
 
     # ------------------------------------------------------------------ whole step: sample -> learn -> priority update
@@ -90,14 +130,12 @@ class Learner(Agent):
         Replays the captured CUDA graph when enable_cuda_graph(mem) was called.  Returns (tree_idxs, loss); in graph
         mode these are static buffers that the next call overwrites."""
         if self._graph is not None and mem is self._graph_mem:
-            dyn = self._dyn
-            nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-            dyn.write(nss, sbc, mem.transitions.get_current_capacity(), mem.priority_weight)
+            self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
             self._graph.replay()
             if self._graph_post is not None:          # data parallel: the collective stays outside the graphs
-                torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
+                self._allreduce_all_grads()
                 self._graph_post.replay()
-            self.optimiser._step += 1
+            self._advance_steps()
             return self._graph_out
         idxs, loss = self.learn(mem, None)
         mem.update_priorities(idxs, loss)
@@ -111,6 +149,8 @@ class Learner(Agent):
         dyn = self._dyn if on else None
         self._dyn_on = bool(on)
         self.optimiser._dyn = dyn
+        if self.fraction_optimiser is not None:
+            self.fraction_optimiser._dyn = dyn.slot(1) if dyn is not None else None
         if mem is not None:
             mem.transitions._dyn = dyn
         self.online_net.begin_step(dyn)
@@ -131,7 +171,7 @@ class Learner(Agent):
         if allreduce:
             self.apply_gradients()
         else:
-            self.optimiser.step()
+            self._step_optimisers()
         mem.update_priorities(idxs, loss)
 
     def _step_body(self, mem):
@@ -147,23 +187,20 @@ class Learner(Agent):
         overlaps the backward on a side stream inside the graph); capture_collectives=False keeps them eager between two
         graphs (the round-1 scheme)."""
         self._capture_collectives = bool(capture_collectives)
-        from .dynstate import DynState
         dev = self.online_net._flat.device
-        self._dyn = DynState(dev)
+        self._dyn = self._new_dyn(dev)
         self._attach_dyn(mem, True)
-        step0 = self.optimiser._step
+        step0 = [o._step for o in self._optimisers()]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for i in range(warmup):                      # eager warm-up on the capture stream (allocator, attributes)
-                nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-                self._dyn.write(nss, sbc, mem.transitions.get_current_capacity(), mem.priority_weight)
+                self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
                 self._step_body(mem)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
-        nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-        self._dyn.write(nss, sbc, mem.transitions.get_current_capacity(), mem.priority_weight)
+        self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
         self.online_net._static_ops_dirty = True     # the captured step must rebuild the conv / iqn_fc operand images
         post = None
         if self.process_group is None or self._capture_collectives:
@@ -178,7 +215,8 @@ class Learner(Agent):
             with torch.cuda.graph(post, pool=graph.pool()):
                 self._step_post(mem, out[0], out[1], allreduce=False)
         # the capture itself does not execute the step: undo the host-side counter it advanced
-        self.optimiser._step = step0 + warmup
+        for o, s0 in zip(self._optimisers(), step0):
+            o._step = s0 + warmup
         self._graph, self._graph_post, self._graph_mem, self._graph_out = graph, post, mem, out
         self._attach_dyn(mem, False)           # eager calls from here on use their by-value arguments again
         return self
@@ -203,13 +241,12 @@ class Learner(Agent):
             self._step_post(mem, self._bg_in[0], loss)
             return loss
 
-        step0 = self.optimiser._step
+        step0 = [o._step for o in self._optimisers()]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
-                nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-                self._dyn.write(nss, sbc, mem.transitions.get_current_capacity(), mem.priority_weight)
+                self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
                 body()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
@@ -225,7 +262,8 @@ class Learner(Agent):
             post = torch.cuda.CUDAGraph()
             with torch.cuda.graph(post, pool=graph.pool()):
                 self._step_post(mem, self._bg_in[0], out, allreduce=False)
-        self.optimiser._step = step0 + 2
+        for o, s0 in zip(self._optimisers(), step0):
+            o._step = s0 + 2
         self._bgraph, self._bgraph_post, self._bg_out = graph, post, out
         self._attach_dyn(mem, False)
         return self
@@ -235,9 +273,8 @@ class Learner(Agent):
         the actor GPUs' shards (apex.ApexTopology.sample).  ``example`` = (states, actions, returns, next_states,
         nonterminals, weights) device tensors defining the shapes; learn_on_graph(batch) copies a batch into the static
         inputs and replays.  Returns self."""
-        from .dynstate import DynState
         if getattr(self, "_dyn", None) is None:
-            self._dyn = DynState(self.online_net._flat.device)
+            self._dyn = self._new_dyn(self.online_net._flat.device)
         self._lg_in = tuple(t.contiguous().clone() for t in example)
 
         def body():
@@ -248,23 +285,22 @@ class Learner(Agent):
             return loss
 
         self._attach_dyn(None, True)
-        step0 = self.optimiser._step
+        step0 = [o._step for o in self._optimisers()]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
-                nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-                self._dyn.write(nss, sbc, 1.0, 0.0)
+                self._write_dyn(1.0, 0.0)
                 body()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
-        nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-        self._dyn.write(nss, sbc, 1.0, 0.0)
+        self._write_dyn(1.0, 0.0)
         self.online_net._static_ops_dirty = True
         with torch.cuda.graph(graph):
             out = body()
-        self.optimiser._step = step0 + 2
+        for o, s0 in zip(self._optimisers(), step0):
+            o._step = s0 + 2
         self._lgraph, self._lg_out = graph, out
         self._attach_dyn(None, False)
         return self
@@ -274,10 +310,9 @@ class Learner(Agent):
         the per-transition loss (static buffer, overwritten by the next call)."""
         for d, src in zip(self._lg_in, batch):
             d.copy_(src, non_blocking=True)
-        nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-        self._dyn.write(nss, sbc, 1.0, 0.0)
+        self._write_dyn(1.0, 0.0)
         self._lgraph.replay()
-        self.optimiser._step += 1
+        self._advance_steps()
         return self._lg_out
 
     def prefetch_host_batch(self, host_batch):
@@ -318,13 +353,12 @@ class Learner(Agent):
             for d, h in zip(self._bg_in, host_batch):
                 d.copy_(h, non_blocking=True)
         mem = self._graph_mem
-        nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-        self._dyn.write(nss, sbc, mem.transitions.get_current_capacity(), mem.priority_weight)
+        self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
         self._bgraph.replay()
         if self._bgraph_post is not None:
-            torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
+            self._allreduce_all_grads()
             self._bgraph_post.replay()
-        self.optimiser._step += 1
+        self._advance_steps()
         return self._bg_out
 
     def set_risk(self, measure, eta=None):

@@ -734,7 +734,8 @@ class DQN(nn.Module):
     def forward(self, x, num_quantiles=None, log=False, tau=None, keep=None, fresh_weights=False, col_cache=None, feat=None,
                 risk=None):
         """model.py:112-157.  Returns (q, quantiles) in IQN mode.  ``feat`` (B, 3136): trunk output computed by the caller
-        (trunk_pair); only valid for no-grad passes.  ``keep``: dict that receives the backward's operands.  ``risk``:
+        (trunk_pair) for a no-grad pass, or, for a gradient pass, ``self.trunk(x, keep)`` run earlier into the same
+        ``keep`` (FQF proposes fractions on it first).  ``keep``: dict that receives the backward's operands.  ``risk``:
         None or (measure, eta), a distortion risk measure (RISK_MEASURES) under which the drawn fractions are beta(tau); the
         returned quantiles are those distorted fractions.  An explicit ``tau`` is embedded as given and ``risk`` then
         draws nothing."""
@@ -746,7 +747,7 @@ class DQN(nn.Module):
             return c51.forward(self, x, log=log, keep=keep, fresh_weights=fresh_weights)
         if not fresh_weights:
             self._compose_weights()
-        if feat is None or keep is not None:
+        if feat is None or (keep is not None and not _trunk_kept(keep, feat)):
             feat = self.trunk(x, keep, col_cache)
         if tau is None:
             tau = self.draw_quantiles(num_quantiles * x.shape[0], risk)
@@ -910,6 +911,12 @@ class DQN(nn.Module):
                      ptr(gv(conv.weight)), ptr(gv(conv.bias)), ptr(din))
             if i > 0:
                 douts[i - 1] = din
+
+
+def _trunk_kept(keep, feat):
+    """Whether ``keep`` already holds the backward operands of the trunk pass that produced ``feat``."""
+    out = keep.get("out")
+    return out is not None and out[2].data_ptr() == feat.data_ptr() and out[2].numel() == feat.numel()
 
 
 def _grad_views(net, training):

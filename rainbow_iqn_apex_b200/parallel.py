@@ -61,6 +61,9 @@ def make_data_parallel(learner, group=None):
             m._noise_calls = 0
         if net._flat.is_cuda:
             net.compose_weights()
+    if getattr(learner, "fraction_net", None) is not None:        # FQF: the fraction proposal's own arena
+        dist.broadcast(learner.fraction_net._flat, src=0, group=group)
+        learner.fraction_optimiser.grad_scale = 1.0 / world
     learner.process_group = group if group is not None else dist.group.WORLD
     learner.optimiser.grad_scale = 1.0 / world
     return learner
@@ -75,6 +78,8 @@ def publish_parameters(agent, src=0, group=None):
         return
     net = agent.online_net
     dist.broadcast(net._flat, src=src, group=group)
+    if getattr(agent, "fraction_net", None) is not None:          # FQF: actors act on the learner's fractions
+        dist.broadcast(agent.fraction_net._flat, src=src, group=group)
     if dist.get_rank(group) != src and net._flat.is_cuda:
         net.compose_weights()
 
