@@ -9,25 +9,39 @@ Under FQF every step also zeroes, fills, (all-reduces) and steps the fraction pr
 (agent.fraction_net, agent.fraction_optimiser).  A user's own loop around ``loss.backward()`` gets the fraction gradients
 from that backward too, and must zero them (fraction_net.zero_grad()) and call fraction_optimiser.step() itself.
 """
+import contextlib
 import io
+from typing import NamedTuple
 
 import torch
 
 from . import compute_loss_iqn
 from .agent import Agent
+from .dynstate import DynState
 
 MODEL_WEIGHT_STR = "model_weight"      # rainbowiqn/constants.py:18
 STEP_LEARNER_STR = "step_learner:"     # rainbowiqn/constants.py:14
 
 
+class _StepGraph(NamedTuple):
+    """A captured learner step."""
+    graph: object        # torch.cuda.CUDAGraph of the step, or of its part before the all-reduce when that stays eager
+    post: object         # the graph of Adam and the priority update after an eager all-reduce, or None
+    mem: object          # the replay memory whose fill and beta every replay writes into the struct, or None
+    inputs: tuple        # the static input buffers a replay copies its batch into, or None (the step samples them)
+    out: object          # the static outputs, overwritten by every replay
+
+
 class Learner(Agent):
     def __init__(self, args, action_space, redis_servor):
+        self._graphs = {}          # captured step graphs by kind: "replay", "batch", "learn" (Agent.__init__ calls set_risk)
         super().__init__(args, action_space, redis_servor)
         self.process_group = None  # set by parallel.make_data_parallel
         self._dp_stream = self._dp_tail = None
         self.overlap_allreduce = True   # data parallel: start the NoisyLinear-gradient all-reduce inside the backward
-        self._graph = None         # CUDA-graph mode (enable_cuda_graph)
-        self._graph_post = None
+        self.capture_collectives = True  # data parallel: capture the all-reduces in the step graphs (enable_cuda_graph)
+        self._dyn = None           # the riqn_dyn_state every step graph of this learner reads (built at the first capture)
+        self._dyn_on = False       # the struct is attached: a step is being warmed up or captured
 
     def learn(self, mem_redis, mp_queue):
         sample = mem_redis.get_sample_from_mp_queue(mp_queue)
@@ -80,22 +94,14 @@ class Learner(Agent):
         for o in self._optimisers():
             o.step()
 
-    def _advance_steps(self):
-        """A captured step was replayed: advance the host step counters its Adam launches stand for."""
-        for o in self._optimisers():
-            o._step += 1
-
-    def _new_dyn(self, dev):
-        """The step's riqn_dyn_state; under FQF with a second struct for the fraction optimiser's Adam."""
-        from .dynstate import DynState
-        return DynState(dev, slots=1 if self.fraction_optimiser is None else 2)
-
-    def _write_dyn(self, capacity, beta):
-        """Stage the next step's device scalars: the Adam bias corrections of every optimiser, capacity and beta."""
+    def _write_dyn(self, mem):
+        """Stage the next step's device scalars: the Adam bias corrections of every optimiser, and the fill and beta of the
+        replay memory ``mem`` ((1, 0) for a step without one)."""
         nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
         more = ()
         if self.fraction_optimiser is not None:
             more = (self.fraction_optimiser.bias_corrections(self.fraction_optimiser._step + 1),)
+        capacity, beta = (1.0, 0.0) if mem is None else (mem.transitions.get_current_capacity(), mem.priority_weight)
         self._dyn.write(nss, sbc, capacity, beta, *more)
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
@@ -129,55 +135,111 @@ class Learner(Agent):
         ReplayMemory.update_priorities of the sampled leaves (launch_learner.py:173-197 without the host queues).
         Replays the captured CUDA graph when enable_cuda_graph(mem) was called.  Returns (tree_idxs, loss); in graph
         mode these are static buffers that the next call overwrites."""
-        if self._graph is not None and mem is self._graph_mem:
-            self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
-            self._graph.replay()
-            if self._graph_post is not None:          # data parallel: the collective stays outside the graphs
-                self._allreduce_all_grads()
-                self._graph_post.replay()
-            self._advance_steps()
-            return self._graph_out
+        g = self._graphs.get("replay")
+        if g is not None and mem is g.mem:
+            return self._replay(g)
         idxs, loss = self.learn(mem, None)
         mem.update_priorities(idxs, loss)
         return idxs, loss
 
-    def _attach_dyn(self, mem, on):
-        """Route the per-step scalars (Philox offsets, Adam bias corrections, beta / capacity) through the device-resident
-        riqn_dyn_state -- ONLY while a step is being warmed up / captured.  A captured graph keeps the struct's address in its
-        kernel arguments; eager calls made after the capture (learn_and_update on another memory, mem.sample(),
-        optimiser.step(), reset_noise()) must read their by-value arguments again, not the last-written struct."""
-        dyn = self._dyn if on else None
-        self._dyn_on = bool(on)
-        self.optimiser._dyn = dyn
-        if self.fraction_optimiser is not None:
-            self.fraction_optimiser._dyn = dyn.slot(1) if dyn is not None else None
-        if mem is not None:
-            mem.transitions._dyn = dyn
+    def _reset_step_streams(self, mem=None):
+        """Start a step: reset the per-step Philox stream indices of both networks (and of ``mem``'s stratified draws),
+        which read the attached riqn_dyn_state, or their by-value arguments when none is attached."""
+        dyn = self._dyn if self._dyn_on else None
         self.online_net.begin_step(dyn)
         self.target_net.begin_step(dyn)
+        if mem is not None:
+            mem.transitions._draws_in_step = 0
+
+    @contextlib.contextmanager
+    def _attached(self, mem):
+        """Route the per-step scalars (Philox offsets, Adam bias corrections, beta / capacity) through the device-resident
+        riqn_dyn_state -- ONLY while a step is being warmed up / captured.  A captured graph keeps the struct's address in its
+        kernel arguments; eager calls made after the capture, or after a capture that raised (learn_and_update on another
+        memory, mem.sample(), optimiser.step(), reset_noise()), must read their by-value arguments again, not the
+        last-written struct."""
+        def route(dyn):
+            self._dyn_on = dyn is not None
+            self.optimiser._dyn = dyn
+            if self.fraction_optimiser is not None:
+                self.fraction_optimiser._dyn = dyn.slot(1) if dyn is not None else None
+            if mem is not None:
+                mem.transitions._dyn = dyn
+            self._reset_step_streams()
+
+        route(self._dyn)
+        try:
+            yield
+        finally:
+            route(None)
 
     def _step_pre(self, mem):
         """sample -> three forwards -> loss -> backward (gradients in the arena)."""
-        dyn = self._dyn if getattr(self, "_dyn_on", False) else None
-        self.online_net.begin_step(dyn)
-        self.target_net.begin_step(dyn)
-        mem.transitions._draws_in_step = 0
+        self._reset_step_streams(mem)
         idxs, states, actions, returns, next_states, nonterminals, weights = mem.get_sample_from_mp_queue(None)
         loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights)
         return idxs, loss
 
     def _step_post(self, mem, idxs, loss, allreduce=True):
-        """(all-reduce) -> Adam -> priority update."""
+        """(all-reduce) -> Adam -> priority update of ``mem``'s sampled leaves (none without a memory)."""
         if allreduce:
             self.apply_gradients()
         else:
             self._step_optimisers()
-        mem.update_priorities(idxs, loss)
+        if mem is not None:
+            mem.update_priorities(idxs, loss)
 
-    def _step_body(self, mem):
-        idxs, loss = self._step_pre(mem)
-        self._step_post(mem, idxs, loss)
-        return idxs, loss
+    def _capture(self, kind, pre, post, warmup, mem, inputs=None):
+        """Capture one learner step as the graph of ``kind``.  ``pre()`` runs the sample or input copy, the loss and the
+        backward and returns the step's outputs; ``post(out, allreduce)`` runs the (all-reduce and) Adam and the priority
+        update.  ``mem``: the replay memory whose fill and beta the struct carries, or None.  Data parallel with
+        capture_collectives False: pre and post become two graphs, with the all-reduce left eager between them."""
+        if self._dyn is None:      # one struct for every graph of this learner: no captured address can go stale
+            self._dyn = DynState(self.online_net._flat.device, slots=1 if self.fraction_optimiser is None else 2)
+        split = self.process_group is not None and not self.capture_collectives
+        step0 = [o._step for o in self._optimisers()]
+        with self._attached(mem):
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(warmup):                  # eager warm-up on a side stream (allocator, attributes)
+                    self._write_dyn(mem)
+                    post(pre(), True)
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            self._write_dyn(mem)
+            self.online_net._static_ops_dirty = True     # the captured step must rebuild the conv / iqn_fc operand images
+            if split:
+                self.overlap_allreduce = False
+            graph, post_graph = torch.cuda.CUDAGraph(), None
+            with torch.cuda.graph(graph):
+                out = pre()
+                if not split:
+                    post(out, True)
+            if split:
+                post_graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(post_graph, pool=graph.pool()):
+                    post(out, False)
+        # the capture itself does not execute the step: undo the host-side counters it advanced
+        for o, s0 in zip(self._optimisers(), step0):
+            o._step = s0 + warmup
+        self._graphs[kind] = _StepGraph(graph, post_graph, mem, inputs, out)
+
+    def _replay(self, g, batch=None):
+        """One step through the captured graph ``g``: ``batch`` (if given) into its static inputs, the struct written from
+        the memory it was captured on, the replay (with an eager all-reduce: then the collective and the post graph).
+        Returns the static outputs."""
+        if batch is not None:
+            for d, src in zip(g.inputs, batch):
+                d.copy_(src, non_blocking=True)
+        self._write_dyn(g.mem)
+        g.graph.replay()
+        if g.post is not None:
+            self._allreduce_all_grads()
+            g.post.replay()
+        for o in self._optimisers():        # advance the host step counters the replayed Adam launches stand for
+            o._step += 1
+        return g.out
 
     def enable_cuda_graph(self, mem, warmup=3, capture_collectives=True):
         """Capture learn_and_update(mem) in a CUDA graph (shapes are static: batch_size, N, N', K).  Everything that
@@ -185,40 +247,10 @@ class Learner(Agent):
         fill are read from a riqn_dyn_state struct that is refreshed by one 32-byte async copy per step.
         Data parallel: the two NCCL all-reduces are captured too (ONE graph launch per step on every rank; the big bucket
         overlaps the backward on a side stream inside the graph); capture_collectives=False keeps them eager between two
-        graphs (the round-1 scheme)."""
-        self._capture_collectives = bool(capture_collectives)
-        dev = self.online_net._flat.device
-        self._dyn = self._new_dyn(dev)
-        self._attach_dyn(mem, True)
-        step0 = [o._step for o in self._optimisers()]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for i in range(warmup):                      # eager warm-up on the capture stream (allocator, attributes)
-                self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
-                self._step_body(mem)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
-        self.online_net._static_ops_dirty = True     # the captured step must rebuild the conv / iqn_fc operand images
-        post = None
-        if self.process_group is None or self._capture_collectives:
-            with torch.cuda.graph(graph):
-                out = self._step_body(mem)
-        else:
-            # data parallel, eager collective: two graphs around one all-reduce of the whole arena
-            self.overlap_allreduce = False
-            with torch.cuda.graph(graph):
-                out = self._step_pre(mem)
-            post = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(post, pool=graph.pool()):
-                self._step_post(mem, out[0], out[1], allreduce=False)
-        # the capture itself does not execute the step: undo the host-side counter it advanced
-        for o, s0 in zip(self._optimisers(), step0):
-            o._step = s0 + warmup
-        self._graph, self._graph_post, self._graph_mem, self._graph_out = graph, post, mem, out
-        self._attach_dyn(mem, False)           # eager calls from here on use their by-value arguments again
+        graphs, in this capture and in the batch and learn graphs captured after it."""
+        self.capture_collectives = bool(capture_collectives)
+        self._capture("replay", lambda: self._step_pre(mem), lambda out, allreduce: self._step_post(mem, *out, allreduce),
+                      warmup, mem)
         return self
 
     def enable_batch_graph(self, mem, example):
@@ -226,46 +258,16 @@ class Learner(Agent):
         learner.py:16): static device input buffers, filled by async copies from pinned host tensors, then
         learn_on_batch + update_priorities replayed.  ``example`` = (idxs, states, actions, returns, next_states,
         nonterminals, weights) device tensors defining the shapes.  Requires enable_cuda_graph(mem) first."""
-        assert self._graph is not None and mem is self._graph_mem
-        self._bg_in = tuple(t.clone() for t in example)
-        self._attach_dyn(mem, True)
+        g = self._graphs.get("replay")
+        assert g is not None and mem is g.mem
+        inputs = tuple(t.clone() for t in example)
 
         def pre():
-            self.online_net.begin_step(self._dyn)
-            self.target_net.begin_step(self._dyn)
-            idxs, st, ac, rt, nx, nt, w = self._bg_in
-            return self.compute_gradients(st, ac, rt, nx, nt, w)
+            self._reset_step_streams()
+            return self.compute_gradients(*inputs[1:])
 
-        def body():
-            loss = pre()
-            self._step_post(mem, self._bg_in[0], loss)
-            return loss
-
-        step0 = [o._step for o in self._optimisers()]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
-                body()
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        self.online_net._static_ops_dirty = True
-        post = None
-        if self.process_group is None or getattr(self, "_capture_collectives", True):
-            with torch.cuda.graph(graph):
-                out = body()
-        else:
-            with torch.cuda.graph(graph):
-                out = pre()
-            post = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(post, pool=graph.pool()):
-                self._step_post(mem, self._bg_in[0], out, allreduce=False)
-        for o, s0 in zip(self._optimisers(), step0):
-            o._step = s0 + 2
-        self._bgraph, self._bgraph_post, self._bg_out = graph, post, out
-        self._attach_dyn(mem, False)
+        self._capture("batch", pre, lambda loss, allreduce: self._step_post(mem, inputs[0], loss, allreduce), 2, mem,
+                      inputs)
         return self
 
     def enable_learn_graph(self, example):
@@ -273,47 +275,19 @@ class Learner(Agent):
         the actor GPUs' shards (apex.ApexTopology.sample).  ``example`` = (states, actions, returns, next_states,
         nonterminals, weights) device tensors defining the shapes; learn_on_graph(batch) copies a batch into the static
         inputs and replays.  Returns self."""
-        if getattr(self, "_dyn", None) is None:
-            self._dyn = self._new_dyn(self.online_net._flat.device)
-        self._lg_in = tuple(t.contiguous().clone() for t in example)
+        inputs = tuple(t.contiguous().clone() for t in example)
 
-        def body():
-            self.online_net.begin_step(self._dyn)
-            self.target_net.begin_step(self._dyn)
-            loss = self.compute_gradients(*self._lg_in)
-            self.apply_gradients()
-            return loss
+        def pre():
+            self._reset_step_streams()
+            return self.compute_gradients(*inputs)
 
-        self._attach_dyn(None, True)
-        step0 = [o._step for o in self._optimisers()]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self._write_dyn(1.0, 0.0)
-                body()
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        self._write_dyn(1.0, 0.0)
-        self.online_net._static_ops_dirty = True
-        with torch.cuda.graph(graph):
-            out = body()
-        for o, s0 in zip(self._optimisers(), step0):
-            o._step = s0 + 2
-        self._lgraph, self._lg_out = graph, out
-        self._attach_dyn(None, False)
+        self._capture("learn", pre, lambda loss, allreduce: self._step_post(None, None, loss, allreduce), 2, None, inputs)
         return self
 
     def learn_on_graph(self, batch):
         """One learner step on ``batch`` (same shapes as enable_learn_graph's example) through the captured graph; returns
         the per-transition loss (static buffer, overwritten by the next call)."""
-        for d, src in zip(self._lg_in, batch):
-            d.copy_(src, non_blocking=True)
-        self._write_dyn(1.0, 0.0)
-        self._lgraph.replay()
-        self._advance_steps()
-        return self._lg_out
+        return self._replay(self._graphs["learn"], batch)
 
     def prefetch_host_batch(self, host_batch):
         """Start the H2D copy of a FUTURE minibatch on a side stream (double-buffered device staging), so that it
@@ -321,7 +295,7 @@ class Learner(Agent):
         (launch_learner.py:24-50).  The next learn_on_host_batch() consumes it."""
         if not hasattr(self, "_pf_stream"):
             self._pf_stream = torch.cuda.Stream()
-            self._pf_buf = [tuple(torch.empty_like(t) for t in self._bg_in) for _ in range(2)]
+            self._pf_buf = [tuple(torch.empty_like(t) for t in self._graphs["batch"].inputs) for _ in range(2)]
             self._pf_slot, self._pf_event = 0, None
             self._pf_read_done = [None, None]
             self._pf_stream.wait_stream(torch.cuda.current_stream())   # fresh staging memory: order after its last user
@@ -342,39 +316,29 @@ class Learner(Agent):
         """host_batch: pinned host tensors (idxs, states u8, actions, returns, next_states u8, nonterminals, weights),
         or None to consume the batch started by prefetch_host_batch().  H2D copies + one graph replay; returns the
         device loss (B,) (static buffer)."""
+        g = self._graphs["batch"]
         if host_batch is None:
             torch.cuda.current_stream().wait_event(self._pf_event)
-            for d, src in zip(self._bg_in, self._pf_buf[self._pf_slot]):
+            for d, src in zip(g.inputs, self._pf_buf[self._pf_slot]):
                 d.copy_(src, non_blocking=True)                          # device-to-device, 29 MB
             ev = torch.cuda.Event()
             ev.record()
             self._pf_read_done[self._pf_slot] = ev                       # this staging slot may be refilled from here on
-        else:
-            for d, h in zip(self._bg_in, host_batch):
-                d.copy_(h, non_blocking=True)
-        mem = self._graph_mem
-        self._write_dyn(mem.transitions.get_current_capacity(), mem.priority_weight)
-        self._bgraph.replay()
-        if self._bgraph_post is not None:
-            self._allreduce_all_grads()
-            self._bgraph_post.replay()
-        self._advance_steps()
-        return self._bg_out
+        return self._replay(g, host_batch)
 
     def set_risk(self, measure, eta=None):
         """Agent.set_risk.  A captured step graph holds the measure and eta as kernel arguments, so it refuses once one
         is captured: release_graphs(), set the risk, then capture again."""
-        if any(getattr(self, g, None) is not None for g in ("_graph", "_bgraph", "_lgraph")):
+        if self._graphs:
             raise RuntimeError("this learner's step is captured in a CUDA graph that holds the current risk measure: "
                                "call release_graphs(), set the risk, then recapture (enable_cuda_graph / "
                                "enable_batch_graph / enable_learn_graph)")
         super().set_risk(measure, eta)
 
     def release_graphs(self):
-        """Drop every captured step graph; learn_and_update runs eagerly again until the next capture."""
-        self._graph = self._graph_post = self._graph_mem = self._graph_out = None
-        self._bgraph = self._bgraph_post = self._bg_out = None
-        self._lgraph = self._lg_out = None
+        """Drop every captured step graph; learn_and_update runs eagerly again until the next capture.  The device step
+        state stays: the next capture reads the same struct."""
+        self._graphs.clear()
 
     # north_star spellings
     update_target = Agent.update_target_net

@@ -520,7 +520,7 @@ def test_fqf_learner_steps_are_bitwise_reproducible(cuda_dev, graph):
 
 
 @pytest.mark.gpu
-def test_graph_replay_steps_the_fraction_adam_with_its_own_rate(cuda_dev):
+def test_replayed_step_moves_the_fraction_arena_by_one_adam_step_at_its_own_rate(cuda_dev):
     """After a replay, the fraction arena is exactly one Adam step (the fraction optimiser's rate and step count, as the
     dyn struct beside the DQN's carries them) from its state before the replay, on the gradients the replay left."""
     from rainbow_iqn_apex_b200._lib import call, ptr
@@ -528,7 +528,7 @@ def test_graph_replay_steps_the_fraction_adam_with_its_own_rate(cuda_dev):
     _, _, _, lr = _bench_learner(cuda_dev, 1 << 14, True, 1, dict(fqf=1, fqf_fraction_lr=1e-4))
     fo = lr.fraction_optimiser
     p0, m0, v0 = (t.clone() for t in (fo._flat, fo._exp_avg, fo._exp_avg_sq))
-    lr.learn_and_update(lr._graph_mem)
+    lr.learn_and_update(lr._graphs["replay"].mem)
     torch.cuda.synchronize()
     g = lr.fraction_net._flat_grad.clone()
     assert bool(g.abs().sum() > 0)
