@@ -368,12 +368,15 @@ int riqn_argmax_weighted(int batch, int n, int action_space, const float* q, con
  * Rainbow-only (C51) head and loss           replaces rainbowiqn/model.py:120-129, rainbowiqn/agent.py:77-141
  * ---------------------------------------------------------------------------------------------- */
 /* zv (batch, atoms), za (batch, A*atoms) -> q = v + a - mean_a a; p / logp (batch, A, atoms) = (log_)softmax over
- * atoms (either may be NULL); a_star (may be NULL) = argmax_a sum_j support[j] p[b,a,j]  (agent.py:92-99). */
+ * atoms (either may be NULL); a_star (may be NULL) = argmax_a sum_j support[j] p[b,a,j], the first maximal index
+ * winning (agent.py:92-99).  atoms <= 64, else cudaErrorInvalidValue before anything is written. */
 int riqn_c51_head_fwd(int batch, int action_space, int atoms, const float* zv, const float* za, const float* support,
                       float* p, float* logp, long long* a_star, void* stream);
 /* Bellman projection of p_target[b, a_star[b], :] onto the support (agent.py:104-133, incl. the l == u fix),
  * loss[b] = -sum_j m_j logp_online[b, actions[b], j] (agent.py:141) and dq (batch, atoms) = dloss/dq[b, actions[b], :].
- * m_out (batch, atoms) optional. */
+ * The projection index b_j = (clamp(tz_j, v_min, v_max) - v_min) / delta_z is clamped to atoms - 1 as well: fp32
+ * rounding can take it just above (v_min = -1, v_max = 1, 62 atoms), where the reference's index_add_ writes the next
+ * sample's atom 0.  With the clamp sum_j m_j = sum_j p_target[b, a_star[b], j].  m_out (batch, atoms) optional. */
 int riqn_c51_loss_fwd_bwd(int batch, int action_space, int atoms, const float* logp_online, const float* p_target,
                           const long long* actions, const long long* a_star, const float* returns,
                           const float* nonterminals, const float* support, float gamma_n, float v_min, float v_max,
@@ -392,7 +395,8 @@ int riqn_zero_f32(float* p, long n, void* stream);
 /* grad[i] = 0 where act[i] <= 0. */
 int riqn_relu_mask(long n, const float* act, float* grad, void* stream);
 /* Strided fp32 linear-layer helpers for the small z-layers: y = x w^T + bias (optional ReLU); dx = dy w;
- * grad_mu += dy^T x, grad_sigma += (dy^T x) * weight_epsilon. */
+ * grad_mu += dy^T x, grad_sigma += (dy^T x) * weight_epsilon (split-K partials added in split order, no atomics:
+ * bitwise reproducible). */
 int riqn_linear_fwd_ld(long rows, int in_features, int out_features, const float* x, long ldx, const float* w,
                        const float* bias, float* y, long ldy, int relu, void* stream);
 int riqn_linear_dgrad_ld(long rows, int in_features, int out_features, const float* dy, long lddy, const float* w,

@@ -64,6 +64,30 @@ def iqn_loss(p_online, p_target, states, actions, returns, next_states, nontermi
     return loss
 
 
+def c51_projection(pns_a, returns, nonterminals, *, atoms=51, v_min=-10.0, v_max=10.0, gamma_n=0.99 ** 3):
+    """Bellman projection of the target distributions pns_a (batch, atoms) onto the support.   agent.py:105-133
+
+    Departs from the reference in one place: the index b is clamped to atoms - 1.  Clamping tz to [v_min, v_max] does
+    not bound b = (tz - v_min) / delta_z in fp32 (v_min = -1, v_max = 1, 62 atoms: tz = v_max gives b = 61.0000038),
+    and there the reference's u = atoms makes index_add_ put the mass on the next sample's atom 0, or out of range
+    for the last sample.  Every b <= atoms - 1 is unchanged.
+    """
+    batch = pns_a.shape[0]
+    support = torch.linspace(v_min, v_max, atoms)
+    delta_z = (v_max - v_min) / (atoms - 1)
+    tz = returns.unsqueeze(1) + nonterminals.unsqueeze(1) * gamma_n * support.unsqueeze(0)
+    tz = tz.clamp(min=v_min, max=v_max)
+    b = ((tz - v_min) / delta_z).clamp(max=atoms - 1)
+    lo, up = b.floor().to(torch.int64), b.ceil().to(torch.int64)
+    lo[(up > 0) * (lo == up)] -= 1            # agent.py:119
+    up[(lo < (atoms - 1)) * (lo == up)] += 1  # agent.py:120
+    m = pns_a.new_zeros(batch, atoms)
+    offset = (torch.arange(batch) * atoms)[:, None].expand(batch, atoms)
+    m.view(-1).index_add_(0, (lo + offset).view(-1), (pns_a * (up.float() - b)).view(-1))
+    m.view(-1).index_add_(0, (up + offset).view(-1), (pns_a * (b - lo.float())).view(-1))
+    return m
+
+
 def c51_loss(p_online, p_target, states, actions, returns, next_states, nonterminals, noises, *,
              atoms=51, v_min=-10.0, v_max=10.0, discount=0.99, n_step=3, keep=None):
     """Categorical (C51) double-DQN n-step loss.                      agent.py:77-141
@@ -73,7 +97,6 @@ def c51_loss(p_online, p_target, states, actions, returns, next_states, nontermi
     batch = states.shape[0]
     acts = p_online["fcnoisy_z_a.bias_mu"].shape[0] // atoms
     support = torch.linspace(v_min, v_max, atoms)
-    delta_z = (v_max - v_min) / (atoms - 1)
     net.apply_noise(p_online, noises[0])
     log_ps = net.dqn_forward_c51(p_online, states, acts, atoms, log=True)
     log_ps_a = log_ps[range(batch), actions]
@@ -83,16 +106,8 @@ def c51_loss(p_online, p_target, states, actions, returns, next_states, nontermi
         a_star = (support.expand_as(pns) * pns).sum(2).argmax(1)
         net.apply_noise(p_target, noises[2])
         pns_a = net.dqn_forward_c51(p_target, next_states, acts, atoms)[range(batch), a_star]
-        tz = returns.unsqueeze(1) + nonterminals.unsqueeze(1) * (discount ** n_step) * support.unsqueeze(0)
-        tz = tz.clamp(min=v_min, max=v_max)
-        b = (tz - v_min) / delta_z
-        lo, up = b.floor().to(torch.int64), b.ceil().to(torch.int64)
-        lo[(up > 0) * (lo == up)] -= 1            # agent.py:119
-        up[(lo < (atoms - 1)) * (lo == up)] += 1  # agent.py:120
-        m = states.new_zeros(batch, atoms)
-        offset = (torch.arange(batch) * atoms)[:, None].expand(batch, atoms)
-        m.view(-1).index_add_(0, (lo + offset).view(-1), (pns_a * (up.float() - b)).view(-1))
-        m.view(-1).index_add_(0, (up + offset).view(-1), (pns_a * (b - lo.float())).view(-1))
+        m = c51_projection(pns_a, returns, nonterminals, atoms=atoms, v_min=v_min, v_max=v_max,
+                           gamma_n=discount ** n_step)
     loss = -(m * log_ps_a).sum(1)
     if keep is not None:
         keep.update(a_star=a_star, m=m, log_ps_a=log_ps_a)

@@ -80,7 +80,10 @@ __global__ void c51_loss_kernel(int A, int atoms, const float* __restrict__ logp
   for (int j = threadIdx.x; j < atoms; j += blockDim.x) {
     float tz = __fadd_rn(returns[b], __fmul_rn(g, support[j]));
     tz = fminf(fmaxf(tz, vmin), vmax);
-    const float bj = __fdiv_rn(__fsub_rn(tz, vmin), delta_z);
+    // The clamp of tz does not bound the index: fp32 rounding of the division can take bj just above atoms - 1
+    // (v_min = -1, v_max = 1, 62 atoms: tz = v_max gives 61.0000038), and u = atoms would add wu past m.  Every
+    // bj <= atoms - 1 is unchanged.  (The reference's index_add_ lands on the next sample's atom 0 instead.)
+    const float bj = fminf(__fdiv_rn(__fsub_rn(tz, vmin), delta_z), (float)(atoms - 1));
     int l = (int)floorf(bj), u = (int)ceilf(bj);
     if (u > 0 && l == u) l -= 1;                   // agent.py:119
     if (l < atoms - 1 && l == u) u += 1;           // agent.py:120
@@ -164,6 +167,17 @@ __global__ void c51_head_bwd_dense_kernel(int A, int atoms, const float* __restr
     dza[(long)b * A * atoms + i] = sdq[i] - dv[i % atoms] / (float)A;
 }
 
+// grad_mu += s ; grad_sigma += s * eps with s = the split-K partials of dy^T x added in split order
+__global__ void noisy_wgrad_finish_kernel(int splits, long n, const float* __restrict__ part, const float* __restrict__ eps,
+                                          float* __restrict__ grad_mu, float* __restrict__ grad_sigma) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float acc = part[i];
+  for (int k = 1; k < splits; ++k) acc += part[(long)k * n + i];
+  grad_mu[i] += acc;
+  grad_sigma[i] += __fmul_rn(acc, eps[i]);
+}
+
 __global__ void relu_mask_kernel(long n, const float* __restrict__ act, float* __restrict__ grad) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && !(act[i] > 0.f)) grad[i] = 0.f;
@@ -237,16 +251,31 @@ RIQN_API int riqn_linear_dgrad_ld(long rows, int in_features, int out_features, 
                   (cudaStream_t)stream);
 }
 
-// grad_mu (out, in) += dy^T x ; grad_sigma += (dy^T x) * eps_w
+// grad_mu (out, in) += dy^T x ; grad_sigma += (dy^T x) * eps_w.  Split-K over the rows (at least 64 per split) to fill
+// the SMs; every split stores its partial product in its own scratch slab and noisy_wgrad_finish_kernel adds the slabs
+// in split order, so the result does not depend on which split finishes first.  One split accumulates in the epilogue.
 RIQN_API int riqn_noisy_wgrad_ld(long rows, int in_features, int out_features, const float* dy, long lddy, const float* x,
                                  long ldx, const float* weight_epsilon, float* grad_mu, float* grad_sigma, void* stream) {
-  riqn::note_launches(1);
+  cudaStream_t s = (cudaStream_t)stream;
   EpiArgs e;
-  e.out2 = grad_sigma;
-  e.eps = weight_epsilon;
   const int tiles = ((out_features + 127) / 128) * ((in_features + 127) / 128);
   int split = (riqn_sms() + tiles - 1) / tiles;
   if ((long)split * 64 > rows) split = (int)((rows + 63) / 64);
-  return gemm_f32(out_features, in_features, (int)rows, dy, 1, lddy, x, 1, ldx, grad_mu, in_features, EPI_NOISY_WGRAD, e, split,
-                  (cudaStream_t)stream);
+  const int splits = gemm_f32_splits((int)rows, split);
+  if (splits <= 1) {
+    riqn::note_launches(1);
+    e.out2 = grad_sigma;
+    e.eps = weight_epsilon;
+    return gemm_f32(out_features, in_features, (int)rows, dy, 1, lddy, x, 1, ldx, grad_mu, in_features, EPI_NOISY_WGRAD, e,
+                    1, s);
+  }
+  riqn::note_launches(2);
+  const long n = (long)out_features * in_features;
+  StreamScratch part;
+  RIQN_CUDA(part.alloc((size_t)splits * n, s));
+  e.slab = n;
+  int rc = gemm_f32(out_features, in_features, (int)rows, dy, 1, lddy, x, 1, ldx, part.p, in_features, EPI_SLAB, e, split, s);
+  if (rc) return rc;
+  noisy_wgrad_finish_kernel<<<riqn_cdiv(n, 256), 256, 0, s>>>(splits, n, part.p, weight_epsilon, grad_mu, grad_sigma);
+  return (int)cudaGetLastError();
 }

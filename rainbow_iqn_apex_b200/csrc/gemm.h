@@ -14,8 +14,9 @@ enum Epi {
   EPI_BIAS_RELU_NCHW = 2,  // m = b*ohw + p ; C[(b*N + n)*ohw + p] = relu(acc + bias[n])
   EPI_EMBED = 3,           // C = feat[(m / batch)*N + n] * relu(acc + bias[n]), batch = rows per sample (model.py:146-151)
   EPI_ATOMIC = 4,          // C += alpha*acc (atomicAdd; split-K capable)
-  EPI_NOISY_WGRAD = 5,     // C += acc ; out2 += acc * eps[m,n]  (dL/dmu, dL/dsigma of NoisyLinear)
+  EPI_NOISY_WGRAD = 5,     // C += acc ; out2 += acc * eps[m,n]  (dL/dmu, dL/dsigma of NoisyLinear; split 1 only)
   EPI_BIAS = 6,            // C = acc + bias[n]
+  EPI_SLAB = 7,            // C[z * slab + m*ldc + n] = acc of split z (split-K partials, summed by the caller in split order)
 };
 
 struct EpiArgs {
@@ -26,9 +27,13 @@ struct EpiArgs {
   float* out2 = nullptr;
   const float* eps = nullptr;
   float alpha = 1.0f;
+  long slab = 0;
 };
 
-// fp32 CUDA-core GEMM with arbitrary operand strides.  Returns a cudaError_t as int.
+// fp32 CUDA-core GEMM with arbitrary operand strides.  Returns a cudaError_t as int.  split_k > 1 (EPI_ATOMIC, EPI_SLAB
+// only) cuts K into gemm_f32_splits(K, split_k) chunks of gemm_f32_kchunk(K, split_k), one grid z-slice each.
+int gemm_f32_kchunk(int K, int split_k);
+int gemm_f32_splits(int K, int split_k);
 int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,
              float* C, long ldc, int epi, const EpiArgs& e, int split_k, cudaStream_t stream);
 

@@ -27,9 +27,11 @@ __device__ __forceinline__ void epi_one(float v, int m, int n, int N, float* __r
     C[(long)m * ldc + n] = e.feat[(long)(m / e.batch) * N + n] * fmaxf(v + e.bias[n], 0.f);
   } else if (EPI == EPI_ATOMIC) {
     atomicAdd(&C[(long)m * ldc + n], e.alpha * v);
-  } else if (EPI == EPI_NOISY_WGRAD) {
-    atomicAdd(&C[(long)m * ldc + n], v);
-    atomicAdd(&e.out2[(long)m * ldc + n], v * e.eps[(long)m * ldc + n]);
+  } else if (EPI == EPI_NOISY_WGRAD) {        // split 1 only: one block owns the element
+    C[(long)m * ldc + n] += v;
+    e.out2[(long)m * ldc + n] += __fmul_rn(v, e.eps[(long)m * ldc + n]);
+  } else if (EPI == EPI_SLAB) {
+    C[(long)m * ldc + n] = v;
   }
 }
 
@@ -107,7 +109,8 @@ gemm_simt_kernel(int M, int N, int K, const float* __restrict__ A, long sAm, lon
     buf ^= 1;
   }
 
-  const bool vec_ok = (EPI == EPI_STORE || EPI == EPI_BIAS_RELU || EPI == EPI_EMBED || EPI == EPI_BIAS) &&
+  if (EPI == EPI_SLAB) C += (long)blockIdx.z * e.slab;
+  const bool vec_ok = (EPI == EPI_STORE || EPI == EPI_BIAS_RELU || EPI == EPI_EMBED || EPI == EPI_BIAS || EPI == EPI_SLAB) &&
                       ((ldc & 3) == 0) && ((N & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -121,7 +124,7 @@ gemm_simt_kernel(int M, int N, int K, const float* __restrict__ A, long sAm, lon
         float4 v = make_float4(acc[i][jh * 4 + 0], acc[i][jh * 4 + 1], acc[i][jh * 4 + 2], acc[i][jh * 4 + 3]);
         if (EPI == EPI_STORE) {
           v.x *= e.alpha; v.y *= e.alpha; v.z *= e.alpha; v.w *= e.alpha;
-        } else {
+        } else if (EPI != EPI_SLAB) {
           const float4 bb = *reinterpret_cast<const float4*>(&e.bias[n]);
           v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
           if (EPI != EPI_BIAS) {
@@ -145,11 +148,8 @@ gemm_simt_kernel(int M, int N, int K, const float* __restrict__ A, long sAm, lon
 template <int EPI>
 static int launch_epi(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,
                       float* C, long ldc, const EpiArgs& e, int split_k, cudaStream_t s) {
-  if (split_k < 1) split_k = 1;
-  int kchunk = (K + split_k - 1) / split_k;
-  kchunk = ((kchunk + BK - 1) / BK) * BK;
-  split_k = (K + kchunk - 1) / kchunk;
-  if (split_k < 1) split_k = 1;
+  const int kchunk = gemm_f32_kchunk(K, split_k);
+  split_k = gemm_f32_splits(K, split_k);
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, split_k);
   const bool akc = (sAk == 1), bkc = (sBk == 1);
 #define RIQN_GEMM_GO(AK_, BK_) \
@@ -162,10 +162,24 @@ static int launch_epi(int M, int N, int K, const float* A, long sAm, long sAk, c
   return (int)cudaGetLastError();
 }
 
+// Rows of K per split: ceil(K / split_k) rounded up to whole k-slabs, so the last split may be shorter or empty.
+int gemm_f32_kchunk(int K, int split_k) {
+  if (split_k < 1) split_k = 1;
+  const int kchunk = (K + split_k - 1) / split_k;
+  return kchunk < BK ? BK : ((kchunk + BK - 1) / BK) * BK;
+}
+
+// Non-empty splits of that cut (<= split_k).
+int gemm_f32_splits(int K, int split_k) {
+  const int kchunk = gemm_f32_kchunk(K, split_k);
+  const int s = (K + kchunk - 1) / kchunk;
+  return s < 1 ? 1 : s;
+}
+
 int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,
              float* C, long ldc, int epi, const EpiArgs& e, int split_k, cudaStream_t s) {
   if (M <= 0 || N <= 0) return 0;
-  if (split_k > 1 && epi != EPI_ATOMIC && epi != EPI_NOISY_WGRAD) return (int)cudaErrorInvalidValue;
+  if (split_k > 1 && epi != EPI_ATOMIC && epi != EPI_SLAB) return (int)cudaErrorInvalidValue;
   switch (epi) {
     case EPI_STORE: return launch_epi<EPI_STORE>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_BIAS: return launch_epi<EPI_BIAS>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
@@ -174,6 +188,7 @@ int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const floa
     case EPI_EMBED: return launch_epi<EPI_EMBED>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_ATOMIC: return launch_epi<EPI_ATOMIC>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_NOISY_WGRAD: return launch_epi<EPI_NOISY_WGRAD>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
+    case EPI_SLAB: return launch_epi<EPI_SLAB>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
   }
   return (int)cudaErrorInvalidValue;
 }

@@ -12,7 +12,7 @@ Method:
 * random regime: Gaussian inputs with ReLU zeros; each element is held to c * K * 2^-24 * sum|a_i b_i| (K = the
   reduction length) plus the output rounding, and each test prints its worst err/bound ratio;
 * where the kernel's value is one correctly rounded fp32 operation (or a chain without a multiply feeding an add: the
-  library builds with FMA contraction on) it is asserted bit for bit through the numpy rounding helpers below;
+  library builds with FMA contraction on) it is asserted bit for bit through the rounding helpers of helpers.py;
 * overwritten outputs start as NaN, accumulated outputs start from a known non-zero pattern, and every output buffer
   carries canaries past its end that must survive.
 """
@@ -20,117 +20,11 @@ import numpy as np
 import pytest
 import torch
 
-U = 2.0 ** -24          # unit roundoff of fp32
+from helpers import (U, Out, assert_bits, assert_canaries, bf16, bf16_bits, check_bound, dptr, f16_bits, f32_bits,
+                     lib_call, prefill_pattern, to_dev, to_dev_bf16)
+
 C_BOUND = 2.0           # the constant c of the random-regime bounds
-PAD = 512               # canary elements past the end of every output buffer
-CANARY = -77.0          # exact in fp32, bf16 and fp16
 HID = 512
-
-
-# ---------------------------------------------------------------------------------------------- rounding helpers
-def bf16_bits(x):
-    """float32 -> bf16 bit patterns, round to nearest even (finite inputs)."""
-    u = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
-    return ((u + (((u >> 16) & 1) + np.uint32(0x7FFF))) >> 16).astype(np.uint16)
-
-
-def bf16(x):
-    """float32 values rounded to bf16 (returned as float32)."""
-    return (bf16_bits(x).astype(np.uint32) << 16).view(np.float32)
-
-
-def f16_bits(x):
-    """float32 -> fp16 bit patterns, round to nearest even (overflow -> inf, as the device conversion)."""
-    with np.errstate(over="ignore"):
-        return np.ascontiguousarray(x, dtype=np.float32).astype(np.float16).view(np.uint16)
-
-
-def f32_bits(x):
-    return np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
-
-
-# ---------------------------------------------------------------------------------------------- device helpers
-def _call(name, *args):
-    from rainbow_iqn_apex_b200._lib import call
-    call(name, *args)
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _dev(a, dev, dtype=torch.float32):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dtype)
-
-
-def _dev_bf16(x, dev):
-    """Device bf16 tensor holding bf16(x) (x float32)."""
-    return torch.from_numpy(bf16_bits(x).view(np.int16)).to(dev).view(torch.bfloat16)
-
-
-class Out:
-    """A flat output buffer of n elements followed by PAD canaries."""
-
-    def __init__(self, n, dev, dtype=torch.float32, fill=float("nan")):
-        self.n = n
-        self.t = torch.full((n + PAD,), CANARY, dtype=dtype, device=dev)
-        if isinstance(fill, np.ndarray):
-            self.t[:n] = torch.from_numpy(np.ascontiguousarray(fill, np.float32).ravel()).to(dev, dtype)
-        else:
-            self.t[:n].fill_(fill)
-
-    @property
-    def p(self):
-        return self.t.data_ptr()
-
-    def canaries_ok(self):
-        return bool(torch.all(self.t[self.n:] == CANARY))
-
-    def f32(self):
-        return self.t[:self.n].float().cpu().numpy()
-
-    def bits(self):
-        """bit patterns of the body: uint16 for 16-bit buffers, uint32 for fp32"""
-        body = self.t[:self.n]
-        if body.element_size() == 2:
-            return body.view(torch.int16).cpu().numpy().view(np.uint16)
-        return body.view(torch.int32).cpu().numpy().view(np.uint32)
-
-
-def _assert_canaries(outs):
-    bad = [k for k, o in outs.items() if o is not None and not o.canaries_ok()]
-    assert not bad, f"writes past the end of {bad}"
-
-
-def _check_bound(what, got, ref, bound):
-    """|got - ref| <= bound elementwise; prints and returns the worst err/bound ratio."""
-    got = np.asarray(got, np.float64)
-    ref = np.asarray(ref, np.float64)
-    assert np.all(np.isfinite(got)), f"{what}: non-finite values"
-    err = np.abs(got - ref)
-    bound = np.asarray(bound, np.float64) + 1e-300
-    ratio = err / bound
-    worst = float(ratio.max()) if ratio.size else 0.0
-    print(f"{what}: worst err/bound {worst:.3g}")
-    if worst > 1.0:
-        i = np.unravel_index(int(np.argmax(ratio)), ratio.shape)
-        raise AssertionError(f"{what}: at {i} got {got[i]!r} ref {ref[i]!r} bound {bound[i]!r}")
-    return worst
-
-
-def _assert_bits(what, got, want):
-    got, want = np.asarray(got), np.asarray(want)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    bad = got != want
-    if bad.any():
-        i = np.argwhere(bad)[0]
-        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.size} elements differ, first at {tuple(i)}: "
-                             f"got {got[tuple(i)]:#x} want {want[tuple(i)]:#x}")
-
-
-def _pattern(n, scale=0.25, mod=13):
-    """A non-zero prefill for accumulated outputs, exact in fp32."""
-    return (((np.arange(n) % mod) - mod // 2) * scale + scale / 2).astype(np.float32)
 
 
 # ---------------------------------------------------------------------------------------------- helpers without a GPU
@@ -152,8 +46,8 @@ def test_bf16_helper_matches_torch():
     rs = np.random.RandomState(0)
     r = rs.randint(0, 2 ** 32, 200000, dtype=np.uint64).astype(np.uint32).view(np.float32)
     x = np.concatenate([x, r[np.isfinite(r)], rs.standard_normal(10000).astype(np.float32)])
-    _assert_bits("bf16 bits", bf16_bits(x), _torch_bits(x, torch.bfloat16))
-    _assert_bits("bf16 values", f32_bits(bf16(x)), f32_bits(torch.from_numpy(x).to(torch.bfloat16).float().numpy()))
+    assert_bits("bf16 bits", bf16_bits(x), _torch_bits(x, torch.bfloat16))
+    assert_bits("bf16 values", f32_bits(bf16(x)), f32_bits(torch.from_numpy(x).to(torch.bfloat16).float().numpy()))
 
 
 def test_fp16_helper_matches_torch():
@@ -162,7 +56,7 @@ def test_fp16_helper_matches_torch():
     rs = np.random.RandomState(1)
     x = np.concatenate([_special_f32([0x7F800000], h), rs.standard_normal(100000).astype(np.float32) * 100,
                         rs.standard_normal(100000).astype(np.float32) * 1e-5])
-    _assert_bits("fp16 bits", f16_bits(x), _torch_bits(x, torch.float16))
+    assert_bits("fp16 bits", f16_bits(x), _torch_bits(x, torch.float16))
 
 
 def test_rounding_helpers_keep_signed_zero():
@@ -204,11 +98,11 @@ def _embed_fwd_call(dev, B, Nq, F, E, mode, inp, x32=True):
         "x_lo_t": Out(F * R, dev, torch.bfloat16) if trans else None,
     }
     p = {k: (v.p if v is not None else None) for k, v in o.items()}
-    _call("riqn_quantile_embed_fwd_tc", B, Nq, E, F, _ptr(inp["tau"]), _ptr(inp["feat"]), _ptr(inp["w_hi"]),
-          _ptr(inp["w_lo"]), _ptr(inp["be"]), p["cos_hi"], p["cos_lo"], p["cos_t_hi"], p["x32"], p["x_hi"], p["x_lo"],
+    lib_call("riqn_quantile_embed_fwd_tc", B, Nq, E, F, dptr(inp["tau"]), dptr(inp["feat"]), dptr(inp["w_hi"]),
+          dptr(inp["w_lo"]), dptr(inp["be"]), p["cos_hi"], p["cos_lo"], p["cos_t_hi"], p["x32"], p["x_hi"], p["x_lo"],
           p["x_hi_t"], p["x_lo_t"], int(f16))
     torch.cuda.synchronize()
-    _assert_canaries(o)
+    assert_canaries(o)
     return o
 
 
@@ -226,8 +120,8 @@ def _embed_fwd_inputs(dev, B, Nq, F, E, seed, zero_weight=False):
     w_hi = bf16(w)
     w_lo = bf16(w - w_hi)
     host = dict(tau=tau, feat=feat, w=w, w_hi=w_hi, w_lo=w_lo, be=be)
-    inp = dict(tau=_dev(tau, dev), feat=_dev(feat, dev), w=_dev(w, dev), w_hi=_dev_bf16(w_hi, dev),
-               w_lo=_dev_bf16(w_lo, dev), be=_dev(be, dev))
+    inp = dict(tau=to_dev(tau, dev), feat=to_dev(feat, dev), w=to_dev(w, dev), w_hi=to_dev_bf16(w_hi, dev),
+               w_lo=to_dev_bf16(w_lo, dev), be=to_dev(be, dev))
     return host, inp
 
 
@@ -251,9 +145,9 @@ def _check_embed_fwd(dev, B, Nq, F, E, mode, seed):
     # CUDA's cosf: 2 ulp (CUDA C Programming Guide, maths functions); a bf16 rounding (of c, or of the residual c - hi
     # into lo) is off by at most half an ulp of its 8-bit significand, 2^-8 of the value
     cos_bound = 2 * sp + (2.0 ** -8 * np.abs(c64 - ch) if split else 2.0 ** -8 * np.abs(c64)) + sp
-    _check_bound(f"cos images {mode}", ch.astype(np.float64) + cl, c64, cos_bound)
+    check_bound(f"cos images {mode}", ch.astype(np.float64) + cl, c64, cos_bound)
     if o["cos_t_hi"] is not None:
-        _assert_bits("cos_t_hi", o["cos_t_hi"].bits().reshape(E, R), o["cos_hi"].bits().reshape(R, E).T)
+        assert_bits("cos_t_hi", o["cos_t_hi"].bits().reshape(E, R), o["cos_hi"].bits().reshape(R, E).T)
     # x32 against feat[r // Nq] * relu(cos W_e^T + b_e) on the kernel's own cos images
     x32 = o["x32"].f32().reshape(R, F)
     rows = _check_rows(R, seed)
@@ -268,29 +162,29 @@ def _check_embed_fwd(dev, B, Nq, F, E, mode, seed):
         k = 3 * E + 2
     fr = host["feat"][rows // Nq].astype(np.float64)
     ref = fr * np.maximum(pre, 0)
-    _check_bound(f"x32 {mode}", x32[rows], ref, C_BOUND * k * U * mag * fr + U * np.abs(ref))
+    check_bound(f"x32 {mode}", x32[rows], ref, C_BOUND * k * U * mag * fr + U * np.abs(ref))
     # the 16-bit images bit for bit from x32
     if mode.startswith("fp16"):
-        _assert_bits("x_hi = fp16(x)", o["x_hi"].bits().reshape(R, F), f16_bits(x32))
+        assert_bits("x_hi = fp16(x)", o["x_hi"].bits().reshape(R, F), f16_bits(x32))
         if o["x_lo"] is not None:
-            _assert_bits("x_lo = bf16(x)", o["x_lo"].bits().reshape(R, F), bf16_bits(x32))
+            assert_bits("x_lo = bf16(x)", o["x_lo"].bits().reshape(R, F), bf16_bits(x32))
     else:
         hi = bf16(x32)
-        _assert_bits("x_hi = bf16(x)", o["x_hi"].bits().reshape(R, F), bf16_bits(x32))
-        _assert_bits("x_lo = bf16(x - hi)", o["x_lo"].bits().reshape(R, F), bf16_bits(x32 - hi))
+        assert_bits("x_hi = bf16(x)", o["x_hi"].bits().reshape(R, F), bf16_bits(x32))
+        assert_bits("x_lo = bf16(x - hi)", o["x_lo"].bits().reshape(R, F), bf16_bits(x32 - hi))
     if o["x_hi_t"] is not None:
-        _assert_bits("x_hi_t", o["x_hi_t"].bits().reshape(F, R), o["x_hi"].bits().reshape(R, F).T)
-        _assert_bits("x_lo_t", o["x_lo_t"].bits().reshape(F, R), o["x_lo"].bits().reshape(R, F).T)
+        assert_bits("x_hi_t", o["x_hi_t"].bits().reshape(F, R), o["x_hi"].bits().reshape(R, F).T)
+        assert_bits("x_lo_t", o["x_lo_t"].bits().reshape(F, R), o["x_lo"].bits().reshape(R, F).T)
     # determinism, and the same images without the fp32 matrix
     o2 = _embed_fwd_call(dev, B, Nq, F, E, mode, inp)
     for key, v in o.items():
         if v is not None:
-            _assert_bits(f"second call {key}", o2[key].bits(), v.bits())
+            assert_bits(f"second call {key}", o2[key].bits(), v.bits())
     if mode != "bf16x3-transposed":
         o3 = _embed_fwd_call(dev, B, Nq, F, E, mode, inp, x32=False)
         for key in ("cos_hi", "cos_lo", "cos_t_hi", "x_hi", "x_lo"):
             if o[key] is not None:
-                _assert_bits(f"x32 = NULL {key}", o3[key].bits(), o[key].bits())
+                assert_bits(f"x32 = NULL {key}", o3[key].bits(), o[key].bits())
 
 
 @pytest.mark.gpu
@@ -315,7 +209,7 @@ def test_embed_fwd_tc_rows_read_their_sample(cuda_dev, Nq, mode):
     B, F, E = 6, 96, 64
     host, inp = _embed_fwd_inputs(cuda_dev, B, Nq, F, E, seed=Nq, zero_weight=True)
     o = _embed_fwd_call(cuda_dev, B, Nq, F, E, mode, inp)
-    _assert_bits("x32 == feat[r // Nq]", f32_bits(o["x32"].f32().reshape(B * Nq, F)),
+    assert_bits("x32 == feat[r // Nq]", f32_bits(o["x32"].f32().reshape(B * Nq, F)),
                  f32_bits(np.repeat(host["feat"], Nq, axis=0)))
 
 
@@ -332,10 +226,10 @@ def test_embed_fwd_tc_rejects_before_writing(cuda_dev):
     for B, Nq, F, E, f16, with_x32, trans, shifted in cases:
         R = B * Nq
         rs = np.random.RandomState(R)
-        tau = _dev(rs.uniform(0, 1, R).astype(np.float32), dev)
-        feat = _dev(np.abs(rs.standard_normal((B, F))).astype(np.float32), dev)
-        w = _dev_bf16(rs.standard_normal((F, E)).astype(np.float32), dev)
-        be = _dev(rs.standard_normal(F).astype(np.float32), dev)
+        tau = to_dev(rs.uniform(0, 1, R).astype(np.float32), dev)
+        feat = to_dev(np.abs(rs.standard_normal((B, F))).astype(np.float32), dev)
+        w = to_dev_bf16(rs.standard_normal((F, E)).astype(np.float32), dev)
+        be = to_dev(rs.standard_normal(F).astype(np.float32), dev)
         o = {"cos_hi": Out(R * E, dev, torch.bfloat16), "cos_lo": Out(R * E, dev, torch.bfloat16),
              "cos_t_hi": Out(E * R, dev, torch.bfloat16), "x32": Out(R * F, dev) if with_x32 else None,
              "x_hi": Out(R * F, dev, torch.float16 if f16 else torch.bfloat16),
@@ -346,10 +240,10 @@ def test_embed_fwd_tc_rejects_before_writing(cuda_dev):
         if shifted:
             p[shifted] += 2
         with pytest.raises(RiqnError):
-            _call("riqn_quantile_embed_fwd_tc", B, Nq, E, F, _ptr(tau), _ptr(feat), _ptr(w), _ptr(w), _ptr(be),
+            lib_call("riqn_quantile_embed_fwd_tc", B, Nq, E, F, dptr(tau), dptr(feat), dptr(w), dptr(w), dptr(be),
                   p["cos_hi"], p["cos_lo"], p["cos_t_hi"], p["x32"], p["x_hi"], p["x_lo"], p["x_hi_t"], p["x_lo_t"], f16)
         torch.cuda.synchronize()
-        _assert_canaries(o)
+        assert_canaries(o)
         for k, v in o.items():
             if v is not None:
                 assert torch.isnan(v.t[:v.n].float()).all(), f"rejected call {(B, Nq, F, E, f16, with_x32, trans, shifted)} wrote {k}"
@@ -394,10 +288,10 @@ def _embed_bwd_call(dev, B, Nq, F, E, dxb, d, pre_w, pre_b):
     R = B * Nq
     o = {"dpre": Out(R * F, dev, torch.bfloat16), "dfeat": Out(B * F, dev), "grad_w": Out(F * E, dev, fill=pre_w),
          "grad_b": Out(F, dev, fill=pre_b)}
-    _call("riqn_quantile_embed_bwd_tc", B, Nq, E, F, _ptr(d["x_hi"]), _ptr(d["x_lo"]), _ptr(d["feat"]), _ptr(d["cos"]),
-          _ptr(d["dx"]), int(dxb), o["dpre"].p, o["dfeat"].p, o["grad_w"].p, o["grad_b"].p)
+    lib_call("riqn_quantile_embed_bwd_tc", B, Nq, E, F, dptr(d["x_hi"]), dptr(d["x_lo"]), dptr(d["feat"]), dptr(d["cos"]),
+          dptr(d["dx"]), int(dxb), o["dpre"].p, o["dfeat"].p, o["grad_w"].p, o["grad_b"].p)
     torch.cuda.synchronize()
-    _assert_canaries(o)
+    assert_canaries(o)
     return o
 
 
@@ -411,16 +305,16 @@ def test_embed_bwd_tc(cuda_dev, variant, B, Nq, F, dxb, xlo, regime):
     E = 64 if F == 3136 else 72
     R = B * Nq
     h = _embed_bwd_inputs(B, Nq, F, E, xlo, dxb, regime, seed=R + F + (7 if regime == "exact" else 0))
-    d = {"x_hi": _dev_bf16(h["x_hi"], dev), "x_lo": _dev_bf16(h["x_lo"], dev) if xlo else None,
-         "feat": _dev(h["feat"], dev), "cos": _dev_bf16(h["cos"], dev),
-         "dx": _dev_bf16(h["dx"], dev) if dxb else _dev(h["dx"], dev)}
-    pre_w, pre_b = _pattern(F * E), _pattern(F, 0.5, 7)
+    d = {"x_hi": to_dev_bf16(h["x_hi"], dev), "x_lo": to_dev_bf16(h["x_lo"], dev) if xlo else None,
+         "feat": to_dev(h["feat"], dev), "cos": to_dev_bf16(h["cos"], dev),
+         "dx": to_dev_bf16(h["dx"], dev) if dxb else to_dev(h["dx"], dev)}
+    pre_w, pre_b = prefill_pattern(F * E), prefill_pattern(F, 0.5, 7)
     o = _embed_bwd_call(dev, B, Nq, F, E, dxb, d, pre_w, pre_b)
     # dpre = bf16(dX * feat) where fp32(x_hi + x_lo) > 0, else 0: one rounding of one product, bit for bit
     x = (h["x_hi"] + h["x_lo"]).astype(np.float32) if xlo else h["x_hi"]
     ft = np.repeat(h["feat"], Nq, axis=0)
     dp = np.where(x > 0, (h["dx"] * ft).astype(np.float32), np.float32(0)).astype(np.float32)
-    _assert_bits("dpre", o["dpre"].bits().reshape(R, F), bf16_bits(dp))
+    assert_bits("dpre", o["dpre"].bits().reshape(R, F), bf16_bits(dp))
     # dfeat = sum_q dX * x / feat, exactly 0 where feat == 0
     dfeat = o["dfeat"].f32().reshape(B, F)
     assert np.all(dfeat[h["feat"] == 0] == 0)
@@ -439,17 +333,17 @@ def test_embed_bwd_tc(cuda_dev, variant, B, Nq, F, dxb, xlo, regime):
     bnd_w = C_BOUND * (R + 1) * U * (np.abs(dpre).T @ np.abs(c64) + np.abs(pre_w.reshape(F, E)))
     got_w = o["grad_w"].f32().reshape(F, E)
     if regime == "exact":
-        _assert_bits("dfeat", f32_bits(dfeat), f32_bits(ref_dfeat))
-        _assert_bits("grad_iqn_b", o["grad_b"].bits(), f32_bits(ref_b))
-        _assert_bits("grad_iqn_w", f32_bits(got_w), f32_bits(ref_w))
+        assert_bits("dfeat", f32_bits(dfeat), f32_bits(ref_dfeat))
+        assert_bits("grad_iqn_b", o["grad_b"].bits(), f32_bits(ref_b))
+        assert_bits("grad_iqn_w", f32_bits(got_w), f32_bits(ref_w))
     else:
-        _check_bound(f"dfeat {variant}", dfeat, ref_dfeat, bnd_dfeat)
-        _check_bound(f"grad_iqn_b {variant}", o["grad_b"].f32(), ref_b, bnd_b)
-        _check_bound(f"grad_iqn_w {variant}", got_w, ref_w, bnd_w)
+        check_bound(f"dfeat {variant}", dfeat, ref_dfeat, bnd_dfeat)
+        check_bound(f"grad_iqn_b {variant}", o["grad_b"].f32(), ref_b, bnd_b)
+        check_bound(f"grad_iqn_w {variant}", got_w, ref_w, bnd_w)
     # determinism: the same call on a fresh prefill gives the same bits everywhere
     o2 = _embed_bwd_call(dev, B, Nq, F, E, dxb, d, pre_w, pre_b)
     for key in o:
-        _assert_bits(f"second call {key}", o2[key].bits(), o[key].bits())
+        assert_bits(f"second call {key}", o2[key].bits(), o[key].bits())
 
 
 @pytest.mark.gpu
@@ -459,19 +353,19 @@ def test_embed_bwd_tc_rejects_before_writing(cuda_dev):
     for B, Nq, F, E in [(3, 3, 104, 64), (4, 2, 100, 64), (4, 2, 104, 60)]:    # rows % 8, feat_dim % 8, embed_dim % 8
         R = B * Nq
         h = _embed_bwd_inputs(B, Nq, F, E, True, False, "random", seed=R)
-        pre_w, pre_b = _pattern(F * E), _pattern(F)
+        pre_w, pre_b = prefill_pattern(F * E), prefill_pattern(F)
         o = {"dpre": Out(R * F, dev, torch.bfloat16), "dfeat": Out(B * F, dev), "grad_w": Out(F * E, dev, fill=pre_w),
              "grad_b": Out(F, dev, fill=pre_b)}
-        d = [_dev_bf16(h["x_hi"], dev), _dev_bf16(h["x_lo"], dev), _dev(h["feat"], dev), _dev_bf16(h["cos"], dev),
-             _dev(h["dx"], dev)]
+        d = [to_dev_bf16(h["x_hi"], dev), to_dev_bf16(h["x_lo"], dev), to_dev(h["feat"], dev), to_dev_bf16(h["cos"], dev),
+             to_dev(h["dx"], dev)]
         with pytest.raises(RiqnError):
-            _call("riqn_quantile_embed_bwd_tc", B, Nq, E, F, *[_ptr(t) for t in d[:4]], _ptr(d[4]), 0, o["dpre"].p,
+            lib_call("riqn_quantile_embed_bwd_tc", B, Nq, E, F, *[dptr(t) for t in d[:4]], dptr(d[4]), 0, o["dpre"].p,
                   o["dfeat"].p, o["grad_w"].p, o["grad_b"].p)
         torch.cuda.synchronize()
-        _assert_canaries(o)
+        assert_canaries(o)
         assert torch.isnan(o["dpre"].t[:R * F].float()).all() and torch.isnan(o["dfeat"].t[:B * F]).all()
-        _assert_bits("grad_iqn_w untouched", o["grad_w"].bits(), f32_bits(pre_w))
-        _assert_bits("grad_iqn_b untouched", o["grad_b"].bits(), f32_bits(pre_b))
+        assert_bits("grad_iqn_w untouched", o["grad_w"].bits(), f32_bits(pre_w))
+        assert_bits("grad_iqn_b untouched", o["grad_b"].bits(), f32_bits(pre_b))
 
 
 # ---------------------------------------------------------------------------------------------- fp32 cross-check twins
@@ -484,10 +378,10 @@ F32_IDS = [f"B{b}-Nq{n}-F{f}-E{e}" for b, n, f, e in F32_SHAPES]
 def _embed_fwd_f32_call(dev, B, Nq, F, E, inp):
     R = B * Nq
     o = {"cos": Out(R * E, dev), "x": Out(R * F, dev)}
-    _call("riqn_quantile_embed_fwd", B, Nq, E, F, _ptr(inp["tau"]), _ptr(inp["feat"]), _ptr(inp["w"]), _ptr(inp["be"]),
+    lib_call("riqn_quantile_embed_fwd", B, Nq, E, F, dptr(inp["tau"]), dptr(inp["feat"]), dptr(inp["w"]), dptr(inp["be"]),
           o["cos"].p, o["x"].p)
     torch.cuda.synchronize()
-    _assert_canaries(o)
+    assert_canaries(o)
     return o
 
 
@@ -501,7 +395,7 @@ def test_embed_fwd_f32(cuda_dev, B, Nq, F, E):
     c64 = _cos_ref(host["tau"], B, Nq, E)
     cos = o["cos"].f32().reshape(R, E)
     sp = np.spacing(np.abs(c64).astype(np.float32)).astype(np.float64)
-    _check_bound("cos f32", cos, c64, 3 * sp)                     # cosf: 2 ulp, plus one ulp of slack
+    check_bound("cos f32", cos, c64, 3 * sp)                     # cosf: 2 ulp, plus one ulp of slack
     # x against feat[r // Nq] * relu(cos W_e^T + b_e) on the kernel's own cos values
     rows = _check_rows(R, B + Nq)
     c = cos[rows].astype(np.float64)
@@ -510,10 +404,10 @@ def test_embed_fwd_f32(cuda_dev, B, Nq, F, E):
     mag = np.abs(c) @ np.abs(w).T + np.abs(host["be"]).astype(np.float64)
     fr = host["feat"][rows // Nq].astype(np.float64)
     ref = fr * np.maximum(pre, 0)
-    _check_bound("x f32", o["x"].f32().reshape(R, F)[rows], ref, C_BOUND * (E + 2) * U * mag * fr + U * np.abs(ref))
+    check_bound("x f32", o["x"].f32().reshape(R, F)[rows], ref, C_BOUND * (E + 2) * U * mag * fr + U * np.abs(ref))
     o2 = _embed_fwd_f32_call(dev, B, Nq, F, E, inp)               # no atomics: deterministic
     for key in o:
-        _assert_bits(f"second call {key}", o2[key].bits(), o[key].bits())
+        assert_bits(f"second call {key}", o2[key].bits(), o[key].bits())
 
 
 @pytest.mark.gpu
@@ -523,7 +417,7 @@ def test_embed_fwd_f32_rows_read_their_sample(cuda_dev, Nq):
     B, F, E = 6, 98, 64
     host, inp = _embed_fwd_inputs(cuda_dev, B, Nq, F, E, seed=Nq + 5, zero_weight=True)
     o = _embed_fwd_f32_call(cuda_dev, B, Nq, F, E, inp)
-    _assert_bits("x == feat[r // Nq]", o["x"].bits().reshape(B * Nq, F), f32_bits(np.repeat(host["feat"], Nq, axis=0)))
+    assert_bits("x == feat[r // Nq]", o["x"].bits().reshape(B * Nq, F), f32_bits(np.repeat(host["feat"], Nq, axis=0)))
 
 
 @pytest.mark.gpu
@@ -536,17 +430,17 @@ def test_embed_bwd_f32(cuda_dev, B, Nq, F, E, regime):
     R = B * Nq
     h = _embed_bwd_inputs(B, Nq, F, E, True, False, regime, seed=R + F + (3 if regime == "exact" else 0))
     x = (h["x_hi"] + h["x_lo"]).astype(np.float32)
-    pre_w, pre_b = _pattern(F * E), _pattern(F, 0.5, 7)
-    x_d, feat_d, cos_d = _dev(x, dev), _dev(h["feat"], dev), _dev(h["cos"], dev)
+    pre_w, pre_b = prefill_pattern(F * E), prefill_pattern(F, 0.5, 7)
+    x_d, feat_d, cos_d = to_dev(x, dev), to_dev(h["feat"], dev), to_dev(h["cos"], dev)
     o = {"dx": Out(R * F, dev, fill=h["dx"]), "dfeat": Out(B * F, dev), "grad_w": Out(F * E, dev, fill=pre_w),
          "grad_b": Out(F, dev, fill=pre_b)}
-    _call("riqn_quantile_embed_bwd", B, Nq, E, F, _ptr(x_d), _ptr(feat_d), _ptr(cos_d), o["dx"].p, o["dfeat"].p,
+    lib_call("riqn_quantile_embed_bwd", B, Nq, E, F, dptr(x_d), dptr(feat_d), dptr(cos_d), o["dx"].p, o["dfeat"].p,
           o["grad_w"].p, o["grad_b"].p)
     torch.cuda.synchronize()
-    _assert_canaries(o)
+    assert_canaries(o)
     ft = np.repeat(h["feat"], Nq, axis=0)
     dp = np.where(x > 0, (h["dx"] * ft).astype(np.float32), np.float32(0)).astype(np.float32)
-    _assert_bits("dpre (in dX)", o["dx"].bits().reshape(R, F), f32_bits(dp))
+    assert_bits("dpre (in dX)", o["dx"].bits().reshape(R, F), f32_bits(dp))
     dfeat = o["dfeat"].f32().reshape(B, F)
     assert np.all(dfeat[h["feat"] == 0] == 0)
     x64, dx64 = x.astype(np.float64).reshape(B, Nq, F), h["dx"].astype(np.float64).reshape(B, Nq, F)
@@ -561,13 +455,13 @@ def test_embed_bwd_f32(cuda_dev, B, Nq, F, E, regime):
     bnd_w = C_BOUND * (R + 2) * U * (np.abs(dp64).T @ np.abs(c64) + np.abs(pre_w.reshape(F, E)))
     got_w = o["grad_w"].f32().reshape(F, E)
     if regime == "exact":
-        _assert_bits("dfeat f32", f32_bits(dfeat), f32_bits(ref_dfeat))
-        _assert_bits("grad_iqn_b f32", o["grad_b"].bits(), f32_bits(ref_b))
-        _assert_bits("grad_iqn_w f32", f32_bits(got_w), f32_bits(ref_w))
+        assert_bits("dfeat f32", f32_bits(dfeat), f32_bits(ref_dfeat))
+        assert_bits("grad_iqn_b f32", o["grad_b"].bits(), f32_bits(ref_b))
+        assert_bits("grad_iqn_w f32", f32_bits(got_w), f32_bits(ref_w))
     else:
-        _check_bound("dfeat f32", dfeat, ref_dfeat, bnd_dfeat)
-        _check_bound("grad_iqn_b f32", o["grad_b"].f32(), ref_b, bnd_b)
-        _check_bound("grad_iqn_w f32", got_w, ref_w, bnd_w)
+        check_bound("dfeat f32", dfeat, ref_dfeat, bnd_dfeat)
+        check_bound("grad_iqn_b f32", o["grad_b"].f32(), ref_b, bnd_b)
+        check_bound("grad_iqn_w f32", got_w, ref_w, bnd_w)
 
 
 # ---------------------------------------------------------------------------------------------- dueling backward
@@ -631,8 +525,8 @@ def _duel_ref(d, B, Nq, A):
 
 
 def _duel_dev(d, dev):
-    return dict(h=_dev(d["h"], dev), h_bf16=_dev_bf16(d["h"], dev), wz=_dev(d["wz"], dev), dtheta=_dev(d["dtheta"], dev),
-                gscale=_dev(d["gscale"], dev), actions=torch.from_numpy(d["actions"]).to(dev))
+    return dict(h=to_dev(d["h"], dev), h_bf16=to_dev_bf16(d["h"], dev), wz=to_dev(d["wz"], dev), dtheta=to_dev(d["dtheta"], dev),
+                gscale=to_dev(d["gscale"], dev), actions=torch.from_numpy(d["actions"]).to(dev))
 
 
 def _duel_bf16_call(dev, B, Nq, A, dd, gmul, use_hb, with_t, fn="riqn_dueling_bwd_bf16"):
@@ -640,15 +534,15 @@ def _duel_bf16_call(dev, B, Nq, A, dd, gmul, use_hb, with_t, fn="riqn_dueling_bw
     o = {"dh_hi": Out(R * 2 * HID, dev, torch.bfloat16), "dh_hi_t": Out(2 * HID * R, dev, torch.bfloat16) if with_t else None,
          "colsum": Out(2 * HID, dev), "dz": Out(R * 32, dev), "dz_bf16": Out(R * 32, dev, torch.bfloat16)}
     p = {k: (v.p if v is not None else None) for k, v in o.items()}
-    hb = _ptr(dd["h_bf16"]) if use_hb else None
+    hb = dptr(dd["h_bf16"]) if use_hb else None
     if fn == "riqn_dueling_bwd_bf16":
-        _call(fn, R, B, HID, A, _ptr(dd["h"]), hb, _ptr(dd["wz"]), _ptr(dd["dtheta"]), _ptr(dd["gscale"]), float(gmul),
-              _ptr(dd["actions"]), p["dh_hi"], p["dh_hi_t"], p["colsum"], p["dz"], p["dz_bf16"])
+        lib_call(fn, R, B, HID, A, dptr(dd["h"]), hb, dptr(dd["wz"]), dptr(dd["dtheta"]), dptr(dd["gscale"]), float(gmul),
+              dptr(dd["actions"]), p["dh_hi"], p["dh_hi_t"], p["colsum"], p["dz"], p["dz_bf16"])
     else:
-        _call(fn, R, B, HID, A, _ptr(dd["h"]), hb, _ptr(dd["wz"]), _ptr(dd["grad_q"]), p["dh_hi"], p["dh_hi_t"],
+        lib_call(fn, R, B, HID, A, dptr(dd["h"]), hb, dptr(dd["wz"]), dptr(dd["grad_q"]), p["dh_hi"], p["dh_hi_t"],
               p["colsum"], p["dz"], p["dz_bf16"])
     torch.cuda.synchronize()
-    _assert_canaries(o)
+    assert_canaries(o)
     return o
 
 
@@ -662,20 +556,20 @@ def test_dueling_bwd_bf16(cuda_dev, B, Nq, A, regime):
     dd = _duel_dev(d, dev)
     dh, dz = _duel_ref(d, B, Nq, A)
     o = _duel_bf16_call(dev, B, Nq, A, dd, d["gmul"], use_hb=False, with_t=True)
-    _assert_bits("dh_hi", o["dh_hi"].bits().reshape(R, 2 * HID), bf16_bits(dh))
-    _assert_bits("dh_hi_t", o["dh_hi_t"].bits().reshape(2 * HID, R), o["dh_hi"].bits().reshape(R, 2 * HID).T)
-    _assert_bits("dz", o["dz"].bits().reshape(R, 32), f32_bits(dz))
-    _assert_bits("dz_bf16", o["dz_bf16"].bits().reshape(R, 32), bf16_bits(dz))
+    assert_bits("dh_hi", o["dh_hi"].bits().reshape(R, 2 * HID), bf16_bits(dh))
+    assert_bits("dh_hi_t", o["dh_hi_t"].bits().reshape(2 * HID, R), o["dh_hi"].bits().reshape(R, 2 * HID).T)
+    assert_bits("dz", o["dz"].bits().reshape(R, 32), f32_bits(dz))
+    assert_bits("dz_bf16", o["dz_bf16"].bits().reshape(R, 32), bf16_bits(dz))
     ref_cs = dh.astype(np.float64).sum(0) + 0.0
     if regime == "exact":
-        _assert_bits("dh_colsum", o["colsum"].bits(), f32_bits(ref_cs))
+        assert_bits("dh_colsum", o["colsum"].bits(), f32_bits(ref_cs))
     else:
-        _check_bound("dh_colsum", o["colsum"].f32(), ref_cs, C_BOUND * R * U * np.abs(dh).astype(np.float64).sum(0))
+        check_bound("dh_colsum", o["colsum"].f32(), ref_cs, C_BOUND * R * U * np.abs(dh).astype(np.float64).sum(0))
     # the bf16 image of h gives the same ReLU mask; without the transposed image the rest is unchanged (and the
     # kernel is deterministic)
     o2 = _duel_bf16_call(dev, B, Nq, A, dd, d["gmul"], use_hb=True, with_t=False)
     for key in ("dh_hi", "colsum", "dz", "dz_bf16"):
-        _assert_bits(f"h_bf16 call {key}", o2[key].bits(), o[key].bits())
+        assert_bits(f"h_bf16 call {key}", o2[key].bits(), o[key].bits())
 
 
 @pytest.mark.gpu
@@ -688,13 +582,13 @@ def test_dueling_bwd_f32(cuda_dev, B, Nq, A, regime):
     dd = _duel_dev(d, dev)
     dh, dz = _duel_ref(d, B, Nq, A)
     o = {"dh": Out(R * 2 * HID, dev), "dz": Out(R * 32, dev), "dz_bf16": Out(R * 32, dev, torch.bfloat16)}
-    _call("riqn_dueling_bwd", R, B, HID, A, _ptr(dd["h"]), _ptr(dd["wz"]), _ptr(dd["dtheta"]), _ptr(dd["gscale"]),
-          float(d["gmul"]), _ptr(dd["actions"]), o["dh"].p, o["dz"].p, o["dz_bf16"].p)
+    lib_call("riqn_dueling_bwd", R, B, HID, A, dptr(dd["h"]), dptr(dd["wz"]), dptr(dd["dtheta"]), dptr(dd["gscale"]),
+          float(d["gmul"]), dptr(dd["actions"]), o["dh"].p, o["dz"].p, o["dz_bf16"].p)
     torch.cuda.synchronize()
-    _assert_canaries(o)
-    _assert_bits("dh", o["dh"].bits().reshape(R, 2 * HID), f32_bits(dh))
-    _assert_bits("dz", o["dz"].bits().reshape(R, 32), f32_bits(dz))
-    _assert_bits("dz_bf16", o["dz_bf16"].bits().reshape(R, 32), bf16_bits(dz))
+    assert_canaries(o)
+    assert_bits("dh", o["dh"].bits().reshape(R, 2 * HID), f32_bits(dh))
+    assert_bits("dz", o["dz"].bits().reshape(R, 32), f32_bits(dz))
+    assert_bits("dz_bf16", o["dz_bf16"].bits().reshape(R, 32), bf16_bits(dz))
 
 
 DENSE_CASES = [(8, 3, 1), (5, 8, 18), (3, 200, 31), (16, 64, 6), (512, 64, 18)]
@@ -711,7 +605,7 @@ def test_dueling_bwd_dense(cuda_dev, B, Nq, A, variant):
     rs = np.random.RandomState(A)
     G = (rs.standard_normal((R, A)) * 0.1).astype(np.float32)          # quantile-major rows q*B + b
     dd = _duel_dev(d, dev)
-    dd["grad_q"] = _dev(G, dev)
+    dd["grad_q"] = to_dev(G, dev)
     r = np.arange(R)
     Gs = G[(r % Nq) * B + r // Nq].astype(np.float64)                   # sample-major
     wz = d["wz"].astype(np.float64)
@@ -730,24 +624,24 @@ def test_dueling_bwd_dense(cuda_dev, B, Nq, A, variant):
     bnd_dz[:, :1 + A] = C_BOUND * k * U * S[:, None]
     if variant == "f32":
         o = {"dh": Out(R * 2 * HID, dev), "dz": Out(R * 32, dev), "dz_bf16": Out(R * 32, dev, torch.bfloat16)}
-        _call("riqn_dueling_bwd_dense", R, B, HID, A, _ptr(dd["h"]), _ptr(dd["wz"]), _ptr(dd["grad_q"]), o["dh"].p,
+        lib_call("riqn_dueling_bwd_dense", R, B, HID, A, dptr(dd["h"]), dptr(dd["wz"]), dptr(dd["grad_q"]), o["dh"].p,
               o["dz"].p, o["dz_bf16"].p)
         torch.cuda.synchronize()
-        _assert_canaries(o)
-        _check_bound("dense dh", o["dh"].f32().reshape(R, 2 * HID), ref_dh, bnd_dh)
+        assert_canaries(o)
+        check_bound("dense dh", o["dh"].f32().reshape(R, 2 * HID), ref_dh, bnd_dh)
     else:
         o = _duel_bf16_call(dev, B, Nq, A, dd, 0.0, use_hb=False, with_t=True, fn="riqn_dueling_bwd_dense_bf16")
         hi = o["dh_hi"].f32().reshape(R, 2 * HID)
-        _check_bound("dense dh_hi", hi, ref_dh, 2 * bnd_dh + 2.0 ** -8 * np.abs(ref_dh))
-        _assert_bits("dense dh_hi_t", o["dh_hi_t"].bits().reshape(2 * HID, R), o["dh_hi"].bits().reshape(R, 2 * HID).T)
-        _check_bound("dense dh_colsum", o["colsum"].f32(), ref_dh.sum(0),
+        check_bound("dense dh_hi", hi, ref_dh, 2 * bnd_dh + 2.0 ** -8 * np.abs(ref_dh))
+        assert_bits("dense dh_hi_t", o["dh_hi_t"].bits().reshape(2 * HID, R), o["dh_hi"].bits().reshape(R, 2 * HID).T)
+        check_bound("dense dh_colsum", o["colsum"].f32(), ref_dh.sum(0),
                      bnd_dh.sum(0) + C_BOUND * R * U * np.abs(ref_dh).sum(0))
         o2 = _duel_bf16_call(dev, B, Nq, A, dd, 0.0, use_hb=True, with_t=False, fn="riqn_dueling_bwd_dense_bf16")
         for key in ("dh_hi", "colsum", "dz", "dz_bf16"):
-            _assert_bits(f"dense h_bf16 call {key}", o2[key].bits(), o[key].bits())
+            assert_bits(f"dense h_bf16 call {key}", o2[key].bits(), o[key].bits())
     dz = o["dz"].f32().reshape(R, 32)
-    _check_bound("dense dz", dz, ref_dz, bnd_dz)
-    _assert_bits("dense dz_bf16", o["dz_bf16"].bits().reshape(R, 32), bf16_bits(dz))
+    check_bound("dense dz", dz, ref_dz, bnd_dz)
+    assert_bits("dense dz_bf16", o["dz_bf16"].bits().reshape(R, 32), bf16_bits(dz))
 
 
 @pytest.mark.gpu
@@ -763,15 +657,15 @@ def test_dueling_bwd_rejects(cuda_dev):
         o = {"dh_hi": Out(32 * 2 * HID, dev, torch.bfloat16), "dh": Out(32 * 2 * HID, dev), "colsum": Out(2 * HID, dev),
              "dz": Out(32 * 32, dev), "dz_bf16": Out(32 * 32, dev, torch.bfloat16)}
         with pytest.raises(RiqnError):
-            _call("riqn_dueling_bwd_bf16", R, B, hid, A, _ptr(dd["h"]), None, _ptr(wz), _ptr(dd["dtheta"]),
-                  _ptr(dd["gscale"]), 1.0, _ptr(dd["actions"]), o["dh_hi"].p, None, o["colsum"].p, o["dz"].p,
+            lib_call("riqn_dueling_bwd_bf16", R, B, hid, A, dptr(dd["h"]), None, dptr(wz), dptr(dd["dtheta"]),
+                  dptr(dd["gscale"]), 1.0, dptr(dd["actions"]), o["dh_hi"].p, None, o["colsum"].p, o["dz"].p,
                   o["dz_bf16"].p)
         if R % 8 == 0:
             with pytest.raises(RiqnError):
-                _call("riqn_dueling_bwd", R, B, hid, A, _ptr(dd["h"]), _ptr(wz), _ptr(dd["dtheta"]), _ptr(dd["gscale"]),
-                      1.0, _ptr(dd["actions"]), o["dh"].p, o["dz"].p, o["dz_bf16"].p)
+                lib_call("riqn_dueling_bwd", R, B, hid, A, dptr(dd["h"]), dptr(wz), dptr(dd["dtheta"]), dptr(dd["gscale"]),
+                      1.0, dptr(dd["actions"]), o["dh"].p, o["dz"].p, o["dz_bf16"].p)
         torch.cuda.synchronize()
-        _assert_canaries(o)
+        assert_canaries(o)
         for k, v in o.items():
             assert torch.isnan(v.t[:v.n].float()).all(), f"rejected call wrote {k}"
 
@@ -788,7 +682,7 @@ def _zw_inputs(rows, A, regime, seed):
         h[rs.uniform(size=h.shape) < 0.3] = 0
         ch = np.array([-2, -1, -0.5, 0.5, 1, 2], np.float32)
         eps = [rs.choice(ch, n) for n in (HID, 1, A * HID, A)]
-        pre = [_pattern(n, 0.5, m) for n, m in ((HID, 11), (HID, 7), (1, 3), (1, 5), (A * HID, 13), (A * HID, 9),
+        pre = [prefill_pattern(n, 0.5, m) for n, m in ((HID, 11), (HID, 7), (1, 3), (1, 5), (A * HID, 13), (A * HID, 9),
                                                  (A, 3), (A, 5))]
     else:
         dz = (rs.standard_normal((rows, 32)) * 0.1).astype(np.float32)
@@ -808,12 +702,12 @@ def _zw_call(dev, variant, rows, A, dzd, dzb, hd, hb, epsd, pre, fill_scratch=fl
     o["dbz"] = Out(32, dev, fill=fill_scratch)
     g = [o[n].p for n in ZW_NAMES]
     if variant == "tc":
-        _call("riqn_z_wgrad_tc", rows, HID, A, _ptr(dzb), _ptr(hb), _ptr(dzd), o["dwz"].p, o["dbz"].p,
-              *[_ptr(e) for e in epsd], *g)
+        lib_call("riqn_z_wgrad_tc", rows, HID, A, dptr(dzb), dptr(hb), dptr(dzd), o["dwz"].p, o["dbz"].p,
+              *[dptr(e) for e in epsd], *g)
     else:
-        _call("riqn_z_wgrad", rows, HID, A, _ptr(dzd), _ptr(hd), o["dwz"].p, o["dbz"].p, *[_ptr(e) for e in epsd], *g)
+        lib_call("riqn_z_wgrad", rows, HID, A, dptr(dzd), dptr(hd), o["dwz"].p, o["dbz"].p, *[dptr(e) for e in epsd], *g)
     torch.cuda.synchronize()
-    _assert_canaries(o)
+    assert_canaries(o)
     return o
 
 
@@ -824,9 +718,9 @@ def _zw_call(dev, variant, rows, A, dzd, dzb, hd, hb, epsd, pre, fill_scratch=fl
 def test_z_wgrad(cuda_dev, rows, A, variant, regime):
     dev = cuda_dev
     dz, h, eps, pre = _zw_inputs(rows, A, regime, seed=rows + A)
-    dzd, hd = _dev(dz, dev), _dev(h, dev)
-    dzb, hb = _dev_bf16(dz, dev), _dev_bf16(h, dev)
-    epsd = [_dev(e, dev) for e in eps]
+    dzd, hd = to_dev(dz, dev), to_dev(h, dev)
+    dzb, hb = to_dev_bf16(dz, dev), to_dev_bf16(h, dev)
+    epsd = [to_dev(e, dev) for e in eps]
     o = _zw_call(dev, variant, rows, A, dzd, dzb, hd, hb, epsd, pre)
     # the weight half reads the operand images the product consumed, the bias half the fp32 dz
     dzi = (bf16(dz) if variant == "tc" else dz).astype(np.float64)
@@ -848,13 +742,13 @@ def test_z_wgrad(cuda_dev, rows, A, variant, regime):
            C_BOUND * k * U * (mag_b[1:] + np.abs(p[6])), C_BOUND * k * U * (mag_b[1:] * np.abs(e_ba) + np.abs(p[7]))]
     for name, r_, b_ in zip(ZW_NAMES, ref, bnd):
         if regime == "exact":
-            _assert_bits(name, o[name].bits(), f32_bits(r_))
+            assert_bits(name, o[name].bits(), f32_bits(r_))
         else:
-            _check_bound(f"{name} {variant}", o[name].f32(), r_, b_)
+            check_bound(f"{name} {variant}", o[name].f32(), r_, b_)
     if variant == "tc":                                                  # determinism of the tensor-core product
         o2 = _zw_call(dev, variant, rows, A, dzd, dzb, hd, hb, epsd, pre)
         for name in ZW_NAMES:
-            _assert_bits(f"second call {name}", o2[name].bits(), o[name].bits())
+            assert_bits(f"second call {name}", o2[name].bits(), o[name].bits())
 
 
 @pytest.mark.gpu
@@ -872,27 +766,27 @@ def test_z_wgrad_rejects_action_space(cuda_dev, variant, A):
     o = {n: Out(x.size, dev, fill=x) for n, x in zip(ZW_NAMES, pre)}
     scratch = Out(32 * 2 * HID, dev, fill=3.0), Out(32, dev, fill=3.0)
     args = [o[n].p for n in ZW_NAMES]
-    epsd = [_dev(e, dev) for e in eps]
-    dzd, dzb, hd, hb = _dev(dz, dev), _dev_bf16(dz, dev), _dev(h, dev), _dev_bf16(h, dev)
+    epsd = [to_dev(e, dev) for e in eps]
+    dzd, dzb, hd, hb = to_dev(dz, dev), to_dev_bf16(dz, dev), to_dev(h, dev), to_dev_bf16(h, dev)
     with pytest.raises(RiqnError):
         if variant == "tc":
-            _call("riqn_z_wgrad_tc", rows, HID, A, _ptr(dzb), _ptr(hb), _ptr(dzd), scratch[0].p, scratch[1].p,
-                  *[_ptr(e) for e in epsd], *args)
+            lib_call("riqn_z_wgrad_tc", rows, HID, A, dptr(dzb), dptr(hb), dptr(dzd), scratch[0].p, scratch[1].p,
+                  *[dptr(e) for e in epsd], *args)
         else:
-            _call("riqn_z_wgrad", rows, HID, A, _ptr(dzd), _ptr(hd), scratch[0].p, scratch[1].p,
-                  *[_ptr(e) for e in epsd], *args)
+            lib_call("riqn_z_wgrad", rows, HID, A, dptr(dzd), dptr(hd), scratch[0].p, scratch[1].p,
+                  *[dptr(e) for e in epsd], *args)
     torch.cuda.synchronize()
     for s in scratch:
         assert torch.all(s.t[:s.n] == 3.0), "the scratch was cleared by a rejected call"
     for n, x in zip(ZW_NAMES, pre):
-        _assert_bits(f"{n} untouched", o[n].bits(), f32_bits(x))
+        assert_bits(f"{n} untouched", o[n].bits(), f32_bits(x))
 
 
 # ---------------------------------------------------------------------------------------------- NoisyLinear bias gradients
 def _nbg_inputs(n, regime, rs):
     if regime == "exact":
         eps = rs.choice(np.array([-2, -1, -0.5, 0.5, 1, 2], np.float32), n)
-        return eps, _pattern(n, 0.5, 11), _pattern(n, 0.5, 7)
+        return eps, prefill_pattern(n, 0.5, 11), prefill_pattern(n, 0.5, 7)
     return (rs.standard_normal(n).astype(np.float32), rs.standard_normal(n).astype(np.float32),
             rs.standard_normal(n).astype(np.float32))
 
@@ -923,18 +817,18 @@ def test_noisy_bias_grad(cuda_dev, rows, regime):
         ref_db, mag = dh.astype(np.float64).sum(0) + 0.0, np.abs(dh).astype(np.float64).sum(0)
         k = rows + 2
     g_mu, g_sig = Out(n, dev, fill=pre_mu), Out(n, dev, fill=pre_sig)
-    dh_d = None if dh is None else _dev(dh, dev)          # (held: a freed input could be reused for the next upload)
-    eps_d = _dev(eps, dev)
-    _call("riqn_noisy_bias_grad", max(rows, 1), n, _ptr(dh_d), _ptr(eps_d), scratch.p, g_mu.p, g_sig.p)
+    dh_d = None if dh is None else to_dev(dh, dev)          # (held: a freed input could be reused for the next upload)
+    eps_d = to_dev(eps, dev)
+    lib_call("riqn_noisy_bias_grad", max(rows, 1), n, dptr(dh_d), dptr(eps_d), scratch.p, g_mu.p, g_sig.p)
     torch.cuda.synchronize()
-    _assert_canaries({"scratch": scratch, "g_bmu": g_mu, "g_bsig": g_sig})
+    assert_canaries({"scratch": scratch, "g_bmu": g_mu, "g_bsig": g_sig})
     e64 = eps.astype(np.float64)
     ref_mu, ref_sig = pre_mu + ref_db, pre_sig + ref_db * e64
     if regime == "exact":
-        _assert_bits("db scratch", scratch.bits(), f32_bits(ref_db))
-        _assert_bits("g_bmu", g_mu.bits(), f32_bits(ref_mu))
-        _assert_bits("g_bsig", g_sig.bits(), f32_bits(ref_sig))
+        assert_bits("db scratch", scratch.bits(), f32_bits(ref_db))
+        assert_bits("g_bmu", g_mu.bits(), f32_bits(ref_mu))
+        assert_bits("g_bsig", g_sig.bits(), f32_bits(ref_sig))
     else:
-        _check_bound("db scratch", scratch.f32(), ref_db, C_BOUND * k * U * mag)
-        _check_bound("g_bmu", g_mu.f32(), ref_mu, C_BOUND * k * U * (mag + np.abs(pre_mu)))
-        _check_bound("g_bsig", g_sig.f32(), ref_sig, C_BOUND * k * U * (mag * np.abs(e64) + np.abs(pre_sig)))
+        check_bound("db scratch", scratch.f32(), ref_db, C_BOUND * k * U * mag)
+        check_bound("g_bmu", g_mu.f32(), ref_mu, C_BOUND * k * U * (mag + np.abs(pre_mu)))
+        check_bound("g_bsig", g_sig.f32(), ref_sig, C_BOUND * k * U * (mag * np.abs(e64) + np.abs(pre_sig)))

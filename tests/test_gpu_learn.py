@@ -334,22 +334,19 @@ def test_c51_loss_api_vs_oracle(cuda_dev):
     assert a == int((p_eval * torch.linspace(-10, 10, 51)).sum(2).argmax(1))
 
 
-@pytest.mark.parametrize("graph", [False, True])
-def test_learner_steps_are_bitwise_reproducible(cuda_dev, graph):
-    """Two learners built from the same seed draw the same prioritized samples and compute bit-identical losses and
-    parameters over several steps at the benchmarked size, eagerly and replayed from the step's CUDA graph.  The losses become the next steps' priorities, so any
-    order-dependent rounding (a float atomic in a cross-block sum) would change which transitions are drawn later."""
+def _assert_steps_bitwise_reproducible(dev, graph, rainbow_only, cap):
     import bench
     from rainbow_iqn_apex_b200 import Learner, ReplayMemory
-    cap = 1 << 14
 
     def run():
         torch.manual_seed(5)
-        a = bench.make_args(cuda_dev, cap)
+        a = bench.make_args(dev, cap, rainbow_only=rainbow_only)
+        if rainbow_only:
+            a.lr, a.adam_eps = 6.25e-5, 1.5e-4                     # bench.c51_leg
         learner = Learner(a, bench.ACTIONS, None)
         learner.train()
         mem = ReplayMemory(a, None)
-        bench.fill_replay(mem, cap, cuda_dev, 7)
+        bench.fill_replay(mem, cap, dev, 7)
         if graph:
             learner.enable_cuda_graph(mem)
         steps = []
@@ -363,4 +360,19 @@ def test_learner_steps_are_bitwise_reproducible(cuda_dev, graph):
     for k, ((i1, l1), (i2, l2)) in enumerate(zip(s1, s2)):
         assert torch.equal(i1, i2), f"step {k}: sampled indices differ"
         assert torch.equal(l1, l2), f"step {k}: losses differ"
-    assert torch.equal(p1, p2)
+    assert torch.equal(p1, p2), "parameters differ"
+
+
+@pytest.mark.parametrize("graph", [False, True])
+def test_learner_steps_are_bitwise_reproducible(cuda_dev, graph):
+    """Two learners built from the same seed draw the same prioritized samples and compute bit-identical losses and
+    parameters over several steps at the benchmarked size, eagerly and replayed from the step's CUDA graph.  The losses become the next steps' priorities, so any
+    order-dependent rounding (a float atomic in a cross-block sum) would change which transitions are drawn later."""
+    _assert_steps_bitwise_reproducible(cuda_dev, graph, rainbow_only=0, cap=1 << 14)
+
+
+@pytest.mark.parametrize("graph", [False, True])
+def test_c51_learner_steps_are_bitwise_reproducible(cuda_dev, graph):
+    """The same for the Rainbow-only (C51) learner at B = 512 (bench.c51_leg's learning rate and Adam epsilon): its
+    z-layer weight gradients are split-K products over the batch rows, whose partials must be added in a fixed order."""
+    _assert_steps_bitwise_reproducible(cuda_dev, graph, rainbow_only=1, cap=1 << 14)
