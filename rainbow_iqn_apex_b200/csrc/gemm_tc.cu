@@ -9,7 +9,8 @@
 //   descriptors; the accumulator lives in their registers,
 // * after a tile's last k-block the consumers pass the accumulator through a shared-memory slab, 64 columns at a time,
 //   so that each warp holds 32 rows x 32 columns with one ROW per lane, and apply the fused epilogue from there while
-//   the producer already fetches the next tile's operands,
+//   the producer already fetches the next tile's operands (the 128x256 forward and bf16 data gradient instead stage
+//   their fragments for TMA stores and go on to the next tile while the stores drain: MODE bit 3, see TcCfg),
 // * persistent CTAs (one per SM) walk (m-tile, n-tile, k-split) work units round-robin.
 //
 // Precision: NSPLIT == 1 multiplies bf16(A) * bf16(B).  NSPLIT == 3 takes each operand as hi + lo bf16 pairs
@@ -43,18 +44,31 @@ constexpr uint32_t kSmemLimit = 232448;           // 227 KB of opt-in shared mem
 
 // NSPLIT 1: a_hi*b_hi.  NSPLIT 3: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi.  NSPLIT 2: A is exact in bf16 (e.g. uint8 pixels),
 // only B is split: a_hi*b_hi + a_hi*b_lo.
-template <int NSPLIT, int BN, int EPI>
+//
+// TMAEPI (128x256 TC_BIAS_RELU / TC_STORE only): the accumulator leaves through TMA stores instead of the slab.  Each
+// consumer warpgroup stages 32-column chunks of its 64 rows in kEpiBufs rotating buffers of kEpiChunkBytes: a 64 x 32
+// fp32 box (8 KB, 128-byte swizzle; TC_BIAS_RELU) and a 64 x 32 bf16 box (4 KB, 64-byte swizzle; the o_hi image).
+// With the 3-stage ring (144 KB) that leaves room for 3 fp32 + bf16 buffers per warpgroup (72 KB) in the forward, and
+// for the whole 128 x 256 bf16 tile (8 buffers, 64 KB) in the data gradient.
+template <int NSPLIT, int BN, int EPI, bool TMAEPI = false>
 struct TcCfg {
   static constexpr int kAOps = NSPLIT == 3 ? 2 : 1, kBOps = NSPLIT == 1 ? 1 : 2;     // hi (+ lo) images per operand
   static constexpr int kOps = kAOps;                                                 // (A images; B tile starts after them)
   static constexpr uint32_t kABytes = TBM * TBK * 2, kBBytes = BN * TBK * 2;
   static constexpr uint32_t kStageBytes = kAOps * kABytes + kBOps * kBBytes;         // 32 / 48 / 64 KB at BN = 128
-  static constexpr uint32_t kEpiBytes = kConsumerWGs * kSlabBytes;
+  static constexpr uint32_t kEpiF32Bytes = EPI == TC_BIAS_RELU ? 64 * 32 * 4 : 0;
+  static constexpr uint32_t kEpiChunkBytes = kEpiF32Bytes + 64 * 32 * 2;
+  static constexpr int kEpiBufsFit = (kSmemLimit - 1024 - 256 - 3 * kStageBytes) / (kConsumerWGs * kEpiChunkBytes);
+  static constexpr int kEpiBufs = kEpiBufsFit > BN / 32 ? BN / 32 : kEpiBufsFit;
+  static constexpr uint32_t kEpiBytes = TMAEPI ? kConsumerWGs * kEpiBufs * kEpiChunkBytes : kConsumerWGs * kSlabBytes;
+  static_assert(!TMAEPI || (BN == 256 && NSPLIT == 1 && (EPI == TC_BIAS_RELU || EPI == TC_STORE) && kEpiBufs >= 2),
+                "TMA-store epilogue: 128x256 single-pass TC_BIAS_RELU / TC_STORE with at least two staging buffers");
   static constexpr uint32_t kFbBytes = EPI == TC_EMBED ? kEpiWarps * 256 : 0;       // per-warp feat / bias broadcast patches
   static constexpr uint32_t kRingBytes = kSmemLimit - 1024 /*align*/ - kEpiBytes - 256 /*barriers*/ - kFbBytes;
   static constexpr int kStages = kRingBytes / kStageBytes > 6 ? 6 : kRingBytes / kStageBytes;
   static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + kEpiBytes + 256 + kFbBytes;
   static_assert(kSmemBytes <= kSmemLimit && kStages >= 2, "exceeds the 227 KB per-CTA shared memory limit");
+  static_assert(!TMAEPI || kStages == 3, "the staging budget above assumes the 3-stage ring");
 };
 
 // ---------------------------------------------------------------------------------------------- PTX wrappers
@@ -96,6 +110,9 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t sr
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// at most N of this thread's most recent bulk store groups may still be reading shared memory
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read_n() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // named barrier over the 128 threads of one warpgroup (id 0 is __syncthreads)
@@ -351,6 +368,7 @@ __device__ __forceinline__ void mma_kblock(float (&d)[TBN / 2], uint32_t sa, uin
 
 struct alignas(64) TcArgs {
   CUtensorMap mapO[2];   // TC_EMBED: TMA-store maps of o_hi / o_lo ((M, N) 16-bit row-major, box 32 x 32, 64-byte swizzle)
+                         // MODE bit 3: C (fp32, box 32 x 64, 128-byte swizzle) / o_hi (bf16, box 32 x 64, 64-byte swizzle)
   int M, N, K;
   int m_tiles, n_tiles, k_splits, kb_per_split, kb_total;
   float* C;
@@ -375,13 +393,14 @@ struct alignas(64) TcArgs {
   long part_stride;      // TC_STORE of split-K partials: split ks writes C + ks * part_stride (0 otherwise)
 };
 
-// MODE (128x256 tiles only; 0 otherwise): bits 0-1 = mn_major, bit 2 = fp16 operands
+// MODE (128x256 tiles only; 0 otherwise): bits 0-1 = mn_major, bit 2 = fp16 operands, bit 3 = TMA-store epilogue
 template <int NSPLIT, int EPI, int BN, int MODE = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                const __grid_constant__ CUtensorMap mapB_hi, const __grid_constant__ CUtensorMap mapB_lo,
                const __grid_constant__ TcArgs p) {
-  using Cfg = TcCfg<NSPLIT, BN, EPI>;
+  constexpr bool kTmaEpi = (MODE & 8) != 0;
+  using Cfg = TcCfg<NSPLIT, BN, EPI, kTmaEpi>;
   constexpr int TBN = BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -504,6 +523,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
   bool conv_grp1 = false;
   int stage = 0;
   uint32_t phase = 0;
+  int epi_seq = 0;                              // TMA-store epilogue: chunks this warpgroup has staged so far
   for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
     const int tiles = p.m_tiles * p.n_tiles;
     const int ks = u / tiles, t = u - ks * tiles;
@@ -575,6 +595,78 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
     if constexpr (EPI == TC_CONV_DGRAD) {
 #pragma unroll
       for (int i = 0; i < TBN / 2; ++i) acc[i] = dg_sum[i];
+    }
+
+    if constexpr (kTmaEpi) {
+      // ---- TMA-store epilogue: the fragments go straight into the swizzled staging boxes (bias + ReLU applied in
+      // registers), one thread per warpgroup issues the bulk tensor stores, and the warpgroup goes on to the next tile
+      // without waiting for them.  A staging buffer is rewritten only after the stores that read it have finished
+      // READING shared memory; their global writes stay in flight.  TMA clips rows >= M and columns >= N.
+      constexpr int kChunks = TBN / 32;
+      constexpr bool kWhole = Cfg::kEpiBufs >= kChunks;   // the whole tile fits: one wait and two barriers per tile
+      const int row0 = mt * TBM + 64 * g;
+      const int nch = min(kChunks, (p.N - nt * TBN + 31) / 32);   // chunks holding real columns
+      const bool elected = wq == 0 && lane == 0;
+      const uint32_t stg = epi_base + g * (Cfg::kEpiBufs * Cfg::kEpiChunkBytes);
+      const int fr = 16 * wq + (lane >> 2);     // fragment rows fr and fr + 8 of this warpgroup's 64
+      if (row0 < p.M) {
+#pragma unroll
+        for (int h = 0; h < kChunks; ++h) {
+          if (h >= nch) break;
+          const int buf = kWhole ? h : epi_seq % Cfg::kEpiBufs;
+          if (!kWhole || h == 0) {
+            if (elected) tma_store_wait_read_n<kWhole ? 0 : Cfg::kEpiBufs - 1>();
+            wg_bar(1 + g);
+          }
+          const uint32_t sf = stg + buf * Cfg::kEpiChunkBytes;   // fp32 box (64 rows x 128 B)
+          const uint32_t sh = sf + Cfg::kEpiF32Bytes;            // bf16 box (64 rows x 64 B)
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * h + jj;               // accumulator column group: tile columns 8 j + 2 (lane % 4) + {0, 1}
+            float b0 = 0.f, b1 = 0.f;
+            if (EPI == TC_BIAS_RELU) {
+              const int n = nt * TBN + 8 * j + 2 * (lane & 3);
+              if (n < p.N) b0 = __ldg(p.bias + n);
+              if (n + 1 < p.N) b1 = __ldg(p.bias + n + 1);
+            }
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int r = fr + 8 * hh;
+              float x0 = acc[4 * j + 2 * hh], x1 = acc[4 * j + 2 * hh + 1];
+              if (EPI == TC_BIAS_RELU) {
+                x0 = fmaxf(x0 + b0, 0.f);
+                x1 = fmaxf(x1 + b1, 0.f);
+                // 128-byte swizzle: 16-byte piece q of row r sits at q ^ (r % 8)
+                const uint32_t q = 2 * jj + ((lane & 3) >> 1);
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(sf + r * 128 + ((q ^ (r & 7)) << 4) + 8 * (lane & 1)),
+                             "f"(x0), "f"(x1) : "memory");
+              }
+              if (EPI == TC_STORE || p.o_hi != nullptr) {
+                // 64-byte swizzle: 16-byte piece q of row r sits at q ^ ((r / 2) % 4)
+                const __nv_bfloat162 hv = __floats2bfloat162_rn(x0, x1);
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(sh + r * 64 + ((jj ^ ((r >> 1) & 3)) << 4) + 4 * (lane & 3)),
+                             "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
+              }
+            }
+          }
+          fence_proxy_async();                      // generic-proxy writes -> visible to the TMA engine
+          if (!kWhole || h == nch - 1) {
+            wg_bar(1 + g);
+            if (elected) {
+#pragma unroll
+              for (int i = kWhole ? 0 : h; i <= h; ++i) {
+                const uint32_t si = kWhole ? stg + i * Cfg::kEpiChunkBytes : sf;
+                const int c0 = nt * TBN + 32 * i;
+                if (EPI == TC_BIAS_RELU) tma_store_2d(&p.mapO[0], si, c0, row0);
+                if (EPI == TC_STORE || p.o_hi != nullptr) tma_store_2d(&p.mapO[1], si + Cfg::kEpiF32Bytes, c0, row0);
+              }
+              tma_store_commit();
+            }
+          }
+          ++epi_seq;
+        }
+      }
+      continue;
     }
 
     // ---- epilogue, one 64-column chunk at a time: fragment -> slab -> (row per lane) v[32] -> fused epilogue
@@ -869,7 +961,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
       }
     }
   }
-  if (EPI == TC_EMBED && lane == 0) tma_store_wait_all();   // bulk stores read this CTA's shared memory
+  if ((EPI == TC_EMBED || kTmaEpi) && lane == 0) tma_store_wait_all();   // bulk stores read this CTA's shared memory
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -900,16 +992,29 @@ static int make_map(CUtensorMap* map, const bf16* base, long rows, long K, int b
   return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
 }
 
-// (rows, cols) row-major 16-bit matrix written by TMA stores of 32 x 32 boxes staged in the 64-byte-swizzle layout
-static int make_store_map(CUtensorMap* map, const bf16* base, long rows, long cols) {
+// (rows, cols) row-major 16-bit matrix written by TMA stores of 32 x box_rows boxes staged in the 64-byte-swizzle layout
+static int make_store_map(CUtensorMap* map, const bf16* base, long rows, long cols, int box_rows = 32) {
   auto enc = get_encode();
   if (!enc) return (int)cudaErrorNotSupported;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)(cols * sizeof(bf16))};
-  cuuint32_t box[2] = {32, 32};
+  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<bf16*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
+}
+// (rows, cols) fp32 matrix with row pitch ld, written by TMA stores of 32 x 64 boxes staged in the 128-byte-swizzle layout
+static int make_store_map_f32(CUtensorMap* map, const float* base, long rows, long cols, long ld) {
+  auto enc = get_encode();
+  if (!enc) return (int)cudaErrorNotSupported;
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)(ld * sizeof(float))};
+  cuuint32_t box[2] = {32, 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
 }
@@ -917,7 +1022,7 @@ static int make_store_map(CUtensorMap* map, const bf16* base, long rows, long co
 template <int NSPLIT, int EPI, int BN, int MODE = 0>
 static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
                      const TcArgs& p, cudaStream_t s) {
-  using Cfg = TcCfg<NSPLIT, BN, EPI>;
+  using Cfg = TcCfg<NSPLIT, BN, EPI, (MODE & 8) != 0>;
   static PerDeviceOnce attr_once;
   const int attr_dev = PerDeviceOnce::device();
   if (!attr_once.done[attr_dev]) {
@@ -1066,6 +1171,17 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
     if (p.o_hi && (rc = make_store_map(&p.mapO[0], p.o_hi, M, N))) return rc;
     if (p.o_lo && (rc = make_store_map(&p.mapO[1], p.o_lo, M, N))) return rc;
   }
+  // 128x256 forward (fp32 C, optional bf16 image) and bf16 data gradient (MN-major weight operand): the accumulator
+  // leaves through TMA stores.  Their bases and row pitches must be 16-byte aligned; the slab epilogue's vector stores
+  // needed the same, so an unaligned output is refused here instead of faulting in the kernel.
+  const bool tma_epi = bn == 256 && (epi == TC_BIAS_RELU || (epi == TC_STORE && p.o_hi != nullptr && (p.mn_major & 2)));
+  if (tma_epi) {
+    const auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    if ((epi == TC_BIAS_RELU && (!al16(C) || ldc % 4)) || (p.o_hi && (!al16(p.o_hi) || N % 8)))
+      return (int)cudaErrorInvalidValue;
+    if (epi == TC_BIAS_RELU && (rc = make_store_map_f32(&p.mapO[0], C, M, N, ldc))) return rc;
+    if (p.o_hi && (rc = make_store_map(&p.mapO[1], p.o_hi, M, N, 64))) return rc;
+  }
   const auto go = [&](int epi) -> int {
 #define RIQN_TC_GO(NS, EP) return launch_tc<NS, EP, 128>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
 #define RIQN_TC_NARROW(NS, EP)                                                                  \
@@ -1089,9 +1205,10 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
         default: return (int)cudaErrorInvalidValue;
       }
     } else if (bn == 256) {
-      const int mode = p.mn_major | ((p.fmt & 3) ? 4 : 0);
+      const int mode = p.mn_major | ((p.fmt & 3) ? 4 : 0) | (tma_epi ? 8 : 0);
 #define RIQN_TC_WIDE(EP, MD) if (epi == EP && mode == MD) return launch_tc<1, EP, 256, MD>(ma_hi, ma_lo, mb_hi, mb_lo, p, s)
-      RIQN_TC_WIDE(TC_BIAS_RELU, 0); RIQN_TC_WIDE(TC_BIAS_RELU, 4);
+      RIQN_TC_WIDE(TC_BIAS_RELU, 8); RIQN_TC_WIDE(TC_BIAS_RELU, 12);
+      RIQN_TC_WIDE(TC_STORE, 10); RIQN_TC_WIDE(TC_STORE, 11); RIQN_TC_WIDE(TC_STORE, 14); RIQN_TC_WIDE(TC_STORE, 15);
       RIQN_TC_WIDE(TC_STORE, 0); RIQN_TC_WIDE(TC_STORE, 2); RIQN_TC_WIDE(TC_STORE, 3);
       RIQN_TC_WIDE(TC_STORE, 4); RIQN_TC_WIDE(TC_STORE, 6); RIQN_TC_WIDE(TC_STORE, 7);
       RIQN_TC_WIDE(TC_NOISY_WGRAD, 0); RIQN_TC_WIDE(TC_NOISY_WGRAD, 2); RIQN_TC_WIDE(TC_NOISY_WGRAD, 3);
