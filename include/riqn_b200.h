@@ -330,6 +330,33 @@ int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_spa
                            float* loss, float* dtheta, float* theta_out, float* target_out, float* bonus_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Value-function rescaling (Pohlen et al. 2018, the transformed Bellman operator; no counterpart in the reference)
+ *   h(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x, evaluated in double in the cancellation-free forms
+ *   h(x):     a = |x|;  m = a / (sqrt(a + 1) + 1);  h = copysign(m, x) + eps x
+ *   h^-1(y):  a = |y|;  u = (a + 1) + eps;  s = sqrt(1 + (4 eps) u);  d = ((4u) a) / (((2u - 1) + s) (s + 1));
+ *             h^-1 = copysign(d (d + 2), y)
+ * with every operation rounded on its own (no FMA), eps the float argument widened to double, and each stored value
+ * rounded once to float.  Every entry point below returns cudaErrorInvalidValue, writing nothing, for eps < 0 or
+ * non-finite, and for the limits it names.
+ * ---------------------------------------------------------------------------------------------- */
+/* out[i] = fl(h(x[i])) (inverse == 0) or fl(h^-1(x[i])) (inverse == 1), i < n.  out must not be NULL. */
+int riqn_value_rescale(long n, const float* x, float eps, int inverse, float* out, void* stream);
+/* riqn_iqn_loss_fwd_bwd against the transformed target, with g = fl(gamma_n * nonterminals[b]) as there:
+ *   target[b,j] = fl(h(returns[b] + g * h^-1(q_target[j*batch+b, a_star[b]])))     (sum and product in double)
+ * theta, loss and dtheta as in riqn_iqn_loss_fwd_bwd.  action_space <= 32. */
+int riqn_iqn_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                            const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                            const float* returns, const float* nonterminals, float gamma_n, float kappa, float eps,
+                            float* loss, float* dtheta, float* theta_out, float* target_out, void* stream);
+/* The expected return on the original scale of h-space quantiles q (n*batch, A), quantile-major, and its argmax:
+ *   values[b,a] = fl(sum_k w[k*batch+b] * h^-1(q[k*batch+b, a]))   (FQF: w = dtau)
+ *   values[b,a] = fl((sum_k h^-1(q[k*batch+b, a])) / n)             (w == NULL: IQN's mean over K fractions)
+ * summed in double over k ascending; a_star[b] = argmax_a values[b,a] on the rounded values, the first maximal index
+ * winning.  values (batch, A) and a_star (batch) may each be NULL, not both.  batch, n >= 1, 1 <= action_space <= 32. */
+int riqn_argmax_expected_h(int batch, int n, int action_space, const float* q, const float* w, float eps, float* values,
+                           long long* a_star, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * FQF: fraction proposal network (Yang et al., NeurIPS 2019; no counterpart in the reference)
  * The proposal's logits (batch, n) = feat W_f^T + b_f come from riqn_linear_fwd_ld (split-1 fp32 store, deterministic).
  * Every entry point below takes 2 <= n <= 256 (and 1 <= action_space <= 32, batch >= 1) and returns
@@ -381,6 +408,14 @@ int riqn_c51_loss_fwd_bwd(int batch, int action_space, int atoms, const float* l
                           const long long* actions, const long long* a_star, const float* returns,
                           const float* nonterminals, const float* support, float gamma_n, float v_min, float v_max,
                           float delta_z, float* loss, float* dq, float* m_out, void* stream);
+/* riqn_c51_loss_fwd_bwd with the transformed Bellman target (value rescaling, see riqn_value_rescale): each atom moves to
+ *   tz_j = fl(h(returns[b] + g * h^-1(support[j])))     g = fl(nonterminals[b] * gamma_n), sum and product in double
+ * before the clamp to [v_min, v_max]; the index, the l == u fix, the projection, loss and dq follow as there.  support is
+ * the h-space support.  atoms <= 64; eps as for riqn_value_rescale. */
+int riqn_c51_loss_fwd_bwd_h(int batch, int action_space, int atoms, const float* logp_online, const float* p_target,
+                            const long long* actions, const long long* a_star, const float* returns,
+                            const float* nonterminals, const float* support, float gamma_n, float v_min, float v_max,
+                            float delta_z, float eps, float* loss, float* dq, float* m_out, void* stream);
 /* dzv (batch, atoms), dza (batch, A*atoms) from dq scaled by gscale[b] (dueling backward). */
 int riqn_c51_head_bwd(int batch, int action_space, int atoms, const float* dq, const float* gscale, float gscale_mul,
                       const long long* actions, float* dzv, float* dza, void* stream);

@@ -79,6 +79,10 @@ SIGNATURES = {
     "riqn_c51_head_fwd":[C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,
                               C.c_float, _P, _P, _P, _P],
+    "riqn_value_rescale": [C.c_long, _P, C.c_float, C.c_int, _P, _P],
+    "riqn_iqn_loss_fwd_bwd_h": [C.c_int] * 4 + [_P] * 7 + [C.c_float] * 3 + [_P] * 5,
+    "riqn_argmax_expected_h": [C.c_int] * 3 + [_P, _P, C.c_float, _P, _P, _P],
+    "riqn_c51_loss_fwd_bwd_h": [C.c_int] * 3 + [_P] * 7 + [C.c_float] * 5 + [_P] * 4,
     "riqn_c51_head_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P, _P],
     "riqn_c51_head_bwd_dense": [C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P],
     "riqn_zero_f32": [_P, C.c_long, _P],

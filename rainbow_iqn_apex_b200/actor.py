@@ -10,6 +10,7 @@ import torch
 from . import fqf
 from ._lib import call, ptr
 from .agent import Agent
+from .compute_loss_iqn import greedy_actions
 from .learner import MODEL_WEIGHT_STR
 
 
@@ -32,55 +33,59 @@ class Actor(Agent):
 
     def _fqf_argmax(self, states_u8):
         q, dtau = self._fqf_pass(states_u8)
-        a = torch.empty(states_u8.shape[0], dtype=torch.int64, device=q.device)
-        call("riqn_argmax_weighted", states_u8.shape[0], self.num_tau_samples, self.action_space, ptr(q), ptr(dtau), ptr(a))
-        return a
+        return greedy_actions(self, states_u8.shape[0], self.num_tau_samples, q, dtau)
 
     def act(self, state_buffer):
         """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN; distorted by ``self.risk``), the
         dtau-weighted mean over the proposed fractions (FQF) or the expected value of the categorical distribution (C51).
-        Frames go to the device as uint8; the /255 of the reference happens inside the conv kernel."""
+        Under value rescaling each of them is the expectation of h^-1 of the network's h-space values, the return's own
+        scale.  Frames go to the device as uint8; the /255 of the reference happens inside the conv kernel."""
         state = torch.from_numpy(np.stack(state_buffer).astype(np.uint8)).to(self.online_net._flat.device)
         with torch.no_grad():
             if self.rainbow_only:
                 p = self.online_net(state.unsqueeze(0))
-                return (p * self.support).sum(2).argmax(1).item()
+                return (p * self.acting_support).sum(2).argmax(1).item()
             if self.fqf is not None:
                 return int(self._fqf_argmax(state.unsqueeze(0)).item())
             quantile_values, _ = self.online_net(state.unsqueeze(0), self.num_quantile_samples, tau=self._pop_tau(),
                                                   risk=self.risk)
-            a = torch.empty(1, dtype=torch.int64, device=state.device)
-            call("riqn_argmax_mean", 1, self.num_quantile_samples, self.action_space, ptr(quantile_values), ptr(a))
-            return int(a.item())
+            return int(greedy_actions(self, 1, self.num_quantile_samples, quantile_values).item())
 
     def act_batch(self, states_u8):
         """Batched greedy actions for many environments at once: states (E, history, 84, 84) uint8 -> (E,)."""
         with torch.no_grad():
             if self.rainbow_only:
-                return (self.online_net(states_u8) * self.support).sum(2).argmax(1)
+                return (self.online_net(states_u8) * self.acting_support).sum(2).argmax(1)
             if self.fqf is not None:
                 return self._fqf_argmax(states_u8)
-            E = states_u8.shape[0]
             q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=self._pop_tau(), risk=self.risk)
-            a = torch.empty(E, dtype=torch.int64, device=q.device)
-            call("riqn_argmax_mean", E, self.num_quantile_samples, self.action_space, ptr(q), ptr(a))
-            return a
+            return greedy_actions(self, states_u8.shape[0], self.num_quantile_samples, q)
 
     def act_batch_values(self, states_u8, tau=None):
         """(E, A) mean quantile values behind act_batch (the argmax input; parity tests and epsilon schedules): Q_beta
         under ``self.risk``, the mean over K fractions beta(tau) unless ``tau`` is given.  FQF: sum_i dtau_i F(s, tau_hat_i, a)
-        over the proposed fractions (``tau`` is not taken)."""
+        over the proposed fractions (``tau`` is not taken).  Under value rescaling: the same expectations of h^-1 of the
+        quantile values, on the return's scale (riqn_argmax_expected_h)."""
         with torch.no_grad():
             E = states_u8.shape[0]
             if self.fqf is not None:
                 if tau is not None:
                     raise ValueError("FQF acts on its proposed fractions: act_batch_values takes no tau")
-                q, dtau = self._fqf_pass(states_u8)
-                return fqf.q_values(q, dtau, E, self.num_tau_samples, self.action_space)
-            q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=tau if tau is not None else self._pop_tau(),
-                                   risk=self.risk)
+                q, w = self._fqf_pass(states_u8)
+                n = self.num_tau_samples
+            else:
+                q, _ = self.online_net(states_u8, self.num_quantile_samples,
+                                       tau=tau if tau is not None else self._pop_tau(), risk=self.risk)
+                w, n = None, self.num_quantile_samples
+            if self.value_rescaling is not None:
+                values = torch.empty(E, self.action_space, device=q.device)
+                call("riqn_argmax_expected_h", E, n, self.action_space, ptr(q), ptr(w), self.value_rescaling, ptr(values),
+                     None)
+                return values
+            if w is not None:
+                return fqf.q_values(q, w, E, n, self.action_space)
             # q rows are quantile-major (k*E + e), like the reference (model.py:149)
-            return q.view(self.num_quantile_samples, E, self.action_space).mean(0)
+            return q.view(n, E, self.action_space).mean(0)
 
     def act_e_greedy(self, state_buffer, epsilon=0.001):
         """actor.py:27-34"""

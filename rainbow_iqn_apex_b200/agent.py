@@ -4,7 +4,8 @@ Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``
 attributes (online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
 compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
-``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions.  The
+``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
+``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards.  The
 networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference
 schema {T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus the fraction network's two
 entries under FQF.
@@ -76,6 +77,23 @@ class Agent:
             if checkpoint is not None and "fraction_net_state_dict" in checkpoint:
                 self.fraction_net.load_state_dict(checkpoint["fraction_net_state_dict"])
                 self.fraction_optimiser.load_state_dict(checkpoint["fraction_optimiser_state_dict"])
+        # value rescaling (the transformed Bellman operator): optional args fields (absent from the reference's namespace:
+        # off).  None, or eps of compute_loss_iqn.check_value_rescaling; fixed for the agent's life, so that a captured
+        # step graph stays valid
+        self.value_rescaling = compute_loss_iqn.check_value_rescaling(
+            getattr(args, "value_rescaling", 0),
+            *(getattr(args, f, v) for f, v in compute_loss_iqn.VALUE_RESCALING_DEFAULTS.items()), munchausen=self.munchausen)
+        if checkpoint is not None and checkpoint.get("value_rescaling_eps") != self.value_rescaling:
+            raise ValueError(f"the checkpoint was trained with value_rescaling_eps = {checkpoint.get('value_rescaling_eps')} "
+                             f"(None: off), the args ask for {self.value_rescaling}: a network trained in h-space acts "
+                             "differently on the linear scale")
+        if self.rainbow_only:
+            # the support the C51 head takes expectations over when it acts: h^-1 of the h-space support under rescaling
+            self.acting_support = self.support
+            if self.value_rescaling is not None:
+                self.acting_support = torch.empty_like(self.support)
+                _lib.call("riqn_value_rescale", self.atoms, _lib.ptr(self.support), self.value_rescaling, 1,
+                          _lib.ptr(self.acting_support))
         # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
         self.risk = None
         self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
@@ -125,7 +143,8 @@ class Agent:
 
     def save(self, path, T_actors, T_learner, name):
         """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
-        fraction_optimiser_state_dict; model_state_dict keeps the reference schema either way."""
+        fraction_optimiser_state_dict, under value rescaling value_rescaling_eps; model_state_dict keeps the reference
+        schema either way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
@@ -135,6 +154,8 @@ class Agent:
         if self.fqf is not None:
             ckpt["fraction_net_state_dict"] = self.fraction_net.state_dict()
             ckpt["fraction_optimiser_state_dict"] = self.fraction_optimiser.state_dict()
+        if self.value_rescaling is not None:
+            ckpt["value_rescaling_eps"] = self.value_rescaling
         torch.save(ckpt, os.path.join(path, name))
 
     def train(self):

@@ -71,7 +71,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     noises = inj["noises"] if inj else (None, None, None)
     on.reset_noise(noises[1])                                              # :95
     a_star = torch.empty(B, dtype=torch.int64, device=dev)
-    forward(on, next_states, fresh_weights=True, want_argmax=a_star, support=agent.support)         # :97-102
+    forward(on, next_states, fresh_weights=True, want_argmax=a_star, support=agent.acting_support)  # :97-102
     tg.reset_noise(noises[2])                                              # :103
     pns = forward(tg, next_states, fresh_weights=True, support=agent.support)                      # :104
     on.reset_noise(noises[0])                                              # agent.py:82
@@ -80,9 +80,13 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     loss = torch.empty(B, device=dev)
     dq = torch.empty(B, atoms, device=dev)
     m_out = torch.empty(B, atoms, device=dev) if debug is not None else None
-    call("riqn_c51_loss_fwd_bwd", B, A, atoms, ptr(log_ps), ptr(pns), ptr(actions), ptr(a_star), ptr(returns),
-         ptr(nonterminals), ptr(agent.support), float(agent.discount ** agent.n), float(agent.Vmin), float(agent.Vmax),
-         float(agent.delta_z), ptr(loss), ptr(dq), ptr(m_out))
+    args = (ptr(log_ps), ptr(pns), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals), ptr(agent.support),
+            float(agent.discount ** agent.n), float(agent.Vmin), float(agent.Vmax), float(agent.delta_z))
+    eps = getattr(agent, "value_rescaling", None)
+    if eps is None:
+        call("riqn_c51_loss_fwd_bwd", B, A, atoms, *args, ptr(loss), ptr(dq), ptr(m_out))
+    else:   # the atoms move to h(R + gamma^n nt h^-1(z_j)) before the projection
+        call("riqn_c51_loss_fwd_bwd_h", B, A, atoms, *args, eps, ptr(loss), ptr(dq), ptr(m_out))
     if debug is not None:
         debug.update(a_star=a_star, m=m_out, log_ps=log_ps)
     version = getattr(on, "_noise_version", 0)       # bumped by every DQN.reset_noise()

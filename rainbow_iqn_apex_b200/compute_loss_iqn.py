@@ -56,6 +56,60 @@ def check_munchausen(munchausen, alpha=0.9, entropy_tau=0.03, l0=-1.0, rainbow_o
     return tuple(vals)
 
 
+VALUE_RESCALING_DEFAULTS = {"value_rescaling_eps": 1e-3}   # R2D2's epsilon
+
+
+def check_value_rescaling(value_rescaling, eps=1e-3, munchausen=None):
+    """Validate a value-rescaling configuration (the transformed Bellman operator, Pohlen et al. 2018).  Returns None when
+    ``value_rescaling`` is off (0 / False), else eps: finite and >= 0 as the kernels receive it (float32).  It applies to
+    the IQN, FQF and C51 losses and does not combine with Munchausen targets (``munchausen`` must be None), whose soft
+    target mixes log-policies of means.  Raises ValueError otherwise."""
+    if isinstance(value_rescaling, bool) or (isinstance(value_rescaling, numbers.Integral) and value_rescaling in (0, 1)):
+        if not value_rescaling:
+            return None
+    else:
+        raise ValueError(f"value_rescaling must be 0 or 1, got {value_rescaling!r}")
+    if isinstance(eps, bool) or not isinstance(eps, numbers.Real):
+        raise ValueError(f"value_rescaling_eps must be a real number, got {eps!r}")
+    f = ctypes.c_float(eps).value
+    if not (math.isfinite(f) and f >= 0.0):
+        raise ValueError(f"value_rescaling_eps must be finite and >= 0 (as a float32), got {eps!r}")
+    if munchausen is not None:
+        raise ValueError("value rescaling and Munchausen targets do not combine: set value_rescaling = 0 or munchausen = 0")
+    return float(eps)
+
+
+def greedy_actions(agent, batch, n, q, w=None):
+    """a* (batch,) int64: the greedy actions of quantile values q (n*batch, A), quantile-major, on the mean over the n
+    fractions (``w`` None, IQN) or the w-weighted sum (FQF: w = dtau).  Under value rescaling (agent.value_rescaling) q
+    lives in h-space and the expectation is taken of h^-1(q), the original scale (riqn_argmax_expected_h); otherwise
+    riqn_argmax_mean / riqn_argmax_weighted."""
+    A = agent.action_space
+    a_star = torch.empty(batch, dtype=torch.int64, device=q.device)
+    eps = getattr(agent, "value_rescaling", None)
+    if eps is not None:
+        call("riqn_argmax_expected_h", batch, n, A, ptr(q), ptr(w), eps, None, ptr(a_star))
+    elif w is None:
+        call("riqn_argmax_mean", batch, n, A, ptr(q), ptr(a_star))
+    else:
+        call("riqn_argmax_weighted", batch, n, A, ptr(q), ptr(w), ptr(a_star))
+    return a_star
+
+
+def _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
+                   target_out):
+    """The double-DQN quantile-Huber loss kernel: riqn_iqn_loss_fwd_bwd, or against the transformed target
+    h(R + gamma^n nt h^-1(Z)) under value rescaling (riqn_iqn_loss_fwd_bwd_h)."""
+    args = (ptr(q_on), ptr(q_tgt), ptr(tau), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals),
+            float(agent.discount ** agent.n), float(agent.kappa))
+    outs = (ptr(loss), ptr(dtheta), ptr(theta_out), ptr(target_out))
+    eps = getattr(agent, "value_rescaling", None)
+    if eps is None:
+        call("riqn_iqn_loss_fwd_bwd", B, N, Np, agent.action_space, *args, *outs)
+    else:
+        call("riqn_iqn_loss_fwd_bwd_h", B, N, Np, agent.action_space, *args, eps, *outs)
+
+
 def _as_device_inputs(agent, states, actions, returns, next_states, nonterminals):
     dev = agent.online_net._flat.device
 
@@ -73,7 +127,6 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
         agent, states, actions, returns, next_states, nonterminals)
     on, tg = agent.online_net, agent.target_net
     B = states.shape[0]
-    A = agent.action_space
     K, Np, N = agent.num_quantile_samples, agent.num_tau_prime_samples, agent.num_tau_samples
     inj = getattr(agent, "_inject", None)
     if isinstance(inj, list):            # a queue of injections: one per call (Actor.compute_priorities chunks)
@@ -94,8 +147,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     # the action selection alone acts under the agent's risk measure (IQN paper, section 3.1): a* = argmax_a Q_beta(x', a)
     q_sel, tau_sel = on.forward(next_states, K, tau=taus[0], fresh_weights=True, col_cache=cache, feat=f_on,
                                 risk=getattr(agent, "risk", None))                                        # :235-237
-    a_star = torch.empty(B, dtype=torch.int64, device=dev)
-    call("riqn_argmax_mean", B, K, A, ptr(q_sel), ptr(a_star))                      # :238-245
+    a_star = greedy_actions(agent, B, K, q_sel)                                     # :238-245
     tg.reset_noise(noises[1])                                                       # :255
     q_tgt, _ = tg.forward(next_states, Np, tau=taus[1], fresh_weights=True, col_cache=cache, feat=f_tg)  # :256-258
     on.reset_noise(noises[2])                                                       # :289
@@ -108,9 +160,8 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, Np, device=dev)
-    call("riqn_iqn_loss_fwd_bwd", B, N, Np, A, ptr(q_on), ptr(q_tgt), ptr(tau), ptr(actions), ptr(a_star),
-         ptr(returns), ptr(nonterminals), float(agent.discount ** agent.n), float(agent.kappa), ptr(loss),
-         ptr(dtheta), ptr(theta_out), ptr(target_out))                              # :262-357
+    _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
+                   target_out)                                                      # :262-357
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on, tau=tau,
                      keep=keep, tau_sel=tau_sel)
@@ -157,7 +208,7 @@ def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises
     boundaries tau_1..tau_{N-1} (no-grad) for the fraction loss's W1 gradient.  With ``keep_graph`` the fraction state
     goes into ``keep["fqf"]`` for fraction_backward."""
     on, tg, fnet = agent.online_net, agent.target_net, agent.fraction_net
-    B, A, N = states.shape[0], agent.action_space, agent.num_tau_samples
+    B, N = states.shape[0], agent.num_tau_samples
     dev = states.device
     on.reset_noise(noises[0])
     cache = {}
@@ -165,8 +216,7 @@ def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises
     f_on, f_tg = pair if pair is not None else (on.trunk(next_states, col_cache=cache), None)
     fr_n = fnet.propose(f_on)                                                         # fractions of s'
     q_sel, _ = on.forward(next_states, N, tau=fr_n["tau_hat"], fresh_weights=True, col_cache=cache, feat=f_on)
-    a_star = torch.empty(B, dtype=torch.int64, device=dev)
-    call("riqn_argmax_weighted", B, N, A, ptr(q_sel), ptr(fr_n["dtau"]), ptr(a_star))
+    a_star = greedy_actions(agent, B, N, q_sel, fr_n["dtau"])
     # the conv trunk is noise-free: the gradient pass's trunk runs here, once, and its features propose the fractions of s
     keep = {} if keep_graph else None
     feat = on.trunk(states, keep)
@@ -186,9 +236,8 @@ def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, N, device=dev)
-    call("riqn_iqn_loss_fwd_bwd", B, N, N, A, ptr(q_on), ptr(q_tgt), ptr(tau_hat), ptr(actions), ptr(a_star),
-         ptr(returns), ptr(nonterminals), float(agent.discount ** agent.n), float(agent.kappa), ptr(loss),
-         ptr(dtheta), ptr(theta_out), ptr(target_out))
+    _quantile_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
+                   target_out)
     if keep is not None:
         keep["fqf"] = dict(fr=fr, q_hat=q_on, q_bnd=q_bnd, actions=actions, debug=debug)
     if debug is not None:

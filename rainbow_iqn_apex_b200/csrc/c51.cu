@@ -4,6 +4,7 @@
 // the cross-entropy and its gradient, plus small strided linear-layer helpers for the (B, 512) x (51 | 918) z-layers.
 #include "common.cuh"
 #include "gemm.h"
+#include "value_rescaling.cuh"
 #include "../../include/riqn_b200.h"
 
 namespace riqn {
@@ -62,11 +63,14 @@ __global__ void c51_head_fwd_kernel(int A, int atoms, const float* __restrict__ 
 
 // One block per sample: categorical projection (agent.py:104-133), loss = -sum_j m_j logp[b, act, j] (agent.py:141)
 // and dq[b, j] = d loss / d q[b, act, j] = -(m_j - p_j sum_k m_k).
+// RESCALE: the atoms move to tz_j = fl(h(R + g * h^-1(support[j]))) (value_rescaling.cuh; the sum and product rounded in
+// double) before the clamp; eps is read only then.
+template <bool RESCALE>
 __global__ void c51_loss_kernel(int A, int atoms, const float* __restrict__ logp_online, const float* __restrict__ p_target,
                                 const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
                                 const float* __restrict__ returns, const float* __restrict__ nonterminals,
                                 const float* __restrict__ support, float gamma_n, float vmin, float vmax, float delta_z,
-                                float* __restrict__ loss, float* __restrict__ dq, float* __restrict__ m_out) {
+                                float* __restrict__ loss, float* __restrict__ dq, float* __restrict__ m_out, float eps) {
   extern __shared__ float sm[];      // m[atoms] | lo[atoms] | up[atoms] | wl[atoms] | wu[atoms]
   float* m = sm;
   int* lo = reinterpret_cast<int*>(sm + atoms);
@@ -78,7 +82,13 @@ __global__ void c51_loss_kernel(int A, int atoms, const float* __restrict__ logp
   const float* pa = p_target + ((long)b * A + as) * atoms;
   const float g = __fmul_rn(nonterminals[b], gamma_n);
   for (int j = threadIdx.x; j < atoms; j += blockDim.x) {
-    float tz = __fadd_rn(returns[b], __fmul_rn(g, support[j]));
+    float tz;
+    if constexpr (RESCALE) {
+      const double z = vr_h_inv((double)support[j], (double)eps);
+      tz = __double2float_rn(vr_h(__dadd_rn((double)returns[b], __dmul_rn((double)g, z)), (double)eps));
+    } else {
+      tz = __fadd_rn(returns[b], __fmul_rn(g, support[j]));
+    }
     tz = fminf(fmaxf(tz, vmin), vmax);
     // The clamp of tz does not bound the index: fp32 rounding of the division can take bj just above atoms - 1
     // (v_min = -1, v_max = 1, 62 atoms: tz = v_max gives 61.0000038), and u = atoms would add wu past m.  Every
@@ -201,9 +211,22 @@ RIQN_API int riqn_c51_loss_fwd_bwd(int batch, int action_space, int atoms, const
                                    const float* nonterminals, const float* support, float gamma_n, float v_min, float v_max,
                                    float delta_z, float* loss, float* dq, float* m_out, void* stream) {
   riqn::note_launches(1);
-  c51_loss_kernel<<<batch, 64, sizeof(float) * 5 * atoms, (cudaStream_t)stream>>>(
+  c51_loss_kernel<false><<<batch, 64, sizeof(float) * 5 * atoms, (cudaStream_t)stream>>>(
       action_space, atoms, logp_online, p_target, (const int64_t*)actions, (const int64_t*)a_star, returns, nonterminals,
-      support, gamma_n, v_min, v_max, delta_z, loss, dq, m_out);
+      support, gamma_n, v_min, v_max, delta_z, loss, dq, m_out, 0.f);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_c51_loss_fwd_bwd_h(int batch, int action_space, int atoms, const float* logp_online,
+                                     const float* p_target, const long long* actions, const long long* a_star,
+                                     const float* returns, const float* nonterminals, const float* support,
+                                     float gamma_n, float v_min, float v_max, float delta_z, float eps, float* loss,
+                                     float* dq, float* m_out, void* stream) {
+  if (!vr_eps_ok(eps) || atoms > 64) return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  c51_loss_kernel<true><<<batch, 64, sizeof(float) * 5 * atoms, (cudaStream_t)stream>>>(
+      action_space, atoms, logp_online, p_target, (const int64_t*)actions, (const int64_t*)a_star, returns, nonterminals,
+      support, gamma_n, v_min, v_max, delta_z, loss, dq, m_out, eps);
   return (int)cudaGetLastError();
 }
 

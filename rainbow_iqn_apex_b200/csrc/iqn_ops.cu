@@ -7,6 +7,7 @@
 // warp-broadcast load and the reduction over a sample's quantiles is contiguous.
 #include "common.cuh"
 #include "gemm.h"
+#include "value_rescaling.cuh"
 #include "../../include/riqn_b200.h"
 
 namespace riqn {
@@ -727,6 +728,46 @@ __global__ void argmax_mean_kernel(int B, int K, int A, const float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
+// Expected return on the original scale of h-space quantiles, and its argmax:
+//   v[b,a] = fl(sum_k w[k*B+b] h^-1(q[k*B+b, a]))   or, w == NULL, fl((sum_k h^-1(q[k*B+b, a])) / K)
+// in double, k ascending; the argmax runs on the rounded values, the first maximal index winning.
+// One warp per sample, lane a for action a (A <= 32).
+// ------------------------------------------------------------------------------------------------
+__global__ void argmax_expected_h_kernel(int B, int K, int A, const float* __restrict__ q, const float* __restrict__ wk,
+                                         double eps, float* __restrict__ values, int64_t* __restrict__ a_star) {
+  const int b = (int)(((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (b >= B) return;
+  float s = -INFINITY;
+  if (lane < A) {
+    double acc = 0.0;
+    for (int k = 0; k < K; ++k) {
+      const double z = vr_h_inv((double)q[((long)k * B + b) * A + lane], eps);
+      acc = __dadd_rn(acc, wk ? __dmul_rn((double)wk[(long)k * B + b], z) : z);
+    }
+    s = __double2float_rn(wk ? acc : __ddiv_rn(acc, (double)K));
+    if (values) values[(long)b * A + lane] = s;
+  }
+  float best = s;
+  int arg = lane;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
+    if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+  }
+  if (a_star && lane == 0) a_star[b] = arg;
+}
+
+// out[i] = fl(h(x[i])) or, inverse, fl(h^-1(x[i]))
+__global__ void value_rescale_kernel(long n, const float* __restrict__ x, double eps, int inverse, float* __restrict__ out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double v = (double)x[i];
+  out[i] = __double2float_rn(inverse ? vr_h_inv(v, eps) : vr_h(v, eps));
+}
+
+// ------------------------------------------------------------------------------------------------
 // Fused IQN quantile-Huber loss, forward + dloss/dtheta            (compute_loss_iqn.py:262-357)
 //   T[b,j]   = R[b] + fl(gamma^n)*nt[b] * q_tgt[(j*B+b), a*[b]]
 //   th[b,i]  = q_on[(i*B+b), act[b]]
@@ -768,19 +809,28 @@ __device__ __forceinline__ void quantile_huber_loss(int B, int N, int Np, int A,
   }
 }
 
+// RESCALE: the transformed Bellman target T[b,j] = fl(h(R[b] + g * h^-1(q_tgt[...])))  (value_rescaling.cuh), with
+// g = fl(gamma^n*nt[b]) as above and the sum and product rounded in double; eps is read only then.
+template <bool RESCALE>
 __global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
                                 const float* __restrict__ q_tgt, const float* __restrict__ tau,
                                 const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
                                 const float* __restrict__ returns, const float* __restrict__ nonterminals,
                                 float gamma_n, float kappa, float* __restrict__ loss, float* __restrict__ dtheta,
-                                float* __restrict__ theta_out, float* __restrict__ target_out) {
+                                float* __restrict__ theta_out, float* __restrict__ target_out, float eps) {
   extern __shared__ float sT[];  // Np targets + 32 reduction slots
   float* red = sT + Np;
   const int b = blockIdx.x, tid = threadIdx.x;
   const int as = (int)a_star[b], ac = (int)actions[b];
   const float g = __fmul_rn(gamma_n, nonterminals[b]);
   for (int j = tid; j < Np; j += blockDim.x) {
-    const float t = __fadd_rn(returns[b], __fmul_rn(g, q_tgt[((long)j * B + b) * A + as]));
+    float t;
+    if constexpr (RESCALE) {
+      const double z = vr_h_inv((double)q_tgt[((long)j * B + b) * A + as], (double)eps);
+      t = __double2float_rn(vr_h(__dadd_rn((double)returns[b], __dmul_rn((double)g, z)), (double)eps));
+    } else {
+      t = __fadd_rn(returns[b], __fmul_rn(g, q_tgt[((long)j * B + b) * A + as]));
+    }
     sT[j] = t;
     if (target_out) target_out[(long)b * Np + j] = t;
   }
@@ -1638,9 +1688,44 @@ RIQN_API int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int ac
   if (threads > 1024) threads = 1024;
   if (threads < 32) threads = 32;
   const size_t smem = sizeof(float) * (n_tau_prime + 32);
-  iqn_loss_kernel<<<batch, threads, smem, (cudaStream_t)stream>>>(
+  iqn_loss_kernel<false><<<batch, threads, smem, (cudaStream_t)stream>>>(
       batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, (const int64_t*)a_star,
-      returns, nonterminals, gamma_n, kappa, loss, dtheta, theta_out, target_out);
+      returns, nonterminals, gamma_n, kappa, loss, dtheta, theta_out, target_out, 0.f);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_iqn_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                                     const float* q_target, const float* tau, const long long* actions,
+                                     const long long* a_star, const float* returns, const float* nonterminals,
+                                     float gamma_n, float kappa, float eps, float* loss, float* dtheta, float* theta_out,
+                                     float* target_out, void* stream) {
+  if (!vr_eps_ok(eps) || action_space > 32) return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;
+  if (threads > 1024) threads = 1024;
+  if (threads < 32) threads = 32;
+  const size_t smem = sizeof(float) * (n_tau_prime + 32);
+  iqn_loss_kernel<true><<<batch, threads, smem, (cudaStream_t)stream>>>(
+      batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, (const int64_t*)a_star,
+      returns, nonterminals, gamma_n, kappa, loss, dtheta, theta_out, target_out, eps);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_argmax_expected_h(int batch, int n, int action_space, const float* q, const float* w, float eps,
+                                    float* values, long long* a_star, void* stream) {
+  if (!vr_eps_ok(eps) || batch < 1 || n < 1 || action_space < 1 || action_space > 32 || (!values && !a_star))
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  argmax_expected_h_kernel<<<riqn_cdiv((long)batch * 32, 128), 128, 0, (cudaStream_t)stream>>>(
+      batch, n, action_space, q, w, (double)eps, values, (int64_t*)a_star);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_value_rescale(long n, const float* x, float eps, int inverse, float* out, void* stream) {
+  if (!vr_eps_ok(eps) || n < 0 || (inverse != 0 && inverse != 1) || !out) return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  if (n == 0) return 0;
+  value_rescale_kernel<<<riqn_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(n, x, (double)eps, inverse, out);
   return (int)cudaGetLastError();
 }
 
