@@ -425,6 +425,29 @@ int riqn_c51_head_bwd(int batch, int action_space, int atoms, const float* dq, c
  * atoms <= 64. */
 int riqn_c51_head_bwd_dense(int batch, int action_space, int atoms, const float* out, const float* grad_out, int is_log,
                             float* dzv, float* dza, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * QR-DQN head (Dabney, Rowland, Bellemare & Munos, AAAI 2018; no counterpart in the reference)
+ * The C51-shaped z-layers zv (batch, n), za (batch, A*n) give n quantile values per action at the fixed fractions
+ * tau_hat_i = (2i+1)/(2n); q is written quantile-major (n*batch, A), row i*batch + b, as the IQN head writes it, so the
+ * quantile-Huber loss, riqn_argmax_mean and riqn_argmax_expected_h read it unchanged.  Every entry point below returns
+ * cudaErrorInvalidValue, writing nothing, unless 2 <= n <= 256, 1 <= action_space <= 32 and batch >= 1.  No atomics:
+ * each output element is computed by one thread in the stated order.
+ * ---------------------------------------------------------------------------------------------- */
+/* The dueling sum per quantile, with every operation rounded to fp32 on its own:
+ *   s_i = sum_a za[b, a*n + i]                         (fp32 adds, a ascending, starting from 0)
+ *   q[(i*batch + b)*A + a] = fl(fl(zv[b,i] + za[b, a*n + i]) - fl(s_i / A)) */
+int riqn_qr_head_fwd(int batch, int action_space, int n, const float* zv, const float* za, float* q, void* stream);
+/* Backward of the loss kernel's one-hot gradient dL/dq[i*batch+b, a] = 1{a == actions[b]} dtheta[i*batch+b] w_b,
+ * w_b = fl(gscale[b] * gscale_mul) (gscale may be NULL: w_b = gscale_mul), with dtheta (n*batch) quantile-major as
+ * riqn_iqn_loss_fwd_bwd writes it.  Rounded as riqn_c51_head_bwd on dq[b, i] = dtheta[i*batch+b] (bit for bit):
+ *   g = fl(dtheta[i*batch+b] * w_b) ;  dzv[b,i] = g ;  dza[b, a*n+i] = fl(g * fl(1{a == actions[b]} - fl(1 / A))) */
+int riqn_qr_head_bwd(int batch, int action_space, int n, const float* dtheta, const float* gscale, float gscale_mul,
+                     const long long* actions, float* dzv, float* dza, void* stream);
+/* Backward of a dense G = dL/dq (n*batch, A), quantile-major:
+ *   dzv[b,i] = sum_a G[i*batch+b, a]   (fp32 adds, a ascending, starting from 0)
+ *   dza[b, a*n+i] = fl(G[i*batch+b, a] - fl(dzv[b,i] / A)) */
+int riqn_qr_head_bwd_dense(int batch, int action_space, int n, const float* grad_q, float* dzv, float* dza, void* stream);
 /* n floats <- 0 (the gradient arena's zero_grad, learner.py:22): cudaMemsetAsync on the caller's stream. */
 int riqn_zero_f32(float* p, long n, void* stream);
 /* grad[i] = 0 where act[i] <= 0. */

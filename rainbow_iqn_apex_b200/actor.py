@@ -37,7 +37,8 @@ class Actor(Agent):
 
     def act(self, state_buffer):
         """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN; distorted by ``self.risk``), the
-        dtau-weighted mean over the proposed fractions (FQF) or the expected value of the categorical distribution (C51).
+        dtau-weighted mean over the proposed fractions (FQF), the mean over the N fixed-fraction quantiles (QR-DQN) or the
+        expected value of the categorical distribution (C51).
         Under value rescaling each of them is the expectation of h^-1 of the network's h-space values, the return's own
         scale.  Frames go to the device as uint8; the /255 of the reference happens inside the conv kernel."""
         state = torch.from_numpy(np.stack(state_buffer).astype(np.uint8)).to(self.online_net._flat.device)
@@ -47,6 +48,9 @@ class Actor(Agent):
                 return (p * self.acting_support).sum(2).argmax(1).item()
             if self.fqf is not None:
                 return int(self._fqf_argmax(state.unsqueeze(0)).item())
+            if self.qr_dqn is not None:
+                q, _ = self.online_net(state.unsqueeze(0))
+                return int(greedy_actions(self, 1, self.qr_dqn, q).item())
             quantile_values, _ = self.online_net(state.unsqueeze(0), self.num_quantile_samples, tau=self._pop_tau(),
                                                   risk=self.risk)
             return int(greedy_actions(self, 1, self.num_quantile_samples, quantile_values).item())
@@ -58,13 +62,17 @@ class Actor(Agent):
                 return (self.online_net(states_u8) * self.acting_support).sum(2).argmax(1)
             if self.fqf is not None:
                 return self._fqf_argmax(states_u8)
+            if self.qr_dqn is not None:
+                q, _ = self.online_net(states_u8)
+                return greedy_actions(self, states_u8.shape[0], self.qr_dqn, q)
             q, _ = self.online_net(states_u8, self.num_quantile_samples, tau=self._pop_tau(), risk=self.risk)
             return greedy_actions(self, states_u8.shape[0], self.num_quantile_samples, q)
 
     def act_batch_values(self, states_u8, tau=None):
         """(E, A) mean quantile values behind act_batch (the argmax input; parity tests and epsilon schedules): Q_beta
         under ``self.risk``, the mean over K fractions beta(tau) unless ``tau`` is given.  FQF: sum_i dtau_i F(s, tau_hat_i, a)
-        over the proposed fractions (``tau`` is not taken).  Under value rescaling: the same expectations of h^-1 of the
+        over the proposed fractions (``tau`` is not taken).  QR-DQN: mean_i q_i(s, a) over its N fixed fractions (``tau`` is
+        not taken).  Under value rescaling: the same expectations of h^-1 of the
         quantile values, on the return's scale (riqn_argmax_expected_h)."""
         with torch.no_grad():
             E = states_u8.shape[0]
@@ -73,6 +81,11 @@ class Actor(Agent):
                     raise ValueError("FQF acts on its proposed fractions: act_batch_values takes no tau")
                 q, w = self._fqf_pass(states_u8)
                 n = self.num_tau_samples
+            elif self.qr_dqn is not None:
+                if tau is not None:
+                    raise ValueError("QR-DQN acts on its N fixed fractions: act_batch_values takes no tau")
+                q, _ = self.online_net(states_u8)
+                w, n = None, self.qr_dqn
             else:
                 q, _ = self.online_net(states_u8, self.num_quantile_samples,
                                        tau=tau if tau is not None else self._pop_tau(), risk=self.risk)

@@ -5,17 +5,17 @@ attributes (online_net, target_net, optimiser, n, history, discount, device, bat
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
 compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
 ``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
-``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards.  The
-networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference
-schema {T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus the fraction network's two
-entries under FQF.
+``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
+``qr_dqn`` for QR-DQN's fixed-fraction quantile head.  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
+optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
 """
 import os
 
 import torch
 
 from . import _lib
-from . import compute_loss_iqn, fqf
+from . import compute_loss_iqn, fqf, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -36,6 +36,13 @@ class Agent:
 
         # online network (+ optional checkpoint, agent.py:26-34), noisy target copy with frozen parameters (:37-41), Adam (:43)
         checkpoint = self._read_checkpoint(getattr(args, "model", None))
+        # QR-DQN: optional args field (absent from the reference's namespace: off).  None, or N of qr.check_qr; checked
+        # against the checkpoint before its weights load (a QR network with N = atoms has the C51 network's shapes)
+        self.qr_dqn = qr.check_qr(getattr(args, "qr_dqn", 0), getattr(args, "num_tau_samples", None), action_space,
+                                  rainbow_only=self.rainbow_only)
+        if checkpoint is not None and checkpoint.get("qr_dqn_quantiles") != self.qr_dqn:
+            raise ValueError(f"the checkpoint was trained with qr_dqn_quantiles = {checkpoint.get('qr_dqn_quantiles')} "
+                             f"(None: not QR-DQN), the args ask for {self.qr_dqn}: the z-layers hold other quantities")
         self.online_net = DQN(args, action_space).to(device=args.device)
         if checkpoint is not None:
             self.online_net.load_state_dict(checkpoint["model_state_dict"])
@@ -54,11 +61,13 @@ class Agent:
                 setattr(self, attr, getattr(args, field))
             self.support = torch.linspace(self.Vmin, self.Vmax, self.atoms).to(device=args.device)
             self.delta_z = (self.Vmax - self.Vmin) / (self.atoms - 1)
+        elif self.qr_dqn is not None:                    # QR-DQN: N fixed fractions, nothing sampled
+            self.kappa, self.num_tau_samples = args.kappa, self.qr_dqn
         else:                                            # IQN sampling sizes (agent.py:58-63)
             for field in self._IQN_FIELDS:
                 setattr(self, field, getattr(args, field))
         self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each;
-        #                      FQF: {"noises": (n0, n1, n2)}
+        #                      FQF and QR-DQN: {"noises": (n0, n1, n2)}
         # Munchausen-IQN targets: optional args fields (absent from the reference's namespace: plain IQN).
         # None, or (alpha, entropy_tau, l0) of compute_loss_iqn.check_munchausen
         self.munchausen = compute_loss_iqn.check_munchausen(
@@ -69,6 +78,8 @@ class Agent:
         self.fqf = fqf.check_fqf(getattr(args, "fqf", 0), *(getattr(args, f, v) for f, v in fqf.FQF_DEFAULTS.items()),
                                  rainbow_only=self.rainbow_only, munchausen=self.munchausen,
                                  num_tau_samples=getattr(args, "num_tau_samples", None))
+        if self.qr_dqn is not None:
+            qr.check_qr(1, self.qr_dqn, munchausen=self.munchausen, fqf=self.fqf)
         self.fraction_net = self.fraction_optimiser = None
         if self.fqf is not None:
             # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed
@@ -109,6 +120,8 @@ class Agent:
             compute_loss_iqn.check_munchausen(1, *self.munchausen, risk=risk)
         if getattr(self, "fqf", None) is not None:
             fqf.check_fqf(1, *self.fqf, risk=risk)
+        if getattr(self, "qr_dqn", None) is not None:
+            qr.check_qr(1, self.qr_dqn, risk=risk)
         self.risk = risk
 
     @staticmethod
@@ -138,13 +151,15 @@ class Agent:
         if self.rainbow_only:
             from . import c51
             return c51.compute_loss_c51(self, states, actions, returns, next_states, nonterminals, debug=debug)
+        if self.qr_dqn is not None:
+            return qr.compute_loss_qr(self, states, actions, returns, next_states, nonterminals, debug=debug)
         return compute_loss_iqn.compute_loss_actor_or_learner_iqn(
             self, states, actions, returns, next_states, nonterminals, debug=debug)
 
     def save(self, path, T_actors, T_learner, name):
         """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
-        fraction_optimiser_state_dict, under value rescaling value_rescaling_eps; model_state_dict keeps the reference
-        schema either way."""
+        fraction_optimiser_state_dict, under value rescaling value_rescaling_eps, under QR-DQN qr_dqn_quantiles (N);
+        model_state_dict keeps the reference schema either way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
@@ -156,6 +171,8 @@ class Agent:
             ckpt["fraction_optimiser_state_dict"] = self.fraction_optimiser.state_dict()
         if self.value_rescaling is not None:
             ckpt["value_rescaling_eps"] = self.value_rescaling
+        if self.qr_dqn is not None:
+            ckpt["qr_dqn_quantiles"] = self.qr_dqn
         torch.save(ckpt, os.path.join(path, name))
 
     def train(self):

@@ -14,13 +14,29 @@ def _tc_mode(B):
 
 def forward(net, x, log=False, keep=None, fresh_weights=False, want_argmax=None, support=None):
     """Returns probabilities (or log-probabilities) (B, A, atoms).  model.py:120-129"""
-    from .model import PRECISION
     if not fresh_weights:
         net._compose_weights()
-    feat = net.trunk(x, keep)
+    zv, za = hidden_z(net, x, keep=keep)
+    B, A, atoms = zv.shape[0], net.action_space, net.atoms
+    out = torch.empty(B, A, atoms, device=zv.device)
+    if support is None:
+        support = net._support(zv.device)
+    call("riqn_c51_head_fwd", B, A, atoms, ptr(zv), ptr(za), ptr(support), None if log else ptr(out),
+         ptr(out) if log else None, ptr(want_argmax))
+    return out
+
+
+def hidden_z(net, x, keep=None, col_cache=None, feat=None):
+    """Trunk, noisy hidden layers [h_v | h_a] and z-layers of the C51-shaped network (C51 and QR-DQN heads): returns
+    zv (B, zv width), za (B, za width), the widths those of fcnoisy_z_v / fcnoisy_z_a.  ``feat``: trunk features computed
+    by the caller (trunk_pair) for a no-grad pass.  ``keep``: dict that receives the backward's operands."""
+    from .model import PRECISION
+    if feat is None:
+        feat = net.trunk(x, keep, col_cache)
     B = feat.shape[0]
     dev = feat.device
-    hid, A, atoms = net.hidden, net.action_space, net.atoms
+    hid = net.hidden
+    nzv, nza = net.fcnoisy_z_v.out_features, net.fcnoisy_z_a.out_features
     h = torch.empty(B, 2 * hid, device=dev)
     x_bf = None
     if _tc_mode(B):
@@ -35,21 +51,16 @@ def forward(net, x, log=False, keep=None, fresh_weights=False, want_argmax=None,
         x_bf = x_lo if f16 else x_hi
     else:
         call("riqn_noisy_linear_fwd", B, FEAT, 2 * hid, ptr(feat), ptr(net._w_eff_h), ptr(net._b_eff_h), ptr(h))
-    zv = torch.empty(B, atoms, device=dev)
-    za = torch.empty(B, A * atoms, device=dev)
-    wz, bz = net._w_eff_z, net._b_eff_z          # rows [0, atoms) = z_v, rows [atoms, atoms + A*atoms) = z_a
+    zv = torch.empty(B, nzv, device=dev)
+    za = torch.empty(B, nza, device=dev)
+    wz, bz = net._w_eff_z, net._b_eff_z          # rows [0, nzv) = z_v, rows [nzv, nzv + nza) = z_a
     hv, ha = h[:, :hid], h[:, hid:]
-    call("riqn_linear_fwd_ld", B, hid, atoms, ptr(hv), 2 * hid, ptr(wz), ptr(bz), ptr(zv), atoms, 0)
-    wza, bza = wz[atoms:], bz[atoms:]
-    call("riqn_linear_fwd_ld", B, hid, A * atoms, ptr(ha), 2 * hid, ptr(wza), ptr(bza), ptr(za), A * atoms, 0)
-    out = torch.empty(B, A, atoms, device=dev)
-    if support is None:
-        support = net._support(dev)
-    call("riqn_c51_head_fwd", B, A, atoms, ptr(zv), ptr(za), ptr(support), None if log else ptr(out),
-         ptr(out) if log else None, ptr(want_argmax))
+    call("riqn_linear_fwd_ld", B, hid, nzv, ptr(hv), 2 * hid, ptr(wz), ptr(bz), ptr(zv), nzv, 0)
+    wza, bza = wz[nzv:], bz[nzv:]
+    call("riqn_linear_fwd_ld", B, hid, nza, ptr(ha), 2 * hid, ptr(wza), ptr(bza), ptr(za), nza, 0)
     if keep is not None:
         keep.update(feat=feat, h=h, B=B, x_bf=x_bf)
-    return out
+    return zv, za
 
 
 def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None):
@@ -114,22 +125,23 @@ def backward_dense(on, keep, out, grad_out, log, gv):
 
 
 def _backward_below_head(on, keep, dzv, dza, gv):
-    """From the z-layer data gradients dzv (B, atoms), dza (B, A*atoms) down to the trunk: z-layer and hidden-layer
-    NoisyLinear gradients, then the convolutions."""
+    """From the z-layer data gradients dzv (B, zv width), dza (B, za width) down to the trunk: z-layer and hidden-layer
+    NoisyLinear gradients, then the convolutions.  The widths are fcnoisy_z_v's and fcnoisy_z_a's (C51: atoms and
+    A*atoms; QR-DQN: N and A*N)."""
     B, dev = keep["B"], dzv.device
-    A, atoms = on.action_space, on.atoms
     hid = on.hidden
     hvL, haL, zvL, zaL = on.fcnoisy_h_v, on.fcnoisy_h_a, on.fcnoisy_z_v, on.fcnoisy_z_a
     h = keep["h"]
     dh = torch.empty(B, 2 * hid, device=dev)
     dhv, dha = dh[:, :hid], dh[:, hid:]
     hv, ha = h[:, :hid], h[:, hid:]
+    nzv, nza = zvL.out_features, zaL.out_features
     w_z = on._w_eff_z
-    wzv, wza = w_z[:atoms], w_z[atoms:]
-    call("riqn_linear_dgrad_ld", B, hid, atoms, ptr(dzv), atoms, ptr(wzv), ptr(dhv), 2 * hid)
-    call("riqn_linear_dgrad_ld", B, hid, A * atoms, ptr(dza), A * atoms, ptr(wza), ptr(dha), 2 * hid)
+    wzv, wza = w_z[:nzv], w_z[nzv:]
+    call("riqn_linear_dgrad_ld", B, hid, nzv, ptr(dzv), nzv, ptr(wzv), ptr(dhv), 2 * hid)
+    call("riqn_linear_dgrad_ld", B, hid, nza, ptr(dza), nza, ptr(wza), ptr(dha), 2 * hid)
     call("riqn_relu_mask", dh.numel(), ptr(h), ptr(dh))
-    scratch = torch.empty(max(A * atoms, 2 * hid), device=dev)
+    scratch = torch.empty(max(nza, 2 * hid), device=dev)
     for layer, d, xin in ((zvL, dzv, hv), (zaL, dza, ha)):
         call("riqn_noisy_wgrad_ld", B, hid, layer.out_features, ptr(d), layer.out_features, ptr(xin), 2 * hid,
              ptr(layer.weight_epsilon), ptr(gv(layer.weight_mu)), ptr(gv(layer.weight_sigma)))
@@ -157,10 +169,13 @@ def _backward_below_head(on, keep, dzv, dza, gv):
     on.backward_trunk(keep, dfeat)
 
 
-class _C51Loss(torch.autograd.Function):
+class _HeadLoss(torch.autograd.Function):
+    """A loss whose ``core(agent, states, actions, returns, next_states, nonterminals, debug=...)`` returns (loss,
+    backward(gscale) closure) -- C51's loss_core, qr.loss_core -- as one autograd node."""
+
     @staticmethod
-    def forward(ctx, agent, states, actions, returns, next_states, nonterminals, debug, *params):
-        loss, bw = loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
+    def forward(ctx, core, agent, states, actions, returns, next_states, nonterminals, debug, *params):
+        loss, bw = core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
         ctx.bw, ctx.n_params = bw, len(params)
         return loss
 
@@ -168,12 +183,12 @@ class _C51Loss(torch.autograd.Function):
     def backward(ctx, grad_loss):
         ctx.bw(grad_loss)
         ctx.bw = None
-        return (None,) * (7 + ctx.n_params)
+        return (None,) * (8 + ctx.n_params)
 
 
 def compute_loss_c51(agent, states, actions, returns, next_states, nonterminals, debug=None):
     if torch.is_grad_enabled():
         params = [p for p in agent.online_net.parameters() if p.requires_grad]
-        return _C51Loss.apply(agent, states, actions, returns, next_states, nonterminals, debug, *params)
+        return _HeadLoss.apply(loss_core, agent, states, actions, returns, next_states, nonterminals, debug, *params)
     loss, _ = loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
     return loss

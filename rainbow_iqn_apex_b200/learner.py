@@ -106,13 +106,18 @@ class Learner(Agent):
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena.
-        ``debug``: dict that receives the IQN loss's intermediates (compute_loss_iqn.loss_core)."""
+        ``debug``: dict that receives the IQN or QR-DQN loss's intermediates (compute_loss_iqn.loss_core, qr.loss_core)."""
         on = self.online_net
         dev = on._flat.device
         weights = weights.to(dev, torch.float32)
         if self.rainbow_only:
             from . import c51
             loss, bw = c51.loss_core(self, states, actions, returns, next_states, nonterminals)
+            on.zero_grad()
+            bw(weights, 1.0 / weights.shape[0])
+        elif self.qr_dqn is not None:
+            from . import qr
+            loss, bw = qr.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug)
             on.zero_grad()
             bw(weights, 1.0 / weights.shape[0])
         else:

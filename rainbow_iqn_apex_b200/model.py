@@ -207,7 +207,8 @@ def _strip_block(g):
 
 
 class DQN(nn.Module):
-    """Reference model.py:56-162 (IQN branch; the C51 branch lives in c51.py)."""
+    """Reference model.py:56-162 (IQN branch; the C51 branch lives in c51.py).  With the optional ``args.qr_dqn = 1``, a
+    QR-DQN network (qr.py): the C51 layer set with z-layer widths N and A*N, N = ``args.num_tau_samples``."""
 
     def __init__(self, args, action_space):
         super().__init__()
@@ -222,7 +223,14 @@ class DQN(nn.Module):
         self.conv1 = nn.Conv2d(args.history_length, 32, 8, stride=4, padding=1)
         self.conv2 = nn.Conv2d(32, 64, 4, stride=2)
         self.conv3 = nn.Conv2d(64, 64, 3)
-        if self.rainbow_only:
+        from . import qr
+        # QR-DQN: N fixed-fraction quantiles per action on the C51 layer set (no quantile embedding); else None
+        self.num_quantiles = qr.check_qr(getattr(args, "qr_dqn", 0), getattr(args, "num_tau_samples", None),
+                                         action_space, rainbow_only=self.rainbow_only)
+        self.qr_dqn = self.num_quantiles is not None
+        if self.qr_dqn:
+            zv, za = self.num_quantiles, action_space * self.num_quantiles
+        elif self.rainbow_only:
             self.atoms = args.atoms
             self._v_min, self._v_max = args.V_min, args.V_max
             zv, za = self.atoms, action_space * self.atoms
@@ -250,11 +258,15 @@ class DQN(nn.Module):
         if self._flat.is_cuda:
             self.reset_noise()
 
+    def _embeds(self):
+        """Whether the network has IQN's quantile embedding iqn_fc (not C51, not QR-DQN)."""
+        return not (self.rainbow_only or self.qr_dqn)
+
     # ------------------------------------------------------------------ arenas
     def _param_groups_in_arena_order(self):
         g = [[self.conv1.weight], [self.conv1.bias], [self.conv2.weight], [self.conv2.bias],
              [self.conv3.weight], [self.conv3.bias]]
-        if not self.rainbow_only:
+        if self._embeds():
             g += [[self.iqn_fc.weight], [self.iqn_fc.bias]]
         hv, ha, zv, za = self.fcnoisy_h_v, self.fcnoisy_h_a, self.fcnoisy_z_v, self.fcnoisy_z_a
         g += [[hv.weight_mu, ha.weight_mu], [hv.weight_sigma, ha.weight_sigma],
@@ -456,7 +468,7 @@ class DQN(nn.Module):
             for name, conv in (("conv1", self.conv1), ("conv2", self.conv2), ("conv3", self.conv3)):
                 co, k = conv.weight.shape[0], conv.weight[0].numel()
                 self._conv_ops[name] = (mk(co, k), mk(co, k), mk(k, co))
-            if not self.rainbow_only:
+            if self._embeds():
                 self._iqn_ops = (mk(FEAT, self.quantile_embedding_dim), mk(FEAT, self.quantile_embedding_dim))
 
     def _refresh_tc_operands(self, force=False, h_done=False):
@@ -495,7 +507,7 @@ class DQN(nn.Module):
                 specs.append((conv.weight, None, 1.0, hi, lo, hiT))                       # original k order (+ transpose)
                 shi, slo = self._strip_ops[name]
                 specs.append((conv.weight, self._strip_perm32[name], 255.0 if name == "conv1" else 1.0, shi, slo, None))
-            if not self.rainbow_only:
+            if self._embeds():
                 specs.append((self.iqn_fc.weight, None, 1.0, self._iqn_ops[0], self._iqn_ops[1], None))
             arr = (SplitJob * len(specs))()
             for j, (src, perm, div, hi, lo, hiT) in zip(arr, specs):
@@ -739,6 +751,20 @@ class DQN(nn.Module):
         None or (measure, eta), a distortion risk measure (RISK_MEASURES) under which the drawn fractions are beta(tau); the
         returned quantiles are those distorted fractions.  An explicit ``tau`` is embedded as given and ``risk`` then
         draws nothing."""
+        if self.qr_dqn:
+            # fixed fractions tau_hat_i = (2i+1)/(2N): nothing to draw, distort or pass in
+            bad = [f"{k}={v!r}" for k, v, ok in (("tau", tau, tau is None), ("risk", risk, risk is None),
+                                                 ("log", log, not log),
+                                                 ("num_quantiles", num_quantiles, num_quantiles in (None, self.num_quantiles)))
+                   if not ok]
+            if bad:
+                raise ValueError(f"the QR-DQN network has N = {self.num_quantiles} fixed quantile fractions and no "
+                                 f"log output: {', '.join(bad)} is not taken")
+            from . import qr
+            if keep is not None and feat is not None and not _trunk_kept(keep, feat):
+                feat = None
+            q = qr.forward(self, x, keep=keep, fresh_weights=fresh_weights, col_cache=col_cache, feat=feat)
+            return q, qr.fractions(self, q.shape[0] // self.num_quantiles).clone()
         risk = check_risk(risk)
         if self.rainbow_only:
             if risk is not None:
@@ -947,6 +973,10 @@ class _DQNForward(torch.autograd.Function):
         if net.rainbow_only:
             ctx.save_for_backward(out)
             return out
+        if net.qr_dqn:
+            q, tau = out
+            ctx.mark_non_differentiable(tau)
+            return q, tau
         keep.pop("q")                # the outputs are not kept in ctx (a reference cycle through the graph)
         keep.pop("tau")
         q, tau = out
@@ -971,6 +1001,9 @@ class _DQNForward(torch.autograd.Function):
             from . import c51
             out, = ctx.saved_tensors
             c51.backward_dense(net, keep, out, g, ctx.log, gv)
+        elif net.qr_dqn:
+            from . import qr
+            qr.backward_dense(net, keep, g, gv)
         else:
             net.backward_iqn_dense(keep, g, gv)
         return (None,) * (6 + ctx.n_params)
