@@ -106,6 +106,17 @@ int riqn_conv_fwd_tc(const riqn_conv_geom* g, const void* in, int in_is_u8, cons
  *                NULL) receive the result as the NEXT layer's block matrix (block edge next_stride, grid next_grid,
  *                within-block order (iy, ix, c)). */
 int riqn_s2d_u8(const riqn_conv_geom* g, const unsigned char* in, void* a_px, void* stream);
+/* Random-shift augmentation (DrQ): edge-replicating shifts of two batches of (C, H, W) images into one contiguous
+ * (nimg, C, H, W) buffer in the inputs' element type (is_u8: uint8, else fp32).  Image i < B reads in0 + i*in0_bstride,
+ * image B + i reads in1 + i*in1_bstride (strides in elements); in1 may be NULL (nimg = B, else 2B).  With (dy, dx) =
+ * (shifts[2i], shifts[2i+1]) of image i,
+ *   out[i, c, y, x] = in_i[c, clamp(y + dy, 0, H-1), clamp(x + dx, 0, W-1)]
+ * i.e. ReplicationPad2d(p) followed by a crop at (dy + p, dx + p) for |dy|, |dx| <= p; larger shifts clamp too.
+ * Returns cudaErrorInvalidValue (and writes nothing) for B, C, H or W < 1, a NULL in0 / shifts / out, is_u8 not 0 or 1,
+ * a batch stride < C*H*W, an in0 / in1 / out address or a batch stride in bytes that is not a multiple of 16, or an
+ * (H, W) plane whose size in bytes is not a multiple of 16 or exceeds 48 KB. */
+int riqn_random_shift(int B, int C, int H, int W, const void* in0, long in0_bstride, const void* in1, long in1_bstride,
+                      int is_u8, const int* shifts, void* out, void* stream);
 int riqn_conv_fwd_strip(const riqn_conv_geom* g, const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,
                         const float* bias, float* out, void* next_hi, void* next_lo, int next_stride, int next_grid,
                         const void* w2_hi, const void* w2_lo, const float* bias2, int share_a, void* stream);
@@ -156,6 +167,13 @@ int riqn_fill_tau_distorted(long n, unsigned long long seed, unsigned long long 
 /* out[i] = sign(x) sqrt|x|, x ~ N(0,1): NoisyLinear._scale_noise (model.py:32-37). */
 int riqn_noisy_sample(long n, unsigned long long seed, unsigned long long stream_id, float* out,
                       const riqn_dyn_state* dyn, void* stream);
+/* n random shifts (dy, dx) in [-pad, pad]^2 for random-shift augmentation (DrQ), out (n, 2) int32.  Component j of pair i
+ * reads the Philox word x that riqn_fill_uniform(2n, seed, stream_id) turns into its value at position 2i + j (same
+ * counters, same dyn->rng_offset); with m = x >> 8, the 24 bits behind that uniform u = (m + 0.5) / 2^24,
+ *   out[2i + j] = ((m (2 pad + 1)) >> 24) - pad        (integer arithmetic: exact, and within [-pad, pad] for every m)
+ * Returns cudaErrorInvalidValue (and writes nothing) for n < 0, pad outside [0, 2^30) or a NULL out with n > 0. */
+int riqn_fill_shifts(long n, int pad, unsigned long long seed, unsigned long long stream_id, int* out,
+                     const riqn_dyn_state* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * NoisyLinear                                             replaces rainbowiqn/model.py:9-53

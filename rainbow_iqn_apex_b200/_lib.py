@@ -51,6 +51,8 @@ SIGNATURES = {
     "riqn_fill_uniform": [C.c_long, C.c_ulonglong, C.c_ulonglong, _P, _P, _P],
     "riqn_fill_tau_distorted": [C.c_long, C.c_ulonglong, C.c_ulonglong, C.c_int, C.c_float, _P, _P, _P],
     "riqn_noisy_sample": [C.c_long, C.c_ulonglong, C.c_ulonglong, _P, _P, _P],
+    "riqn_fill_shifts": [C.c_long, C.c_int, C.c_ulonglong, C.c_ulonglong, _P, _P, _P],
+    "riqn_random_shift": [C.c_int] * 4 + [_P, C.c_long, _P, C.c_long, C.c_int, _P, _P, _P],
     "riqn_noisy_compose": [C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, _P],
     "riqn_noisy_reset_net": [C.c_int, C.POINTER(NoisyLayer), C.c_ulonglong, C.c_int, C.c_int, _P, _P],
     "riqn_noisy_linear_fwd": [C.c_long, C.c_int, C.c_int, _P, _P, _P, _P, _P],

@@ -6,7 +6,8 @@ num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_no
 compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
 ``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
 ``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
-``qr_dqn`` for QR-DQN's fixed-fraction quantile head.  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+``qr_dqn`` for QR-DQN's fixed-fraction quantile head, and ``random_shift`` for the learner's random-shift augmentation
+(augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
 optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
 """
@@ -15,7 +16,7 @@ import os
 import torch
 
 from . import _lib
-from . import compute_loss_iqn, fqf, qr
+from . import augment, compute_loss_iqn, fqf, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -67,7 +68,8 @@ class Agent:
             for field in self._IQN_FIELDS:
                 setattr(self, field, getattr(args, field))
         self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each;
-        #                      FQF and QR-DQN: {"noises": (n0, n1, n2)}
+        #                      FQF and QR-DQN: {"noises": (n0, n1, n2)}; with random_shift, any of these may also carry
+        #                      "shifts": (shifts_states, shifts_next_states), int32 (B, 2) (dy, dx), in place of the draw
         # Munchausen-IQN targets: optional args fields (absent from the reference's namespace: plain IQN).
         # None, or (alpha, entropy_tau, l0) of compute_loss_iqn.check_munchausen
         self.munchausen = compute_loss_iqn.check_munchausen(
@@ -105,6 +107,10 @@ class Agent:
                 self.acting_support = torch.empty_like(self.support)
                 _lib.call("riqn_value_rescale", self.atoms, _lib.ptr(self.support), self.value_rescaling, 1,
                           _lib.ptr(self.acting_support))
+        # random-shift augmentation of the learner's frames: optional args field (absent from the reference's namespace:
+        # off).  None, or the pad p of augment.check_random_shift; fixed for the agent's life, so that a captured step graph
+        # stays valid.  Only Learner.compute_gradients shifts; acting and the actors' priorities see the stored frames
+        self.random_shift = augment.check_random_shift(getattr(args, "random_shift", 0))
         # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
         self.risk = None
         self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))

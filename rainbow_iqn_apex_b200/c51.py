@@ -79,7 +79,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     inj = getattr(agent, "_inject", None)
     if isinstance(inj, list):
         inj = inj.pop(0) if inj else None
-    noises = inj["noises"] if inj else (None, None, None)
+    noises = inj.get("noises", (None, None, None)) if inj else (None, None, None)   # a dict may carry only "shifts"
     on.reset_noise(noises[1])                                              # :95
     a_star = torch.empty(B, dtype=torch.int64, device=dev)
     forward(on, next_states, fresh_weights=True, want_argmax=a_star, support=agent.acting_support)  # :97-102

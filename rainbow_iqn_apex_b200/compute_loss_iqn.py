@@ -131,7 +131,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     inj = getattr(agent, "_inject", None)
     if isinstance(inj, list):            # a queue of injections: one per call (Actor.compute_priorities chunks)
         inj = inj.pop(0) if inj else None
-    noises = inj["noises"] if inj else (None, None, None)
+    noises = inj.get("noises", (None, None, None)) if inj else (None, None, None)   # a dict may carry only "shifts"
     taus = inj.get("taus", (None, None, None)) if inj else (None, None, None)     # FQF's hook has no fractions
     dev = states.device
     if getattr(agent, "munchausen", None) is not None:

@@ -15,7 +15,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import compute_loss_iqn
+from . import augment, compute_loss_iqn
 from .agent import Agent
 from .dynstate import DynState
 
@@ -106,10 +106,13 @@ class Learner(Agent):
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena.
-        ``debug``: dict that receives the IQN or QR-DQN loss's intermediates (compute_loss_iqn.loss_core, qr.loss_core)."""
+        ``debug``: dict that receives the IQN or QR-DQN loss's intermediates (compute_loss_iqn.loss_core, qr.loss_core),
+        and with random_shift the shifts and the shifted frames (_shift_frames)."""
         on = self.online_net
         dev = on._flat.device
         weights = weights.to(dev, torch.float32)
+        if self.random_shift is not None:
+            states, next_states = self._shift_frames(states, next_states, debug)
         if self.rainbow_only:
             from . import c51
             loss, bw = c51.loss_core(self, states, actions, returns, next_states, nonterminals)
@@ -133,6 +136,27 @@ class Learner(Agent):
             on._grads_ready_hook = None
             compute_loss_iqn.fraction_backward(self, keep, weights.contiguous(), 1.0 / weights.shape[0])   # FQF only
         return loss
+
+    def _shift_frames(self, states, next_states, debug=None):
+        """Random-shift augmentation of one step's frames (DrQ with K = M = 1): independent shifts of s_t and s_{t+n}, one
+        per sample, drawn on the device (augment.draw_shifts) or taken from the step's injection dict (``"shifts":
+        (shifts_states, shifts_next_states)``; a list of dicts is peeked, the loss pops it), and ONE riqn_random_shift
+        launch into a [s_{t+n}; s_t] buffer.  Every pass of the loss over a frame set then reads the same shifted frames.
+        The shifts of the last step stay in self._shifts ((2B, 2): rows [0, B) for s_{t+n}; a graph's static buffer)."""
+        on = self.online_net
+        inj = self._inject[0] if isinstance(self._inject, list) and self._inject else self._inject
+        B = states.shape[0]
+        given = inj.get("shifts") if isinstance(inj, dict) else None
+        if given is None:
+            shifts = augment.draw_shifts(on, 2 * B, self.random_shift)
+        else:
+            shifts = torch.cat([torch.as_tensor(s, dtype=torch.int32).reshape(B, 2) for s in (given[1], given[0])])
+            shifts = shifts.to(on._flat.device)
+        next_states, states = augment.random_shift(next_states, states, shifts)
+        self._shifts = shifts
+        if debug is not None:
+            debug.update(shifts=(shifts[B:], shifts[:B]), shifted_states=states, shifted_next_states=next_states)
+        return states, next_states
 
     # ------------------------------------------------------------------ whole step: sample -> learn -> priority update
     def learn_and_update(self, mem):

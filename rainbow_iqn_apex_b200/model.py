@@ -248,6 +248,7 @@ class DQN(nn.Module):
             m._layer_id = i + 1
         self._tau_calls = 0
         self._tau_in_step = 0
+        self._shift_calls = self._shift_in_step = 0   # random-shift draws (augment.draw_shifts), counted like the fractions
         self._dyn = None
         self._tau_stream_offset = 0   # rank-private quantile stream under data parallelism
         self._rng_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -526,7 +527,7 @@ class DQN(nn.Module):
     def begin_step(self, dyn=None):
         """Reset the per-step Philox stream indices (CUDA-graph mode keeps them static across replays)."""
         self._dyn = dyn
-        self._tau_in_step = 0
+        self._tau_in_step = self._shift_in_step = 0
         for _, m in self.noisy_layers():
             m._dyn = dyn
             m._calls_in_step = 0

@@ -101,7 +101,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     inj = getattr(agent, "_inject", None)
     if isinstance(inj, list):
         inj = inj.pop(0) if inj else None
-    noises = inj["noises"] if inj else (None, None, None)
+    noises = inj.get("noises", (None, None, None)) if inj else (None, None, None)   # a dict may carry only "shifts"
     on.reset_noise(noises[0])
     cache = {}   # conv1's pixel block matrix of next_states, shared by the two no-grad passes when they run one by one
     pair = on.trunk_pair(tg, next_states)
