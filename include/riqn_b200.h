@@ -466,6 +466,33 @@ int riqn_qr_head_bwd(int batch, int action_space, int n, const float* dtheta, co
  *   dzv[b,i] = sum_a G[i*batch+b, a]   (fp32 adds, a ascending, starting from 0)
  *   dza[b, a*n+i] = fl(G[i*batch+b, a] - fl(dzv[b,i] / A)) */
 int riqn_qr_head_bwd_dense(int batch, int action_space, int n, const float* grad_q, float* dzv, float* dza, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * MMDQN loss (Nguyen-Tang, Gupta & Venkatesh, AAAI 2021; no counterpart in the reference) on the QR-DQN head's
+ * particles, with g = fl(gamma_n * nonterminals[b]) and a* = a_star[b] as in riqn_iqn_loss_fwd_bwd:
+ *   theta_i = q_online[i*batch + b, actions[b]] ,  T_j = fl(returns[b] + fl(g * q_target[j*batch + b, a*]))
+ *   k(x, y) = sum_h exp(-(x - y)^2 / h)      over the n_bandwidths bandwidths h
+ *   loss[b] = max(0, (1/n^2) sum_i sum_j [k(theta_i, theta_j) + k(T_i, T_j) - 2 k(theta_i, T_j)])
+ *   dtheta[i*batch + b] = (2/n^2) sum_j [k1(theta_i, theta_j) - k1(theta_i, T_j)],
+ *                         k1(x, y) = -sum_h (2 (x - y) / h) exp(-(x - y)^2 / h)   (gradient of the unclamped sum)
+ * dtheta is quantile-major (n*batch), as riqn_qr_head_bwd takes it; theta_out (batch, n) and target_out (batch, n) are
+ * optional (NULL: not written).  `bandwidths` is a HOST array of n_bandwidths floats, read during the call: the kernel
+ * receives the constants c_h = fl(-log2(e) / h) and w_h = fl(2 / h) by value (a captured graph holds them) and evaluates
+ * exp(-(x - y)^2 / h) as exp2f(fl(fl(d * d) * c_h)), d = fl(x - y).  The sums are grouped per (i, j) bracket, j ascending,
+ * so T_j = theta_j for every j gives loss 0 and dtheta 0 exactly.  One CTA per transition, no atomics.  Returns
+ * cudaErrorInvalidValue, writing nothing, unless batch >= 1, 1 <= n <= 256, 1 <= action_space <= 32,
+ * 1 <= n_bandwidths <= 16 and every bandwidth is finite and > 0 with finite c_h and w_h. */
+int riqn_mmd_loss_fwd_bwd(int batch, int n, int action_space, const float* q_online, const float* q_target,
+                          const long long* actions, const long long* a_star, const float* returns,
+                          const float* nonterminals, float gamma_n, int n_bandwidths, const float* bandwidths,
+                          float* loss, float* dtheta, float* theta_out, float* target_out, void* stream);
+/* riqn_mmd_loss_fwd_bwd against the transformed target, as riqn_iqn_loss_fwd_bwd_h forms it:
+ *   T_j = fl(h(returns[b] + g * h^-1(q_target[j*batch + b, a*])))     (sum and product in double)
+ * eps must be finite and >= 0. */
+int riqn_mmd_loss_fwd_bwd_h(int batch, int n, int action_space, const float* q_online, const float* q_target,
+                            const long long* actions, const long long* a_star, const float* returns,
+                            const float* nonterminals, float gamma_n, int n_bandwidths, const float* bandwidths,
+                            float eps, float* loss, float* dtheta, float* theta_out, float* target_out, void* stream);
 /* n floats <- 0 (the gradient arena's zero_grad, learner.py:22): cudaMemsetAsync on the caller's stream. */
 int riqn_zero_f32(float* p, long n, void* stream);
 /* grad[i] = 0 where act[i] <= 0. */

@@ -6,7 +6,8 @@ num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_no
 compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
 ``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
 ``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
-``qr_dqn`` for QR-DQN's fixed-fraction quantile head, and ``random_shift`` for the learner's random-shift augmentation
+``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
+and ``random_shift`` for the learner's random-shift augmentation
 (augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
 optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
@@ -16,7 +17,7 @@ import os
 import torch
 
 from . import _lib
-from . import augment, compute_loss_iqn, fqf, qr
+from . import augment, compute_loss_iqn, fqf, mmd, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -82,6 +83,12 @@ class Agent:
                                  num_tau_samples=getattr(args, "num_tau_samples", None))
         if self.qr_dqn is not None:
             qr.check_qr(1, self.qr_dqn, munchausen=self.munchausen, fqf=self.fqf)
+        # MMDQN: optional args fields (absent from the reference's namespace: off).  None, or the bandwidths of
+        # mmd.check_mmd; fixed for the agent's life, so that a captured step graph stays valid
+        self.mmd = mmd.check_mmd(getattr(args, "mmd", 0),
+                                 getattr(args, "mmd_bandwidths", mmd.MMD_DEFAULTS["mmd_bandwidths"]),
+                                 qr_dqn=self.qr_dqn, rainbow_only=self.rainbow_only, munchausen=self.munchausen,
+                                 fqf=self.fqf)
         self.fraction_net = self.fraction_optimiser = None
         if self.fqf is not None:
             # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed
@@ -128,6 +135,8 @@ class Agent:
             fqf.check_fqf(1, *self.fqf, risk=risk)
         if getattr(self, "qr_dqn", None) is not None:
             qr.check_qr(1, self.qr_dqn, risk=risk)
+        if getattr(self, "mmd", None) is not None:
+            mmd.check_mmd(1, self.mmd, qr_dqn=self.qr_dqn, risk=risk)
         self.risk = risk
 
     @staticmethod

@@ -12,13 +12,14 @@ unclipped returns at the cost of a C51 step.
 
 The learner step runs the IQN path's three passes, each after its own noise reset: online(s') -> a* = argmax_a mean_i q_i,
 target(s') (both trunks in one stacked trunk_pair), online(s) with the backward's operands; then the quantile-Huber loss
-against R + gamma^n nt q_tgt[a*] at the N x N fraction pairs, and riqn_qr_head_bwd below it.
+against R + gamma^n nt q_tgt[a*] at the N x N fraction pairs, and riqn_qr_head_bwd below it.  MMDQN (agent.mmd, mmd.py)
+runs the same step with the MMD loss kernel in place of the quantile-Huber one.
 """
 import numbers
 
 import torch
 
-from . import c51
+from . import c51, mmd
 from ._lib import call, ptr
 from .compute_loss_iqn import _as_device_inputs, _quantile_loss, greedy_actions
 
@@ -120,8 +121,12 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, N, device=dev)
-    _quantile_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
-                   target_out)
+    if getattr(agent, "mmd", None) is None:
+        _quantile_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta,
+                       theta_out, target_out)
+    else:                                              # MMDQN: the same particles under the MMD loss (mmd.py)
+        mmd.mmd_loss(agent, B, N, q_on, q_tgt, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
+                     target_out)
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on,
                      tau=tau_hat, keep=keep)
