@@ -252,8 +252,8 @@ int riqn_quantile_embed_bwd(int batch, int num_quantiles, int embed_dim, int fea
  * are split from x32 by a second launch and therefore need x32 != NULL); x32 (may be NULL) is the fp32 matrix.  cos_hi / cos_lo
  * (rows, embed_dim) and cos_t_hi (embed_dim, rows; may be NULL) are outputs too.  cos_lo == NULL selects the
  * single-bf16 product.  iqn_w_hi / iqn_w_lo: bf16 images of iqn_fc.weight (riqn_split_bf16).  rows % 2, feat_dim % 32
- * and embed_dim % 8 must be 0, and cos_hi, cos_lo, iqn_w_hi, iqn_w_lo, x32, x_hi, x_lo 16-byte aligned; a call rejected
- * for its shapes or alignment (cudaErrorInvalidValue) writes nothing. */
+ * and embed_dim % 8 must be 0, cos_hi, cos_lo, iqn_w_hi, iqn_w_lo, x32, x_hi, x_lo 16-byte aligned, and feat and iqn_b
+ * 8-byte aligned; a call rejected for its shapes or alignment (cudaErrorInvalidValue) writes nothing. */
 int riqn_quantile_embed_fwd_tc(int batch, int num_quantiles, int embed_dim, int feat_dim, const float* tau,
                                const float* feat, const void* iqn_w_hi, const void* iqn_w_lo, const float* iqn_b,
                                void* cos_hi, void* cos_lo, void* cos_t_hi, float* x32, void* x_hi, void* x_lo, void* x_hi_t,

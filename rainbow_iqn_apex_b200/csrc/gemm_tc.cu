@@ -9,8 +9,9 @@
 //   descriptors; the accumulator lives in their registers,
 // * after a tile's last k-block the consumers pass the accumulator through a shared-memory slab, 64 columns at a time,
 //   so that each warp holds 32 rows x 32 columns with one ROW per lane, and apply the fused epilogue from there while
-//   the producer already fetches the next tile's operands (the 128x256 forward and bf16 data gradient instead stage
-//   their fragments for TMA stores and go on to the next tile while the stores drain: MODE bit 3, see TcCfg),
+//   the producer already fetches the next tile's operands (the 128x256 forward, the bf16 data gradient and the quantile
+//   embedding instead stage their fragments for TMA stores and go on to the next tile while the stores drain: MODE
+//   bit 3, see TcCfg),
 // * persistent CTAs (one per SM) walk (m-tile, n-tile, k-split) work units round-robin.
 //
 // Precision: NSPLIT == 1 multiplies bf16(A) * bf16(B).  NSPLIT == 3 takes each operand as hi + lo bf16 pairs
@@ -45,11 +46,17 @@ constexpr uint32_t kSmemLimit = 232448;           // 227 KB of opt-in shared mem
 // NSPLIT 1: a_hi*b_hi.  NSPLIT 3: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi.  NSPLIT 2: A is exact in bf16 (e.g. uint8 pixels),
 // only B is split: a_hi*b_hi + a_hi*b_lo.
 //
-// TMAEPI (128x256 TC_BIAS_RELU / TC_STORE only): the accumulator leaves through TMA stores instead of the slab.  Each
-// consumer warpgroup stages 32-column chunks of its 64 rows in kEpiBufs rotating buffers of kEpiChunkBytes: a 64 x 32
-// fp32 box (8 KB, 128-byte swizzle; TC_BIAS_RELU) and a 64 x 32 bf16 box (4 KB, 64-byte swizzle; the o_hi image).
-// With the 3-stage ring (144 KB) that leaves room for 3 fp32 + bf16 buffers per warpgroup (72 KB) in the forward, and
-// for the whole 128 x 256 bf16 tile (8 buffers, 64 KB) in the data gradient.
+// TMAEPI (128x256 single-pass TC_BIAS_RELU / TC_STORE, and the 128x128 TC_EMBED): the accumulator leaves through TMA
+// stores instead of the slab.  Each consumer warpgroup stages 32-column chunks of its 64 rows in kEpiBufs rotating
+// buffers of kEpiChunkBytes: a 64 x 32 fp32 box (8 KB, 128-byte swizzle; TC_BIAS_RELU) and one 64 x 32 16-bit box per
+// image (4 KB each, 64-byte swizzle; the o_hi image, or the embedding's o_hi and o_lo).  The ring keeps kEpiStages
+// stages and the buffers take what is left, up to kEpiBufsMax:
+//   128x256 (48 KB stages, 3 of them = 144 KB): 3 fp32 + bf16 buffers per warpgroup (72 KB) in the forward, the whole
+//     128 x 256 bf16 tile (8 buffers, 64 KB) in the data gradient;
+//   TC_EMBED (64 KB stages with split operands, 32 KB without): its tiles are ONE k-block long, so two stages already
+//     keep the next tile's operands in flight under every product, and a buffer comes up for rewriting a few hundred
+//     cycles after its stores were issued.  Six 8 KB buffers per warpgroup (96 KB; a tile and a half) let those stores
+//     finish reading behind the next tile's product instead of in front of it; the ring gets 2 (split) / 4 stages.
 template <int NSPLIT, int BN, int EPI, bool TMAEPI = false>
 struct TcCfg {
   static constexpr int kAOps = NSPLIT == 3 ? 2 : 1, kBOps = NSPLIT == 1 ? 1 : 2;     // hi (+ lo) images per operand
@@ -57,18 +64,21 @@ struct TcCfg {
   static constexpr uint32_t kABytes = TBM * TBK * 2, kBBytes = BN * TBK * 2;
   static constexpr uint32_t kStageBytes = kAOps * kABytes + kBOps * kBBytes;         // 32 / 48 / 64 KB at BN = 128
   static constexpr uint32_t kEpiF32Bytes = EPI == TC_BIAS_RELU ? 64 * 32 * 4 : 0;
-  static constexpr uint32_t kEpiChunkBytes = kEpiF32Bytes + 64 * 32 * 2;
-  static constexpr int kEpiBufsFit = (kSmemLimit - 1024 - 256 - 3 * kStageBytes) / (kConsumerWGs * kEpiChunkBytes);
-  static constexpr int kEpiBufs = kEpiBufsFit > BN / 32 ? BN / 32 : kEpiBufsFit;
+  static constexpr uint32_t kEpiChunkBytes = kEpiF32Bytes + (EPI == TC_EMBED ? 2 : 1) * 64 * 32 * 2;
+  static constexpr int kEpiStages = EPI == TC_EMBED ? 2 : 3;
+  static constexpr int kEpiBufsMax = EPI == TC_EMBED ? 6 : BN / 32;
+  static constexpr int kEpiBufsFit = (kSmemLimit - 1024 - 256 - kEpiStages * kStageBytes) / (kConsumerWGs * kEpiChunkBytes);
+  static constexpr int kEpiBufs = kEpiBufsFit > kEpiBufsMax ? kEpiBufsMax : kEpiBufsFit;
   static constexpr uint32_t kEpiBytes = TMAEPI ? kConsumerWGs * kEpiBufs * kEpiChunkBytes : kConsumerWGs * kSlabBytes;
-  static_assert(!TMAEPI || (BN == 256 && NSPLIT == 1 && (EPI == TC_BIAS_RELU || EPI == TC_STORE) && kEpiBufs >= 2),
-                "TMA-store epilogue: 128x256 single-pass TC_BIAS_RELU / TC_STORE with at least two staging buffers");
-  static constexpr uint32_t kFbBytes = EPI == TC_EMBED ? kEpiWarps * 256 : 0;       // per-warp feat / bias broadcast patches
-  static constexpr uint32_t kRingBytes = kSmemLimit - 1024 /*align*/ - kEpiBytes - 256 /*barriers*/ - kFbBytes;
+  static_assert(!TMAEPI || (kEpiBufs >= 2 && (EPI == TC_EMBED ? BN == 128
+                                                              : BN == 256 && NSPLIT == 1 && (EPI == TC_BIAS_RELU || EPI == TC_STORE))),
+                "TMA-store epilogue: 128x256 single-pass TC_BIAS_RELU / TC_STORE or 128x128 TC_EMBED, at least two staging buffers");
+  static_assert(TMAEPI || EPI != TC_EMBED, "the embedding has no slab epilogue");
+  static constexpr uint32_t kRingBytes = kSmemLimit - 1024 /*align*/ - kEpiBytes - 256 /*barriers*/;
   static constexpr int kStages = kRingBytes / kStageBytes > 6 ? 6 : kRingBytes / kStageBytes;
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + kEpiBytes + 256 + kFbBytes;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + kEpiBytes + 256;
   static_assert(kSmemBytes <= kSmemLimit && kStages >= 2, "exceeds the 227 KB per-CTA shared memory limit");
-  static_assert(!TMAEPI || kStages == 3, "the staging budget above assumes the 3-stage ring");
+  static_assert(!TMAEPI || kStages >= kEpiStages, "the staging budget above assumes a ring of kEpiStages");
 };
 
 // ---------------------------------------------------------------------------------------------- PTX wrappers
@@ -115,6 +125,12 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_read_n() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// read-only 8-byte load that keeps its place among the other volatile statements (issued ahead of a wgmma wait)
+__device__ __forceinline__ float2 ldg_nc_f2(const float* p) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
+  return v;
+}
 // named barrier over the 128 threads of one warpgroup (id 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -367,8 +383,8 @@ __device__ __forceinline__ void mma_kblock(float (&d)[TBN / 2], uint32_t sa, uin
 }
 
 struct alignas(64) TcArgs {
-  CUtensorMap mapO[2];   // TC_EMBED: TMA-store maps of o_hi / o_lo ((M, N) 16-bit row-major, box 32 x 32, 64-byte swizzle)
-                         // MODE bit 3: C (fp32, box 32 x 64, 128-byte swizzle) / o_hi (bf16, box 32 x 64, 64-byte swizzle)
+  CUtensorMap mapO[2];   // MODE bit 3: C (fp32, box 32 x 64, 128-byte swizzle) / o_hi (bf16, box 32 x 64, 64-byte swizzle);
+                         // TC_EMBED: o_hi / o_lo ((M, N) 16-bit row-major, box 32 x 64, 64-byte swizzle)
   int M, N, K;
   int m_tiles, n_tiles, k_splits, kb_per_split, kb_total;
   float* C;
@@ -393,7 +409,8 @@ struct alignas(64) TcArgs {
   long part_stride;      // TC_STORE of split-K partials: split ks writes C + ks * part_stride (0 otherwise)
 };
 
-// MODE (128x256 tiles only; 0 otherwise): bits 0-1 = mn_major, bit 2 = fp16 operands, bit 3 = TMA-store epilogue
+// MODE: bits 0-1 = mn_major, bit 2 = fp16 operands (both 128x256 tiles only), bit 3 = TMA-store epilogue (128x256 tiles
+// and TC_EMBED; 0 otherwise)
 template <int NSPLIT, int EPI, int BN, int MODE = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
@@ -404,12 +421,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
   constexpr int TBN = BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // layout: operand ring | accumulator slabs (one per consumer warpgroup, 1 KB aligned) | barriers | feat / bias patches
+  // layout: operand ring | accumulator slabs or staging buffers (per consumer warpgroup, 1 KB aligned) | barriers
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kEpiBytes);
   uint64_t* full = bars;                       // [kStages]  TMA -> MMA
   uint64_t* empty = bars + Cfg::kStages;       // [kStages]  MMA -> TMA (one arrival per consumer warp)
   const uint32_t epi_base = (uint32_t)__cvta_generic_to_shared(smem + Cfg::kStages * Cfg::kStageBytes);
-  const uint32_t epi_fb = epi_base + Cfg::kEpiBytes + 256;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_units = p.m_tiles * p.n_tiles * p.k_splits;
@@ -428,8 +444,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
   if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer (one thread)
     // 128x256 tiles: the producer warpgroup hands its registers to the consumers' 128 accumulators per thread
-    // (128 * 40 + 256 * 232 = the 64512 registers the launch gets at 168 per thread)
-    if constexpr (BN == 256) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    // (128 * 40 + 256 * 232 = the 64512 registers the launch gets at 168 per thread).  The embedding's consumers hold a
+    // tile's feat / bias values (96 registers) beside their 64 accumulators.
+    if constexpr (BN == 256 || EPI == TC_EMBED) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -506,12 +523,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
   }
 
   // -------------------------------------------------------------------- consumer warpgroups (wgmma + epilogue)
-  if constexpr (BN == 256) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  if constexpr (BN == 256 || EPI == TC_EMBED) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   const int g = (warp >> 2) - 1;               // this warpgroup's 64 tile rows start at 64 g
   const int wq = warp & 3;                      // warp in the warpgroup: fragment rows [16 wq, +16)
   const int band = wq & 1, colhalf = wq >> 1;   // epilogue: 32-row band of the slab, 32-column half of each 64-column chunk
   const int quarter = 2 * g + band;             // the tile rows [32 quarter, +32) this warp's lanes hold in the epilogue
-  const int ew = warp - 4;                      // epilogue warp index
   const uint32_t slab = epi_base + g * kSlabBytes;
   const uint32_t st = slab + wq * (32 * kStRow * 4);   // this warp's staging tile (overlays the slab once it is read)
   const bool f16 = (p.fmt & 3) != 0;
@@ -542,6 +558,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
     if constexpr (EPI == TC_CONV_DGRAD) {
 #pragma unroll
       for (int i = 0; i < TBN / 2; ++i) dg_sum[i] = 0.f;
+    }
+    // TC_EMBED: bias and feat of this thread's fragment (column pairs 8 j + 2 (lane % 4) + {0, 1} of rows fr, fr + 8),
+    // loaded here so that their L2 latency passes under the product.  The two rows may belong to different samples
+    // (fewer than 64 rows per sample); rows >= M and columns >= N are only loaded from a valid place, never stored.
+    float2 e_bias[TBN / 8], e_feat[2][TBN / 8];
+    if constexpr (EPI == TC_EMBED) {
+      const int m0 = mt * TBM + 64 * g + 16 * wq + (lane >> 2), m1 = m0 + 8;
+      const float* f0 = p.feat + (long)((m0 < p.M ? m0 : 0) / p.batch) * p.N;
+      const float* f1 = p.feat + (long)((m1 < p.M ? m1 : 0) / p.batch) * p.N;
+#pragma unroll
+      for (int j = 0; j < TBN / 8; ++j) {
+        int n = nt * TBN + 8 * j + 2 * (lane & 3);
+        if (n >= p.N) n = 0;
+        e_bias[j] = ldg_nc_f2(p.bias + n);
+        e_feat[0][j] = ldg_nc_f2(f0 + n);
+        e_feat[1][j] = ldg_nc_f2(f1 + n);
+      }
     }
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
@@ -598,12 +631,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
     }
 
     if constexpr (kTmaEpi) {
-      // ---- TMA-store epilogue: the fragments go straight into the swizzled staging boxes (bias + ReLU applied in
-      // registers), one thread per warpgroup issues the bulk tensor stores, and the warpgroup goes on to the next tile
+      // ---- TMA-store epilogue: the fragments go straight into the swizzled staging boxes (bias + ReLU, or the
+      // embedding's x = feat * relu(acc + bias) (model.py:146-151) and its two 16-bit images, applied in registers),
+      // one thread per warpgroup issues the bulk tensor stores, and the warpgroup goes on to the next tile
       // without waiting for them.  A staging buffer is rewritten only after the stores that read it have finished
       // READING shared memory; their global writes stay in flight.  TMA clips rows >= M and columns >= N.
       constexpr int kChunks = TBN / 32;
-      constexpr bool kWhole = Cfg::kEpiBufs >= kChunks;   // the whole tile fits: one wait and two barriers per tile
+      constexpr bool kWhole = Cfg::kEpiBufs == kChunks;   // one buffer per chunk of the tile: one wait and two barriers per tile
       const int row0 = mt * TBM + 64 * g;
       const int nch = min(kChunks, (p.N - nt * TBN + 31) / 32);   // chunks holding real columns
       const bool elected = wq == 0 && lane == 0;
@@ -623,6 +657,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
             const int j = 4 * h + jj;               // accumulator column group: tile columns 8 j + 2 (lane % 4) + {0, 1}
+            if constexpr (EPI == TC_EMBED) {
+              const bool x_f16 = (p.fmt & 4) != 0;
+#pragma unroll
+              for (int hh = 0; hh < 2; ++hh) {
+                const int r = fr + 8 * hh;
+                const float x0 = e_feat[hh][j].x * fmaxf(acc[4 * j + 2 * hh] + e_bias[j].x, 0.f);
+                const float x1 = e_feat[hh][j].y * fmaxf(acc[4 * j + 2 * hh + 1] + e_bias[j].y, 0.f);
+                if (p.C != nullptr && row0 + r < p.M)   // fp32 x of the cross-check arithmetic modes
+                  *reinterpret_cast<float2*>(p.C + (long)(row0 + r) * p.N + nt * TBN + 8 * j + 2 * (lane & 3)) = make_float2(x0, x1);
+                // fp16(x) feeds the single-pass head forward and bf16(x) the backward products; otherwise bf16 hi + the
+                // residual lo of the split-bf16 x3 head forward
+                const uint32_t w0 = pack16x2(x0, x1, x_f16);
+                const uint32_t w1 = x_f16 ? pack16x2(x0, x1, false)
+                                          : pack16x2(x0 - __uint_as_float(w0 << 16), x1 - __uint_as_float(w0 & 0xffff0000u), false);
+                const uint32_t so = sh + r * 64 + ((jj ^ ((r >> 1) & 3)) << 4) + 4 * (lane & 3);   // 64-byte swizzle, as below
+                if (p.o_hi != nullptr) asm volatile("st.shared.b32 [%0], %1;" ::"r"(so), "r"(w0) : "memory");
+                if (p.o_lo != nullptr) asm volatile("st.shared.b32 [%0], %1;" ::"r"(so + 64 * 32 * 2), "r"(w1) : "memory");
+              }
+              continue;
+            }
             float b0 = 0.f, b1 = 0.f;
             if (EPI == TC_BIAS_RELU) {
               const int n = nt * TBN + 8 * j + 2 * (lane & 3);
@@ -657,6 +711,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
               for (int i = kWhole ? 0 : h; i <= h; ++i) {
                 const uint32_t si = kWhole ? stg + i * Cfg::kEpiChunkBytes : sf;
                 const int c0 = nt * TBN + 32 * i;
+                if (EPI == TC_EMBED) {
+                  if (p.o_hi != nullptr) tma_store_2d(&p.mapO[0], si, c0, row0);
+                  if (p.o_lo != nullptr) tma_store_2d(&p.mapO[1], si + 64 * 32 * 2, c0, row0);
+                  continue;
+                }
                 if (EPI == TC_BIAS_RELU) tma_store_2d(&p.mapO[0], si, c0, row0);
                 if (EPI == TC_STORE || p.o_hi != nullptr) tma_store_2d(&p.mapO[1], si + Cfg::kEpiF32Bytes, c0, row0);
               }
@@ -673,7 +732,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 #pragma unroll
     for (int h = 0; h < (TBN + 63) / 64; ++h) {
       if (BN == 256 && nt * TBN + 64 * h >= p.N) break;         // edge tile: the remaining chunks hold no real column
-      if (EPI == TC_EMBED && lane == 0) tma_store_wait_read();   // bulk stores of the previous chunk read the staging tiles
       wg_bar(1 + g);
       {
         const uint32_t r0 = slab + ((16 * wq + (lane >> 2)) * kSlabStride + 2 * (lane & 3)) * 4;
@@ -702,20 +760,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
       if (c >= TBN) continue;
       const int m = mt * TBM + quarter * 32 + lane;
       const int n0 = nt * TBN + c;
-    // embedding epilogue: lane = row.  The 32 feat / bias values of a chunk are fetched by ONE coalesced load per warp
-    // (lane j loads column j) and broadcast through a 256-byte shared-memory patch; the finished 16-bit tiles are staged
-    // in the TMA 64-byte-swizzle layout and leave through cp.async.bulk.tensor stores -- no per-thread global stores and
-    // no read-back of the staging tile
-    const int e_mbase = mt * TBM + quarter * 32;
-    const bool e_one_sample = (p.batch & 31) == 0;          // sample-major rows: a warp's 32 rows share one feature row
-    const float* embed_feat_row = nullptr;
-    if (EPI == TC_EMBED) embed_feat_row = p.feat + (long)((e_mbase < p.M ? e_mbase : 0) / p.batch) * p.N;
-      // this chunk's feat / bias values
-      float ef = 0.f, eb = 0.f;
-      if (EPI == TC_EMBED && n0 + 32 <= p.N) {
-        eb = __ldg(p.bias + n0 + lane);
-        if (e_one_sample) ef = __ldg(embed_feat_row + n0 + lane);
-      }
       if (m < p.M && n0 < p.N) {
         if (EPI == TC_STORE || EPI == TC_BIAS_RELU) {
           float* crow = p.C + ks * p.part_stride + (long)m * p.ldc + n0;
@@ -756,7 +800,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 #pragma unroll
           for (int j = 0; j < 32; ++j)
             if (n0 + j < p.N) cb[(long)j * p.ohw] = fmaxf(__uint_as_float(v[j]) + p.bias[n0 + j], 0.f);
-        } else if (EPI == TC_EMBED || EPI == TC_COL2IM || EPI == TC_CONV || EPI == TC_CONV_DGRAD) {
+        } else if (EPI == TC_COL2IM || EPI == TC_CONV || EPI == TC_CONV_DGRAD) {
           // handled below with the whole warp
         } else if (!(p.vec_acc && n0 + 32 <= p.N)) {
           float* crow = p.C + (long)m * p.ldc + n0;
@@ -863,7 +907,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
           if (row_ok && off >= 0) base[off] = __uint_as_float(v[j]);
         }
       }
-      if ((EPI == TC_STORE || EPI == TC_EMBED || (EPI == TC_BIAS_RELU && (p.M & 1) == 0) ||
+      if ((EPI == TC_STORE || (EPI == TC_BIAS_RELU && (p.M & 1) == 0) ||
            ((EPI == TC_ATOMIC || EPI == TC_NOISY_WGRAD) && p.vec_acc)) && n0 + 32 <= p.N) {
         const int m_base = mt * TBM + quarter * 32;
         const int rows_valid = min(32, p.M - m_base);            // warp-uniform
@@ -909,59 +953,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
               for (int j = 0; j < 16; ++j) { hw2[j] = hw[j]; hw2[16 + j] = 0u; }
               warp_store_rows_bf16(st, hw2, lane, p.o_hi + (long)m_base * p.N + n0, nullptr, p.N, rows_valid);
             }
-          } else {
-            // x = feat[b] * relu(acc + bias)   (model.py:146-151); N % 32 == 0 is required by the host wrapper.
-            const bool f16 = (p.fmt & 4) != 0;
-            const uint32_t fb = epi_fb + ew * 256;
-            const bool row_ok = m < p.M;
-            const float* frow = p.feat + (long)((row_ok ? m : 0) / p.batch) * p.N + n0;   // per-row feat (several samples per warp)
-            const uint32_t st0 = st;                            // o_hi in the first 2 KB, o_lo in the second
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(fb + lane * 4), "r"(__float_as_uint(ef)) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(fb + 128 + lane * 4), "r"(__float_as_uint(eb)) : "memory");
-            __syncwarp();
-            uint32_t w0[16], w1[16];                            // image 0 / image 1 column pairs of this lane's row
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint4 bu = lds128(fb + 128 + 16 * j);
-              uint4 fu;
-              if (e_one_sample) fu = lds128(fb + 16 * j);
-              else fu = __ldg(reinterpret_cast<const uint4*>(frow) + j);
-              const float x0 = __uint_as_float(fu.x) * fmaxf(__uint_as_float(v[4 * j]) + __uint_as_float(bu.x), 0.f);
-              const float x1 = __uint_as_float(fu.y) * fmaxf(__uint_as_float(v[4 * j + 1]) + __uint_as_float(bu.y), 0.f);
-              const float x2 = __uint_as_float(fu.z) * fmaxf(__uint_as_float(v[4 * j + 2]) + __uint_as_float(bu.z), 0.f);
-              const float x3 = __uint_as_float(fu.w) * fmaxf(__uint_as_float(v[4 * j + 3]) + __uint_as_float(bu.w), 0.f);
-              if (p.C && row_ok) *reinterpret_cast<float4*>(p.C + (long)m * p.N + n0 + 4 * j) = make_float4(x0, x1, x2, x3);
-              if (f16) {            // fp16(x) feeds the single-pass head forward, bf16(x) the backward products
-                w0[2 * j] = pack16x2(x0, x1, true); w0[2 * j + 1] = pack16x2(x2, x3, true);
-                w1[2 * j] = pack16x2(x0, x1, false); w1[2 * j + 1] = pack16x2(x2, x3, false);
-              } else {              // bf16 hi + residual lo (split-bf16 x3 head forward)
-                const uint32_t h0 = pack16x2(x0, x1, false), h1 = pack16x2(x2, x3, false);
-                w0[2 * j] = h0; w0[2 * j + 1] = h1;
-                w1[2 * j] = pack16x2(x0 - __uint_as_float(h0 << 16), x1 - __uint_as_float(h0 & 0xffff0000u), false);
-                w1[2 * j + 1] = pack16x2(x2 - __uint_as_float(h1 << 16), x3 - __uint_as_float(h1 & 0xffff0000u), false);
-              }
-            }
-            // 32 rows x 64 bytes per image in the TMA SWIZZLE_64B layout: 16-byte chunk c of row r sits at chunk c ^ ((r >> 1) & 3)
-            const uint32_t srow = st0 + lane * 64;
-            const int sw = (lane >> 1) & 3;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              if (p.o_hi) sts128(srow + ((c ^ sw) << 4), w0[4 * c], w0[4 * c + 1], w0[4 * c + 2], w0[4 * c + 3]);
-              if (p.o_lo) sts128(srow + 2048 + ((c ^ sw) << 4), w1[4 * c], w1[4 * c + 1], w1[4 * c + 2], w1[4 * c + 3]);
-            }
-            fence_proxy_async();                                // generic-proxy writes -> visible to the TMA engine
-            __syncwarp();
-            if (lane == 0) {
-              if (p.o_hi) tma_store_2d(&p.mapO[0], st0, n0, m_base);
-              if (p.o_lo) tma_store_2d(&p.mapO[1], st0 + 2048, n0, m_base);
-              tma_store_commit();
-            }
           }
         }
       }
     }
   }
-  if ((EPI == TC_EMBED || kTmaEpi) && lane == 0) tma_store_wait_all();   // bulk stores read this CTA's shared memory
+  if (kTmaEpi && lane == 0) tma_store_wait_all();   // bulk stores read this CTA's shared memory
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -1168,8 +1165,8 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
   if ((p.fmt & 4) && epi != TC_EMBED) return (int)cudaErrorInvalidValue;
   if (epi == TC_EMBED && ((N % 32) || (M % 2) || p.o_hiT || p.o_loT)) return (int)cudaErrorInvalidValue;
   if (epi == TC_EMBED) {            // the 16-bit images leave through TMA stores
-    if (p.o_hi && (rc = make_store_map(&p.mapO[0], p.o_hi, M, N))) return rc;
-    if (p.o_lo && (rc = make_store_map(&p.mapO[1], p.o_lo, M, N))) return rc;
+    if (p.o_hi && (rc = make_store_map(&p.mapO[0], p.o_hi, M, N, 64))) return rc;
+    if (p.o_lo && (rc = make_store_map(&p.mapO[1], p.o_lo, M, N, 64))) return rc;
   }
   // 128x256 forward (fp32 C, optional bf16 image) and bf16 data gradient (MN-major weight operand): the accumulator
   // leaves through TMA stores.  Their bases and row pitches must be 16-byte aligned; the slab epilogue's vector stores
@@ -1195,7 +1192,7 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
         case TC_NOISY_WGRAD: RIQN_TC_GO(3, TC_NOISY_WGRAD);
         case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(3, TC_BIAS_RELU_NCHW); RIQN_TC_GO(3, TC_BIAS_RELU_NCHW);
         case TC_CONV: RIQN_TC_NARROW(3, TC_CONV); break;
-        case TC_EMBED: RIQN_TC_GO(3, TC_EMBED);
+        case TC_EMBED: return launch_tc<3, TC_EMBED, 128, 8>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
       }
     } else if (split2) {
       switch (epi) {
@@ -1226,7 +1223,7 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
         case TC_NOISY_WGRAD: RIQN_TC_GO(1, TC_NOISY_WGRAD);
         case TC_BIAS_RELU_NCHW: RIQN_TC_NARROW(1, TC_BIAS_RELU_NCHW); RIQN_TC_GO(1, TC_BIAS_RELU_NCHW);
         case TC_CONV: RIQN_TC_NARROW(1, TC_CONV); break;
-        case TC_EMBED: RIQN_TC_GO(1, TC_EMBED);
+        case TC_EMBED: return launch_tc<1, TC_EMBED, 128, 8>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
       }
     }
 #undef RIQN_TC_NARROW

@@ -1346,12 +1346,13 @@ RIQN_API int riqn_quantile_embed_fwd_tc(int batch, int num_quantiles, int embed_
                                         void* cos_hi, void* cos_lo, void* cosT_hi, float* x32, void* x_hi, void* x_lo,
                                         void* x_hiT, void* x_loT, int x_fp16, void* stream) {
   const long R = (long)batch * num_quantiles;
-  // every shape and operand alignment the product rejects (TMA needs 16-byte aligned bases; the epilogue's x32 stores are
-  // 16 bytes wide) is rejected here, before the cos images are written
+  // every shape and operand alignment the product rejects (TMA needs 16-byte aligned bases; the epilogue reads feat and
+  // the bias and writes x32 as 8-byte column pairs) is rejected here, before the cos images are written
   const bool want_t = x_hiT != nullptr || x_loT != nullptr;    // transposed images (cross-check arithmetic modes only)
   const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  const auto a8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };
   if (R % 2 || feat_dim % 32 || embed_dim % 8 || (want_t && (x32 == nullptr || x_fp16)) || !a16(cos_hi) || !a16(cos_lo) ||
-      !a16(iqn_w_hi) || !a16(iqn_w_lo) || !a16(x32) || !a16(x_hi) || !a16(x_lo))
+      !a16(iqn_w_hi) || !a16(iqn_w_lo) || !a16(x32) || !a16(x_hi) || !a16(x_lo) || !a8(feat) || !a8(iqn_b))
     return (int)cudaErrorInvalidValue;
   riqn::note_launches(2);
   cudaStream_t s = (cudaStream_t)stream;
