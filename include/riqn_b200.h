@@ -271,7 +271,10 @@ int riqn_quantile_embed_bwd_tc(int batch, int num_quantiles, int embed_dim, int 
  * z-layers + dueling aggregation                          replaces rainbowiqn/model.py:153-156
  * ---------------------------------------------------------------------------------------------- */
 /* h (rows, 2*hidden) = [value-stream hidden | advantage-stream hidden]; wz (1+A, hidden) = effective
- * weights of fcnoisy_z_v (row 0) and fcnoisy_z_a; bz (1+A).  q (rows, A) = v + a - mean_a a. */
+ * weights of fcnoisy_z_v (row 0) and fcnoisy_z_a; bz (1+A).  q (rows, A) = v + a - mean_a a, row r of h (sample-major,
+ * r = b*(rows/batch) + k) going to row k*batch + b of q (quantile-major).  Returns cudaErrorInvalidValue, writing
+ * nothing, unless hidden == 512, 1 <= action_space <= 31, batch >= 1, rows % batch == 0, and h and wz are 16-byte
+ * aligned. */
 int riqn_dueling_fwd(long rows, int batch, int hidden, int action_space, const float* h, const float* wz,
                      const float* bz, float* q, void* stream);
 /* Backward for the gathered action: dq[r, actions[b]] = dtheta[r] * gscale[b].  Writes dh (rows, 2*hidden),
@@ -316,14 +319,19 @@ int riqn_z_wgrad(long rows, int hidden, int action_space, const float* dz, const
 /* ------------------------------------------------------------------------------------------------
  * IQN loss                                     replaces rainbowiqn/compute_loss_iqn.py:216-358
  * ---------------------------------------------------------------------------------------------- */
-/* a_star[b] = argmax_a mean_k q[k*batch+b, a]            (compute_loss_iqn.py:238-245) */
+/* a_star[b] = argmax_a mean_k q[k*batch+b, a]            (compute_loss_iqn.py:238-245)
+ * The mean is the fp32 sum over k ascending divided once by num_quantiles; the first maximal index wins.  Returns
+ * cudaErrorInvalidValue, writing nothing, unless batch >= 1, num_quantiles >= 1 and 1 <= action_space <= 32. */
 int riqn_argmax_mean(int batch, int num_quantiles, int action_space, const float* q, long long* a_star, void* stream);
 /* Fused n-step target + pairwise quantile-Huber loss and its gradient (compute_loss_iqn.py:262-357):
  *   target[b,j] = returns[b] + gamma_n*nonterminals[b]*q_target[j*batch+b, a_star[b]]
  *   theta[b,i]  = q_online[i*batch+b, actions[b]]
  *   loss[b]     = mean_j sum_i |tau[i*batch+b] - 1{d<0}| huber_kappa(d)/kappa ,  d = target_j - theta_i
  *   dtheta[i*batch+b] = d loss[b] / d theta[b,i]
- * theta_out (batch, n_tau) / target_out (batch, n_tau_prime) are optional debug outputs (may be NULL). */
+ * theta_out (batch, n_tau) / target_out (batch, n_tau_prime) are optional debug outputs (may be NULL).
+ * Returns cudaErrorInvalidValue, writing nothing, unless batch, n_tau, n_tau_prime >= 1, 1 <= action_space <= 32, kappa
+ * is finite and > 0, and (n_tau_prime + 32) * 4 <= 48 KB (the staged targets).  riqn_iqn_loss_fwd_bwd_h and
+ * riqn_miqn_loss_fwd_bwd take the same limits, the latter less its kernel's static shared memory (1 KB on sm_90a). */
 int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
                           const float* q_target, const float* tau, const long long* actions, const long long* a_star,
                           const float* returns, const float* nonterminals, float gamma_n, float kappa, float* loss,
@@ -340,8 +348,8 @@ int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_spac
  *   theta, loss, dtheta as in riqn_iqn_loss_fwd_bwd.
  * The bonus also enters on terminal transitions.  The log-policy is never formed as log(pi): an underflowing pi gives a
  * finite, very negative l, which the clip takes to l0.  bonus_out (batch), like theta_out / target_out, may be NULL.
- * Returns cudaErrorInvalidValue (and writes nothing) for action_space > 32, entropy_tau <= 0, l0 > 0, alpha < 0, or any of
- * the three non-finite. */
+ * Returns cudaErrorInvalidValue (and writes nothing) outside the limits of riqn_iqn_loss_fwd_bwd, for entropy_tau <= 0,
+ * l0 > 0, alpha < 0, or any of the three non-finite. */
 int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
                            const float* q_target, const float* tau, const long long* actions, const float* returns,
                            const float* nonterminals, float gamma_n, float kappa, float alpha, float entropy_tau, float l0,
@@ -361,7 +369,7 @@ int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_spa
 int riqn_value_rescale(long n, const float* x, float eps, int inverse, float* out, void* stream);
 /* riqn_iqn_loss_fwd_bwd against the transformed target, with g = fl(gamma_n * nonterminals[b]) as there:
  *   target[b,j] = fl(h(returns[b] + g * h^-1(q_target[j*batch+b, a_star[b]])))     (sum and product in double)
- * theta, loss and dtheta as in riqn_iqn_loss_fwd_bwd.  action_space <= 32. */
+ * theta, loss and dtheta as in riqn_iqn_loss_fwd_bwd, and its limits. */
 int riqn_iqn_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
                             const float* q_target, const float* tau, const long long* actions, const long long* a_star,
                             const float* returns, const float* nonterminals, float gamma_n, float kappa, float eps,

@@ -1499,8 +1499,12 @@ RIQN_API int riqn_noisy_bias_grad(long rows, int out_features, const float* dh, 
 
 RIQN_API int riqn_dueling_fwd(long rows, int batch, int hidden, int action_space, const float* h, const float* wz,
                               const float* bz, float* q, void* stream) {
+  // rows % batch: the sample-major -> quantile-major row map is a bijection only on whole samples.  The two A <= 24
+  // kernels read h and wz as float4; the alignment is required for every A so that no path depends on it.
+  if (hidden != 512 || action_space < 1 || action_space > 31 || batch < 1 || rows % batch != 0 ||
+      (reinterpret_cast<uintptr_t>(h) & 15) != 0 || (reinterpret_cast<uintptr_t>(wz) & 15) != 0)
+    return (int)cudaErrorInvalidValue;
   riqn::note_launches(1);
-  if (hidden != 512 || action_space > 31) return (int)cudaErrorInvalidValue;
   const size_t smem = sizeof(float) * (1 + action_space) * hidden;
   static PerDeviceOnce attr_once;
   const int attr_dev = PerDeviceOnce::device();
@@ -1515,7 +1519,7 @@ RIQN_API int riqn_dueling_fwd(long rows, int batch, int hidden, int action_space
       RIQN_CUDA(cudaFuncSetAttribute(z_dueling_fwd4_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
       attr4_once.done[attr4_dev] = true;
     }
-    if (rows >= 4096 && (reinterpret_cast<uintptr_t>(h) & 15) == 0) {      // streamed variant: one CTA per SM
+    if (rows >= 4096) {                                                     // streamed variant: one CTA per SM
       static PerDeviceOnce attrs_once;
       if (!attrs_once.done[attr4_dev]) {
         RIQN_CUDA(cudaFuncSetAttribute(z_dueling_fwd4s_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1672,11 +1676,19 @@ RIQN_API int riqn_z_wgrad_tc(long rows, int hidden, int action_space, const void
 
 RIQN_API int riqn_argmax_mean(int batch, int num_quantiles, int action_space, const float* q, long long* a_star,
                               void* stream) {
+  if (batch < 1 || num_quantiles < 1 || action_space < 1 || action_space > 32) return (int)cudaErrorInvalidValue;
   riqn::note_launches(1);
-  if (action_space > 32) return (int)cudaErrorInvalidValue;
   argmax_mean_kernel<<<riqn_cdiv((long)batch * 32, 128), 128, 0, (cudaStream_t)stream>>>(batch, num_quantiles, action_space, q,
                                                                             (int64_t*)a_star);
   return (int)cudaGetLastError();
+}
+
+// The argument contract of the three quantile-Huber loss entry points.  Each CTA stages the n_tau_prime targets and 32
+// reduction slots in dynamic shared memory, within the 48 KB a launch gets without opting in, less the kernel's static
+// shared memory (static_smem bytes).  A kappa <= 0 makes the loss NaN or meaningless.
+static bool huber_loss_args_ok(int batch, int n_tau, int n_tau_prime, int action_space, float kappa, size_t static_smem) {
+  return batch >= 1 && n_tau >= 1 && n_tau_prime >= 1 && action_space >= 1 && action_space <= 32 && kappa > 0.f &&
+         isfinite(kappa) && ((size_t)n_tau_prime + 32) * sizeof(float) + static_smem <= 48 * 1024;
 }
 
 RIQN_API int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
@@ -1684,6 +1696,7 @@ RIQN_API int riqn_iqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int ac
                                    const long long* a_star, const float* returns, const float* nonterminals,
                                    float gamma_n, float kappa, float* loss, float* dtheta, float* theta_out,
                                    float* target_out, void* stream) {
+  if (!huber_loss_args_ok(batch, n_tau, n_tau_prime, action_space, kappa, 0)) return (int)cudaErrorInvalidValue;
   riqn::note_launches(1);
   int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;
   if (threads > 1024) threads = 1024;
@@ -1700,7 +1713,8 @@ RIQN_API int riqn_iqn_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int 
                                      const long long* a_star, const float* returns, const float* nonterminals,
                                      float gamma_n, float kappa, float eps, float* loss, float* dtheta, float* theta_out,
                                      float* target_out, void* stream) {
-  if (!vr_eps_ok(eps) || action_space > 32) return (int)cudaErrorInvalidValue;
+  if (!vr_eps_ok(eps) || !huber_loss_args_ok(batch, n_tau, n_tau_prime, action_space, kappa, 0))
+    return (int)cudaErrorInvalidValue;
   riqn::note_launches(1);
   int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;
   if (threads > 1024) threads = 1024;
@@ -1735,8 +1749,10 @@ RIQN_API int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int a
                                     const float* returns, const float* nonterminals, float gamma_n, float kappa,
                                     float alpha, float entropy_tau, float l0, float* loss, float* dtheta,
                                     float* theta_out, float* target_out, float* bonus_out, void* stream) {
-  if (action_space > 32 || !(entropy_tau > 0.f) || !isfinite(entropy_tau) || !(l0 <= 0.f) || !isfinite(l0) ||
-      !(alpha >= 0.f) || !isfinite(alpha))
+  cudaFuncAttributes fa;                        // the kernel's static shared memory (s_mean, s_pi, s_lp, s_m)
+  RIQN_CUDA(cudaFuncGetAttributes(&fa, miqn_loss_kernel));
+  if (!huber_loss_args_ok(batch, n_tau, n_tau_prime, action_space, kappa, fa.sharedSizeBytes) || !(entropy_tau > 0.f) ||
+      !isfinite(entropy_tau) || !(l0 <= 0.f) || !isfinite(l0) || !(alpha >= 0.f) || !isfinite(alpha))
     return (int)cudaErrorInvalidValue;
   riqn::note_launches(1);
   int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;

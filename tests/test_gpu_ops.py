@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from helpers import load_params, make_args, rel_err
-from oracle import cases, losses, network as net
+from oracle import cases, network as net
 
 pytestmark = pytest.mark.gpu
 
@@ -135,54 +135,6 @@ def test_forward_injected(cuda_dev, nets):
     d.train()
 
 
-@pytest.mark.parametrize("B,N,Np,kappa", [(7, 8, 8, 1.0), (33, 64, 64, 1.0), (4, 16, 40, 0.5), (3, 100, 9, 2.0)])
-def test_iqn_loss_kernel(cuda_dev, B, N, Np, kappa):
-    call, ptr = _call()
-    rs = np.random.RandomState(B)
-    A = 18
-    q_on = torch.from_numpy(rs.standard_normal((N * B, A)).astype(np.float32)).requires_grad_(True)
-    q_tg = torch.from_numpy(rs.standard_normal((Np * B, A)).astype(np.float32))
-    tau = torch.from_numpy(rs.uniform(0, 1, (N * B, 1)).astype(np.float32))
-    actions = torch.from_numpy(rs.randint(0, A, B).astype(np.int64))
-    a_star = torch.from_numpy(rs.randint(0, A, B).astype(np.int64))
-    returns = torch.from_numpy(rs.standard_normal(B).astype(np.float32))
-    nt = torch.from_numpy((rs.uniform(size=B) < 0.8).astype(np.float32))
-    g = 0.99 ** 3
-    target = (returns[:, None].repeat(Np, 1) + (g * nt[:, None]).repeat(Np, 1)
-              * q_tg.gather(1, a_star[:, None].repeat(Np, 1))).reshape(Np, B).t()
-    theta = q_on.gather(1, actions[:, None].repeat(N, 1)).reshape(N, B).t()
-    ref = losses.iqn_pairwise_loss(theta, target, tau.reshape(N, B).t(), kappa)
-    w = torch.from_numpy(rs.uniform(0.1, 1, B).astype(np.float32))
-    (w * ref).sum().backward()
-    dev = cuda_dev
-    loss = torch.empty(B, device=dev)
-    dth = torch.empty(N * B, device=dev)
-    th_o = torch.empty(B, N, device=dev)
-    tg_o = torch.empty(B, Np, device=dev)
-    d_in = [t.to(dev) for t in (q_on.detach(), q_tg, tau, actions, a_star, returns, nt)]   # keep alive
-    call("riqn_iqn_loss_fwd_bwd", B, N, Np, A, *[ptr(t) for t in d_in], float(g), float(kappa),
-         ptr(loss), ptr(dth), ptr(th_o), ptr(tg_o))
-    assert np.array_equal(tg_o.cpu().numpy(), target.numpy())       # same fp32 op order as the reference
-    assert np.array_equal(th_o.cpu().numpy(), theta.detach().numpy())
-    assert rel_err(loss.cpu().numpy(), ref.detach().numpy()) < 1e-5   # SURVEY 8d: loss kernel alone <= 1e-5
-    # dtheta[i*B+b] * w[b] == dL/dq_on[i*B+b, actions[b]]
-    gref = q_on.grad.gather(1, actions[:, None].repeat(N, 1)).reshape(N, B)
-    got = dth.cpu().reshape(N, B) * w[None, :]
-    assert rel_err(got.numpy(), gref.numpy()) < 1e-5
-
-
-def test_argmax_mean(cuda_dev):
-    call, ptr = _call()
-    rs = np.random.RandomState(1)
-    B, K, A = 37, 32, 18
-    q = torch.from_numpy(rs.standard_normal((K * B, A)).astype(np.float32))
-    ref = q.reshape(K, B, A).mean(0).argmax(1)
-    out = torch.empty(B, dtype=torch.int64, device=cuda_dev)
-    qd = q.to(cuda_dev)
-    call("riqn_argmax_mean", B, K, A, ptr(qd), ptr(out))
-    assert torch.equal(out.cpu(), ref)
-
-
 def test_adam_matches_torch(cuda_dev):
     call, ptr = _call()
     rs = np.random.RandomState(2)
@@ -309,30 +261,3 @@ def test_trunk_pair_equals_two_trunks(cuda_dev):
     ref = net.conv_trunk(net.to_torch(net.make_params(32)), x.cpu().float().div_(255)).numpy()
     assert rel_err(fb.cpu().numpy(), ref) < 3e-5
     assert a.trunk_pair(b_, x[:5]) is None                      # rows per network must fill whole 128-row tiles
-
-
-@pytest.mark.parametrize("R,B,A", [(8203, 1, 18), (4096, 64, 6), (16384, 512, 18)])
-def test_dueling_fwd_streamed_rows(cuda_dev, R, B, A):
-    """riqn_dueling_fwd takes the shared-memory-streamed kernel from 4096 rows up (model.py:153-156).  Same operation
-    order per output as the register kernel: bit-identical to that kernel run on < 4096-row slices (ragged tail
-    included), and equal to the float64 product within fp32 accumulation error."""
-    call, ptr = _call()
-    g = torch.Generator(device="cpu").manual_seed(R + A)
-    h = torch.randn(R, 1024, generator=g).clamp_(min=0).to(cuda_dev)
-    wz = (torch.randn(1 + A, 512, generator=g) * 0.05).to(cuda_dev)
-    bz = torch.randn(1 + A, generator=g).to(cuda_dev)
-    q = torch.full((R, A), float("nan"), device=cuda_dev)
-    call("riqn_dueling_fwd", R, B, 512, A, ptr(h), ptr(wz), ptr(bz), ptr(q))
-    h64, w64, b64 = h.double().cpu(), wz.double().cpu(), bz.double().cpu()
-    v = h64[:, :512] @ w64[0] + b64[0]
-    adv = h64[:, 512:] @ w64[1:].t() + b64[1:]
-    ref = (v[:, None] + adv - adv.mean(1, keepdim=True)).view(B, R // B, A).transpose(0, 1).reshape(R, A)   # row = q_idx*B + b
-    assert rel_err(q.cpu().numpy(), ref.numpy()) < 5e-6
-    if B == 1:      # identity row map: slices of the input are slices of the output
-        parts = []
-        for lo in range(0, R, 4000):
-            n = min(4000, R - lo)
-            qs = torch.empty(n, A, device=cuda_dev)
-            call("riqn_dueling_fwd", n, 1, 512, A, ptr(h[lo:lo + n]), ptr(wz), ptr(bz), ptr(qs))
-            parts.append(qs)
-        assert torch.equal(q, torch.cat(parts))
