@@ -501,6 +501,35 @@ int riqn_mmd_loss_fwd_bwd_h(int batch, int n, int action_space, const float* q_o
                             const long long* actions, const long long* a_star, const float* returns,
                             const float* nonterminals, float gamma_n, int n_bandwidths, const float* bandwidths,
                             float eps, float* loss, float* dtheta, float* theta_out, float* target_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * HL-Gauss loss (Farebrother et al., ICML 2024; Imani & White, ICML 2018; no counterpart in the reference) on the C51
+ * head: cross-entropy against the Gaussian histogram of the scalar double-DQN target.  Operands as riqn_c51_loss_fwd_bwd
+ * (logp_online and p_target (batch, A, atoms), a* = a_star[b]); every double operation is rounded on its own:
+ *   g  = fl(nonterminals[b] * gamma_n) ;  Q' = sum_j fl64(p_target[b, a*, j] * support[j])   (double, j ascending, from 0)
+ *   y  = clamp(returns[b] + g * Q', v_min, v_max)            (double) ;  target_out[b] = fl32(y)
+ *   D  = (v_max - v_min) / (atoms - 1) ;  e_i = v_min + (i - 0.5) * D ;  u_i = (e_i - y) / s ,  s = (sigma_ratio * D) * sqrt(2)
+ *   c_i = 0.5 * erfc(|u_i|)   (i = 0..atoms) ;  mass_j = c_j - c_j+1 if u_j >= 0, c_j+1 - c_j if u_j+1 <= 0, else
+ *   (0.5 - c_j) + (0.5 - c_j+1) ;  m_j = fl32(mass_j / ((0.5 - c_0) + (0.5 - c_atoms)))
+ *   loss[b] = -sum_j fl(m_j * logp_online[b, actions[b], j])   (fp32, lanes 0..31 and 32..63 by the warp_sum butterfly,
+ *             then (0 + warp 0) + warp 1) ;  mt = sum_j m_j in the same order
+ *   dq[b, j] = -fl(m_j - fl(p_j * mt)) ,  p_j = fl32(exp(double logp_online[b, actions[b], j]))
+ * dq (batch, atoms) is the gradient riqn_c51_head_bwd takes; m_out (batch, atoms) and target_out (batch) are optional
+ * (NULL: not written).  One CTA of 64 threads per transition, no atomics.  Returns cudaErrorInvalidValue, writing
+ * nothing, unless batch >= 1, action_space >= 1, 2 <= atoms <= 64, v_min and v_max are finite with v_min < v_max, and
+ * sigma_ratio (sigma in bin widths) is finite with 0 < sigma_ratio <= 1000. */
+int riqn_hl_gauss_loss_fwd_bwd(int batch, int action_space, int atoms, const float* logp_online, const float* p_target,
+                               const long long* actions, const long long* a_star, const float* returns,
+                               const float* nonterminals, const float* support, float gamma_n, float v_min, float v_max,
+                               float sigma_ratio, float* loss, float* dq, float* m_out, float* target_out, void* stream);
+/* riqn_hl_gauss_loss_fwd_bwd with the transformed target (value rescaling): support is the h-space support, and
+ *   Q' = sum_j fl64(p_target[b, a*, j] * h^-1(support[j])) ,  y = clamp(h(returns[b] + g * Q'), v_min, v_max)
+ * (the expectation on the linear scale, the quantity a* is chosen on).  eps as for riqn_value_rescale. */
+int riqn_hl_gauss_loss_fwd_bwd_h(int batch, int action_space, int atoms, const float* logp_online,
+                                 const float* p_target, const long long* actions, const long long* a_star,
+                                 const float* returns, const float* nonterminals, const float* support, float gamma_n,
+                                 float v_min, float v_max, float sigma_ratio, float eps, float* loss, float* dq,
+                                 float* m_out, float* target_out, void* stream);
 /* n floats <- 0 (the gradient arena's zero_grad, learner.py:22): cudaMemsetAsync on the caller's stream. */
 int riqn_zero_f32(float* p, long n, void* stream);
 /* grad[i] = 0 where act[i] <= 0. */

@@ -92,6 +92,8 @@ SIGNATURES = {
     "riqn_qr_head_bwd_dense": [C.c_int] * 3 + [_P] * 4,
     "riqn_mmd_loss_fwd_bwd": [C.c_int] * 3 + [_P] * 6 + [C.c_float, C.c_int, _P] + [_P] * 5,
     "riqn_mmd_loss_fwd_bwd_h": [C.c_int] * 3 + [_P] * 6 + [C.c_float, C.c_int, _P, C.c_float] + [_P] * 5,
+    "riqn_hl_gauss_loss_fwd_bwd": [C.c_int] * 3 + [_P] * 7 + [C.c_float] * 4 + [_P] * 5,
+    "riqn_hl_gauss_loss_fwd_bwd_h": [C.c_int] * 3 + [_P] * 7 + [C.c_float] * 5 + [_P] * 5,
     "riqn_zero_f32": [_P, C.c_long, _P],
     "riqn_relu_mask": [C.c_long, _P, _P, _P],
     "riqn_linear_fwd_ld": [C.c_long, C.c_int, C.c_int, _P, C.c_long, _P, _P, _P, C.c_long, C.c_int, _P],

@@ -7,8 +7,8 @@ compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` 
 ``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
 ``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
 ``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
-and ``random_shift`` for the learner's random-shift augmentation
-(augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51 head (hl_gauss.py), and ``random_shift`` for the
+learner's random-shift augmentation (augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
 optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
 """
@@ -17,7 +17,7 @@ import os
 import torch
 
 from . import _lib
-from . import augment, compute_loss_iqn, fqf, mmd, qr
+from . import augment, compute_loss_iqn, fqf, hl_gauss, mmd, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -89,6 +89,11 @@ class Agent:
                                  getattr(args, "mmd_bandwidths", mmd.MMD_DEFAULTS["mmd_bandwidths"]),
                                  qr_dqn=self.qr_dqn, rainbow_only=self.rainbow_only, munchausen=self.munchausen,
                                  fqf=self.fqf)
+        # HL-Gauss: optional args fields (absent from the reference's namespace: off).  None, or the float32 ratio
+        # sigma / delta_z of hl_gauss.check_hl_gauss; fixed for the agent's life, since a captured step graph holds it
+        self.hl_gauss = hl_gauss.check_hl_gauss(
+            getattr(args, "hl_gauss", 0), getattr(args, "hl_gauss_sigma", hl_gauss.HL_GAUSS_DEFAULTS["hl_gauss_sigma"]),
+            rainbow_only=self.rainbow_only)
         self.fraction_net = self.fraction_optimiser = None
         if self.fqf is not None:
             # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed

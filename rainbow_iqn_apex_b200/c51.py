@@ -1,7 +1,9 @@
 """Rainbow-only (C51) branch of the reference: DQN.forward (model.py:120-129) and the categorical loss
-(agent.py:77-141), on the same CUDA trunk / NoisyLinear ops as the IQN path plus csrc/c51.cu."""
+(agent.py:77-141), on the same CUDA trunk / NoisyLinear ops as the IQN path plus csrc/c51.cu.  HL-Gauss (agent.hl_gauss,
+hl_gauss.py) runs the same step with the Gaussian-histogram loss kernel in place of the projection."""
 import torch
 
+from . import hl_gauss
 from ._lib import call, ptr
 from .model import FEAT
 
@@ -91,15 +93,23 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     loss = torch.empty(B, device=dev)
     dq = torch.empty(B, atoms, device=dev)
     m_out = torch.empty(B, atoms, device=dev) if debug is not None else None
-    args = (ptr(log_ps), ptr(pns), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals), ptr(agent.support),
-            float(agent.discount ** agent.n), float(agent.Vmin), float(agent.Vmax), float(agent.delta_z))
-    eps = getattr(agent, "value_rescaling", None)
-    if eps is None:
-        call("riqn_c51_loss_fwd_bwd", B, A, atoms, *args, ptr(loss), ptr(dq), ptr(m_out))
-    else:   # the atoms move to h(R + gamma^n nt h^-1(z_j)) before the projection
-        call("riqn_c51_loss_fwd_bwd_h", B, A, atoms, *args, eps, ptr(loss), ptr(dq), ptr(m_out))
+    target_out = None
+    if getattr(agent, "hl_gauss", None) is not None:   # HL-Gauss: the histogram of the scalar target (hl_gauss.py)
+        target_out = torch.empty(B, device=dev) if debug is not None else None
+        hl_gauss.hl_gauss_loss(agent, B, log_ps, pns, actions, a_star, returns, nonterminals, loss, dq, m_out,
+                               target_out)
+    else:
+        args = (ptr(log_ps), ptr(pns), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals), ptr(agent.support),
+                float(agent.discount ** agent.n), float(agent.Vmin), float(agent.Vmax), float(agent.delta_z))
+        eps = getattr(agent, "value_rescaling", None)
+        if eps is None:
+            call("riqn_c51_loss_fwd_bwd", B, A, atoms, *args, ptr(loss), ptr(dq), ptr(m_out))
+        else:   # the atoms move to h(R + gamma^n nt h^-1(z_j)) before the projection
+            call("riqn_c51_loss_fwd_bwd_h", B, A, atoms, *args, eps, ptr(loss), ptr(dq), ptr(m_out))
     if debug is not None:
         debug.update(a_star=a_star, m=m_out, log_ps=log_ps)
+        if target_out is not None:                     # HL-Gauss: the scalar targets and the probabilities they came from
+            debug.update(target=target_out, p_target=pns)
     version = getattr(on, "_noise_version", 0)       # bumped by every DQN.reset_noise()
 
     def backward(gscale, gscale_mul=1.0):

@@ -106,7 +106,8 @@ class Learner(Agent):
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena.
-        ``debug``: dict that receives the IQN or QR-DQN loss's intermediates (compute_loss_iqn.loss_core, qr.loss_core),
+        ``debug``: dict that receives the IQN, C51 or QR-DQN loss's intermediates (compute_loss_iqn.loss_core,
+        c51.loss_core, qr.loss_core),
         and with random_shift the shifts and the shifted frames (_shift_frames)."""
         on = self.online_net
         dev = on._flat.device
@@ -115,7 +116,7 @@ class Learner(Agent):
             states, next_states = self._shift_frames(states, next_states, debug)
         if self.rainbow_only:
             from . import c51
-            loss, bw = c51.loss_core(self, states, actions, returns, next_states, nonterminals)
+            loss, bw = c51.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug)
             on.zero_grad()
             bw(weights, 1.0 / weights.shape[0])
         elif self.qr_dqn is not None:
