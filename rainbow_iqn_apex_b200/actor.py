@@ -31,37 +31,24 @@ class Actor(Agent):
         q, _ = on.forward(states_u8, self.num_tau_samples, tau=fr["tau_hat"], fresh_weights=True, feat=feat)
         return q, fr["dtau"]
 
-    def _fqf_argmax(self, states_u8):
-        q, dtau = self._fqf_pass(states_u8)
-        return greedy_actions(self, states_u8.shape[0], self.num_tau_samples, q, dtau)
-
     def act(self, state_buffer):
-        """actor.py:15-25: greedy action from the mean over K sampled quantiles (IQN; distorted by ``self.risk``), the
-        dtau-weighted mean over the proposed fractions (FQF), the mean over the N fixed-fraction quantiles (QR-DQN) or the
-        expected value of the categorical distribution (C51).
-        Under value rescaling each of them is the expectation of h^-1 of the network's h-space values, the return's own
-        scale.  Frames go to the device as uint8; the /255 of the reference happens inside the conv kernel."""
+        """actor.py:15-25: act_batch on the one state of ``state_buffer``, as an int.  Frames go to the device as uint8;
+        the /255 of the reference happens inside the conv kernel."""
         state = torch.from_numpy(np.stack(state_buffer).astype(np.uint8)).to(self.online_net._flat.device)
-        with torch.no_grad():
-            if self.rainbow_only:
-                p = self.online_net(state.unsqueeze(0))
-                return (p * self.acting_support).sum(2).argmax(1).item()
-            if self.fqf is not None:
-                return int(self._fqf_argmax(state.unsqueeze(0)).item())
-            if self.qr_dqn is not None:
-                q, _ = self.online_net(state.unsqueeze(0))
-                return int(greedy_actions(self, 1, self.qr_dqn, q).item())
-            quantile_values, _ = self.online_net(state.unsqueeze(0), self.num_quantile_samples, tau=self._pop_tau(),
-                                                  risk=self.risk)
-            return int(greedy_actions(self, 1, self.num_quantile_samples, quantile_values).item())
+        return int(self.act_batch(state.unsqueeze(0)).item())
 
     def act_batch(self, states_u8):
-        """Batched greedy actions for many environments at once: states (E, history, 84, 84) uint8 -> (E,)."""
+        """Batched greedy actions for many environments at once: states (E, history, 84, 84) uint8 -> (E,).  Each is the
+        argmax of the mean over K sampled quantiles (IQN; distorted by ``self.risk``), the dtau-weighted mean over the
+        proposed fractions (FQF), the mean over the N fixed-fraction quantiles (QR-DQN) or the expected value of the
+        categorical distribution (C51).  Under value rescaling each of them is the expectation of h^-1 of the network's
+        h-space values, the return's own scale."""
         with torch.no_grad():
             if self.rainbow_only:
                 return (self.online_net(states_u8) * self.acting_support).sum(2).argmax(1)
             if self.fqf is not None:
-                return self._fqf_argmax(states_u8)
+                q, dtau = self._fqf_pass(states_u8)
+                return greedy_actions(self, states_u8.shape[0], self.num_tau_samples, q, dtau)
             if self.qr_dqn is not None:
                 q, _ = self.online_net(states_u8)
                 return greedy_actions(self, states_u8.shape[0], self.qr_dqn, q)

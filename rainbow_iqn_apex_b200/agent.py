@@ -3,7 +3,8 @@
 Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``args`` fields, same public
 attributes (online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
-compute_loss_actor_or_learner, save, train, eval), plus ``risk`` / ``set_risk`` for risk-sensitive acting and
+compute_loss_actor_or_learner, save, train, eval), plus ``loss_core`` for the loss the agent trains (c51.loss_core,
+qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-sensitive acting and
 ``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
 ``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
 ``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
@@ -17,7 +18,7 @@ import os
 import torch
 
 from . import _lib
-from . import augment, compute_loss_iqn, fqf, hl_gauss, mmd, qr
+from . import augment, c51, compute_loss_iqn, fqf, hl_gauss, mmd, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -58,16 +59,20 @@ class Agent:
         if checkpoint is not None:
             self.optimiser.load_state_dict(checkpoint["optimiser_state_dict"])
 
+        # the head's sizes and the loss core this agent trains (every core returns (loss, backward))
         if self.rainbow_only:                            # categorical support (agent.py:49-57)
             for attr, field in self._C51_FIELDS:
                 setattr(self, attr, getattr(args, field))
             self.support = torch.linspace(self.Vmin, self.Vmax, self.atoms).to(device=args.device)
             self.delta_z = (self.Vmax - self.Vmin) / (self.atoms - 1)
+            self.loss_core = c51.loss_core
         elif self.qr_dqn is not None:                    # QR-DQN: N fixed fractions, nothing sampled
             self.kappa, self.num_tau_samples = args.kappa, self.qr_dqn
+            self.loss_core = qr.loss_core
         else:                                            # IQN sampling sizes (agent.py:58-63)
             for field in self._IQN_FIELDS:
                 setattr(self, field, getattr(args, field))
+            self.loss_core = compute_loss_iqn.loss_core
         self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each;
         #                      FQF and QR-DQN: {"noises": (n0, n1, n2)}; with random_shift, any of these may also carry
         #                      "shifts": (shifts_states, shifts_next_states), int32 (B, 2) (dy, dx), in place of the draw
@@ -167,14 +172,13 @@ class Agent:
         self.target_net.compose_weights()
 
     def compute_loss_actor_or_learner(self, states, actions, returns, next_states, nonterminals, debug=None):
-        """agent.py:72-147"""
-        if self.rainbow_only:
-            from . import c51
-            return c51.compute_loss_c51(self, states, actions, returns, next_states, nonterminals, debug=debug)
-        if self.qr_dqn is not None:
-            return qr.compute_loss_qr(self, states, actions, returns, next_states, nonterminals, debug=debug)
-        return compute_loss_iqn.compute_loss_actor_or_learner_iqn(
-            self, states, actions, returns, next_states, nonterminals, debug=debug)
+        """agent.py:72-147: the loss (B,) of self.loss_core, differentiable with respect to the online network (and,
+        under FQF, the fraction proposal) when grad mode is on.  ``debug``: dict that receives the core's intermediates."""
+        if torch.is_grad_enabled():
+            params = [p for p in self.online_net.parameters() if p.requires_grad]
+            return _Loss.apply(self, states, actions, returns, next_states, nonterminals, debug, *params)
+        loss, _ = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, keep_graph=False)
+        return loss
 
     def save(self, path, T_actors, T_learner, name):
         """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
@@ -200,3 +204,20 @@ class Agent:
 
     def eval(self):
         self.online_net.eval()
+
+
+class _Loss(torch.autograd.Function):
+    """The agent's loss core as one autograd node.  The online network's parameters are inputs only so that the loss
+    requires grad: the core's backward accumulates straight into the gradient arenas behind every parameter's .grad."""
+
+    @staticmethod
+    def forward(ctx, agent, states, actions, returns, next_states, nonterminals, debug, *params):
+        loss, ctx.bw = agent.loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
+        ctx.n_params = len(params)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        ctx.bw(grad_loss)
+        ctx.bw = None
+        return (None,) * (7 + ctx.n_params)

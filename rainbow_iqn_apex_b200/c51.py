@@ -5,6 +5,7 @@ import torch
 
 from . import hl_gauss
 from ._lib import call, ptr
+from .compute_loss_iqn import _loss_inputs
 from .model import FEAT
 
 
@@ -65,30 +66,27 @@ def hidden_z(net, x, keep=None, col_cache=None, feat=None):
     return zv, za
 
 
-def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None):
-    """agent.py:77-141.  Returns (loss (B,), backward(gscale) closure).
+def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True):
+    """agent.py:77-141.  Returns the loss (B,) and its backward(gscale, gscale_mul=1.0), which accumulates into the online
+    network's gradient arena the gradient of sum_b gscale[b] * gscale_mul * loss[b]; None without ``keep_graph``.
 
     The reference runs online(states) first (:82-83), then the two no-grad passes over next_states (:95-104), each after
     its own reset_noise.  The passes are independent, so they are evaluated here as 2, 3, 1 -- every pass still with its own
     noise sample (injected noises keep their reference slot) -- which leaves the gradient pass's weights and epsilons LIVE
     when the backward runs: no 50 MB of weight / epsilon snapshots per step."""
-    from .compute_loss_iqn import _as_device_inputs
-    states, actions, returns, next_states, nonterminals = _as_device_inputs(
+    (states, actions, returns, next_states, nonterminals), inj = _loss_inputs(
         agent, states, actions, returns, next_states, nonterminals)
     on, tg = agent.online_net, agent.target_net
     B, A, atoms = states.shape[0], agent.action_space, agent.atoms
     dev = states.device
-    inj = getattr(agent, "_inject", None)
-    if isinstance(inj, list):
-        inj = inj.pop(0) if inj else None
-    noises = inj.get("noises", (None, None, None)) if inj else (None, None, None)   # a dict may carry only "shifts"
+    noises = inj.get("noises", (None, None, None))   # a dict may carry only "shifts"
     on.reset_noise(noises[1])                                              # :95
     a_star = torch.empty(B, dtype=torch.int64, device=dev)
     forward(on, next_states, fresh_weights=True, want_argmax=a_star, support=agent.acting_support)  # :97-102
     tg.reset_noise(noises[2])                                              # :103
     pns = forward(tg, next_states, fresh_weights=True, support=agent.support)                      # :104
     on.reset_noise(noises[0])                                              # agent.py:82
-    keep = {}
+    keep = {} if keep_graph else None
     log_ps = forward(on, states, log=True, keep=keep, fresh_weights=True, support=agent.support)   # :83
     loss = torch.empty(B, device=dev)
     dq = torch.empty(B, atoms, device=dev)
@@ -110,6 +108,8 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
         debug.update(a_star=a_star, m=m_out, log_ps=log_ps)
         if target_out is not None:                     # HL-Gauss: the scalar targets and the probabilities they came from
             debug.update(target=target_out, p_target=pns)
+    if keep is None:
+        return loss, None
     version = getattr(on, "_noise_version", 0)       # bumped by every DQN.reset_noise()
 
     def backward(gscale, gscale_mul=1.0):
@@ -177,28 +177,3 @@ def _backward_below_head(on, keep, dzv, dza, gv):
              ptr(gv(hvL.bias_sigma)))
         call("riqn_noisy_linear_dgrad", B, FEAT, 2 * hid, ptr(dh), ptr(on._w_eff_h), ptr(dfeat))
     on.backward_trunk(keep, dfeat)
-
-
-class _HeadLoss(torch.autograd.Function):
-    """A loss whose ``core(agent, states, actions, returns, next_states, nonterminals, debug=...)`` returns (loss,
-    backward(gscale) closure) -- C51's loss_core, qr.loss_core -- as one autograd node."""
-
-    @staticmethod
-    def forward(ctx, core, agent, states, actions, returns, next_states, nonterminals, debug, *params):
-        loss, bw = core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
-        ctx.bw, ctx.n_params = bw, len(params)
-        return loss
-
-    @staticmethod
-    def backward(ctx, grad_loss):
-        ctx.bw(grad_loss)
-        ctx.bw = None
-        return (None,) * (8 + ctx.n_params)
-
-
-def compute_loss_c51(agent, states, actions, returns, next_states, nonterminals, debug=None):
-    if torch.is_grad_enabled():
-        params = [p for p in agent.online_net.parameters() if p.requires_grad]
-        return _HeadLoss.apply(loss_core, agent, states, actions, returns, next_states, nonterminals, debug, *params)
-    loss, _ = loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
-    return loss

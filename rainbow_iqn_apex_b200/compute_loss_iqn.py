@@ -1,9 +1,9 @@
 """IQN loss for actor or learner -- mirror of the reference ``rainbowiqn/compute_loss_iqn.py:216-358``.
 
-Same call signature ``compute_loss_actor_or_learner_iqn(agent, states, actions, returns, next_states,
-nonterminals) -> loss (B,)``; the returned tensor is differentiable w.r.t. the online network: calling
-``(weights * loss).mean().backward()`` (learner.py:23) runs the CUDA backward and leaves the gradients in
-the parameters' ``.grad`` (views of the gradient arena), exactly where the reference leaves them.
+``loss_core(agent, states, actions, returns, next_states, nonterminals) -> (loss (B,), backward)`` is the contract of
+every loss core (c51.loss_core, qr.loss_core).  Agent.compute_loss_actor_or_learner runs the agent's core as one autograd
+node, so ``(weights * loss).mean().backward()`` (learner.py:23) runs the CUDA backward and leaves the gradients in the
+parameters' ``.grad`` (views of the gradient arena), exactly where the reference leaves them.
 
 Three network passes, in the reference's order and with a fresh noise sample before each
 (:234, :255, :289): online(next_states, K) -> a*; target(next_states, N') -> targets; online(states, N).
@@ -16,7 +16,8 @@ as one stacked batch, then online(states, N).
 FQF (Agent.fqf, Yang et al. 2019; see fqf.py) takes every fraction from the online fraction proposal instead of drawing
 them: online(next_states, N at the proposed tau_hat') -> a* by the dtau'-weighted mean; target(next_states, N at the
 tau_hat of states); online(states, N at tau_hat) and, without a reset, online(states, at tau_1..tau_{N-1}) for the fraction
-loss (_fqf_core, fraction_backward).  num_quantile_samples and num_tau_prime_samples are not read under FQF.
+loss (_fqf_core; its gradient is part of loss_core's backward).  num_quantile_samples and num_tau_prime_samples are not
+read under FQF.
 """
 import ctypes
 import math
@@ -110,35 +111,60 @@ def _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, 
         call("riqn_iqn_loss_fwd_bwd_h", B, N, Np, agent.action_space, *args, eps, *outs)
 
 
-def _as_device_inputs(agent, states, actions, returns, next_states, nonterminals):
+def _loss_inputs(agent, states, actions, returns, next_states, nonterminals):
+    """Every loss core's prologue.  Returns the batch on the online network's device (frames uint8 or fp32, actions int64,
+    returns and nonterminals fp32) and the injection dict of this call: ``agent._inject``, or the next entry popped from it
+    when it is a queue (one per call, as Actor.compute_priorities chunks), or {} without one."""
     dev = agent.online_net._flat.device
 
     def frames(x):
         x = x.to(dev)
         return x if x.dtype == torch.uint8 else x.float()
 
-    return (frames(states), actions.to(dev, torch.int64).contiguous(), returns.to(dev, torch.float32).contiguous(),
-            frames(next_states), nonterminals.to(dev, torch.float32).contiguous())
+    inj = getattr(agent, "_inject", None)
+    if isinstance(inj, list):
+        inj = inj.pop(0) if inj else None
+    return ((frames(states), actions.to(dev, torch.int64).contiguous(), returns.to(dev, torch.float32).contiguous(),
+             frames(next_states), nonterminals.to(dev, torch.float32).contiguous()), inj or {})
 
 
-def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_graph=True, debug=None):
-    """Forward passes + fused loss kernel.  Returns (loss (B,), dtheta (N*B,), keep-dict for backward)."""
-    states, actions, returns, next_states, nonterminals = _as_device_inputs(
+def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True):
+    """Forward passes + fused loss kernel.  Returns the loss (B,) and its backward(gscale, gscale_mul=1.0), which
+    accumulates the gradient of sum_b gscale[b] * gscale_mul * loss[b] into the online network's gradient arena and, under
+    FQF, the fraction loss's into agent.fraction_net's; None without ``keep_graph``."""
+    (states, actions, returns, next_states, nonterminals), inj = _loss_inputs(
         agent, states, actions, returns, next_states, nonterminals)
+    noises = inj.get("noises", (None, None, None))   # a dict may carry only "shifts"
+    taus = inj.get("taus", (None, None, None))       # FQF's hook has no fractions
+    batch = (agent, states, actions, returns, next_states, nonterminals)
+    if getattr(agent, "munchausen", None) is not None:
+        loss, dtheta, keep = _munchausen_core(*batch, noises, taus, keep_graph, debug)
+    elif getattr(agent, "fqf", None) is not None:
+        loss, dtheta, keep = _fqf_core(*batch, noises, keep_graph, debug)
+    else:
+        loss, dtheta, keep = _iqn_core(*batch, noises, taus, keep_graph, debug)
+    if keep is None:
+        return loss, None
+
+    def backward(gscale, gscale_mul=1.0):
+        gscale = gscale.contiguous().float()
+        agent.online_net.backward_iqn(keep, dtheta, gscale, actions, gscale_mul)
+        fk = keep.get("fqf")
+        if fk is not None:   # the fraction loss's surrogate of transition b is weighted like its quantile loss
+            dlogits, floss = agent.fraction_net.backward(fk["fr"], fk["q_hat"], fk["q_bnd"], actions, gscale, gscale_mul,
+                                                         agent.fqf[1])
+            if debug is not None:
+                debug.update(dlogits=dlogits, fraction_loss=floss)
+
+    return loss, backward
+
+
+def _iqn_core(agent, states, actions, returns, next_states, nonterminals, noises, taus, keep_graph, debug):
+    """loss_core of plain IQN: (loss (B,), dtheta (N*B,), keep-dict for the backward or None)."""
     on, tg = agent.online_net, agent.target_net
     B = states.shape[0]
     K, Np, N = agent.num_quantile_samples, agent.num_tau_prime_samples, agent.num_tau_samples
-    inj = getattr(agent, "_inject", None)
-    if isinstance(inj, list):            # a queue of injections: one per call (Actor.compute_priorities chunks)
-        inj = inj.pop(0) if inj else None
-    noises = inj.get("noises", (None, None, None)) if inj else (None, None, None)   # a dict may carry only "shifts"
-    taus = inj.get("taus", (None, None, None)) if inj else (None, None, None)     # FQF's hook has no fractions
     dev = states.device
-    if getattr(agent, "munchausen", None) is not None:
-        return _munchausen_core(agent, states, actions, returns, next_states, nonterminals, noises, taus, keep_graph, debug)
-    if getattr(agent, "fqf", None) is not None:
-        return _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises, keep_graph, debug)
-
     on.reset_noise(noises[0])                                                       # :234
     cache = {}   # conv1's pixel block matrix of next_states is shared by the online and the target pass
     # both no-grad passes read next_states: their conv trunks (noise-free weights) run as ONE stacked batch, three launches
@@ -165,7 +191,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, keep_g
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on, tau=tau,
                      keep=keep, tau_sel=tau_sel)
-    return loss, dtheta, keep, actions
+    return loss, dtheta, keep
 
 
 def _munchausen_core(agent, states, actions, returns, next_states, nonterminals, noises, taus, keep_graph, debug):
@@ -195,7 +221,7 @@ def _munchausen_core(agent, states, actions, returns, next_states, nonterminals,
          ptr(dtheta), ptr(theta_out), ptr(target_out), ptr(bonus_out))
     if debug is not None:
         debug.update(bonus=bonus_out, theta=theta_out, target=target_out, q_tgt=q_tgt, q_on=q_on, tau=tau, keep=keep)
-    return loss, dtheta, keep, actions
+    return loss, dtheta, keep
 
 
 def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises, keep_graph, debug):
@@ -206,7 +232,7 @@ def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises
     online proposal select a* = argmax_a sum_i dtau'_i F(s', tau_hat'_i, a); the target network is evaluated on s' at the
     tau_hat of s; the online network at tau_hat (gradient pass) and, with the same composed weights, at the inner
     boundaries tau_1..tau_{N-1} (no-grad) for the fraction loss's W1 gradient.  With ``keep_graph`` the fraction state
-    goes into ``keep["fqf"]`` for fraction_backward."""
+    goes into ``keep["fqf"]`` for the fraction backward."""
     on, tg, fnet = agent.online_net, agent.target_net, agent.fraction_net
     B, N = states.shape[0], agent.num_tau_samples
     dev = states.device
@@ -239,49 +265,9 @@ def _fqf_core(agent, states, actions, returns, next_states, nonterminals, noises
     _quantile_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
                    target_out)
     if keep is not None:
-        keep["fqf"] = dict(fr=fr, q_hat=q_on, q_bnd=q_bnd, actions=actions, debug=debug)
+        keep["fqf"] = dict(fr=fr, q_hat=q_on, q_bnd=q_bnd)
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on, q_bnd=q_bnd,
                      tau=fr["tau"], tau_hat=fr["tau_hat"], dtau=fr["dtau"], logits=fr["logits"], entropy=fr["entropy"],
                      tau_next=fr_n["tau"], dtau_next=fr_n["dtau"], keep=keep)
-    return loss, dtheta, keep, actions
-
-
-def fraction_backward(agent, keep, gscale, gscale_mul=1.0):
-    """The FQF fraction loss's gradient, accumulated into agent.fraction_net's arena, for a loss_core call whose ``keep``
-    it reads; the surrogate of transition b is weighted by gscale[b] * gscale_mul like the quantile loss.  No-op
-    without FQF.  ``debug`` (loss_core's) receives dlogits and fraction_loss."""
-    fk = keep.get("fqf") if keep is not None else None
-    if fk is None:
-        return
-    dlogits, floss = agent.fraction_net.backward(fk["fr"], fk["q_hat"], fk["q_bnd"], fk["actions"], gscale, gscale_mul,
-                                                 agent.fqf[1])
-    if fk["debug"] is not None:
-        fk["debug"].update(dlogits=dlogits, fraction_loss=floss)
-
-
-class _IQNLoss(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, agent, states, actions, returns, next_states, nonterminals, debug, *params):
-        loss, dtheta, keep, actions = loss_core(agent, states, actions, returns, next_states, nonterminals,
-                                                keep_graph=True, debug=debug)
-        ctx.agent, ctx.keep, ctx.dtheta, ctx.actions = agent, keep, dtheta, actions
-        ctx.n_params = len(params)
-        return loss
-
-    @staticmethod
-    def backward(ctx, grad_loss):
-        g = grad_loss.contiguous().float()
-        ctx.agent.online_net.backward_iqn(ctx.keep, ctx.dtheta, g, ctx.actions)
-        fraction_backward(ctx.agent, ctx.keep, g)          # FQF: into agent.fraction_net's arena (fraction_optimiser)
-        ctx.keep = None
-        # gradients were accumulated straight into the arena behind every parameter's .grad
-        return (None,) * (7 + ctx.n_params)
-
-
-def compute_loss_actor_or_learner_iqn(agent, states, actions, returns, next_states, nonterminals, debug=None):
-    if torch.is_grad_enabled():
-        params = [p for p in agent.online_net.parameters() if p.requires_grad]
-        return _IQNLoss.apply(agent, states, actions, returns, next_states, nonterminals, debug, *params)
-    loss, _, _, _ = loss_core(agent, states, actions, returns, next_states, nonterminals, keep_graph=False, debug=debug)
-    return loss
+    return loss, dtheta, keep

@@ -15,7 +15,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment, compute_loss_iqn
+from . import augment
 from .agent import Agent
 from .dynstate import DynState
 
@@ -70,22 +70,24 @@ class Learner(Agent):
     def apply_gradients(self):
         """Gradient all-reduce (data-parallel replicas) + Adam.  learner.py:24"""
         if self.process_group is not None:
-            tail = getattr(self, "_dp_tail", None)
-            if tail is not None:             # the big bucket is already in flight: reduce the rest, then join
-                torch.distributed.all_reduce(self.online_net._flat_grad[:tail], group=self.process_group)
-                torch.cuda.current_stream().wait_stream(self._dp_stream)
-                self._dp_tail = None
-            else:
-                torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
-            if self.fraction_net is not None:   # FQF: the fraction arena (0.8 MB at N = 64) after the DQN's buckets
-                torch.distributed.all_reduce(self.fraction_net._flat_grad, group=self.process_group)
+            self._allreduce_all_grads()
         self._step_optimisers()
 
     def _allreduce_all_grads(self):
-        """Data parallel with the collective outside the captured graphs: every gradient arena, one all-reduce each."""
-        torch.distributed.all_reduce(self.online_net._flat_grad, group=self.process_group)
-        if self.fraction_net is not None:
-            torch.distributed.all_reduce(self.fraction_net._flat_grad, group=self.process_group)
+        """Every gradient arena, one all-reduce each, in _trained_nets order (FQF: the fraction arena, 0.8 MB at N = 64,
+        after the DQN's).  When the backward already started the online arena's tail (_start_tail_allreduce), only its
+        head is left: reduce it, then join the side stream."""
+        for net in self._trained_nets():
+            if net is self.online_net and self._dp_tail is not None:
+                torch.distributed.all_reduce(net._flat_grad[:self._dp_tail], group=self.process_group)
+                torch.cuda.current_stream().wait_stream(self._dp_stream)
+                self._dp_tail = None
+            else:
+                torch.distributed.all_reduce(net._flat_grad, group=self.process_group)
+
+    def _trained_nets(self):
+        """The networks whose gradient arenas a step fills: the online network and, under FQF, the fraction proposal."""
+        return (self.online_net,) if self.fraction_net is None else (self.online_net, self.fraction_net)
 
     def _optimisers(self):
         return (self.optimiser,) if self.fraction_optimiser is None else (self.optimiser, self.fraction_optimiser)
@@ -105,37 +107,20 @@ class Learner(Agent):
         self._dyn.write(nss, sbc, capacity, beta, *more)
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
-        """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arena.
-        ``debug``: dict that receives the IQN, C51 or QR-DQN loss's intermediates (compute_loss_iqn.loss_core,
-        c51.loss_core, qr.loss_core),
-        and with random_shift the shifts and the shifted frames (_shift_frames)."""
+        """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arenas.
+        ``debug``: dict that receives the loss core's intermediates (self.loss_core), and with random_shift the shifts and
+        the shifted frames (_shift_frames)."""
         on = self.online_net
-        dev = on._flat.device
-        weights = weights.to(dev, torch.float32)
+        weights = weights.to(on._flat.device, torch.float32)
         if self.random_shift is not None:
             states, next_states = self._shift_frames(states, next_states, debug)
-        if self.rainbow_only:
-            from . import c51
-            loss, bw = c51.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug)
-            on.zero_grad()
-            bw(weights, 1.0 / weights.shape[0])
-        elif self.qr_dqn is not None:
-            from . import qr
-            loss, bw = qr.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug)
-            on.zero_grad()
-            bw(weights, 1.0 / weights.shape[0])
-        else:
-            loss, dtheta, keep, actions = compute_loss_iqn.loss_core(
-                self, states, actions, returns, next_states, nonterminals, keep_graph=True, debug=debug)
-            if getattr(self, "_debug", None) is not None:                       # parity tests: the pass's activations
-                self._debug.update(keep=keep)
-            on.zero_grad()                                                      # learner.py:22
-            if self.fraction_net is not None:
-                self.fraction_net.zero_grad()
-            on._grads_ready_hook = self._start_tail_allreduce if (self.process_group is not None and self.overlap_allreduce) else None
-            on.backward_iqn(keep, dtheta, weights.contiguous(), actions, 1.0 / weights.shape[0])  # learner.py:23 (.mean())
-            on._grads_ready_hook = None
-            compute_loss_iqn.fraction_backward(self, keep, weights.contiguous(), 1.0 / weights.shape[0])   # FQF only
+        loss, bw = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug)
+        for net in self._trained_nets():                                        # learner.py:22
+            net.zero_grad()
+        # data parallel: DQN.backward_iqn starts the all-reduce of the NoisyLinear gradients as soon as they are final
+        on._grads_ready_hook = self._start_tail_allreduce if (self.process_group is not None and self.overlap_allreduce) else None
+        bw(weights, 1.0 / weights.shape[0])                                     # learner.py:23 (.mean())
+        on._grads_ready_hook = None
         return loss
 
     def _shift_frames(self, states, next_states, debug=None):

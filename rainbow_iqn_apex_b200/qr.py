@@ -21,7 +21,7 @@ import torch
 
 from . import c51, mmd
 from ._lib import call, ptr
-from .compute_loss_iqn import _as_device_inputs, _quantile_loss, greedy_actions
+from .compute_loss_iqn import _loss_inputs, _quantile_loss, greedy_actions
 
 MAX_QUANTILES = 256
 MAX_ACTIONS = 32       # riqn_argmax_mean / riqn_argmax_expected_h
@@ -90,19 +90,17 @@ def backward_dense(on, keep, grad_q, gv):
     c51._backward_below_head(on, keep, dzv, dza, gv)
 
 
-def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None):
-    """The QR-DQN loss (B,) and its backward(gscale, gscale_mul=1.0) closure, which accumulates into the online network's
-    gradient arena the gradient of sum_b gscale[b] * gscale_mul * loss[b].  Injection hook: ``agent._inject =
-    {"noises": (n0, n1, n2)}`` (or a list of them, one per call), the noises of the three passes in their order."""
-    states, actions, returns, next_states, nonterminals = _as_device_inputs(
+def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True):
+    """The QR-DQN loss (B,) and its backward(gscale, gscale_mul=1.0), which accumulates into the online network's
+    gradient arena the gradient of sum_b gscale[b] * gscale_mul * loss[b]; None without ``keep_graph``.  Injection hook:
+    ``agent._inject = {"noises": (n0, n1, n2)}`` (or a list of them, one per call), the noises of the three passes in
+    their order."""
+    (states, actions, returns, next_states, nonterminals), inj = _loss_inputs(
         agent, states, actions, returns, next_states, nonterminals)
     on, tg = agent.online_net, agent.target_net
     B, A, N = states.shape[0], agent.action_space, agent.num_tau_samples
     dev = states.device
-    inj = getattr(agent, "_inject", None)
-    if isinstance(inj, list):
-        inj = inj.pop(0) if inj else None
-    noises = inj.get("noises", (None, None, None)) if inj else (None, None, None)   # a dict may carry only "shifts"
+    noises = inj.get("noises", (None, None, None))   # a dict may carry only "shifts"
     on.reset_noise(noises[0])
     cache = {}   # conv1's pixel block matrix of next_states, shared by the two no-grad passes when they run one by one
     pair = on.trunk_pair(tg, next_states)
@@ -112,7 +110,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     tg.reset_noise(noises[1])
     q_tgt = forward(tg, next_states, fresh_weights=True, col_cache=cache, feat=f_tg)
     on.reset_noise(noises[2])
-    keep = {}
+    keep = {} if keep_graph else None
     q_on = forward(on, states, keep=keep, fresh_weights=True)
     tau_hat = fractions(on, B)
     loss = torch.empty(B, device=dev)
@@ -130,6 +128,8 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on,
                      tau=tau_hat, keep=keep)
+    if keep is None:
+        return loss, None
     version = getattr(on, "_noise_version", 0)
 
     def backward(gscale, gscale_mul=1.0):
@@ -142,13 +142,3 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
         c51._backward_below_head(on, keep, dzv, dza, on.grad_view)
 
     return loss, backward
-
-
-def compute_loss_qr(agent, states, actions, returns, next_states, nonterminals, debug=None):
-    """Agent.compute_loss_actor_or_learner under QR-DQN: the loss (B,), differentiable with respect to the online network
-    when grad mode is on."""
-    if torch.is_grad_enabled():
-        params = [p for p in agent.online_net.parameters() if p.requires_grad]
-        return c51._HeadLoss.apply(loss_core, agent, states, actions, returns, next_states, nonterminals, debug, *params)
-    loss, _ = loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
-    return loss

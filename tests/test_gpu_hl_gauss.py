@@ -328,7 +328,7 @@ def test_learner_step_vs_oracle(cuda_dev, B, eps):
 @pytest.mark.gpu
 @pytest.mark.parametrize("B", [32, 64, 512])
 def test_head_loss_autograd_equals_compute_gradients(cuda_dev, B):
-    """(w * loss).mean().backward() through the _HeadLoss node equals Learner.compute_gradients bit for bit (B a power
+    """(w * loss).mean().backward() through the agent's loss node equals Learner.compute_gradients bit for bit (B a power
     of two, so w / B is exact either way)."""
     from test_gpu_learn import _dev_batch
     params = net.make_params(77 + B, rainbow_only=True)

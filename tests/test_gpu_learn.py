@@ -81,8 +81,9 @@ def test_learn_matches_reference_golden(cuda_dev, golden_dir, name):
         lr._inject = dict(noises=cases.make_noises(seed + 30 + s), taus=taus)
         st, ac, rt, nx, nt = _dev_batch(b, cuda_dev, fp32_frames=(s == 1))
         w = torch.from_numpy(b["weights"]).to(cuda_dev)
-        lr._debug = {}
-        idxs, loss = lr.learn(FakeMem((np.arange(batch), st, ac, rt, nx, nt, w)), None)
+        dbg = {}
+        loss = lr.compute_gradients(st, ac, rt, nx, nt, w, debug=dbg)
+        lr.apply_gradients()
         assert rel_err(loss.cpu().numpy(), g[f"loss_{s}"]) < _loss_tol()
         assert np.max(np.abs(loss.cpu().numpy() - g[f"loss_{s}"]) / np.abs(g[f"loss_{s}"])) < 1e-3  # per transition
         # ReLU kinks: with 4..32 samples a single pre-activation that rounds to opposite sides of 0 on the CPU and the
@@ -93,7 +94,7 @@ def test_learn_matches_reference_golden(cuda_dev, golden_dir, name):
         with torch.no_grad():
             losses.iqn_loss(p_or, net.to_torch(params_np), *cases.batch_to_torch(b), lr._inject["noises"],
                             lr._inject["taus"], **cfg, keep=keep_o)
-        gk = lr._debug["keep"]
+        gk = dbg["keep"]
         fl = [int(((a.cpu() > 0) != (b_ > 0)).sum()) for a, b_ in ((gk["out"][0], keep_o["o1"]), (gk["out"][1], keep_o["o2"]),
                                                                    (gk["out"][2], keep_o["o3"]))]
         upstream = {"conv1": sum(fl), "conv2": fl[1] + fl[2], "conv3": fl[2]}
@@ -257,7 +258,7 @@ def test_full_size_config2_vs_oracle(cuda_dev, batch):
     w = torch.from_numpy(b["weights"]).to(cuda_dev)
     dbg = {}
     from rainbow_iqn_apex_b200 import compute_loss_iqn
-    loss, dtheta, keep_g, _ = compute_loss_iqn.loss_core(lr, st, ac, rt, nx, nt, keep_graph=False, debug=dbg)
+    loss, _ = compute_loss_iqn.loss_core(lr, st, ac, rt, nx, nt, keep_graph=False, debug=dbg)
     p_on, p_tg = net.to_torch(params), net.to_torch(params)
     keep = {}
     with torch.no_grad():

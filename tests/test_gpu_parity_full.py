@@ -72,7 +72,7 @@ def _gpu_forward(dev, c, mode=None):
         lr._inject = dict(noises=c.noises, taus=c.taus)
         st, ac, rt, nx, nt = _dev_batch(c.b, dev)
         dbg = {}
-        loss, _, _, _ = compute_loss_iqn.loss_core(lr, st, ac, rt, nx, nt, keep_graph=False, debug=dbg)
+        loss, _ = compute_loss_iqn.loss_core(lr, st, ac, rt, nx, nt, keep_graph=False, debug=dbg)
         return lr, loss.cpu().numpy(), dbg["a_star"].cpu().numpy()
     finally:
         model.PRECISION.update(old)
@@ -105,10 +105,11 @@ def test_full_size_learn_step_gradients_vs_oracle(cuda_dev, case512):
     w_np[ties] = 0.0                                          # a flipped double-DQN action changes that transition's target
     w = torch.from_numpy(w_np)
     lr._inject = dict(noises=c.noises, taus=c.taus)
-    lr._debug = {}
+    dbg = {}
     st, ac, rt, nx, nt = _dev_batch(c.b, cuda_dev)
     p0 = lr.online_net._flat.clone()
-    _, loss = lr.learn(FakeMem((np.arange(c.batch), st, ac, rt, nx, nt, w.to(cuda_dev))), None)
+    loss = lr.compute_gradients(st, ac, rt, nx, nt, w.to(cuda_dev), debug=dbg)
+    lr.apply_gradients()
     grads_gpu = {k: p.grad.detach().cpu().clone() for k, p in lr.online_net.named_parameters()}
     p_on, p_tg = net.to_torch(c.params, requires_grad=True), net.to_torch(c.params)
     adam = losses.Adam([k for k in p_on if net.is_trainable(k)], lr=5e-5, eps=3.125e-4)
@@ -117,7 +118,7 @@ def test_full_size_learn_step_gradients_vs_oracle(cuda_dev, case512):
     ok = ~ties
     lrel = _rel_loss(loss.cpu().numpy(), o_loss.numpy(), ok)
     assert lrel["max"] < 1e-3, lrel
-    flips = _flips(lr._debug["keep"], keep, c.batch)
+    flips = _flips(dbg["keep"], keep, c.batch)
     report = dict(precision=dict(model.PRECISION), loss=lrel, ties=int(ties.sum()), relu_flips=dict(zip(
         ("conv1", "conv2", "conv3", "h_v", "h_a"), flips)), grads={})
     named = dict(lr.online_net.named_parameters())
