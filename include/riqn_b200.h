@@ -354,6 +354,39 @@ int riqn_miqn_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_spa
                            const float* q_target, const float* tau, const long long* actions, const float* returns,
                            const float* nonterminals, float gamma_n, float kappa, float alpha, float entropy_tau, float l0,
                            float* loss, float* dtheta, float* theta_out, float* target_out, float* bonus_out, void* stream);
+/* CQL (Kumar, Zhou, Tucker & Levine 2020): riqn_iqn_loss_fwd_bwd's loss plus alpha times the log-sum-exp gap of the
+ * online pass.  Per transition b, with N = n_tau and a_t = actions[b]:
+ *   Q_a      = fl(S_a / N),  S_a = fp32 sum over i ascending of q_online[i*batch+b, a]   (riqn_argmax_mean's mean)
+ *   lse      = m + log(sum_a exp(Q_a - m)),  m = max_a Q_a                 (double, a ascending, no atomics)
+ *   pi[b,a]  = fl(exp(Q_a - lse))              (batch, A)   the softmax of the means
+ *   gap[b]   = fl(lse - Q_{a_t}) >= 0
+ *   td_loss[b], dtheta, theta_out, target_out  bit for bit those of riqn_iqn_loss_fwd_bwd on the same inputs
+ *   loss[b]  = fl(td_loss[b] + fl(alpha * gap[b]))
+ * dtheta is the gradient of td_loss alone: the gap's, (alpha / N)(pi[b,a] - 1{a = a_t}) on every row i*batch + b, is
+ * dense over actions and riqn_cql_dense_grad folds it in.  gap, theta_out and target_out may be NULL.  Returns
+ * cudaErrorInvalidValue, writing nothing, outside the limits of riqn_iqn_loss_fwd_bwd, unless alpha is finite and > 0,
+ * or when loss, td_loss, pi or dtheta is NULL. */
+int riqn_cql_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                          const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                          const float* returns, const float* nonterminals, float gamma_n, float kappa, float alpha,
+                          float* loss, float* td_loss, float* pi, float* dtheta, float* gap, float* theta_out,
+                          float* target_out, void* stream);
+/* riqn_cql_loss_fwd_bwd against riqn_iqn_loss_fwd_bwd_h's transformed target; the gap is taken on the h-space outputs.
+ * Its limits, and eps finite and >= 0. */
+int riqn_cql_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                            const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                            const float* returns, const float* nonterminals, float gamma_n, float kappa, float alpha,
+                            float eps, float* loss, float* td_loss, float* pi, float* dtheta, float* gap,
+                            float* theta_out, float* target_out, void* stream);
+/* The dense upstream gradient grad_q (n*batch, A), quantile-major, of sum_b gscale[b]*gscale_mul*loss[b] at the CQL loss,
+ * from its dtheta (n*batch) and pi (batch, A), every operation rounded on its own:
+ *   w_b = fl(gscale[b] * gscale_mul),  c = fl(alpha / n),  g = fl(c * pi[b,a])
+ *   grad_q[i*batch+b, a] = fl(w_b * g)                                  for a != actions[b]
+ *                        = fl(w_b * fl(dtheta[i*batch+b] + fl(g - c)))   for a == actions[b]
+ * for riqn_dueling_bwd_dense / riqn_qr_head_bwd_dense.  Returns cudaErrorInvalidValue, writing nothing, unless batch, n >= 1,
+ * 1 <= action_space <= 32, alpha is finite and > 0 and no pointer is NULL. */
+int riqn_cql_dense_grad(int batch, int n, int action_space, const float* dtheta, const float* pi, const long long* actions,
+                        const float* gscale, float gscale_mul, float alpha, float* grad_q, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Value-function rescaling (Pohlen et al. 2018, the transformed Bellman operator; no counterpart in the reference)

@@ -74,6 +74,9 @@ SIGNATURES = {
     "riqn_iqn_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float,
                               _P, _P, _P, _P, _P],
     "riqn_miqn_loss_fwd_bwd": [C.c_int] * 4 + [_P] * 6 + [C.c_float] * 5 + [_P] * 6,
+    "riqn_cql_loss_fwd_bwd": [C.c_int] * 4 + [_P] * 7 + [C.c_float] * 3 + [_P] * 8,
+    "riqn_cql_loss_fwd_bwd_h": [C.c_int] * 4 + [_P] * 7 + [C.c_float] * 4 + [_P] * 8,
+    "riqn_cql_dense_grad": [C.c_int] * 3 + [_P] * 4 + [C.c_float] * 2 + [_P, _P],
     "riqn_fqf_fractions": [C.c_int, C.c_int] + [_P] * 6,
     "riqn_fqf_fraction_bwd": [C.c_int] * 3 + [_P] * 6 + [C.c_float] * 2 + [_P] * 3,
     "riqn_fqf_fraction_wgrad": [C.c_int] * 3 + [_P] * 5,

@@ -8,7 +8,8 @@ qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-se
 ``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
 ``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
 ``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
-``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51 head (hl_gauss.py), and ``random_shift`` for the
+``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51 head (hl_gauss.py), ``cql`` for the conservative
+regulariser of the IQN and QR-DQN losses (cql.py), and ``random_shift`` for the
 learner's random-shift augmentation (augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
 optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
@@ -18,7 +19,7 @@ import os
 import torch
 
 from . import _lib
-from . import augment, c51, compute_loss_iqn, fqf, hl_gauss, mmd, qr
+from . import augment, c51, compute_loss_iqn, cql, fqf, hl_gauss, mmd, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -99,6 +100,10 @@ class Agent:
         self.hl_gauss = hl_gauss.check_hl_gauss(
             getattr(args, "hl_gauss", 0), getattr(args, "hl_gauss_sigma", hl_gauss.HL_GAUSS_DEFAULTS["hl_gauss_sigma"]),
             rainbow_only=self.rainbow_only)
+        # CQL: optional args fields (absent from the reference's namespace: off).  None, or the float32 alpha of
+        # cql.check_cql; fixed for the agent's life, since a captured step graph holds it
+        self.cql = cql.check_cql(getattr(args, "cql", 0), getattr(args, "cql_alpha", cql.CQL_DEFAULTS["cql_alpha"]),
+                                 rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf, mmd=self.mmd)
         self.fraction_net = self.fraction_optimiser = None
         if self.fqf is not None:
             # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed

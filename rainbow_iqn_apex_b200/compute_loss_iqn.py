@@ -18,6 +18,9 @@ them: online(next_states, N at the proposed tau_hat') -> a* by the dtau'-weighte
 tau_hat of states); online(states, N at tau_hat) and, without a reset, online(states, at tau_1..tau_{N-1}) for the fraction
 loss (_fqf_core; its gradient is part of loss_core's backward).  num_quantile_samples and num_tau_prime_samples are not
 read under FQF.
+
+CQL (Agent.cql, cql.py) adds alpha times the log-sum-exp gap of the online pass to the plain IQN loss; its backward runs
+the head's dense backward on the gradient riqn_cql_dense_grad forms.
 """
 import ctypes
 import math
@@ -25,6 +28,7 @@ import numbers
 
 import torch
 
+from . import cql
 from ._lib import call, ptr
 
 MUNCHAUSEN_DEFAULTS = {"munchausen_alpha": 0.9, "munchausen_tau": 0.03, "munchausen_l0": -1.0}   # the paper's
@@ -148,7 +152,14 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
 
     def backward(gscale, gscale_mul=1.0):
         gscale = gscale.contiguous().float()
-        agent.online_net.backward_iqn(keep, dtheta, gscale, actions, gscale_mul)
+        pi = keep.get("cql_pi")
+        if pi is None:
+            agent.online_net.backward_iqn(keep, dtheta, gscale, actions, gscale_mul)
+        else:                 # CQL: the gap's gradient is dense over actions
+            agent.online_net.check_live(keep)
+            B = actions.shape[0]
+            G = cql.dense_grad(agent, B, dtheta.shape[0] // B, dtheta, pi, actions, gscale, gscale_mul)
+            agent.online_net.backward_iqn_dense(keep, G)
         fk = keep.get("fqf")
         if fk is not None:   # the fraction loss's surrogate of transition b is weighted like its quantile loss
             dlogits, floss = agent.fraction_net.backward(fk["fr"], fk["q_hat"], fk["q_bnd"], actions, gscale, gscale_mul,
@@ -186,8 +197,17 @@ def _iqn_core(agent, states, actions, returns, next_states, nonterminals, noises
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, Np, device=dev)
-    _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
-                   target_out)                                                      # :262-357
+    if getattr(agent, "cql", None) is None:
+        _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
+                       target_out)                                                  # :262-357
+    else:                                                                           # CQL (cql.py)
+        gap = torch.empty(B, device=dev) if debug is not None else None
+        td, pi = cql.cql_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta,
+                              theta_out, target_out, gap)
+        if keep is not None:
+            keep["cql_pi"] = pi
+        if debug is not None:
+            debug.update(td_loss=td, gap=gap, pi=pi)
     if debug is not None:
         debug.update(a_star=a_star, theta=theta_out, target=target_out, q_sel=q_sel, q_tgt=q_tgt, q_on=q_on, tau=tau,
                      keep=keep, tau_sel=tau_sel)

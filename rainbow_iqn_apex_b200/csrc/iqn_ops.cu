@@ -809,19 +809,15 @@ __device__ __forceinline__ void quantile_huber_loss(int B, int N, int Np, int A,
   }
 }
 
+// The double-DQN targets T[b, 0..Np) of transition b into sT (and target_out), shared with cql_loss_kernel.
 // RESCALE: the transformed Bellman target T[b,j] = fl(h(R[b] + g * h^-1(q_tgt[...])))  (value_rescaling.cuh), with
 // g = fl(gamma^n*nt[b]) as above and the sum and product rounded in double; eps is read only then.
 template <bool RESCALE>
-__global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
-                                const float* __restrict__ q_tgt, const float* __restrict__ tau,
-                                const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
-                                const float* __restrict__ returns, const float* __restrict__ nonterminals,
-                                float gamma_n, float kappa, float* __restrict__ loss, float* __restrict__ dtheta,
-                                float* __restrict__ theta_out, float* __restrict__ target_out, float eps) {
-  extern __shared__ float sT[];  // Np targets + 32 reduction slots
-  float* red = sT + Np;
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int as = (int)a_star[b], ac = (int)actions[b];
+__device__ __forceinline__ void stage_double_dqn_targets(int B, int Np, int A, int b, int as, const float* __restrict__ q_tgt,
+                                                         const float* __restrict__ returns,
+                                                         const float* __restrict__ nonterminals, float gamma_n, float eps,
+                                                         float* sT, float* __restrict__ target_out) {
+  const int tid = threadIdx.x;
   const float g = __fmul_rn(gamma_n, nonterminals[b]);
   for (int j = tid; j < Np; j += blockDim.x) {
     float t;
@@ -834,8 +830,86 @@ __global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __rest
     sT[j] = t;
     if (target_out) target_out[(long)b * Np + j] = t;
   }
+}
+
+template <bool RESCALE>
+__global__ void iqn_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
+                                const float* __restrict__ q_tgt, const float* __restrict__ tau,
+                                const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
+                                const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                                float gamma_n, float kappa, float* __restrict__ loss, float* __restrict__ dtheta,
+                                float* __restrict__ theta_out, float* __restrict__ target_out, float eps) {
+  extern __shared__ float sT[];  // Np targets + 32 reduction slots
+  float* red = sT + Np;
+  const int b = blockIdx.x;
+  const int as = (int)a_star[b], ac = (int)actions[b];
+  stage_double_dqn_targets<RESCALE>(B, Np, A, b, as, q_tgt, returns, nonterminals, gamma_n, eps, sT, target_out);
   __syncthreads();
   quantile_huber_loss(B, N, Np, A, b, ac, q_on, tau, kappa, sT, red, loss, dtheta, theta_out);
+}
+
+// ------------------------------------------------------------------------------------------------
+// CQL (Kumar, Zhou, Tucker & Levine 2020): iqn_loss_kernel's loss plus alpha times the log-sum-exp gap of the online pass
+//   Q_a    = fl(S_a / N),  S_a = fp32 sum over i ascending of q_on[i*B+b, a]           (argmax_mean_kernel's mean)
+//   lse    = m + log(sum_a exp(Q_a - m)),  m = max_a Q_a                                 (double, a ascending)
+//   pi[b,a] = fl(exp(Q_a - lse)),  gap[b] = fl(lse - Q_{act[b]})  (>= 0),  loss[b] = fl(td[b] + fl(alpha * gap[b]))
+// td_loss, dtheta, theta_out and target_out are iqn_loss_kernel's.  Warp 0 forms the gap, lane a owning Q_a; every lane
+// runs the same a-ascending sum over shuffles.  The gap's gradient is formed at backward time (cql_dense_grad_kernel).
+// ------------------------------------------------------------------------------------------------
+template <bool RESCALE>
+__global__ void cql_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
+                                const float* __restrict__ q_tgt, const float* __restrict__ tau,
+                                const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
+                                const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                                float gamma_n, float kappa, float alpha, float* __restrict__ loss,
+                                float* __restrict__ td_loss, float* __restrict__ pi, float* __restrict__ dtheta,
+                                float* __restrict__ gap_out, float* __restrict__ theta_out,
+                                float* __restrict__ target_out, float eps) {
+  extern __shared__ float sT[];  // Np targets + 32 reduction slots
+  float* red = sT + Np;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int as = (int)a_star[b], ac = (int)actions[b];
+  stage_double_dqn_targets<RESCALE>(B, Np, A, b, as, q_tgt, returns, nonterminals, gamma_n, eps, sT, target_out);
+  float gap = 0.f;
+  if (tid < 32) {
+    float qa = -INFINITY;
+    if (tid < A) {
+      float s = 0.f;
+      const float* col = q_on + (long)b * A + tid;
+#pragma unroll 8
+      for (int i = 0; i < N; ++i) s = __fadd_rn(s, col[(long)i * B * A]);
+      qa = __fdiv_rn(s, (float)N);
+    }
+    float mf = qa;
+    for (int a = 0; a < A; ++a) mf = fmaxf(mf, __shfl_sync(0xffffffffu, qa, a));
+    const double m = (double)mf;
+    const double e = tid < A ? exp(__dsub_rn((double)qa, m)) : 0.0;
+    double sum = 0.0;
+    for (int a = 0; a < A; ++a) sum = __dadd_rn(sum, __shfl_sync(0xffffffffu, e, a));
+    const double lse = __dadd_rn(m, log(sum));
+    if (tid < A) pi[(long)b * A + tid] = __double2float_rn(exp(__dsub_rn((double)qa, lse)));
+    gap = __double2float_rn(__dsub_rn(lse, (double)__shfl_sync(0xffffffffu, qa, ac)));
+    if (tid == 0 && gap_out) gap_out[b] = gap;
+  }
+  __syncthreads();
+  quantile_huber_loss(B, N, Np, A, b, ac, q_on, tau, kappa, sT, red, td_loss, dtheta, theta_out);
+  if (tid == 0) loss[b] = __fadd_rn(td_loss[b], __fmul_rn(alpha, gap));   // thread 0 wrote td_loss[b]
+}
+
+// The dense upstream gradient of sum_b w_b loss[b] at the CQL loss, one thread per element of G (N*B, A):
+//   w_b = fl(gscale[b] * gmul),  c = fl(alpha / N),  g = fl(c * pi[b,a])
+//   G[i*B+b, a] = fl(w_b * g)  (a != act[b]),   fl(w_b * fl(dtheta[i*B+b] + fl(g - c)))  (a == act[b])
+__global__ void cql_dense_grad_kernel(int B, int N, int A, const float* __restrict__ dtheta, const float* __restrict__ pi,
+                                      const int64_t* __restrict__ actions, const float* __restrict__ gscale, float gmul,
+                                      float alpha, float* __restrict__ G) {
+  const long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long r = e / A;
+  if (r >= (long)N * B) return;
+  const int a = (int)(e - r * A), b = (int)(r % B);
+  const float w = __fmul_rn(gscale[b], gmul);
+  const float c = __fdiv_rn(alpha, (float)N);
+  const float g = __fmul_rn(c, pi[(long)b * A + a]);
+  G[e] = a == (int)actions[b] ? __fmul_rn(w, __fadd_rn(dtheta[r], __fsub_rn(g, c))) : __fmul_rn(w, g);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1723,6 +1797,61 @@ RIQN_API int riqn_iqn_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int 
   iqn_loss_kernel<true><<<batch, threads, smem, (cudaStream_t)stream>>>(
       batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, (const int64_t*)a_star,
       returns, nonterminals, gamma_n, kappa, loss, dtheta, theta_out, target_out, eps);
+  return (int)cudaGetLastError();
+}
+
+template <bool RESCALE>
+static int launch_cql_loss(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                           const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                           const float* returns, const float* nonterminals, float gamma_n, float kappa, float alpha,
+                           float eps, float* loss, float* td_loss, float* pi, float* dtheta, float* gap,
+                           float* theta_out, float* target_out, void* stream) {
+  if (!huber_loss_args_ok(batch, n_tau, n_tau_prime, action_space, kappa, 0) || !(alpha > 0.f) || !isfinite(alpha) ||
+      !loss || !td_loss || !pi || !dtheta)
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;
+  if (threads > 1024) threads = 1024;
+  if (threads < 32) threads = 32;
+  const size_t smem = sizeof(float) * (n_tau_prime + 32);
+  cql_loss_kernel<RESCALE><<<batch, threads, smem, (cudaStream_t)stream>>>(
+      batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, (const int64_t*)a_star,
+      returns, nonterminals, gamma_n, kappa, alpha, loss, td_loss, pi, dtheta, gap, theta_out, target_out, eps);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_cql_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                                   const float* q_target, const float* tau, const long long* actions,
+                                   const long long* a_star, const float* returns, const float* nonterminals,
+                                   float gamma_n, float kappa, float alpha, float* loss, float* td_loss, float* pi,
+                                   float* dtheta, float* gap, float* theta_out, float* target_out, void* stream) {
+  return launch_cql_loss<false>(batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, actions, a_star,
+                                returns, nonterminals, gamma_n, kappa, alpha, 0.f, loss, td_loss, pi, dtheta, gap,
+                                theta_out, target_out, stream);
+}
+
+RIQN_API int riqn_cql_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                                     const float* q_target, const float* tau, const long long* actions,
+                                     const long long* a_star, const float* returns, const float* nonterminals,
+                                     float gamma_n, float kappa, float alpha, float eps, float* loss, float* td_loss,
+                                     float* pi, float* dtheta, float* gap, float* theta_out, float* target_out,
+                                     void* stream) {
+  if (!vr_eps_ok(eps)) return (int)cudaErrorInvalidValue;
+  return launch_cql_loss<true>(batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, actions, a_star,
+                               returns, nonterminals, gamma_n, kappa, alpha, eps, loss, td_loss, pi, dtheta, gap,
+                               theta_out, target_out, stream);
+}
+
+RIQN_API int riqn_cql_dense_grad(int batch, int n, int action_space, const float* dtheta, const float* pi,
+                                 const long long* actions, const float* gscale, float gscale_mul, float alpha,
+                                 float* grad_q, void* stream) {
+  if (batch < 1 || n < 1 || action_space < 1 || action_space > 32 || !(alpha > 0.f) || !isfinite(alpha) || !dtheta ||
+      !pi || !actions || !gscale || !grad_q)
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  const long total = (long)n * batch * action_space;
+  cql_dense_grad_kernel<<<riqn_cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      batch, n, action_space, dtheta, pi, (const int64_t*)actions, gscale, gscale_mul, alpha, grad_q);
   return (int)cudaGetLastError();
 }
 

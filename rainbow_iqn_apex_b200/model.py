@@ -787,9 +787,7 @@ class DQN(nn.Module):
     def backward_iqn(self, keep, dtheta, gscale, actions, gscale_mul=1.0):
         """Accumulate dL/dparams into the gradient arena for the forward recorded in ``keep``, where
         dL/dq[r, actions[b]] = dtheta[r] * gscale[b] * gscale_mul  (r = quantile*B + b)."""
-        if keep.get("noise_version", None) != getattr(self, "_noise_version", 0):
-            raise RuntimeError("the network's noise was resampled between this forward pass and its backward: the composed "
-                               "weights / epsilons of the gradient pass are gone (call backward before the next reset_noise)")
+        self.check_live(keep)
         R, B, hid, A = keep["feat"].shape[0] * keep["num_quantiles"], keep["feat"].shape[0], self.hidden, self.action_space
 
         def one_hot(fused_dh, dh, dh_hi, dbs, dz, dzT):
@@ -800,6 +798,13 @@ class DQN(nn.Module):
                 call("riqn_dueling_bwd", R, B, hid, A, ptr(keep["h"]), ptr(self._w_eff_z), ptr(dtheta), ptr(gscale),
                      float(gscale_mul), ptr(actions), ptr(dh), ptr(dz), ptr(dzT))
         self._backward_head(keep, one_hot, self.grad_view)
+
+    def check_live(self, keep):
+        """Raise unless the composed weights of the forward recorded in ``keep`` are still the network's: its backward
+        reads the live weights."""
+        if keep.get("noise_version", None) != getattr(self, "_noise_version", 0):
+            raise RuntimeError("the network's noise was resampled between this forward pass and its backward: the composed "
+                               "weights / epsilons of the gradient pass are gone (call backward before the next reset_noise)")
 
     def backward_iqn_dense(self, keep, grad_q, gv=None):
         """Accumulate dL/dparams for the forward recorded in ``keep`` given the dense dL/dq ``grad_q`` (Nq*B, A), fp32,

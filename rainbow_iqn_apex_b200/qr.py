@@ -13,13 +13,14 @@ unclipped returns at the cost of a C51 step.
 The learner step runs the IQN path's three passes, each after its own noise reset: online(s') -> a* = argmax_a mean_i q_i,
 target(s') (both trunks in one stacked trunk_pair), online(s) with the backward's operands; then the quantile-Huber loss
 against R + gamma^n nt q_tgt[a*] at the N x N fraction pairs, and riqn_qr_head_bwd below it.  MMDQN (agent.mmd, mmd.py)
-runs the same step with the MMD loss kernel in place of the quantile-Huber one.
+runs the same step with the MMD loss kernel in place of the quantile-Huber one; CQL (agent.cql, cql.py) adds alpha times
+the log-sum-exp gap to the quantile-Huber loss and takes riqn_qr_head_bwd_dense.
 """
 import numbers
 
 import torch
 
-from . import c51, mmd
+from . import c51, cql, mmd
 from ._lib import call, ptr
 from .compute_loss_iqn import _loss_inputs, _quantile_loss, greedy_actions
 
@@ -119,7 +120,14 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, N, device=dev)
-    if getattr(agent, "mmd", None) is None:
+    pi = None
+    if getattr(agent, "cql", None) is not None:       # CQL: the same loss plus alpha * gap (cql.py)
+        gap = torch.empty(B, device=dev) if debug is not None else None
+        td, pi = cql.cql_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta,
+                              theta_out, target_out, gap)
+        if debug is not None:
+            debug.update(td_loss=td, gap=gap, pi=pi)
+    elif getattr(agent, "mmd", None) is None:
         _quantile_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta,
                        theta_out, target_out)
     else:                                              # MMDQN: the same particles under the MMD loss (mmd.py)
@@ -136,6 +144,9 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
         if getattr(on, "_noise_version", 0) != version:
             raise RuntimeError("the online network's noise was resampled between the QR-DQN loss and its backward")
         gscale = gscale.contiguous().float()
+        if pi is not None:                             # CQL: the gap's gradient is dense over actions
+            backward_dense(on, keep, cql.dense_grad(agent, B, N, dtheta, pi, actions, gscale, gscale_mul), on.grad_view)
+            return
         dzv = torch.empty(B, N, device=dev)
         dza = torch.empty(B, A * N, device=dev)
         call("riqn_qr_head_bwd", B, A, N, ptr(dtheta), ptr(gscale), float(gscale_mul), ptr(actions), ptr(dzv), ptr(dza))
