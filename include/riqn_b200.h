@@ -387,6 +387,41 @@ int riqn_cql_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_sp
  * 1 <= action_space <= 32, alpha is finite and > 0 and no pointer is NULL. */
 int riqn_cql_dense_grad(int batch, int n, int action_space, const float* dtheta, const float* pi, const long long* actions,
                         const float* gscale, float gscale_mul, float alpha, float* grad_q, void* stream);
+/* DQfD (Hester et al. 2018): riqn_iqn_loss_fwd_bwd's loss plus lambda times the large-margin imitation loss on the rows
+ * flagged as demonstrations.  Per transition b, with N = n_tau, a_E = actions[b] and l = margin:
+ *   Q_a      = fl(S_a / N),  S_a = fp32 sum over i ascending of q_online[i*batch+b, a]   (riqn_argmax_mean's mean)
+ *   v_a      = Q_a for a = a_E,  fl(Q_a + l) otherwise
+ *   a_hat[b] = the first a (ascending) with v_a = M,  M = max_a v_a
+ *   margin_out[b] = J = fl(M - Q_{a_E}) >= 0
+ *   td_loss[b], dtheta, theta_out, target_out  bit for bit those of riqn_iqn_loss_fwd_bwd on the same inputs
+ *   loss[b]  = fl(td_loss[b] + fl(lambda * J)) if demo[b] != 0, else td_loss[b]
+ * demo: (batch,) flags, or NULL for no demonstration.  dtheta is the gradient of td_loss alone: J's, (1/N)(1{a = a_hat}
+ * - 1{a = a_E}) on every row i*batch + b of a flagged transition, is folded in by riqn_dqfd_dense_grad.  margin_out,
+ * theta_out and target_out may be NULL.  Returns cudaErrorInvalidValue, writing nothing, outside the limits of
+ * riqn_iqn_loss_fwd_bwd, unless margin and lambda are finite and > 0, or when loss, td_loss, a_hat or dtheta is NULL. */
+int riqn_dqfd_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                           const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                           const float* returns, const float* nonterminals, const unsigned char* demo, float gamma_n,
+                           float kappa, float margin, float lambda, float* loss, float* td_loss, float* dtheta,
+                           float* margin_out, long long* a_hat, float* theta_out, float* target_out, void* stream);
+/* riqn_dqfd_loss_fwd_bwd against riqn_iqn_loss_fwd_bwd_h's transformed target; the margin is taken on the h-space outputs,
+ * in h-space units.  Its limits, and eps finite and >= 0. */
+int riqn_dqfd_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                             const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                             const float* returns, const float* nonterminals, const unsigned char* demo, float gamma_n,
+                             float kappa, float margin, float lambda, float eps, float* loss, float* td_loss,
+                             float* dtheta, float* margin_out, long long* a_hat, float* theta_out, float* target_out,
+                             void* stream);
+/* The dense upstream gradient grad_q (n*batch, A), quantile-major, of sum_b gscale[b]*gscale_mul*loss[b] at the DQfD loss,
+ * from its dtheta (n*batch) and a_hat (batch), every operation rounded on its own; zero in every column not named:
+ *   w_b = fl(gscale[b] * gscale_mul),  c = fl(lambda / n)
+ *   demo NULL, demo[b] == 0 or a_hat[b] == actions[b]:  grad_q[i*batch+b, actions[b]] = fl(w_b * dtheta[i*batch+b])
+ *   otherwise:  grad_q[i*batch+b, a_hat[b]] = fl(w_b * c),  grad_q[i*batch+b, actions[b]] = fl(w_b * fl(dtheta - c))
+ * for riqn_dueling_bwd_dense / riqn_qr_head_bwd_dense.  Returns cudaErrorInvalidValue, writing nothing, unless batch, n >= 1,
+ * 1 <= action_space <= 32, lambda is finite and > 0 and no pointer but demo is NULL. */
+int riqn_dqfd_dense_grad(int batch, int n, int action_space, const float* dtheta, const long long* a_hat,
+                         const long long* actions, const unsigned char* demo, const float* gscale, float gscale_mul,
+                         float lambda, float* grad_q, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Value-function rescaling (Pohlen et al. 2018, the transformed Bellman operator; no counterpart in the reference)
@@ -611,6 +646,13 @@ int riqn_sumtree_is_weights(int n, const double* tree, const double* priorities,
 int riqn_sumtree_update(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
                         float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
                         double* max_priority, void* stream);
+/* riqn_sumtree_update with DQfD's demonstration priority bonus eps_d (Hester et al. 2018): after the power, every entry
+ * with tree_idx >= demo_leaf (the leaves of the demonstration segments) takes new = fl(new + bonus).  The diff, the
+ * propagation (duplicates included) and max_priority are riqn_sumtree_update's on those priorities.  Returns
+ * cudaErrorInvalidValue, writing nothing, unless bonus is finite and >= 0 and demo_leaf >= 0. */
+int riqn_sumtree_update_demo(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
+                             float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
+                             double* max_priority, long long demo_leaf, float bonus, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Prioritized replay: frame store            replaces the Redis hashes "transitions<i>" (:184-193)

@@ -77,6 +77,9 @@ SIGNATURES = {
     "riqn_cql_loss_fwd_bwd": [C.c_int] * 4 + [_P] * 7 + [C.c_float] * 3 + [_P] * 8,
     "riqn_cql_loss_fwd_bwd_h": [C.c_int] * 4 + [_P] * 7 + [C.c_float] * 4 + [_P] * 8,
     "riqn_cql_dense_grad": [C.c_int] * 3 + [_P] * 4 + [C.c_float] * 2 + [_P, _P],
+    "riqn_dqfd_loss_fwd_bwd": [C.c_int] * 4 + [_P] * 8 + [C.c_float] * 4 + [_P] * 8,
+    "riqn_dqfd_loss_fwd_bwd_h": [C.c_int] * 4 + [_P] * 8 + [C.c_float] * 5 + [_P] * 8,
+    "riqn_dqfd_dense_grad": [C.c_int] * 3 + [_P] * 5 + [C.c_float] * 2 + [_P, _P],
     "riqn_fqf_fractions": [C.c_int, C.c_int] + [_P] * 6,
     "riqn_fqf_fraction_bwd": [C.c_int] * 3 + [_P] * 6 + [C.c_float] * 2 + [_P] * 3,
     "riqn_fqf_fraction_wgrad": [C.c_int] * 3 + [_P] * 5,
@@ -107,6 +110,8 @@ SIGNATURES = {
     "riqn_sumtree_sample": [C.c_int, C.c_long, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P],
     "riqn_sumtree_is_weights": [C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P, _P, _P],
     "riqn_sumtree_update": [C.c_int, C.c_long, _P, _P, _P, C.c_float, C.c_int, _P, _P, _P, _P],
+    "riqn_sumtree_update_demo": [C.c_int, C.c_long, _P, _P, _P, C.c_float, C.c_int, _P, _P, _P, C.c_longlong, C.c_float,
+                                 _P],
     "riqn_replay_append": [C.c_int, C.c_int, C.c_int, C.c_int] + [_P] * 11,
     "riqn_frame_gather": [C.c_int, C.c_int, C.c_int, C.c_int] + [_P] * 12,
     "riqn_split_bf16_multi": [C.c_int, C.POINTER(SplitJob), _P],

@@ -9,7 +9,8 @@ qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-se
 ``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
 ``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
 ``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51 head (hl_gauss.py), ``cql`` for the conservative
-regulariser of the IQN and QR-DQN losses (cql.py), and ``random_shift`` for the
+regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's large-margin loss on demonstrations (dqfd.py),
+and ``random_shift`` for the
 learner's random-shift augmentation (augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
 optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
@@ -19,7 +20,7 @@ import os
 import torch
 
 from . import _lib
-from . import augment, c51, compute_loss_iqn, cql, fqf, hl_gauss, mmd, qr
+from . import augment, c51, compute_loss_iqn, cql, dqfd, fqf, hl_gauss, mmd, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -104,6 +105,12 @@ class Agent:
         # cql.check_cql; fixed for the agent's life, since a captured step graph holds it
         self.cql = cql.check_cql(getattr(args, "cql", 0), getattr(args, "cql_alpha", cql.CQL_DEFAULTS["cql_alpha"]),
                                  rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf, mmd=self.mmd)
+        # DQfD: optional args fields (absent from the reference's namespace: off).  None, or the float32 (margin, lambda)
+        # of dqfd.check_dqfd; fixed for the agent's life, since a captured step graph holds them
+        self.dqfd = dqfd.check_dqfd(getattr(args, "dqfd", 0),
+                                    *(getattr(args, f, v) for f, v in dqfd.DQFD_DEFAULTS.items()),
+                                    rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf, mmd=self.mmd,
+                                    cql=self.cql)
         self.fraction_net = self.fraction_optimiser = None
         if self.fqf is not None:
             # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed
@@ -152,6 +159,9 @@ class Agent:
             qr.check_qr(1, self.qr_dqn, risk=risk)
         if getattr(self, "mmd", None) is not None:
             mmd.check_mmd(1, self.mmd, qr_dqn=self.qr_dqn, risk=risk)
+        if getattr(self, "dqfd", None) is not None:
+            dqfd.check_dqfd(1, *self.dqfd, rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf,
+                            mmd=self.mmd, cql=self.cql)
         self.risk = risk
 
     @staticmethod
@@ -176,13 +186,15 @@ class Agent:
         self.target_net._eps_flat.copy_(self.online_net._eps_flat)
         self.target_net.compose_weights()
 
-    def compute_loss_actor_or_learner(self, states, actions, returns, next_states, nonterminals, debug=None):
+    def compute_loss_actor_or_learner(self, states, actions, returns, next_states, nonterminals, debug=None, demo=None):
         """agent.py:72-147: the loss (B,) of self.loss_core, differentiable with respect to the online network (and,
-        under FQF, the fraction proposal) when grad mode is on.  ``debug``: dict that receives the core's intermediates."""
+        under FQF, the fraction proposal) when grad mode is on.  ``debug``: dict that receives the core's intermediates.
+        ``demo``: None, or the (B,) demonstration flags of a DQfD agent (dqfd.py)."""
         if torch.is_grad_enabled():
             params = [p for p in self.online_net.parameters() if p.requires_grad]
-            return _Loss.apply(self, states, actions, returns, next_states, nonterminals, debug, *params)
-        loss, _ = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, keep_graph=False)
+            return _Loss.apply(self, states, actions, returns, next_states, nonterminals, debug, demo, *params)
+        loss, _ = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, keep_graph=False,
+                                 demo=demo)
         return loss
 
     def save(self, path, T_actors, T_learner, name):
@@ -216,8 +228,8 @@ class _Loss(torch.autograd.Function):
     requires grad: the core's backward accumulates straight into the gradient arenas behind every parameter's .grad."""
 
     @staticmethod
-    def forward(ctx, agent, states, actions, returns, next_states, nonterminals, debug, *params):
-        loss, ctx.bw = agent.loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug)
+    def forward(ctx, agent, states, actions, returns, next_states, nonterminals, debug, demo, *params):
+        loss, ctx.bw = agent.loss_core(agent, states, actions, returns, next_states, nonterminals, debug=debug, demo=demo)
         ctx.n_params = len(params)
         return loss
 
@@ -225,4 +237,4 @@ class _Loss(torch.autograd.Function):
     def backward(ctx, grad_loss):
         ctx.bw(grad_loss)
         ctx.bw = None
-        return (None,) * (7 + ctx.n_params)
+        return (None,) * (8 + ctx.n_params)

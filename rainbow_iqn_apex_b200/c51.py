@@ -66,14 +66,17 @@ def hidden_z(net, x, keep=None, col_cache=None, feat=None):
     return zv, za
 
 
-def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True):
+def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True, demo=None):
     """agent.py:77-141.  Returns the loss (B,) and its backward(gscale, gscale_mul=1.0), which accumulates into the online
     network's gradient arena the gradient of sum_b gscale[b] * gscale_mul * loss[b]; None without ``keep_graph``.
 
     The reference runs online(states) first (:82-83), then the two no-grad passes over next_states (:95-104), each after
     its own reset_noise.  The passes are independent, so they are evaluated here as 2, 3, 1 -- every pass still with its own
     noise sample (injected noises keep their reference slot) -- which leaves the gradient pass's weights and epsilons LIVE
-    when the backward runs: no 50 MB of weight / epsilon snapshots per step."""
+    when the backward runs: no 50 MB of weight / epsilon snapshots per step.  ``demo`` must be None: DQfD's margin loss
+    is not defined on the categorical head."""
+    if demo is not None:
+        raise ValueError("the C51 and HL-Gauss losses take no demonstration mask: DQfD applies to IQN and QR-DQN")
     (states, actions, returns, next_states, nonterminals), inj = _loss_inputs(
         agent, states, actions, returns, next_states, nonterminals)
     on, tg = agent.online_net, agent.target_net

@@ -20,7 +20,9 @@ loss (_fqf_core; its gradient is part of loss_core's backward).  num_quantile_sa
 read under FQF.
 
 CQL (Agent.cql, cql.py) adds alpha times the log-sum-exp gap of the online pass to the plain IQN loss; its backward runs
-the head's dense backward on the gradient riqn_cql_dense_grad forms.
+the head's dense backward on the gradient riqn_cql_dense_grad forms.  DQfD (Agent.dqfd, dqfd.py) adds lambda times the
+large-margin loss on the rows a ``demo`` mask flags, and its backward runs the same dense backward on the gradient
+riqn_dqfd_dense_grad forms; without a mask the step is the plain IQN step.
 """
 import ctypes
 import math
@@ -28,7 +30,7 @@ import numbers
 
 import torch
 
-from . import cql
+from . import cql, dqfd
 from ._lib import call, ptr
 
 MUNCHAUSEN_DEFAULTS = {"munchausen_alpha": 0.9, "munchausen_tau": 0.03, "munchausen_l0": -1.0}   # the paper's
@@ -132,12 +134,14 @@ def _loss_inputs(agent, states, actions, returns, next_states, nonterminals):
              frames(next_states), nonterminals.to(dev, torch.float32).contiguous()), inj or {})
 
 
-def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True):
+def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True, demo=None):
     """Forward passes + fused loss kernel.  Returns the loss (B,) and its backward(gscale, gscale_mul=1.0), which
     accumulates the gradient of sum_b gscale[b] * gscale_mul * loss[b] into the online network's gradient arena and, under
-    FQF, the fraction loss's into agent.fraction_net's; None without ``keep_graph``."""
+    FQF, the fraction loss's into agent.fraction_net's; None without ``keep_graph``.  ``demo``: None, or the (B,) uint8 /
+    bool demonstration flags of a DQfD agent (dqfd.py)."""
     (states, actions, returns, next_states, nonterminals), inj = _loss_inputs(
         agent, states, actions, returns, next_states, nonterminals)
+    demo = dqfd.demo_flags(agent, demo, states.shape[0])
     noises = inj.get("noises", (None, None, None))   # a dict may carry only "shifts"
     taus = inj.get("taus", (None, None, None))       # FQF's hook has no fractions
     batch = (agent, states, actions, returns, next_states, nonterminals)
@@ -146,20 +150,24 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     elif getattr(agent, "fqf", None) is not None:
         loss, dtheta, keep = _fqf_core(*batch, noises, keep_graph, debug)
     else:
-        loss, dtheta, keep = _iqn_core(*batch, noises, taus, keep_graph, debug)
+        loss, dtheta, keep = _iqn_core(*batch, noises, taus, keep_graph, debug, demo)
     if keep is None:
         return loss, None
 
     def backward(gscale, gscale_mul=1.0):
         gscale = gscale.contiguous().float()
-        pi = keep.get("cql_pi")
-        if pi is None:
-            agent.online_net.backward_iqn(keep, dtheta, gscale, actions, gscale_mul)
-        else:                 # CQL: the gap's gradient is dense over actions
+        pi, a_hat = keep.get("cql_pi"), keep.get("dqfd_a_hat")
+        B = actions.shape[0]
+        if pi is not None:    # CQL: the gap's gradient is dense over actions
             agent.online_net.check_live(keep)
-            B = actions.shape[0]
             G = cql.dense_grad(agent, B, dtheta.shape[0] // B, dtheta, pi, actions, gscale, gscale_mul)
             agent.online_net.backward_iqn_dense(keep, G)
+        elif a_hat is not None:   # DQfD: the margin's gradient reaches a_hat as well as a_E
+            agent.online_net.check_live(keep)
+            G = dqfd.dense_grad(agent, B, dtheta.shape[0] // B, dtheta, a_hat, actions, demo, gscale, gscale_mul)
+            agent.online_net.backward_iqn_dense(keep, G)
+        else:
+            agent.online_net.backward_iqn(keep, dtheta, gscale, actions, gscale_mul)
         fk = keep.get("fqf")
         if fk is not None:   # the fraction loss's surrogate of transition b is weighted like its quantile loss
             dlogits, floss = agent.fraction_net.backward(fk["fr"], fk["q_hat"], fk["q_bnd"], actions, gscale, gscale_mul,
@@ -170,7 +178,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     return loss, backward
 
 
-def _iqn_core(agent, states, actions, returns, next_states, nonterminals, noises, taus, keep_graph, debug):
+def _iqn_core(agent, states, actions, returns, next_states, nonterminals, noises, taus, keep_graph, debug, demo=None):
     """loss_core of plain IQN: (loss (B,), dtheta (N*B,), keep-dict for the backward or None)."""
     on, tg = agent.online_net, agent.target_net
     B = states.shape[0]
@@ -197,7 +205,15 @@ def _iqn_core(agent, states, actions, returns, next_states, nonterminals, noises
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, Np, device=dev)
-    if getattr(agent, "cql", None) is None:
+    if demo is not None:                                                            # DQfD (dqfd.py)
+        margin = torch.empty(B, device=dev) if debug is not None else None
+        td, a_hat = dqfd.dqfd_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, demo, loss,
+                                   dtheta, theta_out, target_out, margin)
+        if keep is not None:
+            keep["dqfd_a_hat"] = a_hat
+        if debug is not None:
+            debug.update(td_loss=td, margin=margin, a_hat=a_hat, demo=demo)
+    elif getattr(agent, "cql", None) is None:
         _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
                        target_out)                                                  # :262-357
     else:                                                                           # CQL (cql.py)

@@ -913,6 +913,86 @@ __global__ void cql_dense_grad_kernel(int B, int N, int A, const float* __restri
 }
 
 // ------------------------------------------------------------------------------------------------
+// DQfD (Hester et al. 2018): iqn_loss_kernel's loss plus lambda times the large-margin imitation loss on the rows flagged
+// as demonstrations.  With a_E = act[b]:
+//   Q_a    = fl(S_a / N),  S_a = fp32 sum over i ascending of q_on[i*B+b, a]           (argmax_mean_kernel's mean)
+//   v_a    = Q_a (a = a_E),  fl(Q_a + l) otherwise;   a_hat = first a ascending with v_a = M,  M = max_a v_a
+//   J[b]   = fl(M - Q_{a_E}) >= 0;   loss[b] = fl(td[b] + fl(lambda * J[b])) if demo[b] != 0, else td[b]
+// td_loss, dtheta, theta_out and target_out are iqn_loss_kernel's.  Warp 0 forms J, lane a owning Q_a; every lane walks
+// the same a-ascending maximum over shuffles.  J's gradient is formed at backward time (dqfd_dense_grad_kernel).
+// ------------------------------------------------------------------------------------------------
+template <bool RESCALE>
+__global__ void dqfd_loss_kernel(int B, int N, int Np, int A, const float* __restrict__ q_on,
+                                 const float* __restrict__ q_tgt, const float* __restrict__ tau,
+                                 const int64_t* __restrict__ actions, const int64_t* __restrict__ a_star,
+                                 const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                                 const unsigned char* __restrict__ demo, float gamma_n, float kappa, float margin,
+                                 float lambda, float* __restrict__ loss, float* __restrict__ td_loss,
+                                 float* __restrict__ dtheta, float* __restrict__ margin_out, int64_t* __restrict__ a_hat,
+                                 float* __restrict__ theta_out, float* __restrict__ target_out, float eps) {
+  extern __shared__ float sT[];  // Np targets + 32 reduction slots
+  float* red = sT + Np;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int as = (int)a_star[b], ac = (int)actions[b];
+  stage_double_dqn_targets<RESCALE>(B, Np, A, b, as, q_tgt, returns, nonterminals, gamma_n, eps, sT, target_out);
+  float J = 0.f;
+  int ah = 0;
+  if (tid < 32) {
+    float qa = -INFINITY, va = -INFINITY;
+    if (tid < A) {
+      float s = 0.f;
+      const float* col = q_on + (long)b * A + tid;
+#pragma unroll 8
+      for (int i = 0; i < N; ++i) s = __fadd_rn(s, col[(long)i * B * A]);
+      qa = __fdiv_rn(s, (float)N);
+      va = tid == ac ? qa : __fadd_rn(qa, margin);
+    }
+    float M = __shfl_sync(0xffffffffu, va, 0);
+    for (int a = 1; a < A; ++a) {
+      const float v = __shfl_sync(0xffffffffu, va, a);
+      if (v > M) { M = v; ah = a; }
+    }
+    J = __fsub_rn(M, __shfl_sync(0xffffffffu, qa, ac));
+    if (tid == 0) {
+      a_hat[b] = ah;
+      if (margin_out) margin_out[b] = J;
+    }
+  }
+  __syncthreads();
+  quantile_huber_loss(B, N, Np, A, b, ac, q_on, tau, kappa, sT, red, td_loss, dtheta, theta_out);
+  if (tid == 0) {                                   // thread 0 wrote td_loss[b]
+    const float td = td_loss[b];
+    loss[b] = demo && demo[b] ? __fadd_rn(td, __fmul_rn(lambda, J)) : td;
+  }
+}
+
+// The dense upstream gradient of sum_b w_b loss[b] at the DQfD loss, one thread per element of G (N*B, A), zero in every
+// column not named:  w_b = fl(gscale[b] * gmul),  c = fl(lambda / N)
+//   demo[b] == 0 or a_hat[b] == a_E:  G[i*B+b, a_E] = fl(w_b * dtheta[i*B+b])
+//   otherwise:                        G[i*B+b, a_hat] = fl(w_b * c),  G[i*B+b, a_E] = fl(w_b * fl(dtheta[i*B+b] - c))
+__global__ void dqfd_dense_grad_kernel(int B, int N, int A, const float* __restrict__ dtheta,
+                                       const int64_t* __restrict__ a_hat, const int64_t* __restrict__ actions,
+                                       const unsigned char* __restrict__ demo, const float* __restrict__ gscale,
+                                       float gmul, float lambda, float* __restrict__ G) {
+  const long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long r = e / A;
+  if (r >= (long)N * B) return;
+  const int a = (int)(e - r * A), b = (int)(r % B);
+  const int ae = (int)actions[b];
+  const int ah = demo && demo[b] ? (int)a_hat[b] : ae;
+  const float w = __fmul_rn(gscale[b], gmul);
+  float g = 0.f;
+  if (ah == ae) {
+    if (a == ae) g = __fmul_rn(w, dtheta[r]);
+  } else {
+    const float c = __fdiv_rn(lambda, (float)N);
+    if (a == ah) g = __fmul_rn(w, c);
+    else if (a == ae) g = __fmul_rn(w, __fsub_rn(dtheta[r], c));
+  }
+  G[e] = g;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Munchausen-IQN loss (Vieillard, Pietquin & Geist 2020), forward + dloss/dtheta.  q_tgt is ONE target-network pass over
 // the stacked frames [next_states; states]: row j*2B + b is s_{t+n}, row j*2B + B + b is s_t of transition b.
 //   qbar'(a) = mean_j q_tgt[j*2B+b, a] ,  qbar(a) = mean_j q_tgt[j*2B+B+b, a]        (j ascending)
@@ -1852,6 +1932,65 @@ RIQN_API int riqn_cql_dense_grad(int batch, int n, int action_space, const float
   const long total = (long)n * batch * action_space;
   cql_dense_grad_kernel<<<riqn_cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
       batch, n, action_space, dtheta, pi, (const int64_t*)actions, gscale, gscale_mul, alpha, grad_q);
+  return (int)cudaGetLastError();
+}
+
+template <bool RESCALE>
+static int launch_dqfd_loss(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                            const float* q_target, const float* tau, const long long* actions, const long long* a_star,
+                            const float* returns, const float* nonterminals, const unsigned char* demo, float gamma_n,
+                            float kappa, float margin, float lambda, float eps, float* loss, float* td_loss,
+                            float* dtheta, float* margin_out, long long* a_hat, float* theta_out, float* target_out,
+                            void* stream) {
+  if (!huber_loss_args_ok(batch, n_tau, n_tau_prime, action_space, kappa, 0) || !(margin > 0.f) || !isfinite(margin) ||
+      !(lambda > 0.f) || !isfinite(lambda) || !loss || !td_loss || !a_hat || !dtheta)
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  int threads = ((n_tau > n_tau_prime ? n_tau : n_tau_prime) + 31) / 32 * 32;
+  if (threads > 1024) threads = 1024;
+  if (threads < 32) threads = 32;
+  const size_t smem = sizeof(float) * (n_tau_prime + 32);
+  dqfd_loss_kernel<RESCALE><<<batch, threads, smem, (cudaStream_t)stream>>>(
+      batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, (const int64_t*)actions, (const int64_t*)a_star,
+      returns, nonterminals, demo, gamma_n, kappa, margin, lambda, loss, td_loss, dtheta, margin_out, (int64_t*)a_hat,
+      theta_out, target_out, eps);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_dqfd_loss_fwd_bwd(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                                    const float* q_target, const float* tau, const long long* actions,
+                                    const long long* a_star, const float* returns, const float* nonterminals,
+                                    const unsigned char* demo, float gamma_n, float kappa, float margin, float lambda,
+                                    float* loss, float* td_loss, float* dtheta, float* margin_out, long long* a_hat,
+                                    float* theta_out, float* target_out, void* stream) {
+  return launch_dqfd_loss<false>(batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, actions, a_star,
+                                 returns, nonterminals, demo, gamma_n, kappa, margin, lambda, 0.f, loss, td_loss, dtheta,
+                                 margin_out, a_hat, theta_out, target_out, stream);
+}
+
+RIQN_API int riqn_dqfd_loss_fwd_bwd_h(int batch, int n_tau, int n_tau_prime, int action_space, const float* q_online,
+                                      const float* q_target, const float* tau, const long long* actions,
+                                      const long long* a_star, const float* returns, const float* nonterminals,
+                                      const unsigned char* demo, float gamma_n, float kappa, float margin, float lambda,
+                                      float eps, float* loss, float* td_loss, float* dtheta, float* margin_out,
+                                      long long* a_hat, float* theta_out, float* target_out, void* stream) {
+  if (!vr_eps_ok(eps)) return (int)cudaErrorInvalidValue;
+  return launch_dqfd_loss<true>(batch, n_tau, n_tau_prime, action_space, q_online, q_target, tau, actions, a_star,
+                                returns, nonterminals, demo, gamma_n, kappa, margin, lambda, eps, loss, td_loss, dtheta,
+                                margin_out, a_hat, theta_out, target_out, stream);
+}
+
+RIQN_API int riqn_dqfd_dense_grad(int batch, int n, int action_space, const float* dtheta, const long long* a_hat,
+                                  const long long* actions, const unsigned char* demo, const float* gscale,
+                                  float gscale_mul, float lambda, float* grad_q, void* stream) {
+  if (batch < 1 || n < 1 || action_space < 1 || action_space > 32 || !(lambda > 0.f) || !isfinite(lambda) || !dtheta ||
+      !a_hat || !actions || !gscale || !grad_q)
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  const long total = (long)n * batch * action_space;
+  dqfd_dense_grad_kernel<<<riqn_cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      batch, n, action_space, dtheta, (const int64_t*)a_hat, (const int64_t*)actions, demo, gscale, gscale_mul, lambda,
+      grad_q);
   return (int)cudaGetLastError();
 }
 

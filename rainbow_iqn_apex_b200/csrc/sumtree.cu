@@ -144,15 +144,20 @@ __global__ void is_weights_kernel(int n, const double* __restrict__ tree, const 
 // ------------------------------------------------------------------------------------------------
 // priorities = np.power(loss_f32, float32(omega))  (redis_memory.py:560) evaluated as a correctly
 // rounded float: double pow then one rounding.  exponent < 0 sentinel => priorities passed through.
+// DEMO: DQfD's demonstration bonus, p = fl(p + bonus) on the leaves idx >= demo_leaf, after the power.
+template <bool DEMO>
 __global__ void update_prepare_kernel(int n, const double* __restrict__ tree, const int64_t* __restrict__ idx,
                                       const float* __restrict__ loss, float exponent, int apply_pow,
                                       float* __restrict__ new_pri, double* __restrict__ diff,
-                                      double* __restrict__ max_priority) {
+                                      double* __restrict__ max_priority, int64_t demo_leaf, float bonus) {
   __shared__ float red[32];
   float mx = -INFINITY;
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
     float p = loss[j];
     if (apply_pow) p = (float)pow((double)p, (double)exponent);
+    if constexpr (DEMO) {
+      if (idx[j] >= demo_leaf) p = __fadd_rn(p, bonus);
+    }
     new_pri[j] = p;
     diff[j] = (double)p - tree[idx[j]];
     mx = fmaxf(mx, p);
@@ -465,15 +470,16 @@ RIQN_API int riqn_sumtree_is_weights(int n, const double* tree, const double* pr
   return (int)cudaGetLastError();
 }
 
-RIQN_API int riqn_sumtree_update(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
+template <bool DEMO>
+static int launch_sumtree_update(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
                                  float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
-                                 double* max_priority, void* stream) {
+                                 double* max_priority, long long demo_leaf, float bonus, void* stream) {
   riqn::note_launches(2);
   if (n <= 0) return 0;
   if (n > 4096) return (int)cudaErrorInvalidValue;  // shared-memory bound of the propagate kernel
   cudaStream_t s = (cudaStream_t)stream;
-  update_prepare_kernel<<<1, 1024, 0, s>>>(n, tree, (const int64_t*)tree_idx, loss, priority_exponent, apply_pow,
-                                           new_priorities, diff_scratch, max_priority);
+  update_prepare_kernel<DEMO><<<1, 1024, 0, s>>>(n, tree, (const int64_t*)tree_idx, loss, priority_exponent, apply_pow,
+                                                 new_priorities, diff_scratch, max_priority, (int64_t)demo_leaf, bonus);
   RIQN_LAUNCH_CHECK();
   int max_depth = 0;  // depth of the deepest leaf (index 2C-2)
   for (long i = 2 * capacity - 2; i > 0; i = (i - 1) / 2) ++max_depth;
@@ -488,6 +494,21 @@ RIQN_API int riqn_sumtree_update(int n, long capacity, double* tree, const long 
   update_propagate_kernel<<<dim3(max_depth + 1, slices), 256, smem, s>>>(n, max_depth, tree, (const int64_t*)tree_idx,
                                                                         diff_scratch);
   return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_sumtree_update(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
+                                 float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
+                                 double* max_priority, void* stream) {
+  return launch_sumtree_update<false>(n, capacity, tree, tree_idx, loss, priority_exponent, apply_pow, new_priorities,
+                                      diff_scratch, max_priority, 0, 0.f, stream);
+}
+
+RIQN_API int riqn_sumtree_update_demo(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
+                                      float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
+                                      double* max_priority, long long demo_leaf, float bonus, void* stream) {
+  if (!(bonus >= 0.f) || !isfinite(bonus) || demo_leaf < 0) return (int)cudaErrorInvalidValue;
+  return launch_sumtree_update<true>(n, capacity, tree, tree_idx, loss, priority_exponent, apply_pow, new_priorities,
+                                     diff_scratch, max_priority, demo_leaf, bonus, stream);
 }
 
 RIQN_API int riqn_replay_append(int n, int actor_capacity, int id_actor, int start, const unsigned char* frames,

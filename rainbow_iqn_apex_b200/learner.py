@@ -46,12 +46,19 @@ class Learner(Agent):
     def learn(self, mem_redis, mp_queue):
         sample = mem_redis.get_sample_from_mp_queue(mp_queue)
         idxs, states, actions, returns, next_states, nonterminals, weights = sample
-        loss = self.learn_on_batch(states, actions, returns, next_states, nonterminals, weights)
+        loss = self.learn_on_batch(states, actions, returns, next_states, nonterminals, weights,
+                                   demo=self._demo_mask(mem_redis, idxs))
         return idxs, loss
 
-    def learn_on_batch(self, states, actions, returns, next_states, nonterminals, weights):
-        """learner.py:18-24 on an already assembled minibatch.  Returns the per-transition loss (B,)."""
-        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights)
+    def _demo_mask(self, mem, idxs):
+        """Under DQfD, the demonstration flags of the sampled tree indices ``idxs`` (ReplayMemory.demo_mask: None when the
+        memory holds no demonstrations); None otherwise."""
+        return mem.demo_mask(idxs) if self.dqfd is not None else None
+
+    def learn_on_batch(self, states, actions, returns, next_states, nonterminals, weights, demo=None):
+        """learner.py:18-24 on an already assembled minibatch.  Returns the per-transition loss (B,).  ``demo``: the
+        DQfD demonstration flags (B,), or None."""
+        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights, demo=demo)
         self.apply_gradients()
         return loss
 
@@ -106,15 +113,15 @@ class Learner(Agent):
         capacity, beta = (1.0, 0.0) if mem is None else (mem.transitions.get_current_capacity(), mem.priority_weight)
         self._dyn.write(nss, sbc, capacity, beta, *more)
 
-    def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None):
+    def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None, demo=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arenas.
         ``debug``: dict that receives the loss core's intermediates (self.loss_core), and with random_shift the shifts and
-        the shifted frames (_shift_frames)."""
+        the shifted frames (_shift_frames).  ``demo``: the DQfD demonstration flags (B,) uint8 / bool, or None."""
         on = self.online_net
         weights = weights.to(on._flat.device, torch.float32)
         if self.random_shift is not None:
             states, next_states = self._shift_frames(states, next_states, debug)
-        loss, bw = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug)
+        loss, bw = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, demo=demo)
         for net in self._trained_nets():                                        # learner.py:22
             net.zero_grad()
         # data parallel: DQN.backward_iqn starts the all-reduce of the NoisyLinear gradients as soon as they are final
@@ -192,7 +199,8 @@ class Learner(Agent):
         """sample -> three forwards -> loss -> backward (gradients in the arena)."""
         self._reset_step_streams(mem)
         idxs, states, actions, returns, next_states, nonterminals, weights = mem.get_sample_from_mp_queue(None)
-        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights)
+        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights,
+                                      demo=self._demo_mask(mem, idxs))
         return idxs, loss
 
     def _step_post(self, mem, idxs, loss, allreduce=True):
@@ -279,7 +287,7 @@ class Learner(Agent):
 
         def pre():
             self._reset_step_streams()
-            return self.compute_gradients(*inputs[1:])
+            return self.compute_gradients(*inputs[1:], demo=self._demo_mask(mem, inputs[0]))
 
         self._capture("batch", pre, lambda loss, allreduce: self._step_post(mem, inputs[0], loss, allreduce), 2, mem,
                       inputs)
@@ -289,7 +297,10 @@ class Learner(Agent):
         """CUDA graph of learn_on_batch alone (no replay on this rank): the Ape-X learner, whose minibatch is gathered from
         the actor GPUs' shards (apex.ApexTopology.sample).  ``example`` = (states, actions, returns, next_states,
         nonterminals, weights) device tensors defining the shapes; learn_on_graph(batch) copies a batch into the static
-        inputs and replays.  Returns self."""
+        inputs and replays.  Returns self.  Not under DQfD: a gathered batch carries no demonstration flags."""
+        if self.dqfd is not None:
+            raise RuntimeError("the learn graph takes batches gathered from the actor shards, which carry no demonstration "
+                               "flags: a DQfD learner steps from its own replay (enable_cuda_graph / enable_batch_graph)")
         inputs = tuple(t.contiguous().clone() for t in example)
 
         def pre():

@@ -14,13 +14,14 @@ The learner step runs the IQN path's three passes, each after its own noise rese
 target(s') (both trunks in one stacked trunk_pair), online(s) with the backward's operands; then the quantile-Huber loss
 against R + gamma^n nt q_tgt[a*] at the N x N fraction pairs, and riqn_qr_head_bwd below it.  MMDQN (agent.mmd, mmd.py)
 runs the same step with the MMD loss kernel in place of the quantile-Huber one; CQL (agent.cql, cql.py) adds alpha times
-the log-sum-exp gap to the quantile-Huber loss and takes riqn_qr_head_bwd_dense.
+the log-sum-exp gap to the quantile-Huber loss and takes riqn_qr_head_bwd_dense, and so does DQfD (agent.dqfd, dqfd.py)
+with lambda times the large-margin loss on the rows a ``demo`` mask flags.
 """
 import numbers
 
 import torch
 
-from . import c51, cql, mmd
+from . import c51, cql, dqfd, mmd
 from ._lib import call, ptr
 from .compute_loss_iqn import _loss_inputs, _quantile_loss, greedy_actions
 
@@ -91,13 +92,14 @@ def backward_dense(on, keep, grad_q, gv):
     c51._backward_below_head(on, keep, dzv, dza, gv)
 
 
-def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True):
+def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=None, keep_graph=True, demo=None):
     """The QR-DQN loss (B,) and its backward(gscale, gscale_mul=1.0), which accumulates into the online network's
     gradient arena the gradient of sum_b gscale[b] * gscale_mul * loss[b]; None without ``keep_graph``.  Injection hook:
     ``agent._inject = {"noises": (n0, n1, n2)}`` (or a list of them, one per call), the noises of the three passes in
-    their order."""
+    their order.  ``demo``: None, or the (B,) uint8 / bool demonstration flags of a DQfD agent (dqfd.py)."""
     (states, actions, returns, next_states, nonterminals), inj = _loss_inputs(
         agent, states, actions, returns, next_states, nonterminals)
+    demo = dqfd.demo_flags(agent, demo, states.shape[0])
     on, tg = agent.online_net, agent.target_net
     B, A, N = states.shape[0], agent.action_space, agent.num_tau_samples
     dev = states.device
@@ -120,8 +122,14 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
     if debug is not None:
         theta_out = torch.empty(B, N, device=dev)
         target_out = torch.empty(B, N, device=dev)
-    pi = None
-    if getattr(agent, "cql", None) is not None:       # CQL: the same loss plus alpha * gap (cql.py)
+    pi = a_hat = None
+    if demo is not None:                               # DQfD: the same loss plus lambda * J on the flagged rows
+        margin = torch.empty(B, device=dev) if debug is not None else None
+        td, a_hat = dqfd.dqfd_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, demo,
+                                   loss, dtheta, theta_out, target_out, margin)
+        if debug is not None:
+            debug.update(td_loss=td, margin=margin, a_hat=a_hat, demo=demo)
+    elif getattr(agent, "cql", None) is not None:       # CQL: the same loss plus alpha * gap (cql.py)
         gap = torch.empty(B, device=dev) if debug is not None else None
         td, pi = cql.cql_loss(agent, B, N, N, q_on, q_tgt, tau_hat, actions, a_star, returns, nonterminals, loss, dtheta,
                               theta_out, target_out, gap)
@@ -146,6 +154,10 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
         gscale = gscale.contiguous().float()
         if pi is not None:                             # CQL: the gap's gradient is dense over actions
             backward_dense(on, keep, cql.dense_grad(agent, B, N, dtheta, pi, actions, gscale, gscale_mul), on.grad_view)
+            return
+        if a_hat is not None:                          # DQfD: the margin's gradient reaches a_hat as well as a_E
+            G = dqfd.dense_grad(agent, B, N, dtheta, a_hat, actions, demo, gscale, gscale_mul)
+            backward_dense(on, keep, G, on.grad_view)
             return
         dzv = torch.empty(B, N, device=dev)
         dza = torch.empty(B, A * N, device=dev)

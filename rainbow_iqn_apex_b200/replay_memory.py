@@ -13,7 +13,7 @@ Class / method names follow the reference so ``launch_learner``-style loops read
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, dqfd
 from ._lib import call, ptr
 
 FRAME = 84 * 84
@@ -194,6 +194,15 @@ class ReplayMemory:
         self._gamma_pow = torch.tensor([self.discount ** k for k in range(self.n)], dtype=torch.float64,
                                        device=self.device)
         self.last_nonpositive = None
+        # DQfD demonstrations: optional args fields (absent from the reference's namespace: none).  The last D segments,
+        # data indices >= (nb_actor - D) * actor_capacity, hold them; the sampler's valid-index shift never leaves a
+        # segment, so a sampled row is a demonstration exactly when its tree index is >= demo_leaf.  update_priorities
+        # adds demo_priority_bonus (DQfD's eps_d) to their new priorities
+        self.demo_segments, self.demo_priority_bonus = dqfd.check_demo_replay(
+            *(getattr(args, f, v) for f, v in dqfd.DEMO_DEFAULTS.items()), args.nb_actor)
+        self.demo_leaf = None
+        if self.demo_segments > 0:
+            self.demo_leaf = (args.nb_actor - self.demo_segments) * args.actor_capacity + self.capacity - 1
 
     def sample_indices(self, batch_size, samples=None):
         """find_multiple_values + importance weights (redis_memory.py:424-475), including the reference's resample loop:
@@ -264,11 +273,31 @@ class ReplayMemory:
         weights = torch.as_tensor(weights).to(self.device, torch.float32)
         return tree_idxs, states, actions, returns, next_states, nonterminals, weights
 
+    def demo_mask(self, tree_idx):
+        """The (B,) uint8 demonstration flags of the sampled tree indices: 1 where tree_idx >= demo_leaf.  None when the
+        memory holds no demonstration segments."""
+        if self.demo_leaf is None:
+            return None
+        return torch.ge(torch.as_tensor(tree_idx).to(self.device), self.demo_leaf).view(torch.uint8)
+
     def update_priorities(self, idxs, priorities):
-        """redis_memory.py:557-573: priorities = loss ** priority_exponent, then the diff-propagating update."""
+        """redis_memory.py:557-573: priorities = loss ** priority_exponent, then the diff-propagating update; with
+        demonstration segments and a bonus eps_d > 0, the demonstrations' priorities are fl32(loss ** omega + eps_d)
+        (riqn_sumtree_update_demo)."""
         idxs = torch.as_tensor(idxs).to(self.device, torch.int64).contiguous()
         priorities = torch.as_tensor(priorities).detach().to(self.device, torch.float32).contiguous()
-        return self.transitions.update_multiple_value(idxs, priorities, apply_pow=True, exponent=self.priority_exponent)
+        tr = self.transitions
+        if self.demo_leaf is None or self.demo_priority_bonus == 0.0:
+            return tr.update_multiple_value(idxs, priorities, apply_pow=True, exponent=self.priority_exponent)
+        n = idxs.numel()
+        if n > 4096:
+            raise ValueError("update_priorities takes at most 4096 entries per call (one reference batch)")
+        new_pri = torch.empty(n, dtype=torch.float32, device=self.device)
+        diff = torch.empty(n, dtype=torch.float64, device=self.device)
+        call("riqn_sumtree_update_demo", n, tr.full_capacity, ptr(tr.tree), ptr(idxs), ptr(priorities),
+             float(self.priority_exponent), 1, ptr(new_pri), ptr(diff), ptr(tr.max_priority), self.demo_leaf,
+             self.demo_priority_bonus)
+        return new_pri
 
 
 # reference spellings
