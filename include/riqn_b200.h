@@ -477,9 +477,15 @@ int riqn_fqf_fraction_bwd(int batch, int n, int action_space, const float* logit
                           const float* q_bnd, const long long* actions, const float* gscale, float gscale_mul,
                           float entropy_coef, float* dlogits, float* loss_out, void* stream);
 /* grad_w (n, feat_dim) += dlogits^T feat, grad_b (n) += sum_b dlogits[b, :]: each element is one fp32 fmaf chain over b
- * ascending, then added once.  No atomics. */
+ * ascending, then added once.  No atomics.  The fraction layer's form of riqn_linear_wgrad (same kernel), with its
+ * 2 <= n <= 256. */
 int riqn_fqf_fraction_wgrad(int batch, int n, int feat_dim, const float* dlogits, const float* feat, float* grad_w,
                             float* grad_b, void* stream);
+/* Generic linear-layer weight gradient: grad_w (n, feat_dim) += dy^T x, grad_b (n) += sum_b dy[b, :], dy (batch, n) and
+ * x (batch, feat_dim) row-major, rounded exactly as riqn_fqf_fraction_wgrad.  Any n >= 1 (CURL's projection: 512 and 128);
+ * batch >= 1, feat_dim >= 1 and non-NULL pointers, else cudaErrorInvalidValue with nothing written. */
+int riqn_linear_wgrad(int batch, int n, int feat_dim, const float* dy, const float* x, float* grad_w, float* grad_b,
+                      void* stream);
 /* a_star[b] = argmax_a sum_k w[k*batch+b] * q[k*batch+b, a]: fp32 fmaf chain over k ascending, the first maximal index
  * winning (as riqn_argmax_mean).  FQF's Q(s, a) = sum_i dtau_i F(s, tau_hat_i, a). */
 int riqn_argmax_weighted(int batch, int n, int action_space, const float* q, const float* w, long long* a_star,
@@ -708,6 +714,44 @@ int riqn_gemm_bf16_tc(int M, int N, int K, const void* a_hi, const void* a_lo, c
  * N % 32 == 0): write the result as bf16 (M, N) there INSTEAD of fp32 into c. */
 int riqn_gemm_bf16_tc_mn(int M, int N, int K, const void* a, const void* b_kn, int a_is_km, float* c, long ldc, int epilogue,
                          float* out2, const float* eps, float alpha, int split_k, void* c_bf16, int fmt, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * CURL (Srinivas, Laskin & Abbeel, ICML 2020; no counterpart in the reference): contrastive auxiliary loss on the trunk
+ * ---------------------------------------------------------------------------------------------- */
+/* Bilinear InfoNCE of anchors z_a (batch, dim) against keys z_k (batch, dim) with W (dim, dim), all row-major fp32, and its
+ * gradient with respect to z_a and W; the positive of anchor i is key i.  With s = fl(coef / batch):
+ *   v_i = W^T z_a,i          v_i[q] = sum_p z_a[i,p] W[p,q]                   (fmaf chain, p ascending)
+ *   l_ij = v_i . z_k,j                                                         (fmaf chain, q ascending)
+ *   m_i = max_j l_ij ;  S_i = sum_j expf(l_ij - m_i)       (lane chains over j = lane + 32k, then the warp_sum butterfly)
+ *   loss_rows[i] = fl(fl(m_i + logf(S_i)) - l_ii)                              (unscaled; the loss is s * sum_i)
+ *   dl_ij = fl(s * fl(fl(expf(l_ij - m_i) * fl(1 / S_i)) - [i == j]))
+ *   g_i[q] = sum_j dl_ij z_k[j,q]   (fmaf, j ascending) ;  dz_a[i,p] = sum_q W[p,q] g_i[q]   (fmaf, q ascending)
+ *   dw[p,q] += sum_i z_a[i,p] g_i[q]                                           (fmaf chain over i ascending, added once)
+ * logits_out (batch, batch) may be NULL.  Two launches (the row kernel, then the dW reduction), scratch from the stream's
+ * pool, no atomics.  dim must be 128 and 2 <= batch <= 4096, coef finite, the other pointers non-NULL; otherwise
+ * cudaErrorInvalidValue and nothing is written. */
+int riqn_curl_infonce_fwd_bwd(int batch, int dim, const float* z_a, const float* z_k, const float* w, float coef,
+                              float* loss_rows, float* dz_a, float* dw, float* logits_out, void* stream);
+/* Row LayerNorm without affine parameters, eps = 1e-5, width 128 or 512 (one warp per row, lane l holding the elements
+ * l + 32k; the sums are lane chains over k then the warp_sum butterfly), of the rows x, or of fl(x + bias[col]) when
+ * bias (width) is non-NULL (the bias of a product whose epilogue has none):
+ *   mean = fl(sum x / width) ;  d = fl(x - mean) ;  rstd = fl(1 / sqrtf(fl(sum d*d / width) + 1e-5)) ;  x_hat = fl(d * rstd)
+ *   y = x_hat, or max(x_hat, 0) when relu != 0.
+ * The backward takes the forward's INPUT x and recomputes x_hat bit for bit; with g = dy (relu: 0 where x_hat <= 0):
+ *   dx = fl(rstd * fl(fl(g - mean(g)) - fl(x_hat * mean(g * x_hat)))).
+ * rows >= 1 and non-NULL pointers, else cudaErrorInvalidValue with nothing written. */
+int riqn_layernorm_fwd(long rows, int width, const float* x, const float* bias, int relu, float* y, void* stream);
+int riqn_layernorm_bwd(long rows, int width, const float* x, const float* bias, const float* dy, int relu, float* dx,
+                       void* stream);
+/* out[c] += sum_r x[r, c] (rows, cols) row-major, in a fixed order (per-block partials added in block order; two
+ * launches, no atomics): the bias gradient of a product on the tensor cores.  rows, cols >= 1 and non-NULL pointers,
+ * else cudaErrorInvalidValue with nothing written. */
+int riqn_colsum_add(long rows, int cols, const float* x, float* out, void* stream);
+/* Momentum update xi[i] = fl(xi[i] + fl(tau * fl(theta[i] - xi[i]))), every operation rounded on its own (no fma).
+ * n >= 1, finite 0 < tau <= 1, non-NULL pointers, else cudaErrorInvalidValue with nothing written. */
+int riqn_ema_f32(long n, const float* theta, float* xi, float tau, void* stream);
+/* out[i] = fl(a[i] + b[i]) (out may alias a or b).  n >= 1 and non-NULL pointers, else cudaErrorInvalidValue. */
+int riqn_add_f32(long n, const float* a, const float* b, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Test hook: plain strided fp32 product C[m,n] = sum_k A[m*sAm + k*sAk] * B[n*sBn + k*sBk].

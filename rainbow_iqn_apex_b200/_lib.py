@@ -83,6 +83,13 @@ SIGNATURES = {
     "riqn_fqf_fractions": [C.c_int, C.c_int] + [_P] * 6,
     "riqn_fqf_fraction_bwd": [C.c_int] * 3 + [_P] * 6 + [C.c_float] * 2 + [_P] * 3,
     "riqn_fqf_fraction_wgrad": [C.c_int] * 3 + [_P] * 5,
+    "riqn_linear_wgrad": [C.c_int] * 3 + [_P] * 5,
+    "riqn_curl_infonce_fwd_bwd": [C.c_int, C.c_int, _P, _P, _P, C.c_float] + [_P] * 5,
+    "riqn_layernorm_fwd": [C.c_long, C.c_int, _P, _P, C.c_int, _P, _P],
+    "riqn_layernorm_bwd": [C.c_long, C.c_int, _P, _P, _P, C.c_int, _P, _P],
+    "riqn_colsum_add": [C.c_long, C.c_int, _P, _P, _P],
+    "riqn_ema_f32": [C.c_long, _P, _P, C.c_float, _P],
+    "riqn_add_f32": [C.c_long, _P, _P, _P, _P],
     "riqn_argmax_weighted": [C.c_int] * 3 + [_P] * 4,
     "riqn_c51_head_fwd":[C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,

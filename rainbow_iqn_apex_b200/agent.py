@@ -10,17 +10,18 @@ qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-se
 ``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
 ``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51 head (hl_gauss.py), ``cql`` for the conservative
 regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's large-margin loss on demonstrations (dqfd.py),
-and ``random_shift`` for the
-learner's random-shift augmentation (augment.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+``random_shift`` for the
+learner's random-shift augmentation (augment.py), and ``curl`` / ``curl_net`` / ``curl_optimiser`` / ``momentum_net`` /
+``momentum_projection`` for CURL's contrastive loss on the trunk (curl.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
-optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF.
+optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF and CURL's three.
 """
 import os
 
 import torch
 
 from . import _lib
-from . import augment, c51, compute_loss_iqn, cql, dqfd, fqf, hl_gauss, mmd, qr
+from . import augment, c51, compute_loss_iqn, cql, curl, dqfd, fqf, hl_gauss, mmd, qr
 from .model import DQN, check_risk
 from .optim import Adam
 
@@ -140,6 +141,15 @@ class Agent:
         # off).  None, or the pad p of augment.check_random_shift; fixed for the agent's life, so that a captured step graph
         # stays valid.  Only Learner.compute_gradients shifts; acting and the actors' priorities see the stored frames
         self.random_shift = augment.check_random_shift(getattr(args, "random_shift", 0))
+        # CURL's contrastive auxiliary loss on the trunk: optional args fields (absent from the reference's namespace: off).
+        # None, or the float32 (lambda, tau) of curl.check_curl; its modules are built last, so that both DQNs (and the
+        # fraction proposal) initialise as a plain agent's from the same seed
+        self.curl = curl.check_curl(getattr(args, "curl", 0),
+                                    *(getattr(args, f, v) for f, v in curl.CURL_DEFAULTS.items()),
+                                    random_shift=self.random_shift, batch_size=self.batch_size)
+        self.curl_net = self.curl_optimiser = self.momentum_net = self.momentum_projection = None
+        if self.curl is not None:
+            curl.build(self, args, checkpoint)
         # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
         self.risk = None
         self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
@@ -189,7 +199,8 @@ class Agent:
     def compute_loss_actor_or_learner(self, states, actions, returns, next_states, nonterminals, debug=None, demo=None):
         """agent.py:72-147: the loss (B,) of self.loss_core, differentiable with respect to the online network (and,
         under FQF, the fraction proposal) when grad mode is on.  ``debug``: dict that receives the core's intermediates.
-        ``demo``: None, or the (B,) demonstration flags of a DQfD agent (dqfd.py)."""
+        ``demo``: None, or the (B,) demonstration flags of a DQfD agent (dqfd.py).  CURL's auxiliary loss is not part of
+        it: only Learner.compute_gradients adds that term."""
         if torch.is_grad_enabled():
             params = [p for p in self.online_net.parameters() if p.requires_grad]
             return _Loss.apply(self, states, actions, returns, next_states, nonterminals, debug, demo, *params)
@@ -199,8 +210,8 @@ class Agent:
 
     def save(self, path, T_actors, T_learner, name):
         """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
-        fraction_optimiser_state_dict, under value rescaling value_rescaling_eps, under QR-DQN qr_dqn_quantiles (N);
-        model_state_dict keeps the reference schema either way."""
+        fraction_optimiser_state_dict, under value rescaling value_rescaling_eps, under QR-DQN qr_dqn_quantiles (N), under CURL
+        curl_state_dict, curl_optimiser_state_dict and curl_momentum_state_dict; model_state_dict keeps the reference schema either way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
@@ -214,6 +225,10 @@ class Agent:
             ckpt["value_rescaling_eps"] = self.value_rescaling
         if self.qr_dqn is not None:
             ckpt["qr_dqn_quantiles"] = self.qr_dqn
+        if self.curl is not None:
+            ckpt["curl_state_dict"] = self.curl_net.state_dict()
+            ckpt["curl_optimiser_state_dict"] = self.curl_optimiser.state_dict()
+            ckpt["curl_momentum_state_dict"] = curl.momentum_state_dict(self)
         torch.save(ckpt, os.path.join(path, name))
 
     def train(self):

@@ -27,18 +27,21 @@ def check_random_shift(value):
     return int(value) if value else None
 
 
-def draw_shifts(net, n, pad):
+def draw_shifts(net, n, pad, key=SHIFT_SEED, advance=True):
     """n shifts (dy, dx) uniform on [-pad, pad]^2, an (n, 2) int32 device tensor, from ``net``'s Philox generator
     (riqn_fill_shifts).  The stream is rank-private (net._tau_stream_offset) and counts per step like the fraction draws'
     (a static index read with the device step state in graph mode, the eager half of the id space otherwise), under a key
-    of its own: a shift draw takes no stream the noise or fraction draws use."""
+    of its own: a shift draw takes no stream the noise or fraction draws use.  ``key`` (xor-ed into net._rng_seed) and
+    ``advance`` = False let a draw of another kind (CURL's positive view) take streams of its own without moving the
+    counters the learner's shifts of s_t and s_{t+n} read."""
     out = torch.empty(n, 2, dtype=torch.int32, device=net._flat.device)
     dyn = getattr(net, "_dyn", None)
     idx = net._shift_in_step if dyn is not None else net._shift_calls
     stream_id = net._tau_stream_offset + idx + (0 if dyn is not None else _EAGER_STREAMS)
-    call("riqn_fill_shifts", n, int(pad), net._rng_seed ^ SHIFT_SEED, stream_id, ptr(out), dyn.ptr() if dyn else None)
-    net._shift_calls += 1
-    net._shift_in_step += 1
+    call("riqn_fill_shifts", n, int(pad), net._rng_seed ^ key, stream_id, ptr(out), dyn.ptr() if dyn else None)
+    if advance:
+        net._shift_calls += 1
+        net._shift_in_step += 1
     return out
 
 

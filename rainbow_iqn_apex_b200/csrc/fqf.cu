@@ -227,6 +227,15 @@ RIQN_API int riqn_fqf_fraction_wgrad(int batch, int n, int feat_dim, const float
   return (int)cudaGetLastError();
 }
 
+RIQN_API int riqn_linear_wgrad(int batch, int n, int feat_dim, const float* dy, const float* x, float* grad_w,
+                               float* grad_b, void* stream) {
+  if (batch < 1 || n < 1 || feat_dim < 1 || !dy || !x || !grad_w || !grad_b) return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  dim3 grid(riqn_cdiv(feat_dim, WG_JT), riqn_cdiv(n, WG_KT));
+  fqf_wgrad_kernel<<<grid, WG_JT, 0, (cudaStream_t)stream>>>(batch, n, feat_dim, dy, x, grad_w, grad_b);
+  return (int)cudaGetLastError();
+}
+
 RIQN_API int riqn_argmax_weighted(int batch, int n, int action_space, const float* q, const float* w, long long* a_star,
                                   void* stream) {
   if (batch < 1 || !fqf_n_ok(n) || action_space < 1 || action_space > 32) return (int)cudaErrorInvalidValue;

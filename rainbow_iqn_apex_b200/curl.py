@@ -1,0 +1,309 @@
+"""CURL: Contrastive Unsupervised Representations for Reinforcement Learning (Srinivas, Laskin & Abbeel, ICML 2020), an
+auxiliary loss on the convolution trunk of every learner.
+
+Two augmentations of the same state should map to nearby features.  The anchor x_a is the randomly shifted s_t that the
+gradient pass already reads (Agent.random_shift); the positive x_k is a second, independent random shift of the same
+unshifted s_t, drawn under a Philox key of its own that moves none of the shift counters, so that the shifts of s_t and
+s_{t+n} stay those of a learner without CURL in every step, eager or replayed.  With f the conv trunk and this project's projection head
+
+  g(feat) = LN(W_c ReLU(LN(W_h feat + b_h)) + b_c)       (3136 -> 512 -> 128; LN: row LayerNorm without affine, eps 1e-5)
+
+  z_a = g_theta(f_theta(x_a)) ,  z_k = g_xi(f_xi(x_k))  (no gradient) ,  logits_ij = z_a,i^T W z_k,j   (B x B)
+  L_CURL = (1/B) sum_i [logsumexp_j logits_ij - logits_ii]
+
+and the step minimises (1/B) sum_b w_b L_RL,b + lambda L_CURL (the CURL term is not importance-weighted).  xi, the key
+encoder, is a momentum copy of the trunk and of the projection (not of W): after the Adam steps
+xi <- xi + tau (theta - xi), each operation rounded on its own (riqn_ema_f32).  Priorities and the returned loss stay the
+RL loss.  The projection sizes, the LayerNorms and the defaults lambda = 1, tau = 0.001 are this project's starting
+point, not tuned and not the paper's settings.
+
+The anchor needs no extra trunk pass: the learner arms DQN._trunk_addend for one backward, and DQN.backward_trunk hands
+it the gradient pass's kept features and the loss core's dfeat; it returns dfeat_RL + dfeat_CURL (riqn_add_f32), so no
+loss core changes.  CURL runs only in Learner.compute_gradients: not in acting, the actors, compute_priorities or the
+autograd path of Agent.compute_loss_actor_or_learner.
+
+Modules, all built after every existing one (so that both DQNs initialise as a plain agent's from the same seed):
+  agent.curl_net        CurlProjection: W_h, b_h, W_c, b_c and W in one flat arena, trained by agent.curl_optimiser
+                        (the arena Adam with the agent's lr and adam_eps)
+  agent.momentum_net    a DQN whose trunk alone ever runs (f_xi), and agent.momentum_projection, the untrained
+                        buffer arena of g_xi (the projection prefix of curl_net's arena layout)
+"""
+import ctypes
+import math
+import numbers
+import weakref
+
+import torch
+from torch import nn
+
+from . import augment
+from ._lib import call, ptr
+from .model import DQN, FEAT, _ALIGN
+
+CURL_DEFAULTS = {"curl_coef": 1.0, "curl_momentum": 0.001}   # this project's starting point, not tuned
+HIDDEN, DIM = 512, 128                                         # projection widths
+MAX_BATCH = 4096                                               # riqn_curl_infonce_fwd_bwd
+CURL_SHIFT_SEED = 0xC0A1                                       # the positive view's draw key (net._rng_seed ^ this)
+
+
+def check_curl(curl, coef=CURL_DEFAULTS["curl_coef"], momentum=CURL_DEFAULTS["curl_momentum"], random_shift=None,
+               batch_size=None):
+    """Validate a CURL configuration.  Returns None when ``curl`` is off (0 / False), else (lambda, tau) as the float32
+    values the kernels receive: lambda finite and > 0, tau finite with 0 < tau <= 1.  CURL contrasts two augmentations, so
+    it needs ``random_shift`` (the pad, not None), and in-batch negatives, so 2 <= ``batch_size`` <= 4096.  Raises
+    ValueError otherwise."""
+    if isinstance(curl, bool) or (isinstance(curl, numbers.Integral) and curl in (0, 1)):
+        if not curl:
+            return None
+    else:
+        raise ValueError(f"curl must be 0 or 1, got {curl!r}")
+    vals = []
+    for name, v, ok, need in (("curl_coef", coef, lambda x: x > 0.0, "> 0"),
+                              ("curl_momentum", momentum, lambda x: 0.0 < x <= 1.0, "in (0, 1]")):
+        if isinstance(v, bool) or not isinstance(v, numbers.Real):
+            raise ValueError(f"{name} must be a real number, got {v!r}")
+        f = ctypes.c_float(float(v)).value
+        if not (math.isfinite(f) and ok(f)):
+            raise ValueError(f"{name} must be finite and {need} as a float32, got {v!r}")
+        vals.append(f)
+    if random_shift is None:
+        raise ValueError("CURL contrasts two random shifts of each state: set random_shift >= 1 (DrQ uses 4)")
+    if batch_size is not None and (isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral)
+                                   or not 2 <= batch_size <= MAX_BATCH):
+        raise ValueError(f"CURL takes its negatives from the batch: it needs 2 <= batch_size <= {MAX_BATCH}, "
+                         f"got {batch_size!r}")
+    return tuple(vals)
+
+
+class CurlProjection(nn.Module):
+    """The online projection g_theta and the bilinear W, views of one flat fp32 arena (``_flat``; gradients in
+    ``_flat_grad``) laid out weight_h (512, 3136) | bias_h | weight_c (128, 512) | bias_c | bilinear (128, 128), each
+    group on a 256-byte boundary; the projection is the prefix [0, proj_numel).  Initialised like nn.Linear (uniform in
+    +-1/sqrt(fan_in)), W like a bias-free nn.Linear(128, 128)."""
+
+    NAMES = ("weight_h", "bias_h", "weight_c", "bias_c", "bilinear")
+
+    def __init__(self, device):
+        super().__init__()
+        h, c, w = nn.Linear(FEAT, HIDDEN), nn.Linear(HIDDEN, DIM), nn.Linear(DIM, DIM, bias=False)
+        for name, t in zip(self.NAMES, (h.weight, h.bias, c.weight, c.bias, w.weight)):
+            setattr(self, name, nn.Parameter(t.detach().clone()))
+        self._flatten(torch.device(device))
+
+    def _flatten(self, dev):
+        total, self._offs = 0, {}
+        for name in self.NAMES:
+            total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
+            self._offs[name] = total
+            total += getattr(self, name).numel()
+        self.proj_numel = self._offs["bilinear"]
+        total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
+        flat = torch.zeros(total, device=dev, dtype=torch.float32)
+        flat_grad = torch.zeros(total, device=dev, dtype=torch.float32)
+        for name in self.NAMES:
+            p, off = getattr(self, name), self._offs[name]
+            n = p.numel()
+            flat[off:off + n].copy_(p.data.reshape(-1).float())
+            p.data = flat[off:off + n].view(p.shape)
+            p.grad = flat_grad[off:off + n].view(p.shape)
+            p._riqn_owner = weakref.ref(self)
+            p._riqn_offset = off
+        self._flat, self._flat_grad = flat, flat_grad
+
+    def _apply(self, fn, *a, **k):
+        out = super()._apply(fn, *a, **k)
+        self._flatten(self.weight_h.device)
+        return out
+
+    def _params_changed(self):
+        """Called by the arena Adam after a step: nothing is cached from these weights."""
+
+    def grad_view(self, p):
+        return self._flat_grad[p._riqn_offset:p._riqn_offset + p.numel()].view(p.shape)
+
+    def zero_grad(self, set_to_none=False):
+        """One memset over the gradient arena; the .grad views stay bound."""
+        call("riqn_zero_f32", ptr(self._flat_grad), self._flat_grad.numel())
+        for name in self.NAMES:
+            p = getattr(self, name)
+            p.grad = self.grad_view(p)
+
+    def views(self, arena):
+        """(weight_h, bias_h, weight_c, bias_c) of the projection laid out in ``arena`` (this arena, or the momentum
+        copy's projection prefix)."""
+        out = []
+        for name in self.NAMES[:4]:
+            p, off = getattr(self, name), self._offs[name]
+            out.append(arena[off:off + p.numel()].view(p.shape))
+        return tuple(out)
+
+
+def _tc(B):
+    """Whether the 3136-wide products of a batch of B run on the tensor cores (split-bf16 x3, fp32-faithful): every
+    reduction length there is a multiple of 8 (the weight gradient's is B).  Otherwise they run on the fp32 SIMT GEMM."""
+    return B % 8 == 0
+
+
+def _split(x, rows, cols, transposed=False):
+    """bf16 (hi, lo) images of the fp32 matrix x (rows, cols), and with ``transposed`` those of x^T (riqn_split_bf16)."""
+    bf = lambda *sh: torch.empty(*sh, dtype=torch.bfloat16, device=x.device)
+    hi, lo = bf(rows, cols), bf(rows, cols)
+    hiT, loT = (bf(cols, rows), bf(cols, rows)) if transposed else (None, None)
+    call("riqn_split_bf16", rows, cols, ptr(x), ptr(hi), ptr(lo), ptr(hiT), ptr(loT), 0)
+    return hi, lo, hiT, loT
+
+
+def project(views, feat, keep=None):
+    """z = g(feat) for the projection ``views`` (CurlProjection.views) and features ``feat`` (B, 3136) fp32.  The
+    3136 -> 512 product runs on riqn_gemm_bf16_tc in split-bf16 x3 mode when _tc(B) (its bias joins in the LayerNorm),
+    else on the fp32 SIMT GEMM; the 512 -> 128 product on the SIMT GEMM.  ``keep``: dict that receives the backward's
+    operands."""
+    B, dev = feat.shape[0], feat.device
+    wh, bh, wc, bc = views
+    h = torch.empty(B, HIDDEN, device=dev)
+    if _tc(B):
+        x_hi, x_lo, x_hiT, x_loT = _split(feat, B, FEAT, transposed=keep is not None)
+        w_hi, w_lo, w_hiT, w_loT = _split(wh, HIDDEN, FEAT, transposed=keep is not None)
+        call("riqn_gemm_bf16_tc", B, HIDDEN, FEAT, ptr(x_hi), ptr(x_lo), ptr(w_hi), ptr(w_lo), ptr(h), HIDDEN, 0, None,
+             None, None, 1, None, None, 0)
+        h_bias = bh
+    else:
+        call("riqn_linear_fwd_ld", B, FEAT, HIDDEN, ptr(feat), FEAT, ptr(wh), ptr(bh), ptr(h), HIDDEN, 0)
+        h_bias = None
+    r = torch.empty(B, HIDDEN, device=dev)
+    call("riqn_layernorm_fwd", B, HIDDEN, ptr(h), ptr(h_bias), 1, ptr(r))
+    c = torch.empty(B, DIM, device=dev)
+    call("riqn_linear_fwd_ld", B, HIDDEN, DIM, ptr(r), HIDDEN, ptr(wc), ptr(bc), ptr(c), DIM, 0)
+    z = torch.empty(B, DIM, device=dev)
+    call("riqn_layernorm_fwd", B, DIM, ptr(c), None, 0, ptr(z))
+    if keep is not None:
+        keep.update(feat=feat, h=h, h_bias=h_bias, r=r, c=c)
+        if _tc(B):
+            keep.update(x_T=(x_hiT, x_loT), w_T=(w_hiT, w_loT))
+    return z
+
+
+def project_backward(net, keep, dz):
+    """Accumulate dL/d(weight_h, bias_h, weight_c, bias_c) into ``net``'s gradient arena for the forward in ``keep`` and
+    the upstream ``dz`` (B, 128); returns dL/dfeat (B, 3136).  The two 3136-wide products (dW_h += dh^T feat and
+    dfeat = dh W_h) take the path the forward took; on the tensor cores the weight gradient is one split, so each
+    element gets one add, and b_h's gradient is riqn_colsum_add's fixed-order column sum."""
+    B, dev = dz.shape[0], dz.device
+    wh, _, wc, _ = net.views(net._flat)
+    gwh, gbh, gwc, gbc = net.views(net._flat_grad)
+    dc = torch.empty(B, DIM, device=dev)
+    call("riqn_layernorm_bwd", B, DIM, ptr(keep["c"]), None, ptr(dz), 0, ptr(dc))
+    call("riqn_linear_wgrad", B, DIM, HIDDEN, ptr(dc), ptr(keep["r"]), ptr(gwc), ptr(gbc))
+    dr = torch.empty(B, HIDDEN, device=dev)
+    call("riqn_linear_dgrad_ld", B, HIDDEN, DIM, ptr(dc), DIM, ptr(wc), ptr(dr), HIDDEN)
+    dh = torch.empty(B, HIDDEN, device=dev)
+    call("riqn_layernorm_bwd", B, HIDDEN, ptr(keep["h"]), ptr(keep["h_bias"]), ptr(dr), 1, ptr(dh))
+    dfeat = torch.empty(B, FEAT, device=dev)
+    if "x_T" in keep:
+        d_hi, d_lo, d_hiT, d_loT = _split(dh, B, HIDDEN, transposed=True)
+        (x_hiT, x_loT), (w_hiT, w_loT) = keep["x_T"], keep["w_T"]
+        call("riqn_gemm_bf16_tc", HIDDEN, FEAT, B, ptr(d_hiT), ptr(d_loT), ptr(x_hiT), ptr(x_loT), ptr(gwh), FEAT, 2, None,
+             None, None, 1, None, None, 0)
+        call("riqn_colsum_add", B, HIDDEN, ptr(dh), ptr(gbh))
+        call("riqn_gemm_bf16_tc", B, FEAT, HIDDEN, ptr(d_hi), ptr(d_lo), ptr(w_hiT), ptr(w_loT), ptr(dfeat), FEAT, 0, None,
+             None, None, 1, None, None, 0)
+    else:
+        call("riqn_linear_wgrad", B, HIDDEN, FEAT, ptr(dh), ptr(keep["feat"]), ptr(gwh), ptr(gbh))
+        call("riqn_linear_dgrad_ld", B, FEAT, HIDDEN, ptr(dh), HIDDEN, ptr(wh), ptr(dfeat), FEAT)
+    return dfeat
+
+
+def build(agent, args, checkpoint):
+    """The CURL modules of ``agent`` (after every other module): curl_net, curl_optimiser, momentum_net and
+    momentum_projection, with xi = theta, or all four restored from ``checkpoint`` when it holds them."""
+    agent.curl_net = CurlProjection(args.device)
+    from .optim import Adam
+    agent.curl_optimiser = Adam(agent.curl_net.parameters(), lr=args.lr, eps=args.adam_eps)
+    agent.momentum_net = DQN(args, agent.action_space).to(device=args.device)
+    agent.momentum_projection = torch.empty(agent.curl_net.proj_numel, device=agent.curl_net._flat.device)
+    if checkpoint is not None and "curl_state_dict" in checkpoint:
+        agent.curl_net.load_state_dict(checkpoint["curl_state_dict"])
+        agent.curl_optimiser.load_state_dict(checkpoint["curl_optimiser_state_dict"])
+        mom = checkpoint["curl_momentum_state_dict"]
+        for name in ("conv1", "conv2", "conv3"):
+            conv = getattr(agent.momentum_net, name)
+            conv.weight.data.copy_(mom[name + ".weight"])
+            conv.bias.data.copy_(mom[name + ".bias"])
+        for v, name in zip(agent.curl_net.views(agent.momentum_projection), CurlProjection.NAMES):
+            v.copy_(mom[name])
+    else:
+        n = trunk_numel(agent.online_net)
+        agent.momentum_net._flat[:n].copy_(agent.online_net._flat[:n])
+        agent.momentum_projection.copy_(agent.curl_net._flat[:agent.curl_net.proj_numel])
+    agent.momentum_net._params_changed()
+
+
+def momentum_state_dict(agent):
+    """curl_momentum_state_dict of a checkpoint: the key encoder's conv1-3 and projection, by name (on the CPU)."""
+    out = {}
+    for name in ("conv1", "conv2", "conv3"):
+        conv = getattr(agent.momentum_net, name)
+        out[name + ".weight"], out[name + ".bias"] = conv.weight.detach().cpu().clone(), conv.bias.detach().cpu().clone()
+    for v, name in zip(agent.curl_net.views(agent.momentum_projection), CurlProjection.NAMES):
+        out[name] = v.detach().cpu().clone()
+    return out
+
+
+def trunk_numel(net):
+    """Length of the conv1-3 prefix of a DQN's parameter arena (the first groups of _param_groups_in_arena_order)."""
+    return net._offsets[id(net.conv3.bias)] + net.conv3.bias.numel()
+
+
+def positives(learner, states, debug=None):
+    """The key view of one step: an independent shift of the unshifted ``states`` (drawn after the step's shifts of s_t
+    and s_{t+n}, under CURL_SHIFT_SEED, or the parity hook's ``"curl_shifts"`` (B, 2) int32), through the momentum trunk
+    and projection.
+    Returns z_k (B, 128)."""
+    on, mom = learner.online_net, learner.momentum_net
+    B = states.shape[0]
+    inj = learner._inject[0] if isinstance(learner._inject, list) and learner._inject else learner._inject
+    given = inj.get("curl_shifts") if isinstance(inj, dict) else None
+    if given is None:
+        # a key of its own, counters untouched: the learner's shifts of s_t and s_{t+n} stay those of a plain learner
+        shifts = augment.draw_shifts(on, B, learner.random_shift, key=CURL_SHIFT_SEED, advance=False)
+    else:
+        shifts = torch.as_tensor(given, dtype=torch.int32).reshape(B, 2).to(on._flat.device)
+    x_k = augment.random_shift(states, None, shifts)
+    # the EMA rewrites the key trunk every step: its operand images are rebuilt here, inside every captured replay
+    mom._refresh_tc_operands(force=True, h_done=True)
+    z_k = project(learner.curl_net.views(learner.momentum_projection), mom.trunk(x_k))
+    if debug is not None:
+        debug.update(curl_shifts=shifts, z_k=z_k)
+    return z_k
+
+
+def trunk_addend(learner, z_k, debug=None):
+    """The one-shot addend DQN.backward_trunk applies (DQN._trunk_addend): given the gradient pass's kept operands and
+    the loss core's dfeat, run the anchor projection on the kept features, the InfoNCE and the projection backward (the
+    CURL gradients land in curl_net's arena) and return dfeat + dfeat_CURL."""
+    net, coef = learner.curl_net, learner.curl[0]
+
+    def addend(keep, dfeat):
+        B = dfeat.shape[0]
+        feat = keep["out"][2].view(B, FEAT)
+        pk = {}
+        z_a = project(net.views(net._flat), feat, pk)
+        rows = torch.empty(B, device=dfeat.device)
+        dz_a = torch.empty(B, DIM, device=dfeat.device)
+        logits = torch.empty(B, B, device=dfeat.device) if debug is not None else None
+        call("riqn_curl_infonce_fwd_bwd", B, DIM, ptr(z_a), ptr(z_k), ptr(net.bilinear), coef, ptr(rows), ptr(dz_a),
+             ptr(net.grad_view(net.bilinear)), ptr(logits))
+        dfeat_curl = project_backward(net, pk, dz_a)
+        out = torch.empty_like(dfeat)
+        call("riqn_add_f32", dfeat.numel(), ptr(dfeat), ptr(dfeat_curl), ptr(out))
+        if debug is not None:
+            debug.update(z_a=z_a, logits=logits, curl_loss=rows, dfeat_curl=dfeat_curl)
+        return out
+    return addend
+
+
+def momentum_update(learner):
+    """xi <- xi + tau (theta - xi) over the trunk's arena prefix and the projection (after the Adam steps)."""
+    on, mom, net, tau = learner.online_net, learner.momentum_net, learner.curl_net, learner.curl[1]
+    call("riqn_ema_f32", trunk_numel(on), ptr(on._flat), ptr(mom._flat), tau)
+    call("riqn_ema_f32", net.proj_numel, ptr(net._flat), ptr(learner.momentum_projection), tau)

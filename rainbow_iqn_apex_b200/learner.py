@@ -8,6 +8,10 @@ gscale[b] = weights[b] / B.  ``north_star`` spellings Agent.learn / Agent.update
 Under FQF every step also zeroes, fills, (all-reduces) and steps the fraction proposal's own arena
 (agent.fraction_net, agent.fraction_optimiser).  A user's own loop around ``loss.backward()`` gets the fraction gradients
 from that backward too, and must zero them (fraction_net.zero_grad()) and call fraction_optimiser.step() itself.
+
+Under CURL (curl.py) every step also contrasts the gradient pass's trunk features with a momentum encoder's, zeroes,
+fills, (all-reduces) and steps the projection's arena (agent.curl_net, agent.curl_optimiser), and after the Adam steps
+moves the momentum encoder towards the online trunk and projection.  Each rank contrasts its own local batch.
 """
 import contextlib
 import io
@@ -15,7 +19,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment
+from . import augment, curl
 from .agent import Agent
 from .dynstate import DynState
 
@@ -93,41 +97,49 @@ class Learner(Agent):
                 torch.distributed.all_reduce(net._flat_grad, group=self.process_group)
 
     def _trained_nets(self):
-        """The networks whose gradient arenas a step fills: the online network and, under FQF, the fraction proposal."""
-        return (self.online_net,) if self.fraction_net is None else (self.online_net, self.fraction_net)
+        """The networks whose gradient arenas a step fills: the online network, under FQF the fraction proposal, under
+        CURL the projection."""
+        return tuple(n for n in (self.online_net, self.fraction_net, self.curl_net) if n is not None)
 
     def _optimisers(self):
-        return (self.optimiser,) if self.fraction_optimiser is None else (self.optimiser, self.fraction_optimiser)
+        return tuple(o for o in (self.optimiser, self.fraction_optimiser, self.curl_optimiser) if o is not None)
 
     def _step_optimisers(self):
         for o in self._optimisers():
             o.step()
+        if self.curl is not None:
+            curl.momentum_update(self)
 
     def _write_dyn(self, mem):
         """Stage the next step's device scalars: the Adam bias corrections of every optimiser, and the fill and beta of the
         replay memory ``mem`` ((1, 0) for a step without one)."""
         nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
-        more = ()
-        if self.fraction_optimiser is not None:
-            more = (self.fraction_optimiser.bias_corrections(self.fraction_optimiser._step + 1),)
+        more = tuple(o.bias_corrections(o._step + 1) for o in self._optimisers()[1:])
         capacity, beta = (1.0, 0.0) if mem is None else (mem.transitions.get_current_capacity(), mem.priority_weight)
         self._dyn.write(nss, sbc, capacity, beta, *more)
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None, demo=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arenas.
-        ``debug``: dict that receives the loss core's intermediates (self.loss_core), and with random_shift the shifts and
-        the shifted frames (_shift_frames).  ``demo``: the DQfD demonstration flags (B,) uint8 / bool, or None."""
+        ``debug``: dict that receives the loss core's intermediates (self.loss_core), with random_shift the shifts and
+        the shifted frames (_shift_frames), and under CURL curl_shifts, z_a, z_k, logits, curl_loss (the per-row InfoNCE
+        terms, (B,)) and dfeat_curl.  ``demo``: the DQfD demonstration flags (B,) uint8 / bool, or None."""
         on = self.online_net
         weights = weights.to(on._flat.device, torch.float32)
+        raw_states = states
         if self.random_shift is not None:
             states, next_states = self._shift_frames(states, next_states, debug)
+        z_k = curl.positives(self, raw_states, debug) if self.curl is not None else None
         loss, bw = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, demo=demo)
         for net in self._trained_nets():                                        # learner.py:22
             net.zero_grad()
         # data parallel: DQN.backward_iqn starts the all-reduce of the NoisyLinear gradients as soon as they are final
         on._grads_ready_hook = self._start_tail_allreduce if (self.process_group is not None and self.overlap_allreduce) else None
-        bw(weights, 1.0 / weights.shape[0])                                     # learner.py:23 (.mean())
-        on._grads_ready_hook = None
+        if z_k is not None:         # CURL's feature gradient joins the loss core's in the trunk backward
+            on._trunk_addend = curl.trunk_addend(self, z_k, debug)
+        try:
+            bw(weights, 1.0 / weights.shape[0])                                 # learner.py:23 (.mean())
+        finally:
+            on._grads_ready_hook = on._trunk_addend = None
         return loss
 
     def _shift_frames(self, states, next_states, debug=None):
@@ -183,8 +195,8 @@ class Learner(Agent):
         def route(dyn):
             self._dyn_on = dyn is not None
             self.optimiser._dyn = dyn
-            if self.fraction_optimiser is not None:
-                self.fraction_optimiser._dyn = dyn.slot(1) if dyn is not None else None
+            for k, o in enumerate(self._optimisers()[1:], 1):     # FQF's fraction optimiser, then CURL's
+                o._dyn = dyn.slot(k) if dyn is not None else None
             if mem is not None:
                 mem.transitions._dyn = dyn
             self._reset_step_streams()
@@ -218,7 +230,7 @@ class Learner(Agent):
         update.  ``mem``: the replay memory whose fill and beta the struct carries, or None.  Data parallel with
         capture_collectives False: pre and post become two graphs, with the all-reduce left eager between them."""
         if self._dyn is None:      # one struct for every graph of this learner: no captured address can go stale
-            self._dyn = DynState(self.online_net._flat.device, slots=1 if self.fraction_optimiser is None else 2)
+            self._dyn = DynState(self.online_net._flat.device, slots=len(self._optimisers()))
         split = self.process_group is not None and not self.capture_collectives
         step0 = [o._step for o in self._optimisers()]
         with self._attached(mem):

@@ -910,6 +910,12 @@ class DQN(nn.Module):
         self.backward_trunk(keep, dfeat)
 
     def backward_trunk(self, keep, dfeat):
+        """conv3 -> conv1 backward of the trunk pass kept in ``keep`` for the feature gradient ``dfeat`` (B, 3136).  An
+        addend armed in ``self._trunk_addend`` (CURL, curl.trunk_addend) is consumed first: ``dfeat`` becomes
+        ``addend(keep, dfeat)``."""
+        addend, self._trunk_addend = getattr(self, "_trunk_addend", None), None
+        if addend is not None:
+            dfeat = addend(keep, dfeat)
         (g1, g2, g3), (out1, out2, out3) = keep["g"], keep["out"]
         dev = dfeat.device
         gv = self.grad_view

@@ -64,6 +64,10 @@ def make_data_parallel(learner, group=None):
     if getattr(learner, "fraction_net", None) is not None:        # FQF: the fraction proposal's own arena
         dist.broadcast(learner.fraction_net._flat, src=0, group=group)
         learner.fraction_optimiser.grad_scale = 1.0 / world
+    if getattr(learner, "curl_net", None) is not None:             # CURL: the projection and the momentum encoder
+        for t in (learner.curl_net._flat, learner.momentum_net._flat, learner.momentum_projection):
+            dist.broadcast(t, src=0, group=group)
+        learner.curl_optimiser.grad_scale = 1.0 / world
     learner.process_group = group if group is not None else dist.group.WORLD
     learner.optimiser.grad_scale = 1.0 / world
     return learner
