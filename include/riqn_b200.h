@@ -682,7 +682,8 @@ int riqn_frame_gather(int batch, int actor_capacity, int history, int n_step, co
 /* fp32 (rows, cols) -> bf16 hi and lo = bf16(x - hi) (either may be NULL); hi_t / lo_t (may be NULL) receive the
  * transposed (cols, rows) copies the weight-gradient product consumes. */
 int riqn_split_bf16(long rows, int cols, const float* src, void* hi, void* lo, void* hi_t, void* lo_t, int fp16, void* stream);
-/* fp16 != 0: hi = fp16(x) and lo (or NULL) = bf16(x) instead (hi_t / lo_t must be NULL). */
+/* fp16 != 0: hi = fp16(x) and lo (or NULL) = bf16(x) instead (hi_t / lo_t must be NULL).  Returns cudaErrorInvalidValue,
+ * writing nothing, for fp16 with hi NULL or hi_t / lo_t set, and for lo_t without hi_t. */
 /* Several small splits in ONE launch (the per-step refresh of the noise-free weight images): for each job
  * out[r, c] = src[r, perm ? perm[c] : c] / div (div == 1: unscaled), written as hi / lo = bf16(x - hi) (lo, hi_t may be
  * NULL; hi_t is the transposed (cols, rows) hi image).  Same values as riqn_split_bf16 / riqn_split_bf16_scaled on a
@@ -697,10 +698,18 @@ typedef struct riqn_split_job {
   void* hi_t;
 } riqn_split_job;
 int riqn_split_bf16_multi(int n_jobs, const riqn_split_job* jobs, void* stream);
-/* C (+)= A B^T with A (M,K), B (N,K) row-major bf16, K % 8 == 0, fp32 accumulation in registers.  a_lo/b_lo non-NULL
- * selects the split-bf16 x3 (fp32-faithful) product.  epilogue: 0 store, 1 relu(acc+bias[n]), 2 atomicAdd into C,
- * 3 atomicAdd into C and acc*eps[m,n] into out2 (NoisyLinear dmu / dsigma).  split_k > 1 needs 2 or 3.
- * c_t_bf16 / c_bf16 (may be NULL; epilogue 1 only): bf16 transposed (N, M) / row-major (M, N) images of the result. */
+/* C (+)= A B^T with A (M,K), B (N,K) row-major bf16, K % 8 == 0, fp32 accumulation in registers.  a_lo and b_lo
+ * non-NULL select the split-bf16 x3 (fp32-faithful) product a_hi b_hi + a_hi b_lo + a_lo b_hi; b_lo alone selects the
+ * split-2 product a_hi (b_hi + b_lo) (epilogue 0 only).  epilogue: 0 store, 1 relu(acc+bias[n]), 2 add into C,
+ * 3 add into C and acc*eps[m,n] into out2 (NoisyLinear dmu / dsigma).  split_k > 1 needs 2 or 3: the splits' partial
+ * products are added in split order, so the result does not depend on scheduling.
+ * c_t_bf16 / c_bf16 (may be NULL; epilogue 1 only): bf16 transposed (N, M) / row-major (M, N) images of the result.
+ * Returns cudaErrorInvalidValue, writing nothing, when: the epilogue is outside 0..3; split_k > 1 with epilogue 0 or 1
+ * (whatever the SM count); a_lo without b_lo; split-2 with epilogue != 0; C is NULL or ldc < N; epilogue 1 with a NULL
+ * bias or epilogue 3 with a NULL out2 or eps; c_bf16 not 16-byte aligned, with an epilogue other than 1, odd M or
+ * N % 32 != 0; c_t_bf16 with an epilogue other than 1.  From N = 32 on, whole 32-column chunks leave as vectors, so
+ * then also when: on epilogues 0 and 1, C is not 16-byte aligned or ldc % 4 != 0; the bias of epilogue 1 is not 16-byte
+ * aligned; at even M, c_t_bf16 is not 4-byte aligned. */
 int riqn_gemm_bf16_tc(int M, int N, int K, const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo,
                       float* c, long ldc, int epilogue, const float* bias, float* out2, const float* eps, int split_k,
                       void* c_t_bf16, void* c_bf16, int fmt, void* stream);
@@ -710,8 +719,10 @@ int riqn_gemm_bf16_tc(int M, int N, int K, const void* a_hi, const void* a_lo, c
  *   a_is_km != 0: C (+)= A^T B with A (K, M) row-major (M % 8 == 0): the reduction runs over the ROWS of both, i.e. a
  *                 weight gradient dW = dY^T X straight from the row-major activations;
  *   a_is_km == 0: C (+)= A B with A (M, K) row-major (K % 8 == 0): a data gradient dX = dY W from the untransposed W.
- * epilogue 0 / 2 / 3 as above (2, 3 scale the accumulator by alpha); single-bf16 product.  c_bf16 (may be NULL; epilogue 0,
- * N % 32 == 0): write the result as bf16 (M, N) there INSTEAD of fp32 into c. */
+ * epilogue 0 / 2 / 3 as above (2 adds alpha * acc into C; 0 and 3 need alpha == 1); single-bf16 product.  c_bf16 (may be
+ * NULL; epilogue 0, N % 32 == 0, 16-byte aligned): write the result as bf16 (M, N) there INSTEAD of fp32 into c (c may
+ * then be NULL).  Refused as riqn_gemm_bf16_tc, and besides when a_is_km != 0 and M % 8 != 0, when N % 8 != 0, when
+ * a_is_km == 0 and K % 8 != 0 (a_is_km != 0: any K), for epilogue 1, and for alpha != 1 unless the epilogue is 2. */
 int riqn_gemm_bf16_tc_mn(int M, int N, int K, const void* a, const void* b_kn, int a_is_km, float* c, long ldc, int epilogue,
                          float* out2, const float* eps, float alpha, int split_k, void* c_bf16, int fmt, void* stream);
 

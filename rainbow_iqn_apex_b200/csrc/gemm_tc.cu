@@ -1355,7 +1355,29 @@ RIQN_API int riqn_split_bf16_multi(int n_jobs, const riqn_split_job* jobs, void*
 RIQN_API int riqn_split_bf16(long rows, int cols, const float* src, void* hi, void* lo, void* hi_t, void* lo_t, int fp16,
                              void* stream) {
   riqn::note_launches(1);
+  if (lo_t != nullptr && hi_t == nullptr) return (int)cudaErrorInvalidValue;   // the kernel writes lo_t beside hi_t only
   return split_bf16(rows, cols, src, (bf16*)hi, (bf16*)lo, (bf16*)hi_t, (bf16*)lo_t, (cudaStream_t)stream, fp16);
+}
+
+// Argument checks of the two C-ABI GEMM entry points (include/riqn_b200.h), made before anything is launched.  Every
+// 32-column chunk that lies wholly inside N leaves as vectors: epilogues 0 / 1 store C as 16-byte row pieces (float4
+// per row at odd M), epilogue 1 reads bias as float4, c_bf16 goes out in 16-byte pieces and c_t_bf16, at even M, in
+// 32-bit pairs.  So from N = 32 on those bases must be aligned and C's pitch a multiple of 4 floats (narrower outputs
+// take the scalar stores); epilogues 2 / 3 choose between vector and scalar accumulation at run time.  split_k > 1 is
+// refused before gemm_bf16_tc clamps it, so that the answer does not depend on the SM count.
+static bool tc_args_ok(int M, int N, float* c, long ldc, int epilogue, bool c_written, const float* bias, float* out2,
+                       const float* eps, int split_k, const void* c_t_bf16, const void* c_bf16) {
+  const auto al = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) == 0; };
+  const bool vec = N >= 32;
+  if (epilogue < TC_STORE || epilogue > TC_NOISY_WGRAD) return false;
+  if (split_k > 1 && epilogue != TC_ATOMIC && epilogue != TC_NOISY_WGRAD) return false;
+  if (c_written && (c == nullptr || ldc < N)) return false;
+  if (c_written && vec && epilogue <= TC_BIAS_RELU && (!al(c, 16) || ldc % 4)) return false;
+  if (epilogue == TC_BIAS_RELU && (bias == nullptr || (vec && !al(bias, 16)))) return false;
+  if (epilogue == TC_NOISY_WGRAD && (out2 == nullptr || eps == nullptr)) return false;
+  if (c_bf16 && !al(c_bf16, 16)) return false;
+  if (c_t_bf16 && (epilogue != TC_BIAS_RELU || (vec && M % 2 == 0 && !al(c_t_bf16, 4)))) return false;
+  return true;
 }
 
 RIQN_API int riqn_gemm_bf16_tc(int M, int N, int K, const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo,
@@ -1367,6 +1389,9 @@ RIQN_API int riqn_gemm_bf16_tc(int M, int N, int K, const void* a_hi, const void
   ex.o_hi = (bf16*)c_bf16;
   ex.fmt = fmt & 3;
   if (c_bf16 && (epilogue != TC_BIAS_RELU || (M & 1) || (N % 32))) return (int)cudaErrorInvalidValue;
+  if (!tc_args_ok(M, N, c, ldc, epilogue, true, bias, out2, eps, split_k, c_t_bf16, c_bf16)) return (int)cudaErrorInvalidValue;
+  if (a_lo != nullptr && b_lo == nullptr) return (int)cudaErrorInvalidValue;        // x3 needs both lo images
+  if (a_lo == nullptr && b_lo != nullptr && epilogue != TC_STORE) return (int)cudaErrorInvalidValue;   // split-2: store only
   return gemm_bf16_tc(M, N, K, (const bf16*)a_hi, (const bf16*)a_lo, (const bf16*)b_hi, (const bf16*)b_lo, c, ldc, epilogue,
                       bias, out2, eps, split_k, (cudaStream_t)stream, &ex);
 }
@@ -1377,6 +1402,9 @@ RIQN_API int riqn_gemm_bf16_tc_mn(int M, int N, int K, const void* a, const void
   riqn::note_launches(1);
   if (epilogue != TC_STORE && epilogue != TC_ATOMIC && epilogue != TC_NOISY_WGRAD) return (int)cudaErrorInvalidValue;
   if (c_bf16 && (epilogue != TC_STORE || (N % 32))) return (int)cudaErrorInvalidValue;
+  if (alpha != 1.f && epilogue != TC_ATOMIC) return (int)cudaErrorInvalidValue;     // only epilogue 2 scales
+  if (!tc_args_ok(M, N, c, ldc, epilogue, c_bf16 == nullptr, nullptr, out2, eps, split_k, nullptr, c_bf16))
+    return (int)cudaErrorInvalidValue;
   TcExtra ex;
   ex.o_hi = (bf16*)c_bf16;
   ex.mn_major = a_is_km ? 3 : 2;

@@ -214,36 +214,6 @@ def test_noisy_reset_net_matches_per_layer_calls(cuda_dev):
     assert torch.equal(keep[3]["b"], keep[3]["bmu"])
 
 
-def test_split_bf16_multi_matches_single_calls(cuda_dev):
-    """riqn_split_bf16_multi (the per-step refresh of the noise-free weight images in one launch) writes exactly what
-    riqn_split_bf16 / riqn_split_bf16_scaled write on the (column-permuted) source."""
-    from rainbow_iqn_apex_b200._lib import SplitJob
-    call, ptr = _call()
-    g = torch.Generator().manual_seed(3)
-    bf = lambda *sh: torch.zeros(*sh, dtype=torch.bfloat16, device=cuda_dev)
-    specs = []
-    for rows, cols, div, with_perm, with_t in ((32, 256, 255.0, True, False), (64, 512, 1.0, True, False),
-                                               (64, 576, 1.0, False, True), (3136, 64, 1.0, False, False)):
-        src = torch.randn(rows, cols, generator=g).to(cuda_dev)
-        perm = torch.randperm(cols, generator=g).to(torch.int32).to(cuda_dev) if with_perm else None
-        specs.append((src, perm, div, bf(rows, cols), bf(rows, cols), bf(cols, rows) if with_t else None))
-    arr = (SplitJob * len(specs))()
-    for j, (src, perm, div, hi, lo, hiT) in zip(arr, specs):
-        j.src, j.perm, j.rows, j.cols, j.div = ptr(src), ptr(perm), src.shape[0], src.shape[1], div
-        j.hi, j.lo, j.hi_t = ptr(hi), ptr(lo), ptr(hiT)
-    call("riqn_split_bf16_multi", len(specs), arr)
-    for src, perm, div, hi, lo, hiT in specs:
-        sp = src[:, perm.long()].contiguous() if perm is not None else src
-        rh, rl = bf(*src.shape), bf(*src.shape)
-        if div != 1.0:
-            call("riqn_split_bf16_scaled", src.shape[0], src.shape[1], ptr(sp), div, ptr(rh), ptr(rl))
-        else:
-            call("riqn_split_bf16", src.shape[0], src.shape[1], ptr(sp), ptr(rh), ptr(rl), None, None, 0)
-        assert torch.equal(hi, rh) and torch.equal(lo, rl)
-        if hiT is not None:
-            assert torch.equal(hiT, rh.t().contiguous())
-
-
 def test_trunk_pair_equals_two_trunks(cuda_dev):
     """Online + target conv trunks over the same frames as ONE stacked batch (three launches, two weight sets selected by
     m-tile) == the two trunks run one after the other, bit for bit."""
