@@ -21,8 +21,8 @@ import os
 import torch
 
 from . import _lib
-from . import augment, c51, compute_loss_iqn, cql, curl, dqfd, fqf, hl_gauss, mmd, qr
-from .model import DQN, check_risk
+from . import c51, compute_loss_iqn, config, curl, fqf, qr
+from .model import DQN
 from .optim import Adam
 
 
@@ -42,13 +42,21 @@ class Agent:
 
         # online network (+ optional checkpoint, agent.py:26-34), noisy target copy with frozen parameters (:37-41), Adam (:43)
         checkpoint = self._read_checkpoint(getattr(args, "model", None))
-        # QR-DQN: optional args field (absent from the reference's namespace: off).  None, or N of qr.check_qr; checked
-        # against the checkpoint before its weights load (a QR network with N = atoms has the C51 network's shapes)
-        self.qr_dqn = qr.check_qr(getattr(args, "qr_dqn", 0), getattr(args, "num_tau_samples", None), action_space,
-                                  rainbow_only=self.rainbow_only)
+        # the head and loss variants and their optional args fields (absent from the reference's namespace: off), read
+        # once (config.py).  Each is fixed for the agent's life, so that a captured step graph stays valid; only the risk
+        # measure has a setter
+        v = config.read(args, action_space)
+        self._head, self._loss = v.pop("head"), v.pop("loss")
+        for attr, value in v.items():
+            setattr(self, attr, value)
+        # both checked before any weights load: a QR network with N = atoms has the C51 network's shapes
         if checkpoint is not None and checkpoint.get("qr_dqn_quantiles") != self.qr_dqn:
             raise ValueError(f"the checkpoint was trained with qr_dqn_quantiles = {checkpoint.get('qr_dqn_quantiles')} "
                              f"(None: not QR-DQN), the args ask for {self.qr_dqn}: the z-layers hold other quantities")
+        if checkpoint is not None and checkpoint.get("value_rescaling_eps") != self.value_rescaling:
+            raise ValueError(f"the checkpoint was trained with value_rescaling_eps = {checkpoint.get('value_rescaling_eps')} "
+                             f"(None: off), the args ask for {self.value_rescaling}: a network trained in h-space acts "
+                             "differently on the linear scale")
         self.online_net = DQN(args, action_space).to(device=args.device)
         if checkpoint is not None:
             self.online_net.load_state_dict(checkpoint["model_state_dict"])
@@ -63,13 +71,13 @@ class Agent:
             self.optimiser.load_state_dict(checkpoint["optimiser_state_dict"])
 
         # the head's sizes and the loss core this agent trains (every core returns (loss, backward))
-        if self.rainbow_only:                            # categorical support (agent.py:49-57)
+        if self._head == "c51":                          # categorical support (agent.py:49-57)
             for attr, field in self._C51_FIELDS:
                 setattr(self, attr, getattr(args, field))
             self.support = torch.linspace(self.Vmin, self.Vmax, self.atoms).to(device=args.device)
             self.delta_z = (self.Vmax - self.Vmin) / (self.atoms - 1)
             self.loss_core = c51.loss_core
-        elif self.qr_dqn is not None:                    # QR-DQN: N fixed fractions, nothing sampled
+        elif self._head == "qr":                         # QR-DQN: N fixed fractions, nothing sampled
             self.kappa, self.num_tau_samples = args.kappa, self.qr_dqn
             self.loss_core = qr.loss_core
         else:                                            # IQN sampling sizes (agent.py:58-63)
@@ -79,39 +87,6 @@ class Agent:
         self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each;
         #                      FQF and QR-DQN: {"noises": (n0, n1, n2)}; with random_shift, any of these may also carry
         #                      "shifts": (shifts_states, shifts_next_states), int32 (B, 2) (dy, dx), in place of the draw
-        # Munchausen-IQN targets: optional args fields (absent from the reference's namespace: plain IQN).
-        # None, or (alpha, entropy_tau, l0) of compute_loss_iqn.check_munchausen
-        self.munchausen = compute_loss_iqn.check_munchausen(
-            getattr(args, "munchausen", 0),
-            *(getattr(args, f, v) for f, v in compute_loss_iqn.MUNCHAUSEN_DEFAULTS.items()), rainbow_only=self.rainbow_only)
-        # FQF fraction proposal: optional args fields (absent from the reference's namespace: plain IQN).
-        # None, or (fraction_lr, entropy_coef) of fqf.check_fqf
-        self.fqf = fqf.check_fqf(getattr(args, "fqf", 0), *(getattr(args, f, v) for f, v in fqf.FQF_DEFAULTS.items()),
-                                 rainbow_only=self.rainbow_only, munchausen=self.munchausen,
-                                 num_tau_samples=getattr(args, "num_tau_samples", None))
-        if self.qr_dqn is not None:
-            qr.check_qr(1, self.qr_dqn, munchausen=self.munchausen, fqf=self.fqf)
-        # MMDQN: optional args fields (absent from the reference's namespace: off).  None, or the bandwidths of
-        # mmd.check_mmd; fixed for the agent's life, so that a captured step graph stays valid
-        self.mmd = mmd.check_mmd(getattr(args, "mmd", 0),
-                                 getattr(args, "mmd_bandwidths", mmd.MMD_DEFAULTS["mmd_bandwidths"]),
-                                 qr_dqn=self.qr_dqn, rainbow_only=self.rainbow_only, munchausen=self.munchausen,
-                                 fqf=self.fqf)
-        # HL-Gauss: optional args fields (absent from the reference's namespace: off).  None, or the float32 ratio
-        # sigma / delta_z of hl_gauss.check_hl_gauss; fixed for the agent's life, since a captured step graph holds it
-        self.hl_gauss = hl_gauss.check_hl_gauss(
-            getattr(args, "hl_gauss", 0), getattr(args, "hl_gauss_sigma", hl_gauss.HL_GAUSS_DEFAULTS["hl_gauss_sigma"]),
-            rainbow_only=self.rainbow_only)
-        # CQL: optional args fields (absent from the reference's namespace: off).  None, or the float32 alpha of
-        # cql.check_cql; fixed for the agent's life, since a captured step graph holds it
-        self.cql = cql.check_cql(getattr(args, "cql", 0), getattr(args, "cql_alpha", cql.CQL_DEFAULTS["cql_alpha"]),
-                                 rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf, mmd=self.mmd)
-        # DQfD: optional args fields (absent from the reference's namespace: off).  None, or the float32 (margin, lambda)
-        # of dqfd.check_dqfd; fixed for the agent's life, since a captured step graph holds them
-        self.dqfd = dqfd.check_dqfd(getattr(args, "dqfd", 0),
-                                    *(getattr(args, f, v) for f, v in dqfd.DQFD_DEFAULTS.items()),
-                                    rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf, mmd=self.mmd,
-                                    cql=self.cql)
         self.fraction_net = self.fraction_optimiser = None
         if self.fqf is not None:
             # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed
@@ -120,16 +95,6 @@ class Agent:
             if checkpoint is not None and "fraction_net_state_dict" in checkpoint:
                 self.fraction_net.load_state_dict(checkpoint["fraction_net_state_dict"])
                 self.fraction_optimiser.load_state_dict(checkpoint["fraction_optimiser_state_dict"])
-        # value rescaling (the transformed Bellman operator): optional args fields (absent from the reference's namespace:
-        # off).  None, or eps of compute_loss_iqn.check_value_rescaling; fixed for the agent's life, so that a captured
-        # step graph stays valid
-        self.value_rescaling = compute_loss_iqn.check_value_rescaling(
-            getattr(args, "value_rescaling", 0),
-            *(getattr(args, f, v) for f, v in compute_loss_iqn.VALUE_RESCALING_DEFAULTS.items()), munchausen=self.munchausen)
-        if checkpoint is not None and checkpoint.get("value_rescaling_eps") != self.value_rescaling:
-            raise ValueError(f"the checkpoint was trained with value_rescaling_eps = {checkpoint.get('value_rescaling_eps')} "
-                             f"(None: off), the args ask for {self.value_rescaling}: a network trained in h-space acts "
-                             "differently on the linear scale")
         if self.rainbow_only:
             # the support the C51 head takes expectations over when it acts: h^-1 of the h-space support under rescaling
             self.acting_support = self.support
@@ -137,42 +102,18 @@ class Agent:
                 self.acting_support = torch.empty_like(self.support)
                 _lib.call("riqn_value_rescale", self.atoms, _lib.ptr(self.support), self.value_rescaling, 1,
                           _lib.ptr(self.acting_support))
-        # random-shift augmentation of the learner's frames: optional args field (absent from the reference's namespace:
-        # off).  None, or the pad p of augment.check_random_shift; fixed for the agent's life, so that a captured step graph
-        # stays valid.  Only Learner.compute_gradients shifts; acting and the actors' priorities see the stored frames
-        self.random_shift = augment.check_random_shift(getattr(args, "random_shift", 0))
-        # CURL's contrastive auxiliary loss on the trunk: optional args fields (absent from the reference's namespace: off).
-        # None, or the float32 (lambda, tau) of curl.check_curl; its modules are built last, so that both DQNs (and the
-        # fraction proposal) initialise as a plain agent's from the same seed
-        self.curl = curl.check_curl(getattr(args, "curl", 0),
-                                    *(getattr(args, f, v) for f, v in curl.CURL_DEFAULTS.items()),
-                                    random_shift=self.random_shift, batch_size=self.batch_size)
+        # random_shift: only Learner.compute_gradients shifts; acting and the actors' priorities see the stored frames.
+        # CURL's modules are built last, so that both DQNs (and the fraction proposal) initialise as a plain agent's
+        # from the same seed
         self.curl_net = self.curl_optimiser = self.momentum_net = self.momentum_projection = None
         if self.curl is not None:
             curl.build(self, args, checkpoint)
-        # risk-sensitive acting: optional args fields (absent from the reference's namespace: risk-neutral)
-        self.risk = None
-        self.set_risk(getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
 
     def set_risk(self, measure, eta=None):
         """Act, and pick the double-DQN target action a*, under a distortion risk measure (IQN paper, section 3.1):
         ``measure`` is "neutral", "cvar", "wang", "cpw", "pow" or "norm" (model.RISK_MEASURES), ``eta`` its parameter.
         The K quantile fractions of those passes become beta(tau); the N and N' fractions of the loss stay uniform."""
-        risk = check_risk((measure, eta))
-        if risk is not None and self.rainbow_only:
-            raise ValueError("risk measures distort the IQN quantile fractions; rainbow_only (C51) acts risk-neutrally")
-        if self.munchausen is not None:
-            compute_loss_iqn.check_munchausen(1, *self.munchausen, risk=risk)
-        if getattr(self, "fqf", None) is not None:
-            fqf.check_fqf(1, *self.fqf, risk=risk)
-        if getattr(self, "qr_dqn", None) is not None:
-            qr.check_qr(1, self.qr_dqn, risk=risk)
-        if getattr(self, "mmd", None) is not None:
-            mmd.check_mmd(1, self.mmd, qr_dqn=self.qr_dqn, risk=risk)
-        if getattr(self, "dqfd", None) is not None:
-            dqfd.check_dqfd(1, *self.dqfd, rainbow_only=self.rainbow_only, munchausen=self.munchausen, fqf=self.fqf,
-                            mmd=self.mmd, cql=self.cql)
-        self.risk = risk
+        self.risk = config.read_risk(self._head, self._loss, measure, eta)
 
     @staticmethod
     def _read_checkpoint(path):

@@ -7,24 +7,12 @@ Pixels stay uint8, so the trunk's pixel block matrix stays exact in bf16.  The l
 and s_{t+n} independently in each step; acting never shifts.  A torch loss written on net(x, N) shifts its frames with
 draw_shifts and random_shift before the forward.
 """
-import numbers
-
 import torch
 
 from ._lib import call, ptr
 from .model import _EAGER_STREAMS
 
 SHIFT_SEED = 0x5D1F7     # the shift draws' key is net._rng_seed ^ SHIFT_SEED: apart from the noise and fraction draws'
-
-
-def check_random_shift(value):
-    """Validate the pad p of random-shift augmentation: an integer with 0 <= p < 84 (not a bool).  Returns None when off
-    (0), else p.  Raises ValueError otherwise."""
-    if isinstance(value, bool) or not isinstance(value, numbers.Integral):
-        raise ValueError(f"random_shift must be an integer pad in pixels (0: off, DrQ uses 4), got {value!r}")
-    if not 0 <= value < 84:
-        raise ValueError(f"random_shift must satisfy 0 <= p < 84, got {value!r}")
-    return int(value) if value else None
 
 
 def draw_shifts(net, n, pad, key=SHIFT_SEED, advance=True):

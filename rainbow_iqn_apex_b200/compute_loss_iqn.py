@@ -24,67 +24,10 @@ the head's dense backward on the gradient riqn_cql_dense_grad forms.  DQfD (Agen
 large-margin loss on the rows a ``demo`` mask flags, and its backward runs the same dense backward on the gradient
 riqn_dqfd_dense_grad forms; without a mask the step is the plain IQN step.
 """
-import ctypes
-import math
-import numbers
-
 import torch
 
 from . import cql, dqfd
 from ._lib import call, ptr
-
-MUNCHAUSEN_DEFAULTS = {"munchausen_alpha": 0.9, "munchausen_tau": 0.03, "munchausen_l0": -1.0}   # the paper's
-
-
-def check_munchausen(munchausen, alpha=0.9, entropy_tau=0.03, l0=-1.0, rainbow_only=False, risk=None):
-    """Validate a Munchausen configuration.  Returns None when ``munchausen`` is off (0 / False), else the float triple
-    ``(alpha, entropy_tau, l0)``: scale alpha >= 0, temperature entropy_tau > 0 and clip l0 <= 0, all finite as the kernel
-    receives them (float32).  Munchausen is IQN-only (not ``rainbow_only``) and risk-neutral (``risk`` must be None, as
-    model.check_risk returns it for the neutral measure).  Raises ValueError otherwise."""
-    if isinstance(munchausen, bool) or (isinstance(munchausen, numbers.Integral) and munchausen in (0, 1)):
-        if not munchausen:
-            return None
-    else:
-        raise ValueError(f"munchausen must be 0 or 1, got {munchausen!r}")
-    vals = []
-    for name, v, ok, need in (("munchausen_alpha", alpha, lambda x: x >= 0.0, ">= 0"),
-                              ("munchausen_tau", entropy_tau, lambda x: x > 0.0, "> 0"),
-                              ("munchausen_l0", l0, lambda x: x <= 0.0, "<= 0")):
-        if isinstance(v, bool) or not isinstance(v, numbers.Real):
-            raise ValueError(f"{name} must be a real number, got {v!r}")
-        f = ctypes.c_float(v).value
-        if not (math.isfinite(f) and ok(f)):
-            raise ValueError(f"{name} must be finite and {need} (as a float32), got {v!r}")
-        vals.append(float(v))
-    if rainbow_only:
-        raise ValueError("Munchausen targets are implemented for the IQN loss; rainbow_only (C51) does not take them")
-    if risk is not None:
-        raise ValueError("Munchausen targets have no target action a* to act risk-sensitively on: use the neutral measure")
-    return tuple(vals)
-
-
-VALUE_RESCALING_DEFAULTS = {"value_rescaling_eps": 1e-3}   # R2D2's epsilon
-
-
-def check_value_rescaling(value_rescaling, eps=1e-3, munchausen=None):
-    """Validate a value-rescaling configuration (the transformed Bellman operator, Pohlen et al. 2018).  Returns None when
-    ``value_rescaling`` is off (0 / False), else eps: finite and >= 0 as the kernels receive it (float32).  It applies to
-    the IQN, FQF and C51 losses and does not combine with Munchausen targets (``munchausen`` must be None), whose soft
-    target mixes log-policies of means.  Raises ValueError otherwise."""
-    if isinstance(value_rescaling, bool) or (isinstance(value_rescaling, numbers.Integral) and value_rescaling in (0, 1)):
-        if not value_rescaling:
-            return None
-    else:
-        raise ValueError(f"value_rescaling must be 0 or 1, got {value_rescaling!r}")
-    if isinstance(eps, bool) or not isinstance(eps, numbers.Real):
-        raise ValueError(f"value_rescaling_eps must be a real number, got {eps!r}")
-    f = ctypes.c_float(eps).value
-    if not (math.isfinite(f) and f >= 0.0):
-        raise ValueError(f"value_rescaling_eps must be finite and >= 0 (as a float32), got {eps!r}")
-    if munchausen is not None:
-        raise ValueError("value rescaling and Munchausen targets do not combine: set value_rescaling = 0 or munchausen = 0")
-    return float(eps)
-
 
 def greedy_actions(agent, batch, n, q, w=None):
     """a* (batch,) int64: the greedy actions of quantile values q (n*batch, A), quantile-major, on the mean over the n

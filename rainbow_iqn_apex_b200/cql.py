@@ -17,38 +17,9 @@ forms the dense upstream gradient G (N*B, A) and the head's dense backward takes
 a* selection included) and QR-DQN; acting, priorities (on the CQL loss), the captured step graphs and checkpoints are the
 plain learner's.
 """
-import ctypes
-import math
-import numbers
-
 import torch
 
 from ._lib import call, ptr
-
-CQL_DEFAULTS = {"cql_alpha": 1.0}     # this project's default, not a value taken from the paper
-
-
-def check_cql(cql, alpha=CQL_DEFAULTS["cql_alpha"], rainbow_only=False, munchausen=None, fqf=None, mmd=None):
-    """Validate a CQL configuration.  Returns None when ``cql`` is off (0 / False), else alpha as the float32 the kernels
-    receive: a real number (not a bool), finite and > 0 in float32.  CQL regularises the quantile heads' IQN and QR-DQN
-    losses, so it does not combine with ``rainbow_only`` (C51, HL-Gauss), Munchausen targets, FQF or MMDQN (``munchausen``,
-    ``fqf``, ``mmd`` not None).  Raises ValueError otherwise."""
-    if isinstance(cql, bool) or (isinstance(cql, numbers.Integral) and cql in (0, 1)):
-        if not cql:
-            return None
-    else:
-        raise ValueError(f"cql must be 0 or 1, got {cql!r}")
-    if isinstance(alpha, bool) or not isinstance(alpha, numbers.Real):
-        raise ValueError(f"cql_alpha must be a real number, got {alpha!r}")
-    f = ctypes.c_float(float(alpha)).value
-    if not (math.isfinite(f) and f > 0.0):
-        raise ValueError(f"cql_alpha must be finite and > 0 as a float32, got {alpha!r}")
-    for on, what in ((rainbow_only, "rainbow_only (C51, HL-Gauss)"), (munchausen is not None, "Munchausen targets"),
-                     (fqf is not None, "FQF"), (mmd is not None, "MMDQN")):
-        if on:
-            raise ValueError(f"CQL regularises the IQN and QR-DQN quantile losses; {what} does not take it: set cql = 0")
-    return f
-
 
 def cql_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonterminals, loss, dtheta, theta_out,
              target_out, gap_out=None):

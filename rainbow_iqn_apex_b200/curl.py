@@ -28,9 +28,6 @@ Modules, all built after every existing one (so that both DQNs initialise as a p
   agent.momentum_net    a DQN whose trunk alone ever runs (f_xi), and agent.momentum_projection, the untrained
                         buffer arena of g_xi (the projection prefix of curl_net's arena layout)
 """
-import ctypes
-import math
-import numbers
 import weakref
 
 import torch
@@ -40,39 +37,8 @@ from . import augment
 from ._lib import call, ptr
 from .model import DQN, FEAT, _ALIGN
 
-CURL_DEFAULTS = {"curl_coef": 1.0, "curl_momentum": 0.001}   # this project's starting point, not tuned
 HIDDEN, DIM = 512, 128                                         # projection widths
-MAX_BATCH = 4096                                               # riqn_curl_infonce_fwd_bwd
 CURL_SHIFT_SEED = 0xC0A1                                       # the positive view's draw key (net._rng_seed ^ this)
-
-
-def check_curl(curl, coef=CURL_DEFAULTS["curl_coef"], momentum=CURL_DEFAULTS["curl_momentum"], random_shift=None,
-               batch_size=None):
-    """Validate a CURL configuration.  Returns None when ``curl`` is off (0 / False), else (lambda, tau) as the float32
-    values the kernels receive: lambda finite and > 0, tau finite with 0 < tau <= 1.  CURL contrasts two augmentations, so
-    it needs ``random_shift`` (the pad, not None), and in-batch negatives, so 2 <= ``batch_size`` <= 4096.  Raises
-    ValueError otherwise."""
-    if isinstance(curl, bool) or (isinstance(curl, numbers.Integral) and curl in (0, 1)):
-        if not curl:
-            return None
-    else:
-        raise ValueError(f"curl must be 0 or 1, got {curl!r}")
-    vals = []
-    for name, v, ok, need in (("curl_coef", coef, lambda x: x > 0.0, "> 0"),
-                              ("curl_momentum", momentum, lambda x: 0.0 < x <= 1.0, "in (0, 1]")):
-        if isinstance(v, bool) or not isinstance(v, numbers.Real):
-            raise ValueError(f"{name} must be a real number, got {v!r}")
-        f = ctypes.c_float(float(v)).value
-        if not (math.isfinite(f) and ok(f)):
-            raise ValueError(f"{name} must be finite and {need} as a float32, got {v!r}")
-        vals.append(f)
-    if random_shift is None:
-        raise ValueError("CURL contrasts two random shifts of each state: set random_shift >= 1 (DrQ uses 4)")
-    if batch_size is not None and (isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral)
-                                   or not 2 <= batch_size <= MAX_BATCH):
-        raise ValueError(f"CURL takes its negatives from the batch: it needs 2 <= batch_size <= {MAX_BATCH}, "
-                         f"got {batch_size!r}")
-    return tuple(vals)
 
 
 class CurlProjection(nn.Module):

@@ -17,62 +17,9 @@ G (N*B, A) and the head's dense backward takes it.  The replay's demonstration p
 riqn_sumtree_update_demo) keeps demonstrations sampled.  DQfD applies to IQN (risk-sensitive a* selection included) and
 QR-DQN; acting, the actors' priorities and checkpoints are the plain learner's.
 """
-import ctypes
-import math
-import numbers
-
 import torch
 
 from ._lib import call, ptr
-
-DQFD_DEFAULTS = {"dqfd_margin": 0.8, "dqfd_lambda": 1.0}            # Hester et al.'s
-DEMO_DEFAULTS = {"demo_segments": 0, "demo_priority_bonus": 0.0}   # no demonstrations
-
-
-def _positive_f32(name, v):
-    if isinstance(v, bool) or not isinstance(v, numbers.Real):
-        raise ValueError(f"{name} must be a real number, got {v!r}")
-    f = ctypes.c_float(float(v)).value
-    if not (math.isfinite(f) and f > 0.0):
-        raise ValueError(f"{name} must be finite and > 0 as a float32, got {v!r}")
-    return f
-
-
-def check_dqfd(dqfd, margin=DQFD_DEFAULTS["dqfd_margin"], lam=DQFD_DEFAULTS["dqfd_lambda"], rainbow_only=False,
-               munchausen=None, fqf=None, mmd=None, cql=None):
-    """Validate a DQfD configuration.  Returns None when ``dqfd`` is off (0 / False), else the float32 pair
-    ``(margin, lambda)`` the kernels receive: real numbers (not bools), finite and > 0 in float32.  The margin loss is
-    fused into the IQN and QR-DQN quantile losses, so it does not combine with ``rainbow_only`` (C51, HL-Gauss), Munchausen
-    targets, FQF, MMDQN or CQL (``munchausen``, ``fqf``, ``mmd``, ``cql`` not None).  Raises ValueError otherwise."""
-    if isinstance(dqfd, bool) or (isinstance(dqfd, numbers.Integral) and dqfd in (0, 1)):
-        if not dqfd:
-            return None
-    else:
-        raise ValueError(f"dqfd must be 0 or 1, got {dqfd!r}")
-    f = (_positive_f32("dqfd_margin", margin), _positive_f32("dqfd_lambda", lam))
-    for on, what in ((rainbow_only, "rainbow_only (C51, HL-Gauss)"), (munchausen is not None, "Munchausen targets"),
-                     (fqf is not None, "FQF"), (mmd is not None, "MMDQN"), (cql is not None, "CQL")):
-        if on:
-            raise ValueError(f"DQfD's margin loss is fused into the IQN and QR-DQN quantile losses; {what} does not take "
-                             "it: set dqfd = 0")
-    return f
-
-
-def check_demo_replay(demo_segments, bonus, nb_actor):
-    """Validate a replay's demonstration fields.  Returns ``(D, eps_d)``: D an integer with 0 <= D <= nb_actor (not a
-    bool), the number of segments, counted from the last, that hold demonstrations; eps_d the float32 priority bonus,
-    finite and >= 0.  Raises ValueError otherwise."""
-    if isinstance(demo_segments, bool) or not isinstance(demo_segments, numbers.Integral):
-        raise ValueError(f"demo_segments must be an integer, got {demo_segments!r}")
-    if not 0 <= int(demo_segments) <= int(nb_actor):
-        raise ValueError(f"demo_segments must be in 0..nb_actor = {nb_actor}, got {demo_segments!r}")
-    if isinstance(bonus, bool) or not isinstance(bonus, numbers.Real):
-        raise ValueError(f"demo_priority_bonus must be a real number, got {bonus!r}")
-    f = ctypes.c_float(float(bonus)).value
-    if not (math.isfinite(f) and f >= 0.0):
-        raise ValueError(f"demo_priority_bonus must be finite and >= 0 as a float32, got {bonus!r}")
-    return int(demo_segments), f
-
 
 def demo_flags(agent, demo, B):
     """The loss cores' ``demo`` argument as (B,) uint8 flags on the online network's device, or None.  A mask needs an

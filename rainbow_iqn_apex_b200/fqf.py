@@ -14,9 +14,6 @@ arena, parameter order and state_dict stay those of the reference.  It lives on 
 by agent.fraction_optimiser, the arena Adam; the paper used RMSProp).  There is no target copy: fractions always come
 from the online proposal.
 """
-import ctypes
-import math
-import numbers
 import weakref
 
 import torch
@@ -24,43 +21,6 @@ from torch import nn
 
 from ._lib import call, ptr
 from .model import FEAT, _ALIGN
-
-FQF_DEFAULTS = {"fqf_fraction_lr": 2.5e-9, "fqf_entropy_coef": 0.0}   # the public FQF Atari configurations' rate
-MAX_FRACTIONS = 256
-
-
-def check_fqf(fqf, fraction_lr=2.5e-9, entropy_coef=0.0, rainbow_only=False, munchausen=None, risk=None,
-              num_tau_samples=None):
-    """Validate an FQF configuration.  Returns None when ``fqf`` is off (0 / False), else ``(fraction_lr,
-    entropy_coef)``: fraction_lr > 0 and entropy_coef >= 0, both finite as float32.  FQF is IQN-only (not
-    ``rainbow_only``), does not combine with Munchausen targets (``munchausen`` must be None) and is risk-neutral (``risk``
-    must be None); ``num_tau_samples`` (N) must lie in 2..256.  Raises ValueError otherwise."""
-    if isinstance(fqf, bool) or (isinstance(fqf, numbers.Integral) and fqf in (0, 1)):
-        if not fqf:
-            return None
-    else:
-        raise ValueError(f"fqf must be 0 or 1, got {fqf!r}")
-    vals = []
-    for name, v, ok, need in (("fqf_fraction_lr", fraction_lr, lambda x: x > 0.0, "> 0"),
-                              ("fqf_entropy_coef", entropy_coef, lambda x: x >= 0.0, ">= 0")):
-        if isinstance(v, bool) or not isinstance(v, numbers.Real):
-            raise ValueError(f"{name} must be a real number, got {v!r}")
-        f = ctypes.c_float(v).value
-        if not (math.isfinite(f) and ok(f)):
-            raise ValueError(f"{name} must be finite and {need} (as a float32), got {v!r}")
-        vals.append(float(v))
-    if rainbow_only:
-        raise ValueError("FQF proposes quantile fractions for the IQN head; rainbow_only (C51) has none")
-    if munchausen is not None:
-        raise ValueError("FQF and Munchausen targets do not combine: set munchausen = 0 or fqf = 0")
-    if risk is not None:
-        raise ValueError("FQF acts on its proposed fractions: a risk measure has no fractions to distort; use the neutral "
-                         "measure")
-    if num_tau_samples is not None and (isinstance(num_tau_samples, bool) or not isinstance(num_tau_samples, numbers.Integral)
-                                        or not 2 <= num_tau_samples <= MAX_FRACTIONS):
-        raise ValueError(f"FQF needs num_tau_samples in 2..{MAX_FRACTIONS}, got {num_tau_samples!r}")
-    return tuple(vals)
-
 
 class FractionProposal(nn.Module):
     """The fraction proposal network: one linear layer ``weight`` (N, 3136), ``bias`` (N), views of one flat fp32 arena

@@ -12,40 +12,7 @@ v_max + delta_z / 2].  The loss is the cross-entropy -sum_j m_j log p_j(s, a), o
 backward takes unchanged.  Everything else is C51's: the three passes, a*, acting, the captured step graphs and
 checkpoints.
 """
-import ctypes
-import math
-import numbers
-
 from ._lib import call, ptr
-
-HL_GAUSS_DEFAULTS = {"hl_gauss_sigma": 0.75}
-MAX_SIGMA_RATIO = 1000.0
-
-
-def _f32(x):
-    return ctypes.c_float(x).value
-
-
-def check_hl_gauss(hl_gauss, sigma=HL_GAUSS_DEFAULTS["hl_gauss_sigma"], rainbow_only=False):
-    """Validate an HL-Gauss configuration.  Returns None when ``hl_gauss`` is off (0 / False), else the ratio sigma /
-    delta_z as the float32 the kernel receives: a real number (not a bool), finite, > 0 and <= 1000 in float32.  HL-Gauss
-    trains the C51 head, so it needs ``rainbow_only``; that also excludes QR-DQN, MMDQN, FQF and Munchausen targets,
-    which reject rainbow_only.  Raises ValueError otherwise."""
-    if isinstance(hl_gauss, bool) or (isinstance(hl_gauss, numbers.Integral) and hl_gauss in (0, 1)):
-        if not hl_gauss:
-            return None
-    else:
-        raise ValueError(f"hl_gauss must be 0 or 1, got {hl_gauss!r}")
-    if isinstance(sigma, bool) or not isinstance(sigma, numbers.Real):
-        raise ValueError(f"hl_gauss_sigma must be a real number, got {sigma!r}")
-    f = _f32(float(sigma))
-    if not (math.isfinite(f) and 0.0 < f <= MAX_SIGMA_RATIO):
-        raise ValueError(f"hl_gauss_sigma (sigma in bin widths) must be finite, > 0 and <= {MAX_SIGMA_RATIO:g} as a "
-                         f"float32, got {sigma!r}")
-    if not rainbow_only:
-        raise ValueError("hl_gauss trains the C51 head's categorical output: set rainbow_only = 1 as well")
-    return f
-
 
 def hl_gauss_loss(agent, B, log_ps, pns, actions, a_star, returns, nonterminals, loss, dq, m_out, target_out):
     """The HL-Gauss cross-entropy at ratio ``agent.hl_gauss``: riqn_hl_gauss_loss_fwd_bwd, or the transformed target

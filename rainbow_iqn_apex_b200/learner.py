@@ -38,7 +38,7 @@ class _StepGraph(NamedTuple):
 
 class Learner(Agent):
     def __init__(self, args, action_space, redis_servor):
-        self._graphs = {}          # captured step graphs by kind: "replay", "batch", "learn" (Agent.__init__ calls set_risk)
+        self._graphs = {}          # captured step graphs by kind: "replay", "batch", "learn"
         super().__init__(args, action_space, redis_servor)
         self.process_group = None  # set by parallel.make_data_parallel
         self._dp_stream = self._dp_tail = None

@@ -12,60 +12,8 @@ the one-hot head backward (the loss writes dtheta quantile-major, as the quantil
 the particles, and checkpoints.  The network's second output, QR-DQN's fixed fractions, is not read.
 """
 import ctypes
-import math
-import numbers
 
 from ._lib import call, ptr
-
-MMD_DEFAULTS = {"mmd_bandwidths": tuple(float(h) for h in range(1, 11))}
-MAX_BANDWIDTHS = 16
-_LOG2E = 1.4426950408889634
-
-
-def _f32(x):
-    return ctypes.c_float(x).value
-
-
-def check_mmd(mmd, bandwidths=MMD_DEFAULTS["mmd_bandwidths"], qr_dqn=None, rainbow_only=False, munchausen=None,
-              fqf=None, risk=None):
-    """Validate an MMDQN configuration.  Returns None when ``mmd`` is off (0 / False), else ``bandwidths`` as a tuple of
-    floats: a sequence (not a string) of 1..16 real numbers, each finite and > 0 as the float32 the kernel receives, with
-    the kernel's constants log2(e)/h and 2/h finite in float32.  MMDQN trains the QR-DQN network, so it needs ``qr_dqn``
-    (N, as qr.check_qr returns it, not None) and inherits QR-DQN's exclusions: ``rainbow_only``, Munchausen targets
-    (``munchausen`` not None), FQF (``fqf`` not None) and a risk measure (``risk`` not None).  Raises ValueError
-    otherwise."""
-    if isinstance(mmd, bool) or (isinstance(mmd, numbers.Integral) and mmd in (0, 1)):
-        if not mmd:
-            return None
-    else:
-        raise ValueError(f"mmd must be 0 or 1, got {mmd!r}")
-    if isinstance(bandwidths, (str, bytes)):
-        raise ValueError(f"mmd_bandwidths must be a sequence of numbers, not a string: {bandwidths!r}")
-    try:
-        vals = tuple(bandwidths)
-    except TypeError:
-        raise ValueError(f"mmd_bandwidths must be a sequence of numbers, got {bandwidths!r}") from None
-    if not 1 <= len(vals) <= MAX_BANDWIDTHS:
-        raise ValueError(f"mmd_bandwidths needs 1..{MAX_BANDWIDTHS} bandwidths, got {len(vals)}")
-    for v in vals:
-        if isinstance(v, bool) or not isinstance(v, numbers.Real):
-            raise ValueError(f"each of mmd_bandwidths must be a real number, got {v!r}")
-        f = _f32(v)
-        if not (math.isfinite(f) and f > 0.0 and math.isfinite(_f32(_LOG2E / f)) and math.isfinite(_f32(2.0 / f))):
-            raise ValueError(f"each of mmd_bandwidths must be finite and > 0 (as a float32, with 2/h finite), got {v!r}")
-    if qr_dqn is None:
-        raise ValueError("mmd trains the QR-DQN network's particles: set qr_dqn = 1 as well")
-    if rainbow_only:
-        raise ValueError("mmd trains the QR-DQN head, and rainbow_only selects the C51 head: set one of them")
-    if munchausen is not None:
-        raise ValueError("MMDQN and Munchausen targets do not combine: set munchausen = 0 or mmd = 0")
-    if fqf is not None:
-        raise ValueError("MMDQN has no fractions for FQF to learn: set fqf = 0 or mmd = 0")
-    if risk is not None:
-        raise ValueError("MMDQN's particles carry no quantile fractions for a risk measure to distort; use the neutral "
-                         "measure")
-    return tuple(float(v) for v in vals)
-
 
 def mmd_loss(agent, B, N, q_on, q_tgt, actions, a_star, returns, nonterminals, loss, dtheta, theta_out, target_out):
     """The double-DQN MMD loss kernel over the bandwidths ``agent.mmd``: riqn_mmd_loss_fwd_bwd, or against the

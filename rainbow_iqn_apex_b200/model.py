@@ -223,11 +223,10 @@ class DQN(nn.Module):
         self.conv1 = nn.Conv2d(args.history_length, 32, 8, stride=4, padding=1)
         self.conv2 = nn.Conv2d(32, 64, 4, stride=2)
         self.conv3 = nn.Conv2d(64, 64, 3)
-        from . import qr
+        from . import config
         # QR-DQN: N fixed-fraction quantiles per action on the C51 layer set (no quantile embedding); else None
-        self.num_quantiles = qr.check_qr(getattr(args, "qr_dqn", 0), getattr(args, "num_tau_samples", None),
-                                         action_space, rainbow_only=self.rainbow_only)
-        self.qr_dqn = self.num_quantiles is not None
+        head, self.num_quantiles = config.read_head(args, action_space)
+        self.qr_dqn = head == "qr"
         if self.qr_dqn:
             zv, za = self.num_quantiles, action_space * self.num_quantiles
         elif self.rainbow_only:

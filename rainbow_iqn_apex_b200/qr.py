@@ -17,44 +17,11 @@ runs the same step with the MMD loss kernel in place of the quantile-Huber one; 
 the log-sum-exp gap to the quantile-Huber loss and takes riqn_qr_head_bwd_dense, and so does DQfD (agent.dqfd, dqfd.py)
 with lambda times the large-margin loss on the rows a ``demo`` mask flags.
 """
-import numbers
-
 import torch
 
 from . import c51, cql, dqfd, mmd
 from ._lib import call, ptr
 from .compute_loss_iqn import _loss_inputs, _quantile_loss, greedy_actions
-
-MAX_QUANTILES = 256
-MAX_ACTIONS = 32       # riqn_argmax_mean / riqn_argmax_expected_h
-
-
-def check_qr(qr_dqn, num_tau_samples=None, action_space=None, rainbow_only=False, munchausen=None, fqf=None, risk=None):
-    """Validate a QR-DQN configuration.  Returns None when ``qr_dqn`` is off (0 / False), else N = ``num_tau_samples``,
-    an integer in 2..256.  ``action_space`` must not exceed 32; QR-DQN does not combine with ``rainbow_only``, Munchausen
-    targets (``munchausen`` not None) or FQF (``fqf`` not None), and acts risk-neutrally (``risk`` None, as
-    model.check_risk returns it for the neutral measure).  Raises ValueError otherwise."""
-    if isinstance(qr_dqn, bool) or (isinstance(qr_dqn, numbers.Integral) and qr_dqn in (0, 1)):
-        if not qr_dqn:
-            return None
-    else:
-        raise ValueError(f"qr_dqn must be 0 or 1, got {qr_dqn!r}")
-    if (isinstance(num_tau_samples, bool) or not isinstance(num_tau_samples, numbers.Integral)
-            or not 2 <= num_tau_samples <= MAX_QUANTILES):
-        raise ValueError(f"QR-DQN needs num_tau_samples (its N) in 2..{MAX_QUANTILES}, got {num_tau_samples!r}")
-    if action_space is not None and not 1 <= action_space <= MAX_ACTIONS:
-        raise ValueError(f"QR-DQN supports 1..{MAX_ACTIONS} actions, got {action_space!r}")
-    if rainbow_only:
-        raise ValueError("qr_dqn and rainbow_only are two different heads on the same network: set one of them")
-    if munchausen is not None:
-        raise ValueError("QR-DQN and Munchausen targets do not combine: set munchausen = 0 or qr_dqn = 0")
-    if fqf is not None:
-        raise ValueError("QR-DQN has fixed fractions and FQF learned ones: set fqf = 0 or qr_dqn = 0")
-    if risk is not None:
-        raise ValueError("QR-DQN has fixed quantile fractions: a risk measure has nothing to distort; use the neutral "
-                         "measure")
-    return int(num_tau_samples)
-
 
 def fractions(net, batch):
     """The fixed fractions tau_hat_i = fl((2i+1)/(2N)) as an (N*batch, 1) array, quantile-major (row i*batch + b); built

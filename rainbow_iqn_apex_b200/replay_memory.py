@@ -13,7 +13,7 @@ Class / method names follow the reference so ``launch_learner``-style loops read
 import numpy as np
 import torch
 
-from . import _lib, dqfd
+from . import _lib, config
 from ._lib import call, ptr
 
 FRAME = 84 * 84
@@ -198,8 +198,7 @@ class ReplayMemory:
         # data indices >= (nb_actor - D) * actor_capacity, hold them; the sampler's valid-index shift never leaves a
         # segment, so a sampled row is a demonstration exactly when its tree index is >= demo_leaf.  update_priorities
         # adds demo_priority_bonus (DQfD's eps_d) to their new priorities
-        self.demo_segments, self.demo_priority_bonus = dqfd.check_demo_replay(
-            *(getattr(args, f, v) for f, v in dqfd.DEMO_DEFAULTS.items()), args.nb_actor)
+        self.demo_segments, self.demo_priority_bonus = config.read_demo(args)
         self.demo_leaf = None
         if self.demo_segments > 0:
             self.demo_leaf = (args.nb_actor - self.demo_segments) * args.actor_capacity + self.capacity - 1

@@ -133,15 +133,6 @@ def test_philox_statement_known_answers():
     assert list(philox_np(0, 0, 1)) == [0x6627E8D5, 0xE169C58D, 0xBC57AC4C, 0x9B00DBD8]
 
 
-def test_check_random_shift():
-    from rainbow_iqn_apex_b200.augment import check_random_shift
-    assert check_random_shift(0) is None and check_random_shift(4) == 4 and check_random_shift(np.int64(83)) == 83
-    assert check_random_shift(np.int32(1)) == 1
-    for v in (True, False, 1.5, 4.0, -1, 84, float("nan"), "4", None):
-        with pytest.raises(ValueError):
-            check_random_shift(v)
-
-
 # ------------------------------------------------------------------------------------------------ kernels (GPU)
 def _u8_out(n, dev):
     t = torch.full((n + PAD,), CANARY, dtype=torch.uint8, device=dev)

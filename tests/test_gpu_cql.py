@@ -98,23 +98,6 @@ def test_float64_and_torch_fp32_statements_agree(kind, eps):
     assert np.max(np.abs(loss.detach().numpy() - l64) / np.abs(l64)) < 1e-6
 
 
-def test_check_cql():
-    from rainbow_iqn_apex_b200.cql import CQL_DEFAULTS, check_cql
-    assert CQL_DEFAULTS == {"cql_alpha": 1.0}
-    assert check_cql(0) is None and check_cql(False) is None and check_cql(0, "x", rainbow_only=1) is None
-    assert check_cql(1) == 1.0 and check_cql(True, 4) == 4.0 and check_cql(np.int64(1), np.float32(0.1)) == float(F32(0.1))
-    assert check_cql(1, 0.1) == float(F32(0.1)) and check_cql(1, 1e-40) > 0 and check_cql(1, 3e38) == float(F32(3e38))
-    bad = [dict(cql=2), dict(cql=-1), dict(cql=0.5), dict(cql=1.0), dict(cql="1"), dict(cql=None), dict(alpha=0.0),
-           dict(alpha=-1.0), dict(alpha=math.nan), dict(alpha=math.inf), dict(alpha=-math.inf), dict(alpha=1e39),
-           dict(alpha=1e-50), dict(alpha=True), dict(alpha="1"), dict(alpha=None), dict(alpha=(1.0,)),
-           dict(rainbow_only=1), dict(rainbow_only=True), dict(munchausen=(0.9, 0.03, -1.0)), dict(fqf=(2.5e-9, 0.0)),
-           dict(mmd=(1.0,))]
-    for kw in bad:
-        kw = dict(dict(cql=1, alpha=1.0), **kw)
-        with pytest.raises(ValueError):
-            check_cql(**kw)
-
-
 # ------------------------------------------------------------------------------------------------ kernels (GPU)
 # (B, A, N, N'): N, N' from 1 up to the IQN kernel tests' (1500, 64) and (64, 2000)
 KERNEL_SHAPES = [(1, 1, 1, 1), (7, 4, 8, 5), (32, 18, 64, 64), (512, 18, 64, 64), (4096, 4, 32, 32), (32, 32, 200, 200),

@@ -246,22 +246,6 @@ def test_rejected_calls_write_nothing(cuda_dev):
 
 
 # ------------------------------------------------------------------------------------------------ validation
-def test_check_curl():
-    from rainbow_iqn_apex_b200.curl import check_curl
-    assert check_curl(0) is None and check_curl(False) is None
-    assert check_curl(1, random_shift=4, batch_size=32) == (1.0, np.float32(0.001))
-    assert check_curl(True, 0.5, 1, random_shift=1, batch_size=2) == (0.5, 1.0)
-    for kw in (dict(curl=2), dict(curl=1.0), dict(curl=-1), dict(curl="1"), dict(coef=0.0), dict(coef=-1.0),
-               dict(coef=float("nan")), dict(coef=float("inf")), dict(coef=1e39), dict(coef=True), dict(coef=1e-46),
-               dict(momentum=0.0), dict(momentum=1.5), dict(momentum=float("nan")), dict(momentum=-0.1),
-               dict(momentum=False), dict(random_shift=None), dict(batch_size=1), dict(batch_size=0),
-               dict(batch_size=4097), dict(batch_size=2.0)):
-        a = dict(curl=1, coef=1.0, momentum=0.001, random_shift=4, batch_size=32)
-        a.update(kw)
-        with pytest.raises(ValueError):
-            check_curl(a.pop("curl"), a.pop("coef"), a.pop("momentum"), **a)
-
-
 def test_oracle_statements():
     """The oracle's InfoNCE equals the float64 statement, and its EMA is the float32 one (the CPU half of the checks)."""
     rs = np.random.RandomState(3)

@@ -133,40 +133,6 @@ def test_bonus_priorities_on_the_oracle_tree():
     assert t.check() < 1e-12
 
 
-def test_check_dqfd():
-    from rainbow_iqn_apex_b200.dqfd import DQFD_DEFAULTS, check_dqfd
-    assert DQFD_DEFAULTS == {"dqfd_margin": 0.8, "dqfd_lambda": 1.0}
-    assert check_dqfd(0) is None and check_dqfd(False) is None and check_dqfd(0, "x", None, rainbow_only=1) is None
-    assert check_dqfd(1) == (float(F32(0.8)), 1.0) and check_dqfd(True, 2, 4) == (2.0, 4.0)
-    assert check_dqfd(np.int64(1), np.float32(0.1), 1e-40)[0] == float(F32(0.1))
-    assert check_dqfd(1, 3e38, 3e38) == (float(F32(3e38)),) * 2
-    bad = [dict(dqfd=2), dict(dqfd=-1), dict(dqfd=0.5), dict(dqfd=1.0), dict(dqfd="1"), dict(dqfd=None)]
-    for name in ("margin", "lam"):
-        bad += [{name: v} for v in (0.0, -1.0, math.nan, math.inf, -math.inf, 1e39, 1e-50, True, "1", None, (1.0,))]
-    bad += [dict(rainbow_only=1), dict(rainbow_only=True), dict(munchausen=(0.9, 0.03, -1.0)), dict(fqf=(2.5e-9, 0.0)),
-            dict(mmd=(1.0,)), dict(cql=1.0)]
-    for kw in bad:
-        kw = dict(dict(dqfd=1, margin=0.8, lam=1.0), **kw)
-        with pytest.raises(ValueError):
-            check_dqfd(**kw)
-
-
-def test_check_demo_replay():
-    from rainbow_iqn_apex_b200.dqfd import DEMO_DEFAULTS, check_demo_replay
-    assert DEMO_DEFAULTS == {"demo_segments": 0, "demo_priority_bonus": 0.0}
-    for nb in (1, 2, 7):
-        for d in range(nb + 1):
-            assert check_demo_replay(d, 0.0, nb) == (d, 0.0)
-            assert check_demo_replay(np.int64(d), np.float32(1e-3), nb) == (d, float(F32(1e-3)))
-        for d in (-1, nb + 1, 1.0, 0.5, True, "1", None):
-            with pytest.raises(ValueError):
-                check_demo_replay(d, 0.0, nb)
-    assert check_demo_replay(1, 3e38, 1)[1] == float(F32(3e38)) and check_demo_replay(1, 1e-50, 1)[1] == 0.0
-    for v in (-1e-3, -1.0, math.nan, math.inf, -math.inf, 1e39, True, "1", None, (1.0,)):
-        with pytest.raises(ValueError):
-            check_demo_replay(1, v, 2)
-
-
 # ------------------------------------------------------------------------------------------------ kernels (GPU)
 # (B, A, N, N'): the CQL kernel tests' shapes
 KERNEL_SHAPES = [(1, 1, 1, 1), (7, 4, 8, 5), (32, 18, 64, 64), (512, 18, 64, 64), (4096, 4, 32, 32), (32, 32, 200, 200),

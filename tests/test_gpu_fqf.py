@@ -89,22 +89,6 @@ def test_torch_fp32_fractions_agree_with_float64():
     assert rel_err(H.numpy(), fr["entropy"]) < 1e-6
 
 
-def test_check_fqf():
-    from rainbow_iqn_apex_b200.fqf import check_fqf
-    assert check_fqf(0) is None and check_fqf(False) is None and check_fqf(0, -1.0, -1.0, rainbow_only=True) is None
-    assert check_fqf(1) == (2.5e-9, 0.0)
-    assert check_fqf(np.int64(1), np.float32(1e-4), 1, num_tau_samples=256) == (float(np.float32(1e-4)), 1.0)
-    bad = [dict(fqf=2), dict(fqf=0.5), dict(fqf="1"), dict(fqf=None), dict(fraction_lr=0.0), dict(fraction_lr=-1e-9),
-           dict(fraction_lr=1e-50), dict(fraction_lr=math.nan), dict(fraction_lr=math.inf), dict(fraction_lr=1e39),
-           dict(fraction_lr=True), dict(fraction_lr="1e-9"), dict(entropy_coef=-0.1), dict(entropy_coef=math.nan),
-           dict(entropy_coef=math.inf), dict(entropy_coef=None), dict(rainbow_only=True), dict(munchausen=(0.9, 0.03, -1.0)),
-           dict(risk=("cvar", 0.25)), dict(num_tau_samples=1), dict(num_tau_samples=257), dict(num_tau_samples=8.0)]
-    for kw in bad:
-        kw = dict(dict(fqf=1), **kw)
-        with pytest.raises(ValueError):
-            check_fqf(**kw)
-
-
 def test_dqn_layout_is_unchanged_under_fqf():
     """The DQN's state_dict keys, parameter order and census do not see the fraction proposal, which has its own arena."""
     from rainbow_iqn_apex_b200.fqf import FractionProposal

@@ -137,27 +137,6 @@ def test_float64_and_torch_fp32_statements_agree(eps):
     assert np.max(np.abs(loss.numpy() - l64) / l64) < 1e-6
 
 
-def test_check_hl_gauss():
-    from rainbow_iqn_apex_b200.hl_gauss import HL_GAUSS_DEFAULTS, check_hl_gauss
-    assert HL_GAUSS_DEFAULTS == {"hl_gauss_sigma": 0.75}
-    assert check_hl_gauss(0) is None and check_hl_gauss(False) is None and check_hl_gauss(0, "x") is None
-    assert check_hl_gauss(1, rainbow_only=1) == 0.75 and check_hl_gauss(True, 2, rainbow_only=True) == 2.0
-    assert check_hl_gauss(np.int64(1), np.float32(0.1), rainbow_only=1) == float(np.float32(0.1))
-    assert check_hl_gauss(1, 0.1, rainbow_only=1) == float(np.float32(0.1))
-    assert check_hl_gauss(1, 1000, rainbow_only=1) == 1000.0 and check_hl_gauss(1, 1e-40, rainbow_only=1) > 0
-    assert check_hl_gauss(1, 1000.00001, rainbow_only=1) == 1000.0          # 1000 as a float32
-    bad = [dict(hl_gauss=2), dict(hl_gauss=-1), dict(hl_gauss=0.5), dict(hl_gauss=1.0), dict(hl_gauss="1"),
-           dict(hl_gauss=None), dict(sigma=0.0), dict(sigma=-0.75), dict(sigma=math.nan), dict(sigma=math.inf),
-           dict(sigma=-math.inf), dict(sigma=1000.001), dict(sigma=1e39), dict(sigma=1e-50), dict(sigma=True),
-           dict(sigma="0.75"), dict(sigma=None), dict(sigma=(0.75,)), dict(rainbow_only=0), dict(rainbow_only=False)]
-    for kw in bad:
-        kw = dict(dict(hl_gauss=1, sigma=0.75, rainbow_only=1), **kw)
-        with pytest.raises(ValueError):
-            check_hl_gauss(**kw)
-    with pytest.raises(ValueError, match="rainbow_only"):
-        check_hl_gauss(1, 0.75)
-
-
 # ------------------------------------------------------------------------------------------------ kernels (GPU)
 KERNEL_CASES = [(1, 1, 2, -10.0, 10.0), (7, 4, 21, -3.0, 40.0), (32, 18, 51, -10.0, 10.0), (512, 32, 64, -3.0, 40.0),
                 (4096, 18, 51, -10.0, 10.0), (32, 1, 64, -10.0, 10.0), (512, 4, 21, -10.0, 10.0), (7, 32, 2, -3.0, 40.0)]

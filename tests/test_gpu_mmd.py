@@ -116,28 +116,6 @@ def test_float64_and_torch_fp32_statements_agree(eps):
     assert np.max(np.abs(th.grad.numpy() - g)) <= 1e-6 * np.max(np.abs(g))
 
 
-def test_check_mmd():
-    from rainbow_iqn_apex_b200.mmd import MMD_DEFAULTS, check_mmd
-    assert MMD_DEFAULTS["mmd_bandwidths"] == BW_DEFAULT
-    assert check_mmd(0) is None and check_mmd(False) is None and check_mmd(0, "x", rainbow_only=True) is None
-    assert check_mmd(1, qr_dqn=64) == BW_DEFAULT
-    assert check_mmd(True, [2, 0.5], qr_dqn=8) == (2.0, 0.5) and check_mmd(np.int64(1), np.float32([3]), qr_dqn=2) == (3.0,)
-    assert check_mmd(1, BW_WIDE, qr_dqn=200) == BW_WIDE
-    bad = [dict(mmd=2), dict(mmd=-1), dict(mmd=0.5), dict(mmd=1.0), dict(mmd="1"), dict(mmd=None),
-           dict(bandwidths="1,2"), dict(bandwidths=b"12"), dict(bandwidths=3.0), dict(bandwidths=None),
-           dict(bandwidths=(1.0, True)), dict(bandwidths=(False,)), dict(bandwidths=(1.0, float("nan"))),
-           dict(bandwidths=(float("inf"),)), dict(bandwidths=(-float("inf"),)), dict(bandwidths=(0.0,)),
-           dict(bandwidths=(1.0, -2.0)), dict(bandwidths=(1e-50,)), dict(bandwidths=(1e-39,)), dict(bandwidths=(1e39,)),
-           dict(bandwidths=("1",)), dict(bandwidths=(1.0,) * 17), dict(bandwidths=()), dict(bandwidths=[]),
-           dict(qr_dqn=None), dict(rainbow_only=1), dict(munchausen=(0.9, 0.03, -1.0)), dict(fqf=(2.5e-9, 0.0)),
-           dict(risk=("cvar", 0.25))]
-    for kw in bad:
-        kw = dict(dict(mmd=1, bandwidths=BW_DEFAULT, qr_dqn=64), **kw)
-        with pytest.raises(ValueError):
-            check_mmd(**kw)
-    assert check_mmd(1, (1.0,) * 16, qr_dqn=2) == (1.0,) * 16
-
-
 # ------------------------------------------------------------------------------------------------ kernels (GPU)
 KERNEL_CASES = [(1, 1, 2, BW_DEFAULT), (5, 4, 7, (1.0,)), (33, 32, 64, BW_WIDE), (512, 18, 200, BW_DEFAULT),
                 (64, 18, 256, BW_DEFAULT), (4096, 4, 7, BW_DEFAULT), (7, 1, 256, BW_WIDE), (100, 32, 2, BW_WIDE),

@@ -86,23 +86,6 @@ def test_torch_oracle_agrees_with_float64(spread):
     assert rel_err(b32.numpy(), b64) < 1e-6 and np.all(np.isfinite(t32.numpy()))
 
 
-def test_check_munchausen():
-    from rainbow_iqn_apex_b200.compute_loss_iqn import check_munchausen
-    assert check_munchausen(0) is None and check_munchausen(False) is None and check_munchausen(0, -1.0, 0.0, 1.0) is None
-    assert check_munchausen(1) == (0.9, 0.03, -1.0)
-    assert check_munchausen(True, np.float32(0.5), 1, 0) == (0.5, 1.0, 0.0)
-    assert check_munchausen(np.int64(1), 0.0, 1e-6, -0.0) == (0.0, 1e-6, -0.0)
-    bad = [dict(munchausen=2), dict(munchausen=0.5), dict(munchausen="1"), dict(munchausen=None),
-           dict(alpha=-0.1), dict(alpha=math.nan), dict(alpha=math.inf), dict(alpha=1e39), dict(alpha=True),
-           dict(alpha="0.9"), dict(entropy_tau=0.0), dict(entropy_tau=-0.03), dict(entropy_tau=1e-50),
-           dict(entropy_tau=math.nan), dict(entropy_tau=math.inf), dict(l0=0.1), dict(l0=math.nan), dict(l0=-math.inf),
-           dict(l0=None), dict(rainbow_only=True), dict(risk=("cvar", 0.25))]
-    for kw in bad:
-        kw = dict(dict(munchausen=1, **DEFAULTS), **kw)
-        with pytest.raises(ValueError):
-            check_munchausen(**kw)
-
-
 # ------------------------------------------------------------------------------------------------ kernel (GPU)
 def _kernel(c, B, N, Np, A, g, kappa, alpha, entropy_tau, l0, outs=None):
     from rainbow_iqn_apex_b200._lib import call, ptr

@@ -116,20 +116,6 @@ def test_float64_and_torch_fp32_statements_agree(eps):
     assert rel_err(loss.numpy(), oq.loss_np(keep["theta"].numpy(), tgt)) < 1e-6
 
 
-def test_check_qr():
-    from rainbow_iqn_apex_b200.qr import check_qr
-    assert check_qr(0) is None and check_qr(False) is None and check_qr(0, 1, 99, rainbow_only=True) is None
-    assert check_qr(1, 64, 18) == 64 and check_qr(np.int64(1), np.int32(2), 32) == 2 and check_qr(True, 256, 1) == 256
-    bad = [dict(qr_dqn=2), dict(qr_dqn=0.5), dict(qr_dqn=1.0), dict(qr_dqn="1"), dict(qr_dqn=None),
-           dict(num_tau_samples=1), dict(num_tau_samples=257), dict(num_tau_samples=64.0), dict(num_tau_samples=True),
-           dict(num_tau_samples=None), dict(action_space=33), dict(action_space=0), dict(rainbow_only=1),
-           dict(munchausen=(0.9, 0.03, -1.0)), dict(fqf=(2.5e-9, 0.0)), dict(risk=("cvar", 0.25))]
-    for kw in bad:
-        kw = dict(dict(qr_dqn=1, num_tau_samples=64, action_space=18), **kw)
-        with pytest.raises(ValueError):
-            check_qr(**kw)
-
-
 @pytest.mark.parametrize("n", [64, 200])
 def test_qr_state_dict_layout(n):
     """Host logic on CPU tensors only: the C51 layer set with z-layer widths N and A*N, the C51 parameter order, the

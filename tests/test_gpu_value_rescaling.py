@@ -83,21 +83,6 @@ def test_target_map_is_monotone(eps):
     assert np.array_equal(t1, t2)
 
 
-def test_check_value_rescaling():
-    from rainbow_iqn_apex_b200.compute_loss_iqn import check_value_rescaling
-    assert check_value_rescaling(0) is None and check_value_rescaling(False) is None
-    assert check_value_rescaling(0, -1.0, munchausen=(0.9, 0.03, -1.0)) is None
-    assert check_value_rescaling(1) == 1e-3 and check_value_rescaling(True, 0) == 0.0
-    assert check_value_rescaling(np.int64(1), np.float32(0.01)) == float(np.float32(0.01))
-    bad = [dict(value_rescaling=2), dict(value_rescaling=0.5), dict(value_rescaling="1"), dict(value_rescaling=None),
-           dict(eps=-1e-3), dict(eps=math.nan), dict(eps=math.inf), dict(eps=-math.inf), dict(eps=1e39), dict(eps=True),
-           dict(eps="0.001"), dict(eps=None), dict(munchausen=(0.9, 0.03, -1.0))]
-    for kw in bad:
-        kw = dict(dict(value_rescaling=1), **kw)
-        with pytest.raises(ValueError):
-            check_value_rescaling(**kw)
-
-
 # The existing instantiations of the two loss kernels compile to the SASS they had before the rescaled instantiations
 # were added: normalized `cuobjdump -sass` (symbol names and column alignment aside), CUDA 12.9, sm_90a.
 SASS_DIGESTS = {"iqn_loss_kernel": "51ff206e68935cde47f787404dacf0220602e77c4ef41e242d2676b58a226b59",
