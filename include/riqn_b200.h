@@ -675,6 +675,18 @@ int riqn_frame_gather(int batch, int actor_capacity, int history, int n_step, co
                       const unsigned char* s_frames, const int* s_timestep, const int* s_action, const float* s_reward,
                       const unsigned char* s_nonterminal, const double* gamma_pow, unsigned char* window,
                       long long* actions, float* returns, float* nonterminals, void* stream);
+/* SPR's K-step sequence (Schwarzer et al., ICLR 2021): window (batch, history+K, 84, 84) uint8 with the slots and blank
+ * frames of riqn_frame_gather at n_step = K (so window[:, :history] is its states, bit for bit), actions (batch, K) int64
+ * a_t .. a_{t+K-1} as stored (actions[:, 0] is riqn_frame_gather's), and valid (batch, K) uint8: valid[b, k-1] = 1 iff
+ * the last frame of s_{t+k} (window index history-1+k) is not blank and, with p the sampled position in its segment and
+ * h = index_actor[segment] (read on the device), the distance (h - p) mod actor_capacity is not in 1..k (the walk
+ * p+1 .. p+k never reaches the write head, past which lie an older episode or unwritten slots).  Returns
+ * cudaErrorInvalidValue, writing nothing, for batch, actor_capacity, history or K < 1, history + K > 16, or a NULL
+ * pointer. */
+int riqn_sequence_gather(int batch, int actor_capacity, int history, int K, const long long* data_idx,
+                         const long long* index_actor, const unsigned char* s_frames, const int* s_timestep,
+                         const int* s_action, const unsigned char* s_nonterminal, unsigned char* window,
+                         long long* actions, unsigned char* valid, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Tensor-core building blocks of the NoisyLinear products (wgmma + TMA; csrc/gemm_tc.cu).
@@ -763,6 +775,43 @@ int riqn_colsum_add(long rows, int cols, const float* x, float* out, void* strea
 int riqn_ema_f32(long n, const float* theta, float* xi, float tau, void* stream);
 /* out[i] = fl(a[i] + b[i]) (out may alias a or b).  n >= 1 and non-NULL pointers, else cudaErrorInvalidValue. */
 int riqn_add_f32(long n, const float* a, const float* b, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * SPR (Schwarzer et al., ICLR 2021; no counterpart in the reference): the transition model on the (B, 64, 7, 7) latent
+ * runs on riqn_conv_fwd_strip / riqn_conv_bwd_strip with conv3's geometry (3x3, stride 1, pad 0, H = W = 9) over the
+ * zero-bordered latent.
+ * ---------------------------------------------------------------------------------------------- */
+/* The A operand of that strip convolution: hi / lo (batch*81, channels) bf16 (lo = bf16(x - hi)), row (b, gy, gx) of
+ * the 9x9 grid, column c: latent[b, c, gy-1, gx-1] for c < 64 inside the border; with channels = 128, also the one-hot
+ * action planes, 1 at c = 64 + actions[b * action_stride] for 64 <= c < 64 + num_actions inside the border; 0 elsewhere
+ * (an action outside 0..num_actions-1 sets no plane).  channels = 64 takes actions == NULL; channels = 128 a non-NULL
+ * actions, 1 <= num_actions <= 64 and action_stride >= 1.  Otherwise cudaErrorInvalidValue with nothing written. */
+int riqn_spr_pack(int batch, int channels, const float* latent, const long long* actions, int action_stride,
+                  int num_actions, void* hi, void* lo, void* stream);
+/* Adjoint of riqn_spr_pack's latent part: out (batch, 64, 7, 7) = fl(acc + din[:, :64, 1:8, 1:8]) element by element, or
+ * the crop alone when acc is NULL; din (batch, channels, 9, 9) fp32 is riqn_conv_bwd_strip's data gradient.  out may
+ * alias acc.  channels 64 or 128, non-NULL din / out, else cudaErrorInvalidValue. */
+int riqn_spr_unpack_grad(int batch, int channels, const float* din, const float* acc, float* out, void* stream);
+/* bf16 images of a 3x3 convolution weight w (cout, cin, 3, 3) fp32 zero-padded to cpad input channels: hi / lo
+ * (cout, 9*cpad) in strip order, column (dy*3 + dx)*cpad + c (riqn_conv_fwd_strip's w_hi / w_lo), and hi_orig
+ * (cout, cpad*9) in the original order c*9 + dy*3 + dx (riqn_conv_bwd_strip's w_hi).  1 <= cout <= 64,
+ * 1 <= cin <= cpad, cpad % 64 == 0 and non-NULL pointers, else cudaErrorInvalidValue. */
+int riqn_spr_weight_images(int cout, int cin, int cpad, const float* w, void* hi, void* lo, void* hi_orig, void* stream);
+/* gw[o, c, s] = fl(gw[o, c, s] + gpad[o, c, s]) for c < cin: a padded weight gradient (cout, cpad, 9) into the
+ * unpadded one (cout, cin, 9).  cout, cin >= 1, cin <= cpad, non-NULL pointers, else cudaErrorInvalidValue. */
+int riqn_spr_weight_grad_add(int cout, int cin, int cpad, const float* gpad, float* gw, void* stream);
+/* Masked negative cosine of predictions p = pred[k*rows + b] against targets t = target[k*rows + b] ((K, rows, dim)
+ * fp32), its loss per sample and its gradient with respect to the predictions.  With s = fl(coef / rows), v =
+ * valid[b*K + k] ((rows, K) uint8) and lanes l holding elements l + 32j (j = 0..3):
+ *   P = sum p*p, T = sum t*t, Q = sum p*t       (lane chains of fl(fl(a*b) + acc) over j, then the warp_sum butterfly)
+ *   |p| = sqrtf(P) ; np = max(|p|, 1e-12) ; nt = max(sqrtf(T), 1e-12) ; cos = fl(Q / fl(np * nt))
+ *   loss_rows[b] = sum_k (v ? -cos : 0)          (k ascending; the loss is s * sum_b loss_rows[b])
+ *   dpred = fl((v ? -s : 0) * fl(g / np)),  g = fl(fl(t / nt) - fl(cos * fl(p / np))) when |p| > 1e-12, else fl(t / nt)
+ * i.e. the gradient of -s v cos(F.normalize(p), F.normalize(t)) with eps 1e-12 on both norms.  One CTA per sample, no
+ * atomics.  dim must be 128, 1 <= K <= 12, 1 <= rows <= 4096, coef finite, the pointers non-NULL; otherwise
+ * cudaErrorInvalidValue and nothing is written. */
+int riqn_spr_cosine_fwd_bwd(int rows, int K, int dim, const float* pred, const float* target, const unsigned char* valid,
+                            float coef, float* loss_rows, float* dpred, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Test hook: plain strided fp32 product C[m,n] = sum_k A[m*sAm + k*sAk] * B[n*sBn + k*sBk].

@@ -90,6 +90,12 @@ SIGNATURES = {
     "riqn_colsum_add": [C.c_long, C.c_int, _P, _P, _P],
     "riqn_ema_f32": [C.c_long, _P, _P, C.c_float, _P],
     "riqn_add_f32": [C.c_long, _P, _P, _P, _P],
+    "riqn_spr_pack": [C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P],
+    "riqn_spr_unpack_grad": [C.c_int, C.c_int, _P, _P, _P, _P],
+    "riqn_spr_weight_images": [C.c_int] * 3 + [_P] * 5,
+    "riqn_spr_weight_grad_add": [C.c_int] * 3 + [_P] * 3,
+    "riqn_spr_cosine_fwd_bwd": [C.c_int] * 3 + [_P] * 3 + [C.c_float, _P, _P, _P],
+    "riqn_sequence_gather": [C.c_int] * 4 + [_P] * 10,
     "riqn_argmax_weighted": [C.c_int] * 3 + [_P] * 4,
     "riqn_c51_head_fwd":[C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,

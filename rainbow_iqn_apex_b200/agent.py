@@ -12,16 +12,17 @@ qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-se
 regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's large-margin loss on demonstrations (dqfd.py),
 ``random_shift`` for the
 learner's random-shift augmentation (augment.py), and ``curl`` / ``curl_net`` / ``curl_optimiser`` / ``momentum_net`` /
-``momentum_projection`` for CURL's contrastive loss on the trunk (curl.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
+``momentum_projection`` for CURL's contrastive loss on the trunk (curl.py), and ``spr`` / ``spr_net`` /
+``spr_optimiser`` for SPR's self-predictive loss on the trunk (spr.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
 optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
-optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF and CURL's three.
+optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF, CURL's three and SPR's two.
 """
 import os
 
 import torch
 
 from . import _lib
-from . import c51, compute_loss_iqn, config, curl, fqf, qr
+from . import c51, compute_loss_iqn, config, curl, fqf, qr, spr
 from .model import DQN
 from .optim import Adam
 
@@ -108,6 +109,9 @@ class Agent:
         self.curl_net = self.curl_optimiser = self.momentum_net = self.momentum_projection = None
         if self.curl is not None:
             curl.build(self, args, checkpoint)
+        self.spr_net = self.spr_optimiser = None       # SPR's too (never with CURL)
+        if self.spr is not None:
+            spr.build(self, args, checkpoint)
 
     def set_risk(self, measure, eta=None):
         """Act, and pick the double-DQN target action a*, under a distortion risk measure (IQN paper, section 3.1):
@@ -141,7 +145,7 @@ class Agent:
         """agent.py:72-147: the loss (B,) of self.loss_core, differentiable with respect to the online network (and,
         under FQF, the fraction proposal) when grad mode is on.  ``debug``: dict that receives the core's intermediates.
         ``demo``: None, or the (B,) demonstration flags of a DQfD agent (dqfd.py).  CURL's auxiliary loss is not part of
-        it: only Learner.compute_gradients adds that term."""
+        it, nor SPR's: only Learner.compute_gradients adds those terms."""
         if torch.is_grad_enabled():
             params = [p for p in self.online_net.parameters() if p.requires_grad]
             return _Loss.apply(self, states, actions, returns, next_states, nonterminals, debug, demo, *params)
@@ -152,7 +156,8 @@ class Agent:
     def save(self, path, T_actors, T_learner, name):
         """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
         fraction_optimiser_state_dict, under value rescaling value_rescaling_eps, under QR-DQN qr_dqn_quantiles (N), under CURL
-        curl_state_dict, curl_optimiser_state_dict and curl_momentum_state_dict; model_state_dict keeps the reference schema either way."""
+        curl_state_dict, curl_optimiser_state_dict and curl_momentum_state_dict, under SPR spr_state_dict and
+        spr_optimiser_state_dict; model_state_dict keeps the reference schema either way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
@@ -170,6 +175,9 @@ class Agent:
             ckpt["curl_state_dict"] = self.curl_net.state_dict()
             ckpt["curl_optimiser_state_dict"] = self.curl_optimiser.state_dict()
             ckpt["curl_momentum_state_dict"] = curl.momentum_state_dict(self)
+        if self.spr is not None:
+            ckpt["spr_state_dict"] = self.spr_net.state_dict()
+            ckpt["spr_optimiser_state_dict"] = self.spr_optimiser.state_dict()
         torch.save(ckpt, os.path.join(path, name))
 
     def train(self):

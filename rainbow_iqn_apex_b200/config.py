@@ -16,7 +16,9 @@ MAX_N = 256                # QR-DQN's quantiles and FQF's fractions (num_tau_sam
 MAX_ACTIONS = 32           # QR-DQN: riqn_argmax_mean / riqn_argmax_expected_h
 MAX_BANDWIDTHS = 16        # riqn_mmd_loss_fwd_bwd
 MAX_SIGMA_RATIO = 1000.0   # riqn_hl_gauss_loss_fwd_bwd
-MAX_BATCH = 4096           # riqn_curl_infonce_fwd_bwd
+MAX_BATCH = 4096           # riqn_curl_infonce_fwd_bwd, riqn_spr_cosine_fwd_bwd
+MAX_SPR_STEPS = 12         # riqn_spr_cosine_fwd_bwd; riqn_sequence_gather's history + K <= 16 at history 4
+MAX_SPR_ACTIONS = 64       # riqn_spr_pack: the one-hot planes share conv1's 128 input channels with the latent's 64
 _LOG2E = 1.4426950408889634
 
 
@@ -96,6 +98,9 @@ FIELDS = {
     "curl": (0, switch),
     "curl_coef": (1.0, real(lambda x: x > 0.0, "> 0")),           # this project's starting point, not tuned
     "curl_momentum": (0.001, real(lambda x: 0.0 < x <= 1.0, "in (0, 1]")),
+    "spr": (0, switch),
+    "spr_steps": (5, integer(1, MAX_SPR_STEPS)),                  # the paper's Atari K and lambda
+    "spr_coef": (2.0, real(lambda x: x > 0.0, "> 0")),
     "demo_segments": (0, integer(0, math.inf)),                   # at most nb_actor (read_demo)
     "demo_priority_bonus": (0.0, real(lambda x: x >= 0.0, ">= 0")),
 }
@@ -147,12 +152,12 @@ def read_risk(head, loss, measure, eta=None):
 
 def read(args, action_space):
     """Validate the optional fields of ``args`` and return what the agent stores, as a dict: qr_dqn (N or None); per
-    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl) None when off, else its parameter
+    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr) None when off, else its parameter
     or the tuple of its parameters; random_shift (the pad, or None); risk (model.check_risk's); and the "head" and the
     "loss" variant (or None) they select."""
     head, n = read_head(args, action_space)
     v = {"qr_dqn": n}
-    for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl"):
+    for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl", "spr"):
         v[name] = None
         if field(args, name):
             params = tuple(field(args, f) for f in FIELDS if f.startswith(name + "_"))
@@ -174,6 +179,18 @@ def read(args, action_space):
         if v["random_shift"] is None:
             raise ValueError("curl = 1 contrasts two random shifts of each state: set random_shift >= 1 (DrQ uses 4)")
         integer(2, MAX_BATCH)("batch_size", args.batch_size)      # CURL's negatives are the batch's other states
+    if v["spr"] is not None:
+        if v["curl"] is not None:
+            raise ValueError("spr and curl are both auxiliary losses on the trunk's feature gradient, of which one at most "
+                             "can be on")
+        if not 1 <= action_space <= MAX_SPR_ACTIONS:
+            raise ValueError(f"spr supports 1..{MAX_SPR_ACTIONS} actions (its transition model's one-hot action planes), "
+                             f"got {action_space!r}")
+        integer(1, MAX_BATCH)("batch_size", args.batch_size)
+        history = getattr(args, "history_length", 4)
+        if history + v["spr"][0] > 16:
+            raise ValueError(f"spr_steps + history_length must be at most 16 (the sequence window), got "
+                             f"{v['spr'][0]} + {history}")
     v["risk"] = read_risk(head, loss, getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
     return dict(v, head=head, loss=loss)
 

@@ -437,6 +437,51 @@ __global__ void frame_gather_kernel(int B, int actor_cap, int history, int n_ste
   }
 }
 
+// SPR's multi-step window: frame_gather_kernel's slots and blanking over history + K frames (no return), the K logged
+// actions a_t .. a_{t+K-1}, and valid[b, k-1] for the step to s_{t+k}: its last frame is not blank and the walk
+// p+1 .. p+k from the sampled ring position p does not reach the write head (past it lie older or unwritten slots).
+__global__ void sequence_gather_kernel(int B, int actor_cap, int history, int K, const int64_t* __restrict__ data_idx,
+                                       const int64_t* __restrict__ index_actor, const uint8_t* __restrict__ s_frames,
+                                       const int32_t* __restrict__ s_timestep, const int32_t* __restrict__ s_action,
+                                       const uint8_t* __restrict__ s_nonterminal, uint8_t* __restrict__ window,
+                                       int64_t* __restrict__ actions, uint8_t* __restrict__ valid) {
+  const int b = blockIdx.x;
+  const int L = history + K;
+  __shared__ long slots[16];
+  __shared__ int blank[16];
+  if (threadIdx.x == 0) {
+    const long d = data_idx[b];
+    const long actor = d / actor_cap;
+    int ts[16], nt[16];
+    for (int k = 0; k < L; ++k) {
+      long pos = (k + d - history + 1) % actor_cap;
+      if (pos < 0) pos += actor_cap;
+      slots[k] = pos + actor * actor_cap;
+      ts[k] = s_timestep[slots[k]];
+      nt[k] = s_nonterminal[slots[k]];
+      blank[k] = 0;
+    }
+    for (int t = history - 2; t >= 0; --t)
+      if (ts[t + 1] == 0) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
+    for (int t = history; t < L; ++t)
+      if (!nt[t - 1]) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
+    long head = (index_actor[actor] - d % actor_cap) % actor_cap;       // distance from p to the write head
+    if (head < 0) head += actor_cap;
+    for (int k = 0; k < K; ++k) {
+      actions[(long)b * K + k] = s_action[slots[history - 1 + k]];
+      valid[(long)b * K + k] = (!blank[history + k] && !(head >= 1 && head <= k + 1)) ? 1 : 0;
+    }
+  }
+  __syncthreads();
+  constexpr int V = FRAME_BYTES / 16;
+  for (int t = threadIdx.x; t < L * V; t += blockDim.x) {
+    const int k = t / V, o = t % V;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (!blank[k]) v = reinterpret_cast<const uint4*>(s_frames + slots[k] * FRAME_BYTES)[o];
+    reinterpret_cast<uint4*>(window + ((long)b * L + k) * FRAME_BYTES)[o] = v;
+  }
+}
+
 }  // namespace riqn
 
 using namespace riqn;
@@ -535,5 +580,19 @@ RIQN_API int riqn_frame_gather(int batch, int actor_capacity, int history, int n
                                                                (const int64_t*)data_idx, s_frames, s_timestep, s_action,
                                                                s_reward, s_nonterminal, gamma_pow, window,
                                                                (int64_t*)actions, returns, nonterminals);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_sequence_gather(int batch, int actor_capacity, int history, int K, const long long* data_idx,
+                                  const long long* index_actor, const unsigned char* s_frames, const int* s_timestep,
+                                  const int* s_action, const unsigned char* s_nonterminal, unsigned char* window,
+                                  long long* actions, unsigned char* valid, void* stream) {
+  if (batch < 1 || actor_capacity < 1 || history < 1 || K < 1 || history + K > 16 || !data_idx || !index_actor ||
+      !s_frames || !s_timestep || !s_action || !s_nonterminal || !window || !actions || !valid)
+    return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  sequence_gather_kernel<<<batch, 256, 0, (cudaStream_t)stream>>>(
+      batch, actor_capacity, history, K, (const int64_t*)data_idx, (const int64_t*)index_actor, s_frames, s_timestep,
+      s_action, s_nonterminal, window, (int64_t*)actions, valid);
   return (int)cudaGetLastError();
 }

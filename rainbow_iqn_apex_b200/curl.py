@@ -41,33 +41,25 @@ HIDDEN, DIM = 512, 128                                         # projection widt
 CURL_SHIFT_SEED = 0xC0A1                                       # the positive view's draw key (net._rng_seed ^ this)
 
 
-class CurlProjection(nn.Module):
-    """The online projection g_theta and the bilinear W, views of one flat fp32 arena (``_flat``; gradients in
-    ``_flat_grad``) laid out weight_h (512, 3136) | bias_h | weight_c (128, 512) | bias_c | bilinear (128, 128), each
-    group on a 256-byte boundary; the projection is the prefix [0, proj_numel).  Initialised like nn.Linear (uniform in
-    +-1/sqrt(fan_in)), W like a bias-free nn.Linear(128, 128)."""
+class ArenaModule(nn.Module):
+    """Parameters ``NAMES`` (dotted names allowed) as views of one flat fp32 arena (``_flat``; gradients in
+    ``_flat_grad``), each group on a 256-byte boundary, in NAMES order.  The first four are a projection (weight_h,
+    bias_h, weight_c, bias_c), the prefix [0, proj_numel)."""
 
-    NAMES = ("weight_h", "bias_h", "weight_c", "bias_c", "bilinear")
-
-    def __init__(self, device):
-        super().__init__()
-        h, c, w = nn.Linear(FEAT, HIDDEN), nn.Linear(HIDDEN, DIM), nn.Linear(DIM, DIM, bias=False)
-        for name, t in zip(self.NAMES, (h.weight, h.bias, c.weight, c.bias, w.weight)):
-            setattr(self, name, nn.Parameter(t.detach().clone()))
-        self._flatten(torch.device(device))
+    NAMES = ()
 
     def _flatten(self, dev):
         total, self._offs = 0, {}
         for name in self.NAMES:
             total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
             self._offs[name] = total
-            total += getattr(self, name).numel()
-        self.proj_numel = self._offs["bilinear"]
+            total += self.get_parameter(name).numel()
+        self.proj_numel = self._offs[self.NAMES[4]]
         total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
         flat = torch.zeros(total, device=dev, dtype=torch.float32)
         flat_grad = torch.zeros(total, device=dev, dtype=torch.float32)
         for name in self.NAMES:
-            p, off = getattr(self, name), self._offs[name]
+            p, off = self.get_parameter(name), self._offs[name]
             n = p.numel()
             flat[off:off + n].copy_(p.data.reshape(-1).float())
             p.data = flat[off:off + n].view(p.shape)
@@ -78,7 +70,7 @@ class CurlProjection(nn.Module):
 
     def _apply(self, fn, *a, **k):
         out = super()._apply(fn, *a, **k)
-        self._flatten(self.weight_h.device)
+        self._flatten(self.get_parameter(self.NAMES[0]).device)
         return out
 
     def _params_changed(self):
@@ -91,17 +83,32 @@ class CurlProjection(nn.Module):
         """One memset over the gradient arena; the .grad views stay bound."""
         call("riqn_zero_f32", ptr(self._flat_grad), self._flat_grad.numel())
         for name in self.NAMES:
-            p = getattr(self, name)
+            p = self.get_parameter(name)
             p.grad = self.grad_view(p)
 
     def views(self, arena):
-        """(weight_h, bias_h, weight_c, bias_c) of the projection laid out in ``arena`` (this arena, or the momentum
-        copy's projection prefix)."""
+        """(weight_h, bias_h, weight_c, bias_c) of the projection laid out in ``arena`` (this arena, or a copy of its
+        projection prefix)."""
         out = []
         for name in self.NAMES[:4]:
-            p, off = getattr(self, name), self._offs[name]
+            p, off = self.get_parameter(name), self._offs[name]
             out.append(arena[off:off + p.numel()].view(p.shape))
         return tuple(out)
+
+
+class CurlProjection(ArenaModule):
+    """The online projection g_theta and the bilinear W, views of one flat fp32 arena laid out weight_h (512, 3136) |
+    bias_h | weight_c (128, 512) | bias_c | bilinear (128, 128).  Initialised like nn.Linear (uniform in
+    +-1/sqrt(fan_in)), W like a bias-free nn.Linear(128, 128)."""
+
+    NAMES = ("weight_h", "bias_h", "weight_c", "bias_c", "bilinear")
+
+    def __init__(self, device):
+        super().__init__()
+        h, c, w = nn.Linear(FEAT, HIDDEN), nn.Linear(HIDDEN, DIM), nn.Linear(DIM, DIM, bias=False)
+        for name, t in zip(self.NAMES, (h.weight, h.bias, c.weight, c.bias, w.weight)):
+            setattr(self, name, nn.Parameter(t.detach().clone()))
+        self._flatten(torch.device(device))
 
 
 def _tc(B):

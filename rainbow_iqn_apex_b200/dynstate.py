@@ -3,7 +3,8 @@ CUDA graph once and replayed: the host rewrites this 32-byte struct with one asy
 
 An FQF learner keeps a second struct beside the first (``slots=2``), written by the same copy: its Adam fields are the
 fraction optimiser's bias corrections (its own learning rate), its rng_offset repeats the first one's.  A CURL learner
-adds one more for the projection's optimiser, after FQF's when both are on."""
+adds one more for the projection's optimiser, after FQF's when both are on; an SPR learner likewise one for its
+arena's optimiser."""
 import struct
 
 import torch

@@ -12,6 +12,11 @@ from that backward too, and must zero them (fraction_net.zero_grad()) and call f
 Under CURL (curl.py) every step also contrasts the gradient pass's trunk features with a momentum encoder's, zeroes,
 fills, (all-reduces) and steps the projection's arena (agent.curl_net, agent.curl_optimiser), and after the Adam steps
 moves the momentum encoder towards the online trunk and projection.  Each rank contrasts its own local batch.
+
+Under SPR (spr.py) every step also gathers the sampled transitions' K-step sequences (ReplayMemory.sample_sequence),
+predicts their latents through the transition model, zeroes, fills, (all-reduces) and steps SPR's arena (agent.spr_net,
+agent.spr_optimiser).  Each rank predicts its own local batch.  Entry points that receive an already assembled minibatch
+without its sequence (learn_on_batch without ``sequence``, the batch and learn graphs, learn_on_host_batch) refuse.
 """
 import contextlib
 import io
@@ -19,7 +24,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment, curl
+from . import augment, curl, spr
 from .agent import Agent
 from .dynstate import DynState
 
@@ -51,7 +56,7 @@ class Learner(Agent):
         sample = mem_redis.get_sample_from_mp_queue(mp_queue)
         idxs, states, actions, returns, next_states, nonterminals, weights = sample
         loss = self.learn_on_batch(states, actions, returns, next_states, nonterminals, weights,
-                                   demo=self._demo_mask(mem_redis, idxs))
+                                   demo=self._demo_mask(mem_redis, idxs), sequence=self._sequence(mem_redis, idxs))
         return idxs, loss
 
     def _demo_mask(self, mem, idxs):
@@ -59,10 +64,25 @@ class Learner(Agent):
         memory holds no demonstrations); None otherwise."""
         return mem.demo_mask(idxs) if self.dqfd is not None else None
 
-    def learn_on_batch(self, states, actions, returns, next_states, nonterminals, weights, demo=None):
+    def _sequence(self, mem, idxs):
+        """Under SPR, the K-step sequences of the sampled tree indices ``idxs`` (ReplayMemory.sample_sequence); None
+        otherwise."""
+        return mem.sample_sequence(idxs, self.spr[0]) if self.spr is not None else None
+
+    def _refuse_spr(self, what):
+        if self.spr is not None:
+            raise ValueError(f"spr = 1 predicts the K states after each sampled one: {what} receives an assembled "
+                             "minibatch without its sequences; step an SPR learner with learn / learn_and_update (and "
+                             "enable_cuda_graph), or pass learn_on_batch the sequence= of ReplayMemory.sample_sequence")
+
+    def learn_on_batch(self, states, actions, returns, next_states, nonterminals, weights, demo=None, sequence=None):
         """learner.py:18-24 on an already assembled minibatch.  Returns the per-transition loss (B,).  ``demo``: the
-        DQfD demonstration flags (B,), or None."""
-        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights, demo=demo)
+        DQfD demonstration flags (B,), or None.  ``sequence``: under SPR (required there), the minibatch's
+        ReplayMemory.sample_sequence."""
+        if sequence is None:
+            self._refuse_spr("learn_on_batch without sequence=")
+        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights, demo=demo,
+                                      sequence=sequence)
         self.apply_gradients()
         return loss
 
@@ -98,11 +118,12 @@ class Learner(Agent):
 
     def _trained_nets(self):
         """The networks whose gradient arenas a step fills: the online network, under FQF the fraction proposal, under
-        CURL the projection."""
-        return tuple(n for n in (self.online_net, self.fraction_net, self.curl_net) if n is not None)
+        CURL the projection, under SPR its arena."""
+        return tuple(n for n in (self.online_net, self.fraction_net, self.curl_net, self.spr_net) if n is not None)
 
     def _optimisers(self):
-        return tuple(o for o in (self.optimiser, self.fraction_optimiser, self.curl_optimiser) if o is not None)
+        return tuple(o for o in (self.optimiser, self.fraction_optimiser, self.curl_optimiser, self.spr_optimiser)
+                     if o is not None)
 
     def _step_optimisers(self):
         for o in self._optimisers():
@@ -118,17 +139,23 @@ class Learner(Agent):
         capacity, beta = (1.0, 0.0) if mem is None else (mem.transitions.get_current_capacity(), mem.priority_weight)
         self._dyn.write(nss, sbc, capacity, beta, *more)
 
-    def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None, demo=None):
+    def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None, demo=None,
+                          sequence=None):
         """loss -> zero_grad -> backward of (weights*loss).mean()   (learner.py:18-23); gradients land in the arenas.
         ``debug``: dict that receives the loss core's intermediates (self.loss_core), with random_shift the shifts and
-        the shifted frames (_shift_frames), and under CURL curl_shifts, z_a, z_k, logits, curl_loss (the per-row InfoNCE
-        terms, (B,)) and dfeat_curl.  ``demo``: the DQfD demonstration flags (B,) uint8 / bool, or None."""
+        the shifted frames (_shift_frames), under CURL curl_shifts, z_a, z_k, logits, curl_loss (the per-row InfoNCE
+        terms, (B,)) and dfeat_curl, and under SPR spr_shifts, spr_targets, spr_latents, spr_pred, spr_loss (the
+        per-sample sums of the masked negative cosines, (B,)) and dfeat_spr.  ``demo``: the DQfD demonstration flags (B,)
+        uint8 / bool, or None.  ``sequence``: under SPR (required there), ReplayMemory.sample_sequence of the batch."""
         on = self.online_net
+        if sequence is None:
+            self._refuse_spr("compute_gradients without sequence=")
         weights = weights.to(on._flat.device, torch.float32)
         raw_states = states
         if self.random_shift is not None:
             states, next_states = self._shift_frames(states, next_states, debug)
         z_k = curl.positives(self, raw_states, debug) if self.curl is not None else None
+        spr_t = spr.targets(self, sequence[0], debug) if self.spr is not None else None
         loss, bw = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, demo=demo)
         for net in self._trained_nets():                                        # learner.py:22
             net.zero_grad()
@@ -136,6 +163,8 @@ class Learner(Agent):
         on._grads_ready_hook = self._start_tail_allreduce if (self.process_group is not None and self.overlap_allreduce) else None
         if z_k is not None:         # CURL's feature gradient joins the loss core's in the trunk backward
             on._trunk_addend = curl.trunk_addend(self, z_k, debug)
+        if spr_t is not None:       # SPR's likewise
+            on._trunk_addend = spr.trunk_addend(self, sequence, spr_t, debug)
         try:
             bw(weights, 1.0 / weights.shape[0])                                 # learner.py:23 (.mean())
         finally:
@@ -195,7 +224,7 @@ class Learner(Agent):
         def route(dyn):
             self._dyn_on = dyn is not None
             self.optimiser._dyn = dyn
-            for k, o in enumerate(self._optimisers()[1:], 1):     # FQF's fraction optimiser, then CURL's
+            for k, o in enumerate(self._optimisers()[1:], 1):     # FQF's fraction optimiser, then CURL's or SPR's
                 o._dyn = dyn.slot(k) if dyn is not None else None
             if mem is not None:
                 mem.transitions._dyn = dyn
@@ -212,7 +241,7 @@ class Learner(Agent):
         self._reset_step_streams(mem)
         idxs, states, actions, returns, next_states, nonterminals, weights = mem.get_sample_from_mp_queue(None)
         loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights,
-                                      demo=self._demo_mask(mem, idxs))
+                                      demo=self._demo_mask(mem, idxs), sequence=self._sequence(mem, idxs))
         return idxs, loss
 
     def _step_post(self, mem, idxs, loss, allreduce=True):
@@ -292,7 +321,9 @@ class Learner(Agent):
         """Second captured graph for minibatches that arrive from the HOST (the reference's mp-queue hand-off,
         learner.py:16): static device input buffers, filled by async copies from pinned host tensors, then
         learn_on_batch + update_priorities replayed.  ``example`` = (idxs, states, actions, returns, next_states,
-        nonterminals, weights) device tensors defining the shapes.  Requires enable_cuda_graph(mem) first."""
+        nonterminals, weights) device tensors defining the shapes.  Requires enable_cuda_graph(mem) first.  Not under
+        SPR: the host batch carries no sequences."""
+        self._refuse_spr("enable_batch_graph")
         g = self._graphs.get("replay")
         assert g is not None and mem is g.mem
         inputs = tuple(t.clone() for t in example)
@@ -313,6 +344,7 @@ class Learner(Agent):
         if self.dqfd is not None:
             raise RuntimeError("the learn graph takes batches gathered from the actor shards, which carry no demonstration "
                                "flags: a DQfD learner steps from its own replay (enable_cuda_graph / enable_batch_graph)")
+        self._refuse_spr("enable_learn_graph")
         inputs = tuple(t.contiguous().clone() for t in example)
 
         def pre():
@@ -354,6 +386,7 @@ class Learner(Agent):
         """host_batch: pinned host tensors (idxs, states u8, actions, returns, next_states u8, nonterminals, weights),
         or None to consume the batch started by prefetch_host_batch().  H2D copies + one graph replay; returns the
         device loss (B,) (static buffer)."""
+        self._refuse_spr("learn_on_host_batch")
         g = self._graphs["batch"]
         if host_batch is None:
             torch.cuda.current_stream().wait_event(self._pf_event)

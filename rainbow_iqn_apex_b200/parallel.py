@@ -68,6 +68,9 @@ def make_data_parallel(learner, group=None):
         for t in (learner.curl_net._flat, learner.momentum_net._flat, learner.momentum_projection):
             dist.broadcast(t, src=0, group=group)
         learner.curl_optimiser.grad_scale = 1.0 / world
+    if getattr(learner, "spr_net", None) is not None:              # SPR: projection, transition model, predictor
+        dist.broadcast(learner.spr_net._flat, src=0, group=group)
+        learner.spr_optimiser.grad_scale = 1.0 / world
     learner.process_group = group if group is not None else dist.group.WORLD
     learner.optimiser.grad_scale = 1.0 / world
     return learner

@@ -245,6 +245,24 @@ class ReplayMemory:
              ptr(actions), ptr(returns), ptr(nonterminals))
         return window, actions, returns, nonterminals
 
+    def sample_sequence(self, tree_idx, K):
+        """SPR's K-step sequence of the sampled tree indices ``tree_idx`` (data index tree_idx - capacity + 1), as device
+        tensors (riqn_sequence_gather): window (B, history + K, 84, 84) uint8 whose first history frames are the
+        sample's states bit for bit, actions (B, K) int64 a_t .. a_{t+K-1} (actions[:, 0] is the sample's), and valid
+        (B, K) uint8, valid[:, k-1] = 0 where s_{t+k} crosses a terminal or the segment's write head.  The sampler is not
+        changed: steps it did not guarantee are masked, never resampled."""
+        tr = self.transitions
+        if not tr.store_frames:
+            raise RuntimeError("this replay was built with store_frames=False (tree only): nothing to assemble")
+        data_idx = (torch.as_tensor(tree_idx).to(self.device, torch.int64) - (self.capacity - 1)).contiguous()
+        B = data_idx.numel()
+        window = torch.empty(B, self.history + K, 84, 84, dtype=torch.uint8, device=self.device)
+        actions = torch.empty(B, K, dtype=torch.int64, device=self.device)
+        valid = torch.empty(B, K, dtype=torch.uint8, device=self.device)
+        call("riqn_sequence_gather", B, tr.actor_capacity, self.history, K, ptr(data_idx), ptr(tr.index_actor),
+             ptr(tr.frames), ptr(tr.timestep), ptr(tr.action), ptr(tr.nonterminal), ptr(window), ptr(actions), ptr(valid))
+        return window, actions, valid
+
     def sample(self, batch_size, samples=None):
         """Everything Learner.learn needs, as device tensors:
         (tree_idxs, states u8, actions, returns, next_states u8, nonterminals, weights)."""
