@@ -630,16 +630,25 @@ int riqn_adam_step(long n, float* params, const float* grads, float* exp_avg, fl
  * Prioritized replay: sum-tree          replaces RedisSegmentTree / ReplayRedisMemory, redis_memory.py
  * tree: 2*capacity-1 float64 nodes in HBM, leaf of data index d at d + capacity - 1.
  * ---------------------------------------------------------------------------------------------- */
-/* Stratified sample values, one per segment of total/n, shuffled (redis_memory.py:276-287). n <= 12000. */
+/* Stratified sample values, one per segment of total/n, shuffled (redis_memory.py:276-287): value s is
+ * a + (b - a) * u with a = s*seg, b = (s+1)*seg, seg = tree[0] / n, u = (((x << 32 | y) >> 11) + 0.5) * 2^-53 of the words
+ * x, y of Philox draw s at stream_id (+ dyn->rng_offset when dyn != NULL); it goes to output slot rank(key_s), keys =
+ * word x of the draws at stream_id ^ 0x5bd1e995, ties broken by s.  Returns cudaErrorInvalidValue, writing nothing,
+ * unless 1 <= n <= 12000, or for a NULL tree or values. */
 int riqn_sumtree_stratified(int n, unsigned long long seed, unsigned long long stream_id, const double* tree,
                             double* values, const riqn_dyn_state* dyn, void* stream);
 /* Descent (_retrieve_multiple_values :205-229) + transform_to_valid_tree_indexes (:242-264) + priority
- * read (:315-321).  index_actor: per-actor write heads (int64).  Bit-exact with the reference. */
+ * read (:315-321).  index_actor: per-actor write heads (int64).  Bit-exact with the reference.  Returns
+ * cudaErrorInvalidValue, writing nothing, for capacity or actor_capacity < 1, a capacity that is not a multiple of
+ * actor_capacity, history or n_step < 0, or a NULL pointer; n <= 0 does nothing. */
 int riqn_sumtree_sample(int n, long capacity, int actor_capacity, const double* tree, const double* values,
                         const long long* index_actor, int history, int n_step, long long* tree_idx,
                         long long* data_idx, double* priorities, void* stream);
 /* Importance-sampling weights (sample_byte :465-475); n_nonpositive (device int, may be NULL) counts the
- * priorities <= 0 that were replaced by 1/capacity (:446-456). */
+ * priorities <= 0 that were replaced by 1/capacity (:446-456).  With dyn != NULL, dyn->is_capacity and dyn->is_beta
+ * replace current_capacity and priority_weight.  Returns cudaErrorInvalidValue, writing nothing, for n < 1, a NULL
+ * tree, priorities, w64 or w32, or (dyn == NULL) a current_capacity or priority_weight that is not finite and >= 0.
+ * current_capacity 0 gives the reference's NaN weights ((0 * p)^-beta / max). */
 int riqn_sumtree_is_weights(int n, const double* tree, const double* priorities, double current_capacity,
                             double priority_weight, double* w64, float* w32, int* n_nonpositive,
                             const riqn_dyn_state* dyn, void* stream);
@@ -648,14 +657,16 @@ int riqn_sumtree_is_weights(int n, const double* tree, const double* priorities,
  * diff_scratch (n doubles) are outputs/workspace; *max_priority (device double) is raised if needed.
  * n <= 4096.  The tree arithmetic is bit-exact with the reference (including duplicated indices) given the
  * float32 priorities; the power itself is the correctly rounded float32 value, which numpy/libm powf only
- * approximates (<= 1 ulp apart, platform dependent). */
+ * approximates (<= 1 ulp apart, platform dependent).  Returns cudaErrorInvalidValue, writing nothing, for n > 4096,
+ * capacity < 1 or a NULL pointer; n <= 0 does nothing. */
 int riqn_sumtree_update(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
                         float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
                         double* max_priority, void* stream);
 /* riqn_sumtree_update with DQfD's demonstration priority bonus eps_d (Hester et al. 2018): after the power, every entry
  * with tree_idx >= demo_leaf (the leaves of the demonstration segments) takes new = fl(new + bonus).  The diff, the
  * propagation (duplicates included) and max_priority are riqn_sumtree_update's on those priorities.  Returns
- * cudaErrorInvalidValue, writing nothing, unless bonus is finite and >= 0 and demo_leaf >= 0. */
+ * cudaErrorInvalidValue, writing nothing, unless bonus is finite and >= 0 and demo_leaf >= 0, and for the arguments
+ * riqn_sumtree_update refuses. */
 int riqn_sumtree_update_demo(int n, long capacity, double* tree, const long long* tree_idx, const float* loss,
                              float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
                              double* max_priority, long long demo_leaf, float bonus, void* stream);
@@ -663,14 +674,18 @@ int riqn_sumtree_update_demo(int n, long capacity, double* tree, const long long
 /* ------------------------------------------------------------------------------------------------
  * Prioritized replay: frame store            replaces the Redis hashes "transitions<i>" (:184-193)
  * ---------------------------------------------------------------------------------------------- */
-/* Frame half of append_actor_buffer (:159-199): n consecutive transitions of one actor into its ring. */
+/* Frame half of append_actor_buffer (:159-199): n consecutive transitions of one actor into its ring, slot
+ * (start + i) % actor_capacity + id_actor * actor_capacity.  Returns cudaErrorInvalidValue, writing nothing, for
+ * actor_capacity < 1, id_actor < 0, start outside [0, actor_capacity), n > actor_capacity (a slot written twice in one
+ * launch) or a NULL pointer; n <= 0 does nothing. */
 int riqn_replay_append(int n, int actor_capacity, int id_actor, int start, const unsigned char* frames,
                        const int* timestep, const int* action, const float* reward, const unsigned char* nonterminal,
                        unsigned char* s_frames, int* s_timestep, int* s_action, float* s_reward,
                        unsigned char* s_nonterminal, void* stream);
 /* Transition assembly (:347-369, :479-541): window (batch, history+n_step, 84, 84) uint8 with blank frames
  * across episode boundaries; states = window[:, :history], next_states = window[:, n_step:].
- * gamma_pow: n_step doubles, discount**k. */
+ * gamma_pow: n_step doubles, discount**k.  Returns cudaErrorInvalidValue, writing nothing, for actor_capacity, history
+ * or n_step < 1, history + n_step > 16, or a NULL pointer; batch <= 0 does nothing. */
 int riqn_frame_gather(int batch, int actor_capacity, int history, int n_step, const long long* data_idx,
                       const unsigned char* s_frames, const int* s_timestep, const int* s_action, const float* s_reward,
                       const unsigned char* s_nonterminal, const double* gamma_pow, unsigned char* window,

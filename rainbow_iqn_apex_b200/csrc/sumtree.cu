@@ -489,7 +489,7 @@ using namespace riqn;
 RIQN_API int riqn_sumtree_stratified(int n, unsigned long long seed, unsigned long long stream_id, const double* tree,
                                      double* values, const riqn_dyn_state* dyn, void* stream) {
   riqn::note_launches(1);
-  if (n <= 0 || n > 12000) return (int)cudaErrorInvalidValue;
+  if (n <= 0 || n > 12000 || !tree || !values) return (int)cudaErrorInvalidValue;
   stratified_kernel<<<1, 1024, sizeof(int) * n, (cudaStream_t)stream>>>(n, seed, stream_id, tree, values, dyn);
   return (int)cudaGetLastError();
 }
@@ -498,6 +498,10 @@ RIQN_API int riqn_sumtree_sample(int n, long capacity, int actor_capacity, const
                                  const long long* index_actor, int history, int n_step, long long* tree_idx,
                                  long long* data_idx, double* priorities, void* stream) {
   riqn::note_launches(1);
+  // the segment of a leaf is d / actor_capacity, so the segments must tile the tree exactly
+  if (capacity < 1 || actor_capacity < 1 || capacity % actor_capacity != 0 || history < 0 || n_step < 0 || !tree ||
+      !values || !index_actor || !tree_idx || !data_idx || !priorities)
+    return (int)cudaErrorInvalidValue;
   if (n <= 0) return 0;
   const int warps_per_block = 4;
   sumtree_sample_kernel<<<riqn_cdiv(n, warps_per_block), warps_per_block * 32, 0, (cudaStream_t)stream>>>(
@@ -510,6 +514,12 @@ RIQN_API int riqn_sumtree_is_weights(int n, const double* tree, const double* pr
                                      double priority_weight, double* w64, float* w32, int* n_nonpositive,
                                      const riqn_dyn_state* dyn, void* stream) {
   riqn::note_launches(1);
+  if (n < 1 || !tree || !priorities || !w64 || !w32) return (int)cudaErrorInvalidValue;
+  // with dyn the device values replace these (checked by whoever writes them).  A capacity of 0 (a tree filled without
+  // the fill count) is accepted: like the reference's numpy, (0 * p)^-beta / max gives NaN weights
+  if (!dyn && (!isfinite(current_capacity) || !(current_capacity >= 0.0) || !isfinite(priority_weight) ||
+               !(priority_weight >= 0.0)))
+    return (int)cudaErrorInvalidValue;
   is_weights_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(n, tree, priorities, current_capacity, priority_weight, w64,
                                                           w32, n_nonpositive, dyn);
   return (int)cudaGetLastError();
@@ -520,6 +530,8 @@ static int launch_sumtree_update(int n, long capacity, double* tree, const long 
                                  float priority_exponent, int apply_pow, float* new_priorities, double* diff_scratch,
                                  double* max_priority, long long demo_leaf, float bonus, void* stream) {
   riqn::note_launches(2);
+  if (capacity < 1 || !tree || !tree_idx || !loss || !new_priorities || !diff_scratch || !max_priority)
+    return (int)cudaErrorInvalidValue;
   if (n <= 0) return 0;
   if (n > 4096) return (int)cudaErrorInvalidValue;  // shared-memory bound of the propagate kernel
   cudaStream_t s = (cudaStream_t)stream;
@@ -561,6 +573,11 @@ RIQN_API int riqn_replay_append(int n, int actor_capacity, int id_actor, int sta
                                 const unsigned char* nonterminal, unsigned char* s_frames, int* s_timestep, int* s_action,
                                 float* s_reward, unsigned char* s_nonterminal, void* stream) {
   riqn::note_launches(1);
+  // n <= actor_capacity: one launch writes every slot at most once (more would let two blocks race on a slot)
+  if (actor_capacity < 1 || id_actor < 0 || start < 0 || start >= actor_capacity || n > actor_capacity || !frames ||
+      !timestep || !action || !reward || !nonterminal || !s_frames || !s_timestep || !s_action || !s_reward ||
+      !s_nonterminal)
+    return (int)cudaErrorInvalidValue;
   if (n <= 0) return 0;
   replay_append_kernel<<<n, 128, 0, (cudaStream_t)stream>>>(n, actor_capacity, id_actor, start, frames, timestep, action,
                                                             reward, nonterminal, s_frames, s_timestep, s_action, s_reward,
@@ -574,8 +591,11 @@ RIQN_API int riqn_frame_gather(int batch, int actor_capacity, int history, int n
                                unsigned char* window, long long* actions, float* returns, float* nonterminals,
                                void* stream) {
   riqn::note_launches(1);
+  if (actor_capacity < 1 || history < 1 || n_step < 1 || history + n_step > 16 || !data_idx || !s_frames ||
+      !s_timestep || !s_action || !s_reward || !s_nonterminal || !gamma_pow || !window || !actions || !returns ||
+      !nonterminals)
+    return (int)cudaErrorInvalidValue;
   if (batch <= 0) return 0;
-  if (history + n_step > 16) return (int)cudaErrorInvalidValue;
   frame_gather_kernel<<<batch, 256, 0, (cudaStream_t)stream>>>(batch, actor_capacity, history, n_step,
                                                                (const int64_t*)data_idx, s_frames, s_timestep, s_action,
                                                                s_reward, s_nonterminal, gamma_pow, window,

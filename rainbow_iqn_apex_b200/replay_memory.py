@@ -27,6 +27,8 @@ class SegmentTree:
         self.full_capacity = self.actor_capacity * self.nb_actor
         self.actor_full = False
         self.memory_full = False
+        if self.actor_capacity < 1 or self.nb_actor < 1:
+            raise ValueError(f"actor_capacity {actor_capacity} and nb_actor {nb_actor} must be >= 1")
         self.device = torch.device(device)
         self.store_frames = store_frames
         self._rng_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -92,6 +94,15 @@ class SegmentTree:
              float(exponent), 1 if apply_pow else 0, ptr(new_pri), ptr(diff), ptr(self.max_priority))
         return new_pri
 
+    def _check_append(self, id_actor, start, n):
+        """Refuse, before the tree is touched, an append the frame store would refuse: n steps of segment ``id_actor``
+        at ring position ``start`` must fit the segment once (more would write one slot twice in one launch)."""
+        if not 0 <= int(id_actor) < self.nb_actor or not 0 <= int(start) < self.actor_capacity \
+                or n > self.actor_capacity:
+            raise ValueError(f"append of {n} steps at position {start} of segment {id_actor}: needs 0 <= segment < "
+                             f"{self.nb_actor}, 0 <= position < {self.actor_capacity} and at most "
+                             f"{self.actor_capacity} steps")
+
     def append_arrays(self, id_actor, start, timesteps, frames, actions, rewards, dones, priorities, T_actor=0):
         """append_actor_buffer (redis_memory.py:153-202) on arrays: n consecutive steps of actor ``id_actor``
         written at ring position ``start``; priorities (n,) already exponentiated (launch_actor.py:123-133)."""
@@ -100,6 +111,7 @@ class SegmentTree:
         cap = self.actor_capacity
         if not self.store_frames:
             raise RuntimeError("this SegmentTree was built with store_frames=False (tree only): no transition store")
+        self._check_append(id_actor, start, n)
         pos = (np.arange(start, start + n) % cap) + id_actor * cap
         tree_idx = torch.from_numpy(pos + self.full_capacity - 1).to(dev)
         pri = torch.as_tensor(np.asarray(priorities, np.float32)).to(dev)
@@ -129,6 +141,7 @@ class SegmentTree:
             raise RuntimeError("this SegmentTree was built with store_frames=False (tree only): no transition store")
         dev, cap = self.device, self.actor_capacity
         n = int(actions.numel())
+        self._check_append(id_actor, start, n)
         pos = (torch.arange(start, start + n, device=dev) % cap) + id_actor * cap
         self.update_multiple_value(pos + self.full_capacity - 1, priorities.to(dev, torch.float32).contiguous())
         fr = frames.to(dev, torch.uint8).reshape(n, FRAME).contiguous()
@@ -206,12 +219,13 @@ class ReplayMemory:
     def sample_indices(self, batch_size, samples=None):
         """find_multiple_values + importance weights (redis_memory.py:424-475), including the reference's resample loop:
         while some sampled priority is <= 0 (a slot next to a write head of a partially filled segment) the batch is
-        redrawn, up to 10 times (:432-445); after that -- and always inside a captured CUDA graph or with injected
-        ``samples``, where a host-side retry is impossible -- the reference's final fallback applies (:446-456: those
-        probabilities become 1/capacity).  The count of such samples is left in ``last_nonpositive`` (device int)."""
+        drawn again, up to 10 more times, 11 draws in all (:432-438); after that -- and always inside a captured CUDA
+        graph or with injected ``samples``, where a host-side retry is impossible -- the reference's final fallback
+        applies (:446-456: those probabilities become 1/capacity).  The count of such samples is left in
+        ``last_nonpositive`` (device int)."""
         tr = self.transitions
         retry = samples is None and tr._dyn is None and not torch.cuda.is_current_stream_capturing()
-        for attempt in range(10 if retry else 1):
+        for attempt in range(11 if retry else 1):
             pri, data_idx, tree_idx = tr.find_multiple_values(self.history, self.n, batch_size, samples)
             w64 = torch.empty(batch_size, dtype=torch.float64, device=self.device)
             w32 = torch.empty(batch_size, dtype=torch.float32, device=self.device)

@@ -145,3 +145,20 @@ def assert_bits(what, got, want):
 def prefill_pattern(n, scale=0.25, mod=13):
     """A non-zero prefill for accumulated outputs, exact in fp32."""
     return (((np.arange(n) % mod) - mod // 2) * scale + scale / 2).astype(np.float32)
+
+
+_M32 = np.uint64(0xFFFFFFFF)
+
+
+def philox_np(seed, stream, count):
+    """Philox4x32-10 (Salmon et al. 2011) words of counters 0 .. count-1 under (seed, stream), in the order
+    riqn_fill_uniform consumes them: word 4i + j is component j of draw i.  (count * 4,) uint32."""
+    idx = np.arange(count, dtype=np.uint64)
+    c = [idx & _M32, idx >> np.uint64(32), np.full(count, stream & 0xFFFFFFFF, np.uint64),
+         np.full(count, stream >> 32, np.uint64)]
+    k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64(seed >> 32)
+    for _ in range(10):
+        p0, p1 = np.uint64(0xD2511F53) * c[0], np.uint64(0xCD9E8D57) * c[2]
+        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & _M32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & _M32]
+        k0, k1 = (k0 + np.uint64(0x9E3779B9)) & _M32, (k1 + np.uint64(0xBB67AE85)) & _M32
+    return np.stack(c, 1).astype(np.uint32).ravel()

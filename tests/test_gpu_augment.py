@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import assert_bits, dptr, f32_bits, lib_call, load_params, make_args
+from helpers import assert_bits, dptr, f32_bits, lib_call, load_params, make_args, philox_np
 from oracle import cases, losses, network as net, qr as oq
 
 HW = 84
@@ -39,23 +39,6 @@ def shift_np(x, shifts):
 def draw_from_m(m, pad):
     """The shift of the 24-bit integer m: floor(m (2p+1) / 2^24) - p, in integers."""
     return ((np.asarray(m, np.int64) * (2 * pad + 1)) >> 24) - pad
-
-
-_M32 = np.uint64(0xFFFFFFFF)
-
-
-def philox_np(seed, stream, count):
-    """Philox4x32-10 (Salmon et al. 2011) words of counters 0 .. count-1 under (seed, stream), in the order
-    riqn_fill_uniform consumes them: word 4i + j is component j of draw i.  (count * 4,) uint32."""
-    idx = np.arange(count, dtype=np.uint64)
-    c = [idx & _M32, idx >> np.uint64(32), np.full(count, stream & 0xFFFFFFFF, np.uint64),
-         np.full(count, stream >> 32, np.uint64)]
-    k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64(seed >> 32)
-    for _ in range(10):
-        p0, p1 = np.uint64(0xD2511F53) * c[0], np.uint64(0xCD9E8D57) * c[2]
-        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & _M32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & _M32]
-        k0, k1 = (k0 + np.uint64(0x9E3779B9)) & _M32, (k1 + np.uint64(0xBB67AE85)) & _M32
-    return np.stack(c, 1).astype(np.uint32).ravel()
 
 
 def uniform_of_m(m):
