@@ -829,6 +829,34 @@ int riqn_spr_cosine_fwd_bwd(int rows, int K, int dim, const float* pred, const f
                             float coef, float* loss_rows, float* dpred, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Periodic network resets (SR-SPR, D'Oro et al. 2023; BBF, Schwarzer et al. 2023; no counterpart in the reference)
+ * ---------------------------------------------------------------------------------------------- */
+#define RIQN_RESET_MAX_SEGMENTS 64
+#define RIQN_RESET_UNIFORM 0    /* fresh draw U(-value, value) */
+#define RIQN_RESET_CONSTANT 1   /* fresh draw = value          */
+typedef struct riqn_reset_segment {
+  long long begin, end;   /* the arena elements [begin, end)                                       */
+  int kind;               /* RIQN_RESET_UNIFORM or RIQN_RESET_CONSTANT                              */
+  float value;            /* the uniform bound b, or the constant                                  */
+  float alpha;            /* the share of the old value that is kept, 0 <= alpha < 1               */
+} riqn_reset_segment;
+/* Reset the segments `segs` (a HOST array of nseg, passed by value to one launch) of the fp32 arena params[0:n], and
+ * restart its Adam moments: exp_avg[0:n] = exp_avg_sq[0:n] = 0 when both are non-NULL (both NULL: no moments).
+ * Element i of a segment becomes
+ *   u_i    = the (0,1) uniform riqn_fill_uniform(n, seed, stream_id, dyn = NULL) writes at position i (Philox4x32-10 word
+ *            i % 4 of draw i / 4, x -> fl(fl((x >> 8) + 0.5) / 2^24));
+ *   theta0 = fl(value * (2 u_i - 1)) for a uniform segment (2 u_i - 1 is exact in fp32), value for a constant one;
+ *   theta' = fl(fl(alpha * theta) + fl(fl(1 - alpha) * theta0)), each operation rounded on its own (no fma);
+ *            alpha = 0 writes theta0 itself (the same value for every finite theta; a non-finite theta is replaced too).
+ * The draw depends on (seed, stream_id, i) only, not on the launch geometry.  Elements in no segment (alignment padding,
+ * parameters a reset keeps) keep their bits.  Refused with cudaErrorInvalidValue, nothing written, when n < 1, params is
+ * NULL, exactly one moment pointer is NULL, segs is NULL, nseg is not in 1..64, the segments are not sorted, disjoint
+ * and non-empty inside [0, n) (0 <= begin < end <= n, begin >= the previous end), a kind is unknown, a uniform bound is
+ * not finite and > 0, a constant is not finite, or an alpha is not in [0, 1). */
+int riqn_arena_reset(long n, float* params, float* exp_avg, float* exp_avg_sq, int nseg, const riqn_reset_segment* segs,
+                     unsigned long long seed, unsigned long long stream_id, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Test hook: plain strided fp32 product C[m,n] = sum_k A[m*sAm + k*sAk] * B[n*sBn + k*sBk].
  * ---------------------------------------------------------------------------------------------- */
 int riqn_gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,

@@ -28,6 +28,12 @@ class NoisyLayer(C.Structure):
                 ("stream_out", C.c_ulonglong), ("w_hi", _P), ("w_lo", _P), ("w_fp16", C.c_int)]
 
 
+class ResetSegment(C.Structure):
+    """riqn_reset_segment (include/riqn_b200.h)"""
+    _fields_ = [("begin", C.c_longlong), ("end", C.c_longlong), ("kind", C.c_int), ("value", C.c_float),
+                ("alpha", C.c_float)]
+
+
 class SplitJob(C.Structure):
     """riqn_split_job (include/riqn_b200.h)"""
     _fields_ = [("src", _P), ("perm", _P), ("rows", C.c_int), ("cols", C.c_int), ("div", C.c_float), ("hi", _P),
@@ -96,6 +102,7 @@ SIGNATURES = {
     "riqn_spr_weight_grad_add": [C.c_int] * 3 + [_P] * 3,
     "riqn_spr_cosine_fwd_bwd": [C.c_int] * 3 + [_P] * 3 + [C.c_float, _P, _P, _P],
     "riqn_sequence_gather": [C.c_int] * 4 + [_P] * 10,
+    "riqn_arena_reset": [C.c_long, _P, _P, _P, C.c_int, C.POINTER(ResetSegment), C.c_ulonglong, C.c_ulonglong, _P],
     "riqn_argmax_weighted": [C.c_int] * 3 + [_P] * 4,
     "riqn_c51_head_fwd":[C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P],
     "riqn_c51_loss_fwd_bwd": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,

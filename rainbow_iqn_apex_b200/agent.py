@@ -13,9 +13,11 @@ regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's large-mar
 ``random_shift`` for the
 learner's random-shift augmentation (augment.py), and ``curl`` / ``curl_net`` / ``curl_optimiser`` / ``momentum_net`` /
 ``momentum_projection`` for CURL's contrastive loss on the trunk (curl.py), and ``spr`` / ``spr_net`` /
-``spr_optimiser`` for SPR's self-predictive loss on the trunk (spr.py).  The networks are rainbow_iqn_apex_b200.model.DQN (CUDA) and the
-optimiser is the arena Adam; checkpoints keep the reference schema {T_actors, T_learner, model_state_dict,
-optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries under FQF, CURL's three and SPR's two.
+``spr_optimiser`` for SPR's self-predictive loss on the trunk (spr.py), and ``reset`` (reset_interval, reset_shrink) with
+``updates`` / ``resets`` for the learner's periodic network resets (reset.py).  The networks are
+rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference schema
+{T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries
+under FQF, CURL's three, SPR's two and, under resets, reset_state.
 """
 import os
 
@@ -112,6 +114,11 @@ class Agent:
         self.spr_net = self.spr_optimiser = None       # SPR's too (never with CURL)
         if self.spr is not None:
             spr.build(self, args, checkpoint)
+        # optimiser steps run and resets done (Learner.reset_networks): a resumed run resets at the same updates with the
+        # same draws
+        self.updates = self.resets = 0
+        if self.reset is not None and checkpoint is not None and "reset_state" in checkpoint:
+            self.updates, self.resets = (int(x) for x in checkpoint["reset_state"])
 
     def set_risk(self, measure, eta=None):
         """Act, and pick the double-DQN target action a*, under a distortion risk measure (IQN paper, section 3.1):
@@ -157,7 +164,8 @@ class Agent:
         """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
         fraction_optimiser_state_dict, under value rescaling value_rescaling_eps, under QR-DQN qr_dqn_quantiles (N), under CURL
         curl_state_dict, curl_optimiser_state_dict and curl_momentum_state_dict, under SPR spr_state_dict and
-        spr_optimiser_state_dict; model_state_dict keeps the reference schema either way."""
+        spr_optimiser_state_dict, under resets reset_state = (updates, resets); model_state_dict keeps the reference schema
+        either way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
@@ -178,6 +186,8 @@ class Agent:
         if self.spr is not None:
             ckpt["spr_state_dict"] = self.spr_net.state_dict()
             ckpt["spr_optimiser_state_dict"] = self.spr_optimiser.state_dict()
+        if self.reset is not None:
+            ckpt["reset_state"] = (self.updates, self.resets)
         torch.save(ckpt, os.path.join(path, name))
 
     def train(self):

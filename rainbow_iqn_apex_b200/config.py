@@ -101,6 +101,9 @@ FIELDS = {
     "spr": (0, switch),
     "spr_steps": (5, integer(1, MAX_SPR_STEPS)),                  # the paper's Atari K and lambda
     "spr_coef": (2.0, real(lambda x: x > 0.0, "> 0")),
+    "reset": (0, switch),
+    "reset_interval": (40000, integer(1, math.inf)),              # this project's starting point, not tuned
+    "reset_shrink": (0.5, real(lambda x: 0.0 <= x <= 1.0, "in [0, 1]")),
     "demo_segments": (0, integer(0, math.inf)),                   # at most nb_actor (read_demo)
     "demo_priority_bonus": (0.0, real(lambda x: x >= 0.0, ">= 0")),
 }
@@ -152,12 +155,12 @@ def read_risk(head, loss, measure, eta=None):
 
 def read(args, action_space):
     """Validate the optional fields of ``args`` and return what the agent stores, as a dict: qr_dqn (N or None); per
-    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr) None when off, else its parameter
-    or the tuple of its parameters; random_shift (the pad, or None); risk (model.check_risk's); and the "head" and the
-    "loss" variant (or None) they select."""
+    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr, reset) None when off, else its
+    parameter or the tuple of its parameters; random_shift (the pad, or None); risk (model.check_risk's); and the "head"
+    and the "loss" variant (or None) they select.  Resets combine with every head and variant."""
     head, n = read_head(args, action_space)
     v = {"qr_dqn": n}
-    for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl", "spr"):
+    for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl", "spr", "reset"):
         v[name] = None
         if field(args, name):
             params = tuple(field(args, f) for f in FIELDS if f.startswith(name + "_"))

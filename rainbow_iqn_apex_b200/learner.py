@@ -17,6 +17,13 @@ Under SPR (spr.py) every step also gathers the sampled transitions' K-step seque
 predicts their latents through the transition model, zeroes, fills, (all-reduces) and steps SPR's arena (agent.spr_net,
 agent.spr_optimiser).  Each rank predicts its own local batch.  Entry points that receive an already assembled minibatch
 without its sequence (learn_on_batch without ``sequence``, the batch and learn graphs, learn_on_host_batch) refuse.
+
+Under resets (reset.py) ``updates`` counts the optimiser steps this learner has run, and after every reset_interval-th
+update the step entry points (learn_on_batch and learn through it, learn_and_update eager or replayed, learn_on_graph,
+learn_on_host_batch) call reset_networks() before they return: one eager launch per arena between two steps, never
+inside a captured graph.  The warm-up steps of a capture count; a reset that falls due during them runs when the
+enable_* call returns (one, however many fell due).  reset_networks() is public, for a schedule of one's own or a loop
+of one's own around loss.backward().
 """
 import contextlib
 import io
@@ -24,7 +31,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment, curl, spr
+from . import augment, curl, reset, spr
 from .agent import Agent
 from .dynstate import DynState
 
@@ -84,7 +91,22 @@ class Learner(Agent):
         loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights, demo=demo,
                                       sequence=sequence)
         self.apply_gradients()
+        self._count_updates(1)
         return loss
+
+    def reset_networks(self):
+        """Reset the networks now (reset.py): redraw the last layers, shrink and perturb the trunk and SPR's transition
+        model by reset_shrink (its default, 0.5, when reset = 0), restart every optimiser of a reset arena, and count
+        the reset (the next one draws from the next streams)."""
+        reset.reset(self, self.resets)
+        self.resets += 1
+
+    def _count_updates(self, n):
+        """Count ``n`` optimiser steps; under resets, reset once if one of them completed a reset_interval."""
+        before = self.updates
+        self.updates += n
+        if self.reset is not None and self.updates // self.reset[0] > before // self.reset[0]:
+            self.reset_networks()
 
     def _start_tail_allreduce(self, offset):
         """Called by DQN.backward_iqn once the NoisyLinear gradients (arena[offset:], 25.8 of 26.9 MB) are final: their
@@ -288,6 +310,7 @@ class Learner(Agent):
         for o, s0 in zip(self._optimisers(), step0):
             o._step = s0 + warmup
         self._graphs[kind] = _StepGraph(graph, post_graph, mem, inputs, out)
+        self._count_updates(warmup)     # after the counters are set: a reset here restarts them for good
 
     def _replay(self, g, batch=None):
         """One step through the captured graph ``g``: ``batch`` (if given) into its static inputs, the struct written from
@@ -303,6 +326,7 @@ class Learner(Agent):
             g.post.replay()
         for o in self._optimisers():        # advance the host step counters the replayed Adam launches stand for
             o._step += 1
+        self._count_updates(1)
         return g.out
 
     def enable_cuda_graph(self, mem, warmup=3, capture_collectives=True):

@@ -59,6 +59,12 @@ class Adam(torch.optim.Optimizer):
              float(g["eps"]), float(self.grad_scale), self._dyn.ptr() if self._dyn is not None else None)
         self._net._params_changed()             # conv / iqn_fc operand images are rebuilt by the next reset_noise()
 
+    def restart(self):
+        """Become a freshly constructed optimiser once the caller has zeroed the moment arenas (riqn_arena_reset): step
+        0, no per-parameter state, so that the next step takes the step-1 bias corrections."""
+        self._step = 0
+        self.state.clear()
+
     def bias_corrections(self, step):
         """(-(lr / (1 - b1^t)), sqrt(1 - b2^t)) of step t, as torch.optim.Adam computes them."""
         g = self.param_groups[0]
