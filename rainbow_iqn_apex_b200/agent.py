@@ -1,23 +1,22 @@
 """Agent -- mirror of the reference ``rainbowiqn/agent.py:10-166`` (shared by Learner and Actor).
 
-Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``args`` fields, same public
-attributes (online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
+Same constructor ``Agent(args, action_space, redis_servor)`` reading the same ``args`` fields, same public attributes
+(online_net, target_net, optimiser, n, history, discount, device, batch_size, kappa, num_tau_samples,
 num_tau_prime_samples, num_quantile_samples, support, ...) and methods (reset_noise, update_target_net,
 compute_loss_actor_or_learner, save, train, eval), plus ``loss_core`` for the loss the agent trains (c51.loss_core,
-qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-sensitive acting and
-``munchausen`` for Munchausen-IQN targets, ``fqf`` / ``fraction_net`` / ``fraction_optimiser`` for FQF fractions,
-``value_rescaling`` (and, for C51, ``acting_support``) for the transformed Bellman operator on unclipped rewards, and
-``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd`` for MMDQN's moment-matching loss on that head (mmd.py),
-``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51 head (hl_gauss.py), ``cql`` for the conservative
-regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's large-margin loss on demonstrations (dqfd.py),
-``random_shift`` for the
-learner's random-shift augmentation (augment.py), and ``curl`` / ``curl_net`` / ``curl_optimiser`` / ``momentum_net`` /
-``momentum_projection`` for CURL's contrastive loss on the trunk (curl.py), and ``spr`` / ``spr_net`` /
-``spr_optimiser`` for SPR's self-predictive loss on the trunk (spr.py), and ``reset`` (reset_interval, reset_shrink) with
-``updates`` / ``resets`` for the learner's periodic network resets (reset.py).  The networks are
+qr.loss_core or compute_loss_iqn.loss_core), ``risk`` / ``set_risk`` for risk-sensitive acting and ``munchausen`` for
+Munchausen-IQN targets, ``fqf`` for FQF fractions (fqf.py), ``value_rescaling`` (and, for C51, ``acting_support``) for
+the transformed Bellman operator on unclipped rewards, and ``qr_dqn`` for QR-DQN's fixed-fraction quantile head, ``mmd``
+for MMDQN's moment-matching loss on that head (mmd.py), ``hl_gauss`` for HL-Gauss's Gaussian-histogram loss on the C51
+head (hl_gauss.py), ``cql`` for the conservative regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's
+large-margin loss on demonstrations (dqfd.py), ``random_shift`` for the learner's random-shift augmentation
+(augment.py), ``curl`` for CURL's contrastive loss on the trunk (curl.py), ``spr`` for SPR's self-predictive loss on the
+trunk (spr.py), and ``reset`` (reset_interval, reset_shrink) with ``updates`` / ``resets`` for the learner's periodic
+network resets (reset.py).  The networks FQF, CURL and SPR train beside the DQN and their optimisers are set by those
+modules' ``build`` (None when off), and ``sides`` lists them (arena.Side).  The networks are
 rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference schema
-{T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus the fraction network's two entries
-under FQF, CURL's three, SPR's two and, under resets, reset_state.
+{T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus, under resets, reset_state and
+each side's entries.
 """
 import os
 
@@ -90,14 +89,6 @@ class Agent:
         self._inject = None  # parity hook: {"noises": (n0, n1, n2), "taus": (t0, t1, t2)}; Munchausen: two of each;
         #                      FQF and QR-DQN: {"noises": (n0, n1, n2)}; with random_shift, any of these may also carry
         #                      "shifts": (shifts_states, shifts_next_states), int32 (B, 2) (dy, dx), in place of the draw
-        self.fraction_net = self.fraction_optimiser = None
-        if self.fqf is not None:
-            # drawn after both DQNs, so that their initialisation is that of a plain IQN agent from the same seed
-            self.fraction_net = fqf.FractionProposal(self.num_tau_samples, args.device)
-            self.fraction_optimiser = Adam(self.fraction_net.parameters(), lr=self.fqf[0], eps=args.adam_eps)
-            if checkpoint is not None and "fraction_net_state_dict" in checkpoint:
-                self.fraction_net.load_state_dict(checkpoint["fraction_net_state_dict"])
-                self.fraction_optimiser.load_state_dict(checkpoint["fraction_optimiser_state_dict"])
         if self.rainbow_only:
             # the support the C51 head takes expectations over when it acts: h^-1 of the h-space support under rescaling
             self.acting_support = self.support
@@ -106,14 +97,13 @@ class Agent:
                 _lib.call("riqn_value_rescale", self.atoms, _lib.ptr(self.support), self.value_rescaling, 1,
                           _lib.ptr(self.acting_support))
         # random_shift: only Learner.compute_gradients shifts; acting and the actors' priorities see the stored frames.
-        # CURL's modules are built last, so that both DQNs (and the fraction proposal) initialise as a plain agent's
-        # from the same seed
+        # The side networks (arena.py), set by their modules' build (None when off), come after both DQNs in the fixed
+        # order FQF, CURL, SPR: every network initialises from a seed as it would without the later ones
+        self.fraction_net = self.fraction_optimiser = None
         self.curl_net = self.curl_optimiser = self.momentum_net = self.momentum_projection = None
-        if self.curl is not None:
-            curl.build(self, args, checkpoint)
-        self.spr_net = self.spr_optimiser = None       # SPR's too (never with CURL)
-        if self.spr is not None:
-            spr.build(self, args, checkpoint)
+        self.spr_net = self.spr_optimiser = None
+        self.sides = tuple(module.build(self, args, checkpoint)
+                           for on, module in ((self.fqf, fqf), (self.curl, curl), (self.spr, spr)) if on is not None)
         # optimiser steps run and resets done (Learner.reset_networks): a resumed run resets at the same updates with the
         # same draws
         self.updates = self.resets = 0
@@ -161,33 +151,23 @@ class Agent:
         return loss
 
     def save(self, path, T_actors, T_learner, name):
-        """agent.py:150-160.  Under FQF the checkpoint also holds fraction_net_state_dict and
-        fraction_optimiser_state_dict, under value rescaling value_rescaling_eps, under QR-DQN qr_dqn_quantiles (N), under CURL
-        curl_state_dict, curl_optimiser_state_dict and curl_momentum_state_dict, under SPR spr_state_dict and
-        spr_optimiser_state_dict, under resets reset_state = (updates, resets); model_state_dict keeps the reference schema
-        either way."""
+        """agent.py:150-160.  Under value rescaling the checkpoint also holds value_rescaling_eps, under QR-DQN
+        qr_dqn_quantiles (N), under resets reset_state = (updates, resets), and each side network's entries (Side.checkpoint);
+        model_state_dict keeps the reference schema either way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
             "model_state_dict": self.online_net.state_dict(),
             "optimiser_state_dict": self.optimiser.state_dict(),
         }
-        if self.fqf is not None:
-            ckpt["fraction_net_state_dict"] = self.fraction_net.state_dict()
-            ckpt["fraction_optimiser_state_dict"] = self.fraction_optimiser.state_dict()
         if self.value_rescaling is not None:
             ckpt["value_rescaling_eps"] = self.value_rescaling
         if self.qr_dqn is not None:
             ckpt["qr_dqn_quantiles"] = self.qr_dqn
-        if self.curl is not None:
-            ckpt["curl_state_dict"] = self.curl_net.state_dict()
-            ckpt["curl_optimiser_state_dict"] = self.curl_optimiser.state_dict()
-            ckpt["curl_momentum_state_dict"] = curl.momentum_state_dict(self)
-        if self.spr is not None:
-            ckpt["spr_state_dict"] = self.spr_net.state_dict()
-            ckpt["spr_optimiser_state_dict"] = self.spr_optimiser.state_dict()
         if self.reset is not None:
             ckpt["reset_state"] = (self.updates, self.resets)
+        for side in self.sides:
+            ckpt.update(side.checkpoint())
         torch.save(ckpt, os.path.join(path, name))
 
     def train(self):

@@ -33,6 +33,23 @@ def draw_shifts(net, n, pad, key=SHIFT_SEED, advance=True):
     return out
 
 
+def injection(learner):
+    """The injection dict of the step ``learner`` is about to run: its ``_inject``, or the first of a list of them
+    (peeked: the loss core pops it); an empty dict without one."""
+    inj = learner._inject[0] if isinstance(learner._inject, list) and learner._inject else learner._inject
+    return inj if isinstance(inj, dict) else {}
+
+
+def view_shifts(learner, name, n, key):
+    """n shifts (n, 2) int32 for a further view of one step's frames (CURL's positive, SPR's targets): the injection's
+    ``name``, or a draw under ``key`` that moves none of the counters, so that the learner's shifts of s_t and s_{t+n}
+    stay those of a learner without the view."""
+    given = injection(learner).get(name)
+    if given is None:
+        return draw_shifts(learner.online_net, n, learner.random_shift, key=key, advance=False)
+    return torch.as_tensor(given, dtype=torch.int32).reshape(n, 2).to(learner.online_net._flat.device)
+
+
 def _frames(x, dev):
     """Frames the kernel reads: on ``dev``, uint8 or fp32, each sample (C, H, W)-contiguous with a 16-byte aligned start
     (replay-window views qualify as they are)."""

@@ -28,75 +28,34 @@ Modules, all built after every existing one (so that both DQNs initialise as a p
   agent.momentum_net    a DQN whose trunk alone ever runs (f_xi), and agent.momentum_projection, the untrained
                         buffer arena of g_xi (the projection prefix of curl_net's arena layout)
 """
-import weakref
-
 import torch
 from torch import nn
 
 from . import augment
 from ._lib import call, ptr
-from .model import DQN, FEAT, _ALIGN
+from .arena import ArenaModule, Side
+from .model import DQN, FEAT
 
 HIDDEN, DIM = 512, 128                                         # projection widths
 CURL_SHIFT_SEED = 0xC0A1                                       # the positive view's draw key (net._rng_seed ^ this)
 
 
-class ArenaModule(nn.Module):
-    """Parameters ``NAMES`` (dotted names allowed) as views of one flat fp32 arena (``_flat``; gradients in
-    ``_flat_grad``), each group on a 256-byte boundary, in NAMES order.  The first four are a projection (weight_h,
-    bias_h, weight_c, bias_c), the prefix [0, proj_numel)."""
+class ProjectionArena(ArenaModule):
+    """An arena whose first four groups are a projection g (weight_h, bias_h, weight_c, bias_c): the prefix
+    [0, proj_numel) that project and project_backward read.  CURL's and SPR's arenas."""
 
-    NAMES = ()
-
-    def _flatten(self, dev):
-        total, self._offs = 0, {}
-        for name in self.NAMES:
-            total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
-            self._offs[name] = total
-            total += self.get_parameter(name).numel()
-        self.proj_numel = self._offs[self.NAMES[4]]
-        total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
-        flat = torch.zeros(total, device=dev, dtype=torch.float32)
-        flat_grad = torch.zeros(total, device=dev, dtype=torch.float32)
-        for name in self.NAMES:
-            p, off = self.get_parameter(name), self._offs[name]
-            n = p.numel()
-            flat[off:off + n].copy_(p.data.reshape(-1).float())
-            p.data = flat[off:off + n].view(p.shape)
-            p.grad = flat_grad[off:off + n].view(p.shape)
-            p._riqn_owner = weakref.ref(self)
-            p._riqn_offset = off
-        self._flat, self._flat_grad = flat, flat_grad
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self._flatten(self.get_parameter(self.NAMES[0]).device)
-        return out
-
-    def _params_changed(self):
-        """Called by the arena Adam after a step: nothing is cached from these weights."""
-
-    def grad_view(self, p):
-        return self._flat_grad[p._riqn_offset:p._riqn_offset + p.numel()].view(p.shape)
-
-    def zero_grad(self, set_to_none=False):
-        """One memset over the gradient arena; the .grad views stay bound."""
-        call("riqn_zero_f32", ptr(self._flat_grad), self._flat_grad.numel())
-        for name in self.NAMES:
-            p = self.get_parameter(name)
-            p.grad = self.grad_view(p)
+    @property
+    def proj_numel(self):
+        return self.get_parameter(self.NAMES[4])._riqn_offset
 
     def views(self, arena):
         """(weight_h, bias_h, weight_c, bias_c) of the projection laid out in ``arena`` (this arena, or a copy of its
         projection prefix)."""
-        out = []
-        for name in self.NAMES[:4]:
-            p, off = self.get_parameter(name), self._offs[name]
-            out.append(arena[off:off + p.numel()].view(p.shape))
-        return tuple(out)
+        params = [self.get_parameter(name) for name in self.NAMES[:4]]
+        return tuple(arena[p._riqn_offset:p._riqn_offset + p.numel()].view(p.shape) for p in params)
 
 
-class CurlProjection(ArenaModule):
+class CurlProjection(ProjectionArena):
     """The online projection g_theta and the bilinear W, views of one flat fp32 arena laid out weight_h (512, 3136) |
     bias_h | weight_c (128, 512) | bias_c | bilinear (128, 128).  Initialised like nn.Linear (uniform in
     +-1/sqrt(fan_in)), W like a bias-free nn.Linear(128, 128)."""
@@ -187,28 +146,39 @@ def project_backward(net, keep, dz):
 
 
 def build(agent, args, checkpoint):
-    """The CURL modules of ``agent`` (after every other module): curl_net, curl_optimiser, momentum_net and
-    momentum_projection, with xi = theta, or all four restored from ``checkpoint`` when it holds them."""
-    agent.curl_net = CurlProjection(args.device)
+    """The CURL modules of ``agent`` (after both DQNs and the fraction proposal): curl_net, curl_optimiser, momentum_net
+    and momentum_projection, with xi = theta, or all four restored from ``checkpoint`` when it holds them.  Returns
+    CURL's Side."""
+    net = agent.curl_net = CurlProjection(args.device)
     from .optim import Adam
-    agent.curl_optimiser = Adam(agent.curl_net.parameters(), lr=args.lr, eps=args.adam_eps)
+    opt = agent.curl_optimiser = Adam(net.parameters(), lr=args.lr, eps=args.adam_eps)
     agent.momentum_net = DQN(args, agent.action_space).to(device=args.device)
-    agent.momentum_projection = torch.empty(agent.curl_net.proj_numel, device=agent.curl_net._flat.device)
+    agent.momentum_projection = torch.empty(net.proj_numel, device=net._flat.device)
     if checkpoint is not None and "curl_state_dict" in checkpoint:
-        agent.curl_net.load_state_dict(checkpoint["curl_state_dict"])
-        agent.curl_optimiser.load_state_dict(checkpoint["curl_optimiser_state_dict"])
+        net.load_state_dict(checkpoint["curl_state_dict"])
+        opt.load_state_dict(checkpoint["curl_optimiser_state_dict"])
         mom = checkpoint["curl_momentum_state_dict"]
         for name in ("conv1", "conv2", "conv3"):
             conv = getattr(agent.momentum_net, name)
             conv.weight.data.copy_(mom[name + ".weight"])
             conv.bias.data.copy_(mom[name + ".bias"])
-        for v, name in zip(agent.curl_net.views(agent.momentum_projection), CurlProjection.NAMES):
+        for v, name in zip(net.views(agent.momentum_projection), CurlProjection.NAMES):
             v.copy_(mom[name])
     else:
         n = trunk_numel(agent.online_net)
         agent.momentum_net._flat[:n].copy_(agent.online_net._flat[:n])
-        agent.momentum_projection.copy_(agent.curl_net._flat[:agent.curl_net.proj_numel])
+        copy_projection(agent)
     agent.momentum_net._params_changed()
+    return Side(2, net, opt,
+                lambda: {"curl_state_dict": net.state_dict(), "curl_optimiser_state_dict": opt.state_dict(),
+                         "curl_momentum_state_dict": momentum_state_dict(agent)},
+                broadcast=(net._flat, agent.momentum_net._flat, agent.momentum_projection),
+                after_step=momentum_update, after_reset=copy_projection, trunk_term=trunk_term)
+
+
+def copy_projection(agent):
+    """g_xi <- g_theta: the momentum projection set to the online one (at construction and after a reset)."""
+    agent.momentum_projection.copy_(agent.curl_net._flat[:agent.curl_net.proj_numel])
 
 
 def momentum_state_dict(agent):
@@ -232,15 +202,8 @@ def positives(learner, states, debug=None):
     and s_{t+n}, under CURL_SHIFT_SEED, or the parity hook's ``"curl_shifts"`` (B, 2) int32), through the momentum trunk
     and projection.
     Returns z_k (B, 128)."""
-    on, mom = learner.online_net, learner.momentum_net
-    B = states.shape[0]
-    inj = learner._inject[0] if isinstance(learner._inject, list) and learner._inject else learner._inject
-    given = inj.get("curl_shifts") if isinstance(inj, dict) else None
-    if given is None:
-        # a key of its own, counters untouched: the learner's shifts of s_t and s_{t+n} stay those of a plain learner
-        shifts = augment.draw_shifts(on, B, learner.random_shift, key=CURL_SHIFT_SEED, advance=False)
-    else:
-        shifts = torch.as_tensor(given, dtype=torch.int32).reshape(B, 2).to(on._flat.device)
+    mom = learner.momentum_net
+    shifts = augment.view_shifts(learner, "curl_shifts", states.shape[0], CURL_SHIFT_SEED)
     x_k = augment.random_shift(states, None, shifts)
     # the EMA rewrites the key trunk every step: its operand images are rebuilt here, inside every captured replay
     mom._refresh_tc_operands(force=True, h_done=True)
@@ -250,10 +213,12 @@ def positives(learner, states, debug=None):
     return z_k
 
 
-def trunk_addend(learner, z_k, debug=None):
-    """The one-shot addend DQN.backward_trunk applies (DQN._trunk_addend): given the gradient pass's kept operands and
-    the loss core's dfeat, run the anchor projection on the kept features, the InfoNCE and the projection backward (the
-    CURL gradients land in curl_net's arena) and return dfeat + dfeat_CURL."""
+def trunk_term(learner, raw_states, sequence, debug=None):
+    """CURL's term of one step on the unshifted ``raw_states``: the positives, drawn now, and the one-shot addend
+    DQN.backward_trunk applies (DQN._trunk_addend): given the gradient pass's kept operands and the loss core's dfeat,
+    run the anchor projection on the kept features, the InfoNCE and the projection backward (the CURL gradients land in
+    curl_net's arena) and return dfeat + dfeat_CURL."""
+    z_k = positives(learner, raw_states, debug)
     net, coef = learner.curl_net, learner.curl[0]
 
     def addend(keep, dfeat):

@@ -1,10 +1,8 @@
 """Device-resident per-step scalars (riqn_dyn_state, include/riqn_b200.h) so that a learner step can be captured in a
 CUDA graph once and replayed: the host rewrites this 32-byte struct with one async copy before each replay.
 
-An FQF learner keeps a second struct beside the first (``slots=2``), written by the same copy: its Adam fields are the
-fraction optimiser's bias corrections (its own learning rate), its rng_offset repeats the first one's.  A CURL learner
-adds one more for the projection's optimiser, after FQF's when both are on; an SPR learner likewise one for its
-arena's optimiser."""
+A learner keeps one slot per Learner._optimisers() entry, in that order, written by the same copy: each slot's Adam
+fields are that optimiser's bias corrections (its own learning rate), and every rng_offset repeats the first one's."""
 import struct
 
 import torch

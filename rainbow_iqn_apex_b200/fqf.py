@@ -14,18 +14,19 @@ arena, parameter order and state_dict stay those of the reference.  It lives on 
 by agent.fraction_optimiser, the arena Adam; the paper used RMSProp).  There is no target copy: fractions always come
 from the online proposal.
 """
-import weakref
-
 import torch
 from torch import nn
 
 from ._lib import call, ptr
-from .model import FEAT, _ALIGN
+from .arena import ArenaModule, Side
+from .model import FEAT
 
-class FractionProposal(nn.Module):
-    """The fraction proposal network: one linear layer ``weight`` (N, 3136), ``bias`` (N), views of one flat fp32 arena
-    (``_flat``; gradients in ``_flat_grad``) that the arena Adam steps and data parallelism reduces in one piece.
+
+class FractionProposal(ArenaModule):
+    """The fraction proposal network: one linear layer ``weight`` (N, 3136), ``bias`` (N), views of one flat fp32 arena.
     Xavier-uniform weights with gain 0.01 and a zero bias: the starting fractions are nearly uniform."""
+
+    NAMES = ("weight", "bias")
 
     def __init__(self, num_fractions, device, feat_dim=FEAT):
         super().__init__()
@@ -34,41 +35,6 @@ class FractionProposal(nn.Module):
         self.bias = nn.Parameter(torch.zeros(self.num_fractions))
         nn.init.xavier_uniform_(self.weight.data, gain=0.01)
         self._flatten(torch.device(device))
-
-    def _flatten(self, dev):
-        nw = self.weight.numel()
-        boff = (nw + _ALIGN - 1) // _ALIGN * _ALIGN
-        total = (boff + self.bias.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
-        flat = torch.zeros(total, device=dev, dtype=torch.float32)
-        flat_grad = torch.zeros(total, device=dev, dtype=torch.float32)
-        for p, off in ((self.weight, 0), (self.bias, boff)):
-            n = p.numel()
-            flat[off:off + n].copy_(p.data.reshape(-1).float())
-            p.data = flat[off:off + n].view(p.shape)
-            p.grad = flat_grad[off:off + n].view(p.shape)
-            p._riqn_owner = weakref.ref(self)
-            p._riqn_offset = off
-        self._flat, self._flat_grad = flat, flat_grad
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self._flatten(self.weight.device)
-        return out
-
-    def _params_changed(self):
-        """Called by the arena Adam after a step: nothing is cached from these weights."""
-
-    def grad_view(self, p):
-        return self._flat_grad[p._riqn_offset:p._riqn_offset + p.numel()].view(p.shape)
-
-    def zero_grad(self, set_to_none=False):
-        """One memset over the gradient arena; the .grad views stay bound."""
-        if self._flat_grad.is_cuda:
-            call("riqn_zero_f32", ptr(self._flat_grad), self._flat_grad.numel())
-        else:
-            self._flat_grad.zero_()
-        for p in (self.weight, self.bias):
-            p.grad = self.grad_view(p)
 
     def propose(self, feat):
         """Fractions of the states behind ``feat`` (B, 3136) fp32 (read only; nothing flows back into the trunk).
@@ -99,6 +65,20 @@ class FractionProposal(nn.Module):
         call("riqn_fqf_fraction_wgrad", B, N, self.feat_dim, ptr(dlogits), ptr(fr["feat"]), ptr(self.grad_view(self.weight)),
              ptr(self.grad_view(self.bias)))
         return dlogits, floss
+
+
+def build(agent, args, checkpoint):
+    """agent.fraction_net and agent.fraction_optimiser (learning rate agent.fqf[0]), restored from ``checkpoint`` when it
+    holds them.  Returns FQF's Side: the actors act on the learner's fractions, so Ape-X publishes its arena."""
+    from .optim import Adam
+    net = agent.fraction_net = FractionProposal(agent.num_tau_samples, args.device)
+    opt = agent.fraction_optimiser = Adam(net.parameters(), lr=agent.fqf[0], eps=args.adam_eps)
+    if checkpoint is not None and "fraction_net_state_dict" in checkpoint:
+        net.load_state_dict(checkpoint["fraction_net_state_dict"])
+        opt.load_state_dict(checkpoint["fraction_optimiser_state_dict"])
+    return Side(1, net, opt,
+                lambda: {"fraction_net_state_dict": net.state_dict(), "fraction_optimiser_state_dict": opt.state_dict()},
+                broadcast=(net._flat,), publish=True)
 
 
 def q_values(q, dtau, batch, num_fractions, action_space):

@@ -5,18 +5,13 @@ sample -> loss -> zero_grad -> (weights*loss).mean().backward() -> Adam.step (le
 backward driven directly (no autograd graph) and the IS weights folded into the upstream gradient
 gscale[b] = weights[b] / B.  ``north_star`` spellings Agent.learn / Agent.update_target are aliased.
 
-Under FQF every step also zeroes, fills, (all-reduces) and steps the fraction proposal's own arena
-(agent.fraction_net, agent.fraction_optimiser).  A user's own loop around ``loss.backward()`` gets the fraction gradients
-from that backward too, and must zero them (fraction_net.zero_grad()) and call fraction_optimiser.step() itself.
-
-Under CURL (curl.py) every step also contrasts the gradient pass's trunk features with a momentum encoder's, zeroes,
-fills, (all-reduces) and steps the projection's arena (agent.curl_net, agent.curl_optimiser), and after the Adam steps
-moves the momentum encoder towards the online trunk and projection.  Each rank contrasts its own local batch.
-
-Under SPR (spr.py) every step also gathers the sampled transitions' K-step sequences (ReplayMemory.sample_sequence),
-predicts their latents through the transition model, zeroes, fills, (all-reduces) and steps SPR's arena (agent.spr_net,
-agent.spr_optimiser).  Each rank predicts its own local batch.  Entry points that receive an already assembled minibatch
-without its sequence (learn_on_batch without ``sequence``, the batch and learn graphs, learn_on_host_batch) refuse.
+Every step also zeroes, fills, (all-reduces) and steps the arena of each side network (Agent.sides).  A user's own loop
+around ``loss.backward()`` gets FQF's fraction gradients from that backward too, and must zero and step that arena itself.
+Under CURL (curl.py) the step also contrasts the gradient pass's trunk features with a momentum encoder's, and after the
+Adam steps moves the momentum encoder towards the online trunk and projection.  Under SPR (spr.py) it gathers the sampled
+transitions' K-step sequences (ReplayMemory.sample_sequence) and predicts their latents; entry points that receive an
+already assembled minibatch without its sequence (learn_on_batch without ``sequence``, the batch and learn graphs,
+learn_on_host_batch) refuse.  Each rank contrasts or predicts its own local batch.
 
 Under resets (reset.py) ``updates`` counts the optimiser steps this learner has run, and after every reset_interval-th
 update the step entry points (learn_on_batch and learn through it, learn_and_update eager or replayed, learn_on_graph,
@@ -31,7 +26,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment, curl, reset, spr
+from . import augment, reset
 from .agent import Agent
 from .dynstate import DynState
 
@@ -139,19 +134,18 @@ class Learner(Agent):
                 torch.distributed.all_reduce(net._flat_grad, group=self.process_group)
 
     def _trained_nets(self):
-        """The networks whose gradient arenas a step fills: the online network, under FQF the fraction proposal, under
-        CURL the projection, under SPR its arena."""
-        return tuple(n for n in (self.online_net, self.fraction_net, self.curl_net, self.spr_net) if n is not None)
+        """The networks whose gradient arenas a step fills: the online network, then the sides'."""
+        return (self.online_net,) + tuple(side.net for side in self.sides)
 
     def _optimisers(self):
-        return tuple(o for o in (self.optimiser, self.fraction_optimiser, self.curl_optimiser, self.spr_optimiser)
-                     if o is not None)
+        return (self.optimiser,) + tuple(side.optimiser for side in self.sides)
 
     def _step_optimisers(self):
         for o in self._optimisers():
             o.step()
-        if self.curl is not None:
-            curl.momentum_update(self)
+        for side in self.sides:
+            if side.after_step is not None:
+                side.after_step(self)
 
     def _write_dyn(self, mem):
         """Stage the next step's device scalars: the Adam bias corrections of every optimiser, and the fill and beta of the
@@ -176,17 +170,16 @@ class Learner(Agent):
         raw_states = states
         if self.random_shift is not None:
             states, next_states = self._shift_frames(states, next_states, debug)
-        z_k = curl.positives(self, raw_states, debug) if self.curl is not None else None
-        spr_t = spr.targets(self, sequence[0], debug) if self.spr is not None else None
+        # CURL's or SPR's feature gradient joins the loss core's in the trunk backward (config.read allows one of them)
+        terms = [side.trunk_term(self, raw_states, sequence, debug) for side in self.sides if side.trunk_term is not None]
+        assert len(terms) <= 1, "at most one side network adds a trunk term"
         loss, bw = self.loss_core(self, states, actions, returns, next_states, nonterminals, debug=debug, demo=demo)
         for net in self._trained_nets():                                        # learner.py:22
             net.zero_grad()
         # data parallel: DQN.backward_iqn starts the all-reduce of the NoisyLinear gradients as soon as they are final
         on._grads_ready_hook = self._start_tail_allreduce if (self.process_group is not None and self.overlap_allreduce) else None
-        if z_k is not None:         # CURL's feature gradient joins the loss core's in the trunk backward
-            on._trunk_addend = curl.trunk_addend(self, z_k, debug)
-        if spr_t is not None:       # SPR's likewise
-            on._trunk_addend = spr.trunk_addend(self, sequence, spr_t, debug)
+        if terms:
+            on._trunk_addend = terms[0]
         try:
             bw(weights, 1.0 / weights.shape[0])                                 # learner.py:23 (.mean())
         finally:
@@ -200,9 +193,8 @@ class Learner(Agent):
         launch into a [s_{t+n}; s_t] buffer.  Every pass of the loss over a frame set then reads the same shifted frames.
         The shifts of the last step stay in self._shifts ((2B, 2): rows [0, B) for s_{t+n}; a graph's static buffer)."""
         on = self.online_net
-        inj = self._inject[0] if isinstance(self._inject, list) and self._inject else self._inject
         B = states.shape[0]
-        given = inj.get("shifts") if isinstance(inj, dict) else None
+        given = augment.injection(self).get("shifts")
         if given is None:
             shifts = augment.draw_shifts(on, 2 * B, self.random_shift)
         else:
@@ -246,7 +238,7 @@ class Learner(Agent):
         def route(dyn):
             self._dyn_on = dyn is not None
             self.optimiser._dyn = dyn
-            for k, o in enumerate(self._optimisers()[1:], 1):     # FQF's fraction optimiser, then CURL's or SPR's
+            for k, o in enumerate(self._optimisers()[1:], 1):     # the sides' optimisers, in Agent.sides order
                 o._dyn = dyn.slot(k) if dyn is not None else None
             if mem is not None:
                 mem.transitions._dyn = dyn

@@ -26,12 +26,12 @@ from torch import nn
 
 from . import _lib
 from ._lib import ConvGeom, NoisyLayer, SplitJob, call, ptr
+from .arena import _ALIGN, layout
 
 FEAT = 3136
 # Philox stream ids: CUDA-graph steps use (static per-step index + the device-side rng_offset = 64 * epoch); eager calls count
 # on the host.  The eager counters live in their own half of the id space so that the two can never reuse a stream.
 _EAGER_STREAMS = 1 << 39
-_ALIGN = 64  # floats; arena groups start on 256-byte boundaries
 
 # Arithmetic of the hidden NoisyLinear products (x W^T, dh W, dh^T x -- 91% of the step's FLOPs):
 #   "bf16x3": wgmma tensor cores, every operand split into bf16 hi + lo, 3 MMAs per k-step (fp32-faithful)
@@ -279,49 +279,32 @@ class DQN(nn.Module):
         """(Re)build the flat parameter / gradient / epsilon arenas on the parameters' current device."""
         groups = self._param_groups_in_arena_order()
         dev = groups[0][0].device
-        total = 0
-        offsets = []
-        for grp in groups:
-            total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
-            for p in grp:
-                offsets.append(total)
-                total += p.numel()
-        total = (total + _ALIGN - 1) // _ALIGN * _ALIGN
+        offsets, total = layout([[p.numel() for p in grp] for grp in groups])
         flat = torch.zeros(total, device=dev, dtype=torch.float32)
         flat_grad = torch.zeros(total, device=dev, dtype=torch.float32)
-        i = 0
         self._offsets = {}
-        for grp in groups:
-            for p in grp:
-                off, n = offsets[i], p.numel()
-                flat[off:off + n].copy_(p.data.reshape(-1).float())
-                p.data = flat[off:off + n].view(p.shape)
-                p.grad = flat_grad[off:off + n].view(p.shape)
-                self._offsets[id(p)] = off
-                p._riqn_owner = weakref.ref(self)
-                p._riqn_offset = off
-                i += 1
+        for p, off in zip((p for grp in groups for p in grp), offsets):
+            n = p.numel()
+            flat[off:off + n].copy_(p.data.reshape(-1).float())
+            p.data = flat[off:off + n].view(p.shape)
+            p.grad = flat_grad[off:off + n].view(p.shape)
+            self._offsets[id(p)] = off
+            p._riqn_owner = weakref.ref(self)
+            p._riqn_offset = off
         self._flat, self._flat_grad = flat, flat_grad
         self._params_changed()
-        # epsilon arena: [h_v.weight_epsilon | h_a.weight_epsilon], h bias eps, [z_v | z_a] weight eps, z bias eps
+        # epsilon arena: [h_v.weight_epsilon | h_a.weight_epsilon], h bias eps, [z_v | z_a] weight eps, z bias eps, then
+        # _ALIGN floats past the last one
         hv, ha, zv, za = self.fcnoisy_h_v, self.fcnoisy_h_a, self.fcnoisy_z_v, self.fcnoisy_z_a
         eg = [[(hv, "weight_epsilon"), (ha, "weight_epsilon")], [(hv, "bias_epsilon"), (ha, "bias_epsilon")],
               [(zv, "weight_epsilon"), (za, "weight_epsilon")], [(zv, "bias_epsilon"), (za, "bias_epsilon")]]
-        etotal, eoffs = 0, []
-        for grp in eg:
-            etotal = (etotal + _ALIGN - 1) // _ALIGN * _ALIGN
-            for m, name in grp:
-                eoffs.append(etotal)
-                etotal += m._buffers[name].numel()
-        eflat = torch.zeros(etotal + _ALIGN, device=dev, dtype=torch.float32)
-        i = 0
-        for grp in eg:
-            for m, name in grp:
-                old = m._buffers[name]
-                n = old.numel()
-                eflat[eoffs[i]:eoffs[i] + n].copy_(old.reshape(-1).float())
-                m._buffers[name] = eflat[eoffs[i]:eoffs[i] + n].view(old.shape)
-                i += 1
+        bufs = [(m, name, m._buffers[name]) for grp in eg for m, name in grp]
+        eoffs, _ = layout([[m._buffers[name].numel() for m, name in grp] for grp in eg])
+        eflat = torch.zeros(eoffs[-1] + bufs[-1][2].numel() + _ALIGN, device=dev, dtype=torch.float32)
+        for (m, name, old), off in zip(bufs, eoffs):
+            n = old.numel()
+            eflat[off:off + n].copy_(old.reshape(-1).float())
+            m._buffers[name] = eflat[off:off + n].view(old.shape)
         self._eps_flat = eflat
         # composed (effective) weights, concatenated like the arenas
         hid = self.hidden
@@ -910,7 +893,7 @@ class DQN(nn.Module):
 
     def backward_trunk(self, keep, dfeat):
         """conv3 -> conv1 backward of the trunk pass kept in ``keep`` for the feature gradient ``dfeat`` (B, 3136).  An
-        addend armed in ``self._trunk_addend`` (CURL, curl.trunk_addend) is consumed first: ``dfeat`` becomes
+        addend armed in ``self._trunk_addend`` (CURL's or SPR's trunk_term) is consumed first: ``dfeat`` becomes
         ``addend(keep, dfeat)``."""
         addend, self._trunk_addend = getattr(self, "_trunk_addend", None), None
         if addend is not None:

@@ -61,16 +61,10 @@ def make_data_parallel(learner, group=None):
             m._noise_calls = 0
         if net._flat.is_cuda:
             net.compose_weights()
-    if getattr(learner, "fraction_net", None) is not None:        # FQF: the fraction proposal's own arena
-        dist.broadcast(learner.fraction_net._flat, src=0, group=group)
-        learner.fraction_optimiser.grad_scale = 1.0 / world
-    if getattr(learner, "curl_net", None) is not None:             # CURL: the projection and the momentum encoder
-        for t in (learner.curl_net._flat, learner.momentum_net._flat, learner.momentum_projection):
+    for side in getattr(learner, "sides", ()):                     # the side networks' arenas (arena.Side)
+        for t in side.broadcast:
             dist.broadcast(t, src=0, group=group)
-        learner.curl_optimiser.grad_scale = 1.0 / world
-    if getattr(learner, "spr_net", None) is not None:              # SPR: projection, transition model, predictor
-        dist.broadcast(learner.spr_net._flat, src=0, group=group)
-        learner.spr_optimiser.grad_scale = 1.0 / world
+        side.optimiser.grad_scale = 1.0 / world
     learner.process_group = group if group is not None else dist.group.WORLD
     learner.optimiser.grad_scale = 1.0 / world
     return learner
@@ -85,8 +79,9 @@ def publish_parameters(agent, src=0, group=None):
         return
     net = agent.online_net
     dist.broadcast(net._flat, src=src, group=group)
-    if getattr(agent, "fraction_net", None) is not None:          # FQF: actors act on the learner's fractions
-        dist.broadcast(agent.fraction_net._flat, src=src, group=group)
+    for side in getattr(agent, "sides", ()):                       # FQF: actors act on the learner's fractions
+        if side.publish:
+            dist.broadcast(side.net._flat, src=src, group=group)
     if dist.get_rank(group) != src and net._flat.is_cuda:
         net.compose_weights()
 

@@ -61,13 +61,9 @@ def shrink(agent):
     return agent.reset[1] if agent.reset is not None else config.FIELDS["reset_shrink"][0]
 
 
-def tables(agent):
-    """[(arena index, module, optimiser, sorted segments)] of every arena ``agent`` trains."""
-    a_s = shrink(agent)
-    keep_trunk = a_s == 1.0
-    on = agent.online_net
+def _online_segments(on, a_s):
     segs = []
-    if not keep_trunk:
+    if a_s != 1.0:
         for conv in (on.conv1, on.conv2, on.conv3):
             segs += _linear(conv.weight, conv.bias, conv.weight[0].numel(), a_s)
     if on._embeds():
@@ -77,23 +73,36 @@ def tables(agent):
         segs += [_seg(m.weight_mu, UNIFORM, bound, 0.0), _seg(m.bias_mu, UNIFORM, bound, 0.0),
                  _seg(m.weight_sigma, CONSTANT, m.std_init / math.sqrt(m.in_features), 0.0),
                  _seg(m.bias_sigma, CONSTANT, m.std_init / math.sqrt(m.out_features), 0.0)]
-    out = [(0, on, agent.optimiser, segs)]
-    if agent.fraction_net is not None:
-        f = agent.fraction_net
-        bound = 0.01 * math.sqrt(6.0 / (f.feat_dim + f.num_fractions))
-        out.append((1, f, agent.fraction_optimiser, [_seg(f.weight, UNIFORM, bound, 0.0), _seg(f.bias, CONSTANT, 0.0, 0.0)]))
-    if agent.curl_net is not None:
-        c = agent.curl_net
-        segs = _linear(c.weight_h, c.bias_h, FEAT, 0.0) + _linear(c.weight_c, c.bias_c, c.weight_c.shape[1], 0.0)
-        out.append((2, c, agent.curl_optimiser, segs + _linear(c.bilinear, None, c.bilinear.shape[1], 0.0)))
-    if agent.spr_net is not None:
-        s = agent.spr_net
-        segs = _linear(s.weight_h, s.bias_h, FEAT, 0.0) + _linear(s.weight_c, s.bias_c, s.weight_c.shape[1], 0.0)
-        if not keep_trunk:
-            for conv in (s.conv1, s.conv2):
-                segs += _linear(conv.weight, conv.bias, conv.weight[0].numel(), a_s)
-        out.append((3, s, agent.spr_optimiser, segs + _linear(s.weight_q, s.bias_q, s.weight_q.shape[1], 0.0)))
-    return [(k, net, opt, sorted(segs)) for k, net, opt, segs in out]
+    return segs
+
+
+def _fraction_segments(f, a_s):
+    bound = 0.01 * math.sqrt(6.0 / (f.feat_dim + f.num_fractions))
+    return [_seg(f.weight, UNIFORM, bound, 0.0), _seg(f.bias, CONSTANT, 0.0, 0.0)]
+
+
+def _curl_segments(c, a_s):
+    segs = _linear(c.weight_h, c.bias_h, FEAT, 0.0) + _linear(c.weight_c, c.bias_c, c.weight_c.shape[1], 0.0)
+    return segs + _linear(c.bilinear, None, c.bilinear.shape[1], 0.0)
+
+
+def _spr_segments(s, a_s):
+    segs = _linear(s.weight_h, s.bias_h, FEAT, 0.0) + _linear(s.weight_c, s.bias_c, s.weight_c.shape[1], 0.0)
+    if a_s != 1.0:
+        for conv in (s.conv1, s.conv2):
+            segs += _linear(conv.weight, conv.bias, conv.weight[0].numel(), a_s)
+    return segs + _linear(s.weight_q, s.bias_q, s.weight_q.shape[1], 0.0)
+
+
+_SEGMENTS = (_online_segments, _fraction_segments, _curl_segments, _spr_segments)    # by arena index, as ARENAS
+
+
+def tables(agent):
+    """[(arena index, module, optimiser, sorted segments)] of every arena ``agent`` trains: the online network's, then
+    the sides'."""
+    a_s = shrink(agent)
+    arenas = [(0, agent.online_net, agent.optimiser)] + [(s.index, s.net, s.optimiser) for s in agent.sides]
+    return [(k, net, opt, sorted(_SEGMENTS[k](net, a_s))) for k, net, opt in arenas]
 
 
 def reset_arena(net, optimiser, segs, seed, stream_id):
@@ -109,7 +118,8 @@ def reset(agent, index):
     seed = agent.online_net._rng_seed ^ RESET_SEED
     for k, net, opt, segs in tables(agent):
         reset_arena(net, opt, segs, seed, index * len(ARENAS) + k)
-    if agent.curl_net is not None:
-        agent.momentum_projection.copy_(agent.curl_net._flat[:agent.curl_net.proj_numel])
+    for side in agent.sides:
+        if side.after_reset is not None:
+            side.after_reset(agent)
     agent.online_net._params_changed()
     agent.online_net.compose_weights()

@@ -42,7 +42,8 @@ from torch import nn
 
 from . import augment
 from ._lib import call, ptr
-from .curl import DIM, HIDDEN, ArenaModule, project, project_backward
+from .arena import Side
+from .curl import DIM, HIDDEN, ProjectionArena, project, project_backward
 from .model import FEAT, _geom, _strip_perm
 
 SPR_SHIFT_SEED = 0x59E2          # the target views' draw key (net._rng_seed ^ this)
@@ -50,7 +51,7 @@ CH, EDGE, GRID = 64, 7, 9        # latent channels and edge, zero-bordered edge
 CPAD = 128                       # conv1's input channels: the latent, the one-hot action planes, zeros
 
 
-class SprNet(ArenaModule):
+class SprNet(ProjectionArena):
     """SPR's trained parameters, views of one flat fp32 arena laid out weight_h (512, 3136) | bias_h | weight_c
     (128, 512) | bias_c | conv1.weight (64, 64 + A, 3, 3) | conv1.bias | conv2.weight (64, 64, 3, 3) | conv2.bias |
     weight_q (128, 128) | bias_q, the projection first so that curl.project / curl.project_backward serve it.  Initialised
@@ -88,13 +89,15 @@ class SprNet(ArenaModule):
 
 def build(agent, args, checkpoint):
     """agent.spr_net and agent.spr_optimiser (after every other module), restored from ``checkpoint`` when it holds
-    them."""
+    them.  Returns SPR's Side."""
     from .optim import Adam
-    agent.spr_net = SprNet(agent.action_space, args.device)
-    agent.spr_optimiser = Adam(agent.spr_net.parameters(), lr=args.lr, eps=args.adam_eps)
+    net = agent.spr_net = SprNet(agent.action_space, args.device)
+    opt = agent.spr_optimiser = Adam(net.parameters(), lr=args.lr, eps=args.adam_eps)
     if checkpoint is not None and "spr_state_dict" in checkpoint:
-        agent.spr_net.load_state_dict(checkpoint["spr_state_dict"])
-        agent.spr_optimiser.load_state_dict(checkpoint["spr_optimiser_state_dict"])
+        net.load_state_dict(checkpoint["spr_state_dict"])
+        opt.load_state_dict(checkpoint["spr_optimiser_state_dict"])
+    return Side(3, net, opt, lambda: {"spr_state_dict": net.state_dict(), "spr_optimiser_state_dict": opt.state_dict()},
+                broadcast=(net._flat,), trunk_term=trunk_term)
 
 
 def _bf(rows, cols, dev):
@@ -148,12 +151,7 @@ def targets(learner, window, debug=None):
     x = torch.empty(K * B, H, 84, 84, dtype=torch.uint8, device=dev)
     shifts = None
     if learner.random_shift is not None:
-        inj = learner._inject[0] if isinstance(learner._inject, list) and learner._inject else learner._inject
-        given = inj.get("spr_shifts") if isinstance(inj, dict) else None
-        if given is None:
-            shifts = augment.draw_shifts(on, K * B, learner.random_shift, key=SPR_SHIFT_SEED, advance=False)
-        else:
-            shifts = torch.as_tensor(given, dtype=torch.int32).reshape(K * B, 2).to(dev)
+        shifts = augment.view_shifts(learner, "spr_shifts", K * B, SPR_SHIFT_SEED)
         for k in range(K):
             v = window[:, k + 1:k + 1 + H]
             call("riqn_random_shift", B, H, 84, 84, ptr(v), v.stride(0), None, 0, 1, ptr(shifts[k * B:]), ptr(x[k * B:]))
@@ -169,11 +167,13 @@ def targets(learner, window, debug=None):
     return t
 
 
-def trunk_addend(learner, sequence, t, debug=None):
-    """The one-shot addend DQN.backward_trunk applies (DQN._trunk_addend): from the gradient pass's kept conv3 output,
-    unroll T over the sequence's actions, project and predict, run the masked cosine and backpropagate (the SPR
-    gradients land in spr_net's arena); return dfeat + dfeat_SPR.  ``sequence``: (window, actions (B, K), valid (B, K))
-    of ReplayMemory.sample_sequence; ``t``: targets()."""
+def trunk_term(learner, raw_states, sequence, debug=None):
+    """SPR's term of one step on its ``sequence`` ((window, actions (B, K), valid (B, K)) of
+    ReplayMemory.sample_sequence): the targets, computed now, and the one-shot addend DQN.backward_trunk applies
+    (DQN._trunk_addend): from the gradient pass's kept conv3 output, unroll T over the sequence's actions, project and
+    predict, run the masked cosine and backpropagate (the SPR gradients land in spr_net's arena); return
+    dfeat + dfeat_SPR."""
+    t = targets(learner, sequence[0], debug)
     net, (K, coef) = learner.spr_net, learner.spr
     _, actions, valid = sequence
 
