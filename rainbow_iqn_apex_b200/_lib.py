@@ -126,6 +126,7 @@ SIGNATURES = {
     "riqn_linear_dgrad_ld": [C.c_long, C.c_int, C.c_int, _P, C.c_long, _P, _P, C.c_long, _P],
     "riqn_noisy_wgrad_ld": [C.c_long, C.c_int, C.c_int, _P, C.c_long, _P, C.c_long, _P, _P, _P, _P],
     "riqn_adam_step": [C.c_long, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _P, _P],
+    "riqn_adamw_step": [C.c_long, _P, _P, _P, _P, C.c_int] + [C.c_float] * 6 + [_P, _P],
     "riqn_sumtree_stratified": [C.c_int, C.c_ulonglong, C.c_ulonglong, _P, _P, _P, _P],
     "riqn_sumtree_sample": [C.c_int, C.c_long, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P],
     "riqn_sumtree_is_weights": [C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P, _P, _P],

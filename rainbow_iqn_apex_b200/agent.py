@@ -11,9 +11,11 @@ for MMDQN's moment-matching loss on that head (mmd.py), ``hl_gauss`` for HL-Gaus
 head (hl_gauss.py), ``cql`` for the conservative regulariser of the IQN and QR-DQN losses (cql.py), ``dqfd`` for DQfD's
 large-margin loss on demonstrations (dqfd.py), ``random_shift`` for the learner's random-shift augmentation
 (augment.py), ``curl`` for CURL's contrastive loss on the trunk (curl.py), ``spr`` for SPR's self-predictive loss on the
-trunk (spr.py), and ``reset`` (reset_interval, reset_shrink) with ``updates`` / ``resets`` for the learner's periodic
-network resets (reset.py).  The networks FQF, CURL and SPR train beside the DQN and their optimisers are set by those
-modules' ``build`` (None when off), and ``sides`` lists them (arena.Side).  The networks are
+trunk (spr.py), ``reset`` (reset_interval, reset_shrink) with ``updates`` / ``resets`` for the learner's periodic
+network resets (reset.py), ``target_ema`` (tau) for the learner's EMA target network (target.py) and ``adamw`` (the
+weight decay) for AdamW in every optimiser the agent builds.  The networks FQF, CURL and SPR train beside the DQN and
+their optimisers are set by those modules' ``build`` (None when off), and ``sides`` lists them (arena.Side).  The
+networks are
 rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference schema
 {T_actors, T_learner, model_state_dict, optimiser_state_dict} (agent.py:150-160), plus, under resets, reset_state and
 each side's entries.
@@ -64,11 +66,14 @@ class Agent:
             self.online_net.load_state_dict(checkpoint["model_state_dict"])
         self.target_net = DQN(args, action_space).to(device=args.device)
         self.update_target_net()
+        if self.target_ema is not None and checkpoint is not None and "target_state_dict" in checkpoint:
+            self.target_net.load_state_dict(checkpoint["target_state_dict"])     # an EMA target is not the online net
+            self.target_net.compose_weights()
         for net in (self.online_net, self.target_net):
             net.train()                                  # the target stays in train mode: it is noisy too
         for p in self.target_net.parameters():
             p.requires_grad = False
-        self.optimiser = Adam(self.online_net.parameters(), lr=args.lr, eps=args.adam_eps)
+        self.optimiser = Adam(self.online_net.parameters(), lr=args.lr, eps=args.adam_eps, weight_decay=self.adamw or 0.0)
         if checkpoint is not None:
             self.optimiser.load_state_dict(checkpoint["optimiser_state_dict"])
 
@@ -101,7 +106,7 @@ class Agent:
         # order FQF, CURL, SPR: every network initialises from a seed as it would without the later ones
         self.fraction_net = self.fraction_optimiser = None
         self.curl_net = self.curl_optimiser = self.momentum_net = self.momentum_projection = None
-        self.spr_net = self.spr_optimiser = None
+        self.spr_net = self.spr_optimiser = self.spr_ema_projection = None
         self.sides = tuple(module.build(self, args, checkpoint)
                            for on, module in ((self.fqf, fqf), (self.curl, curl), (self.spr, spr)) if on is not None)
         # optimiser steps run and resets done (Learner.reset_networks): a resumed run resets at the same updates with the
@@ -152,8 +157,10 @@ class Agent:
 
     def save(self, path, T_actors, T_learner, name):
         """agent.py:150-160.  Under value rescaling the checkpoint also holds value_rescaling_eps, under QR-DQN
-        qr_dqn_quantiles (N), under resets reset_state = (updates, resets), and each side network's entries (Side.checkpoint);
-        model_state_dict keeps the reference schema either way."""
+        qr_dqn_quantiles (N), under resets reset_state = (updates, resets), under target_ema target_state_dict (the EMA
+        target, which the online network no longer determines; a checkpoint without it starts the target at the online
+        network), and each side network's entries (Side.checkpoint); model_state_dict keeps the reference schema either
+        way."""
         ckpt = {
             "T_actors": T_actors,
             "T_learner": T_learner,
@@ -166,6 +173,8 @@ class Agent:
             ckpt["qr_dqn_quantiles"] = self.qr_dqn
         if self.reset is not None:
             ckpt["reset_state"] = (self.updates, self.resets)
+        if self.target_ema is not None:
+            ckpt["target_state_dict"] = self.target_net.state_dict()
         for side in self.sides:
             ckpt.update(side.checkpoint())
         torch.save(ckpt, os.path.join(path, name))

@@ -104,6 +104,10 @@ FIELDS = {
     "reset": (0, switch),
     "reset_interval": (40000, integer(1, math.inf)),              # this project's starting point, not tuned
     "reset_shrink": (0.5, real(lambda x: 0.0 <= x <= 1.0, "in [0, 1]")),
+    "target_ema": (0, switch),
+    "target_ema_tau": (0.005, real(lambda x: 0.0 < x <= 1.0, "in (0, 1]")),      # BBF's two
+    "adamw": (0, switch),
+    "adamw_weight_decay": (0.1, real(lambda x: x >= 0.0, ">= 0")),
     "demo_segments": (0, integer(0, math.inf)),                   # at most nb_actor (read_demo)
     "demo_priority_bonus": (0.0, real(lambda x: x >= 0.0, ">= 0")),
 }
@@ -155,12 +159,15 @@ def read_risk(head, loss, measure, eta=None):
 
 def read(args, action_space):
     """Validate the optional fields of ``args`` and return what the agent stores, as a dict: qr_dqn (N or None); per
-    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr, reset) None when off, else its
-    parameter or the tuple of its parameters; random_shift (the pad, or None); risk (model.check_risk's); and the "head"
-    and the "loss" variant (or None) they select.  Resets combine with every head and variant."""
+    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr, reset, target_ema, adamw) None
+    when off, else its parameter or the tuple of its parameters; random_shift (the pad, or None); risk
+    (model.check_risk's); and the "head" and the "loss" variant (or None) they select.  Resets, the EMA target
+    (target_ema: tau) and AdamW (adamw: the weight decay lambda) combine with every head and variant; AdamW needs
+    lr * lambda < 1 for the agent's lr and, under FQF, for fqf_fraction_lr, as the float32 values the optimiser receives."""
     head, n = read_head(args, action_space)
     v = {"qr_dqn": n}
-    for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl", "spr", "reset"):
+    for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl", "spr", "reset",
+                 "target_ema", "adamw"):
         v[name] = None
         if field(args, name):
             params = tuple(field(args, f) for f in FIELDS if f.startswith(name + "_"))
@@ -194,6 +201,12 @@ def read(args, action_space):
         if history + v["spr"][0] > 16:
             raise ValueError(f"spr_steps + history_length must be at most 16 (the sequence window), got "
                              f"{v['spr'][0]} + {history}")
+    if v["adamw"] is not None:
+        lrs = [("lr", args.lr)] + ([("fqf_fraction_lr", v["fqf"][0])] if v["fqf"] is not None else [])
+        for name, lr in lrs:
+            if not 0.0 <= _f32(lr) * v["adamw"] < 1.0:       # riqn_adamw_step's decay 1 - lr * lambda in (0, 1]
+                raise ValueError(f"adamw_weight_decay decays by 1 - {name} * adamw_weight_decay, which must be in (0, 1]: "
+                                 f"{name} = {lr!r}, adamw_weight_decay = {v['adamw']!r}")
     v["risk"] = read_risk(head, loss, getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
     return dict(v, head=head, loss=loss)
 

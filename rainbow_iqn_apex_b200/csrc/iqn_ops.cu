@@ -1368,11 +1368,14 @@ __global__ void embed_bwd_elem_kernel(int B, int Nq, int F, const float* __restr
 }
 
 // ------------------------------------------------------------------------------------------------
-// Adam over a flat fp32 arena (torch.optim.Adam semantics; agent.py:43, learner.py:24)
+// Adam over a flat fp32 arena (torch.optim.Adam semantics; agent.py:43, learner.py:24).  kDecay: AdamW's decoupled
+// decay first, theta <- fl(theta * decay) with decay = fl32(1 - lr * weight_decay), then the same update on the decayed
+// theta (torch.optim.AdamW).  `decay` is the last parameter, so that the Adam instantiation keeps its parameter layout
 // ------------------------------------------------------------------------------------------------
+template <bool kDecay>
 __global__ void adam_kernel(long n, float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                             float* __restrict__ v, float neg_step_size, float sqrt_bc2, float eps, float b1, float b2,
-                            float grad_scale, const riqn_dyn_state* __restrict__ dyn) {
+                            float grad_scale, const riqn_dyn_state* __restrict__ dyn, float decay) {
   if (dyn) { neg_step_size = dyn->adam_neg_step_size; sqrt_bc2 = dyn->adam_sqrt_bc2; }
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     const float gi = g[i] * grad_scale;
@@ -1381,7 +1384,8 @@ __global__ void adam_kernel(long n, float* __restrict__ p, const float* __restri
     m[i] = mi;
     v[i] = vi;
     const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), sqrt_bc2), eps);   // (v.sqrt() / sqrt(bc2)).add_(eps)
-    p[i] = __fadd_rn(p[i], __fdiv_rn(__fmul_rn(neg_step_size, mi), denom)); // addcdiv_(m, denom, value=-step_size)
+    const float pi = kDecay ? __fmul_rn(p[i], decay) : p[i];              // AdamW: param.mul_(1 - lr * weight_decay)
+    p[i] = __fadd_rn(pi, __fdiv_rn(__fmul_rn(neg_step_size, mi), denom));   // addcdiv_(m, denom, value=-step_size)
   }
 }
 
@@ -2039,7 +2043,24 @@ RIQN_API int riqn_adam_step(long n, float* params, const float* grads, float* ex
   riqn::note_launches(1);
   const double bc1 = 1.0 - pow((double)beta1, (double)step);
   const double bc2 = 1.0 - pow((double)beta2, (double)step);
-  adam_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(n, params, grads, exp_avg, exp_avg_sq, (float)(-(lr / bc1)),
-                                                            (float)sqrt(bc2), eps, beta1, beta2, grad_scale, dyn);
+  adam_kernel<false><<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(n, params, grads, exp_avg, exp_avg_sq,
+                                                                   (float)(-(lr / bc1)), (float)sqrt(bc2), eps, beta1,
+                                                                   beta2, grad_scale, dyn, 1.f);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_adamw_step(long n, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int step,
+                             float lr, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
+                             const riqn_dyn_state* dyn, void* stream) {
+  if (n < 1 || !params || !grads || !exp_avg || !exp_avg_sq || !isfinite(weight_decay) || weight_decay < 0.f)
+    return (int)cudaErrorInvalidValue;
+  const float decay = (float)(1.0 - (double)lr * (double)weight_decay);
+  if (!(decay > 0.f) || !(decay <= 1.f)) return (int)cudaErrorInvalidValue;
+  riqn::note_launches(1);
+  const double bc1 = 1.0 - pow((double)beta1, (double)step);
+  const double bc2 = 1.0 - pow((double)beta2, (double)step);
+  adam_kernel<true><<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(n, params, grads, exp_avg, exp_avg_sq,
+                                                                  (float)(-(lr / bc1)), (float)sqrt(bc2), eps, beta1,
+                                                                  beta2, grad_scale, dyn, decay);
   return (int)cudaGetLastError();
 }

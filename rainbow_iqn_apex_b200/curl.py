@@ -151,7 +151,7 @@ def build(agent, args, checkpoint):
     CURL's Side."""
     net = agent.curl_net = CurlProjection(args.device)
     from .optim import Adam
-    opt = agent.curl_optimiser = Adam(net.parameters(), lr=args.lr, eps=args.adam_eps)
+    opt = agent.curl_optimiser = Adam(net.parameters(), lr=args.lr, eps=args.adam_eps, weight_decay=agent.adamw or 0.0)
     agent.momentum_net = DQN(args, agent.action_space).to(device=args.device)
     agent.momentum_projection = torch.empty(net.proj_numel, device=net._flat.device)
     if checkpoint is not None and "curl_state_dict" in checkpoint:

@@ -72,7 +72,8 @@ def build(agent, args, checkpoint):
     holds them.  Returns FQF's Side: the actors act on the learner's fractions, so Ape-X publishes its arena."""
     from .optim import Adam
     net = agent.fraction_net = FractionProposal(agent.num_tau_samples, args.device)
-    opt = agent.fraction_optimiser = Adam(net.parameters(), lr=agent.fqf[0], eps=args.adam_eps)
+    opt = agent.fraction_optimiser = Adam(net.parameters(), lr=agent.fqf[0], eps=args.adam_eps,
+                                                weight_decay=agent.adamw or 0.0)
     if checkpoint is not None and "fraction_net_state_dict" in checkpoint:
         net.load_state_dict(checkpoint["fraction_net_state_dict"])
         opt.load_state_dict(checkpoint["fraction_optimiser_state_dict"])

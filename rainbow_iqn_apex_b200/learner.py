@@ -19,6 +19,10 @@ learn_on_host_batch) call reset_networks() before they return: one eager launch 
 inside a captured graph.  The warm-up steps of a capture count; a reset that falls due during them runs when the
 enable_* call returns (one, however many fell due).  reset_networks() is public, for a schedule of one's own or a loop
 of one's own around loss.backward().
+
+Under target_ema (target.py) every step ends with the EMA of the target network, after the optimisers and the sides'
+after_step hooks, eagerly and in every captured graph.  Under adamw every optimiser is AdamW; a captured graph holds
+each one's decay 1 - lr * weight_decay by value, so a replay after an lr or weight_decay change raises.
 """
 import contextlib
 import io
@@ -26,7 +30,7 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment, reset
+from . import augment, reset, target
 from .agent import Agent
 from .dynstate import DynState
 
@@ -41,6 +45,7 @@ class _StepGraph(NamedTuple):
     mem: object          # the replay memory whose fill and beta every replay writes into the struct, or None
     inputs: tuple        # the static input buffers a replay copies its batch into, or None (the step samples them)
     out: object          # the static outputs, overwritten by every replay
+    decay: tuple         # every optimiser's AdamW decay factor (Adam.decay) that the graph holds by value
 
 
 class Learner(Agent):
@@ -146,6 +151,7 @@ class Learner(Agent):
         for side in self.sides:
             if side.after_step is not None:
                 side.after_step(self)
+        target.update(self)
 
     def _write_dyn(self, mem):
         """Stage the next step's device scalars: the Adam bias corrections of every optimiser, and the fill and beta of the
@@ -287,6 +293,8 @@ class Learner(Agent):
             torch.cuda.synchronize()
             self._write_dyn(mem)
             self.online_net._static_ops_dirty = True     # the captured step must rebuild the conv / iqn_fc operand images
+            if self.target_ema is not None:              # and, as the EMA rewrites it every step, the target's
+                self.target_net._static_ops_dirty = True
             if split:
                 self.overlap_allreduce = False
             graph, post_graph = torch.cuda.CUDAGraph(), None
@@ -301,13 +309,17 @@ class Learner(Agent):
         # the capture itself does not execute the step: undo the host-side counters it advanced
         for o, s0 in zip(self._optimisers(), step0):
             o._step = s0 + warmup
-        self._graphs[kind] = _StepGraph(graph, post_graph, mem, inputs, out)
+        self._graphs[kind] = _StepGraph(graph, post_graph, mem, inputs, out, self._decays())
         self._count_updates(warmup)     # after the counters are set: a reset here restarts them for good
 
     def _replay(self, g, batch=None):
         """One step through the captured graph ``g``: ``batch`` (if given) into its static inputs, the struct written from
         the memory it was captured on, the replay (with an eager all-reduce: then the collective and the post graph).
         Returns the static outputs."""
+        if self._decays() != g.decay:
+            raise RuntimeError("this learner's step is captured in a CUDA graph that holds each optimiser's AdamW decay "
+                               "1 - lr * weight_decay, and an lr or weight_decay has changed since: call release_graphs(), "
+                               "then recapture (enable_cuda_graph / enable_batch_graph / enable_learn_graph)")
         if batch is not None:
             for d, src in zip(g.inputs, batch):
                 d.copy_(src, non_blocking=True)
@@ -320,6 +332,9 @@ class Learner(Agent):
             o._step += 1
         self._count_updates(1)
         return g.out
+
+    def _decays(self):
+        return tuple(o.decay() for o in self._optimisers())
 
     def enable_cuda_graph(self, mem, warmup=3, capture_collectives=True):
         """Capture learn_and_update(mem) in a CUDA graph (shapes are static: batch_size, N, N', K).  Everything that

@@ -22,8 +22,8 @@ step 0, so the next step takes torch's step-1 bias corrections, eagerly and in a
 momentum projection is set to the new projection (as curl.build does at construction) and the online network's
 composed weights are rebuilt, so acting right after a reset sees the new weights.
 
-Untouched: the target network (it bootstraps from the pre-reset network until the next update_target_net), the epsilon
-arenas, and CURL's momentum trunk (it keeps following the online trunk by EMA).  Each draw is keyed by
+Untouched: the target network (it bootstraps from the pre-reset network until the next update_target_net; under
+target_ema it follows the reset online network at rate tau from the next step on, target.py), the epsilon arenas, and CURL's momentum trunk (it keeps following the online trunk by EMA).  Each draw is keyed by
 online_net._rng_seed ^ RESET_SEED with stream id (reset index) * 4 + arena index; data-parallel replicas share that seed
 (parallel.make_data_parallel), so every rank draws the same reset without a collective.  Under Ape-X only the learner
 rank resets; the actors receive the reset weights with the next publication.

@@ -9,6 +9,8 @@ learner's (shifted) state, a_t .. a_{t+K-1} the logged actions and valid_k the m
   z_k = T(z_{k-1}, a_{t+k-1}),  k = 1..K,  T(z, a) = ReLU(conv2(ReLU(conv1([z ; onehot(a)]))))   (3x3, padding 1, 64)
   y_k = q(g(z_k))                          q: Linear(128, 128) with bias (the predictor)
   t_k = g(f_theta(s'_{t+k}))               no gradient; s'_{t+k} an independent random shift of s_{t+k}
+                                           (under target_ema: g_xi(f_xi(s'_{t+k})), the EMA target network's trunk and
+                                           an EMA copy of g at the target's tau, BBF's setting)
   g(feat) = LN(W_c ReLU(LN(W_h feat + b_h)) + b_c)          (3136 -> 512 -> 128, curl.project, SPR's own parameters)
   L_SPR = (1/B) sum_b sum_k valid_{b,k} (-cos(y_{b,k}, t_{b,k}))   (F.normalize's eps 1e-12 on both norms)
 
@@ -88,16 +90,39 @@ class SprNet(ProjectionArena):
 
 
 def build(agent, args, checkpoint):
-    """agent.spr_net and agent.spr_optimiser (after every other module), restored from ``checkpoint`` when it holds
-    them.  Returns SPR's Side."""
+    """agent.spr_net and agent.spr_optimiser (after every other module), and under target_ema agent.spr_ema_projection
+    (g_xi, set to g_theta), restored from ``checkpoint`` when it holds them.  Returns SPR's Side."""
     from .optim import Adam
     net = agent.spr_net = SprNet(agent.action_space, args.device)
-    opt = agent.spr_optimiser = Adam(net.parameters(), lr=args.lr, eps=args.adam_eps)
+    opt = agent.spr_optimiser = Adam(net.parameters(), lr=args.lr, eps=args.adam_eps, weight_decay=agent.adamw or 0.0)
+    agent.spr_ema_projection = None
     if checkpoint is not None and "spr_state_dict" in checkpoint:
         net.load_state_dict(checkpoint["spr_state_dict"])
         opt.load_state_dict(checkpoint["spr_optimiser_state_dict"])
-    return Side(3, net, opt, lambda: {"spr_state_dict": net.state_dict(), "spr_optimiser_state_dict": opt.state_dict()},
-                broadcast=(net._flat,), trunk_term=trunk_term)
+    if agent.target_ema is None:
+        return Side(3, net, opt, lambda: {"spr_state_dict": net.state_dict(), "spr_optimiser_state_dict": opt.state_dict()},
+                    broadcast=(net._flat,), trunk_term=trunk_term)
+    agent.spr_ema_projection = torch.empty(net.proj_numel, device=net._flat.device)
+    if checkpoint is not None and "spr_ema_projection" in checkpoint:
+        agent.spr_ema_projection.copy_(checkpoint["spr_ema_projection"])
+    else:
+        copy_projection(agent)
+    return Side(3, net, opt,
+                lambda: {"spr_state_dict": net.state_dict(), "spr_optimiser_state_dict": opt.state_dict(),
+                         "spr_ema_projection": agent.spr_ema_projection.detach().cpu().clone()},
+                broadcast=(net._flat, agent.spr_ema_projection), after_step=ema_projection_update,
+                after_reset=copy_projection, trunk_term=trunk_term)
+
+
+def copy_projection(agent):
+    """g_xi <- g_theta: the EMA projection set to the online one (at construction and after a reset)."""
+    agent.spr_ema_projection.copy_(agent.spr_net._flat[:agent.spr_net.proj_numel])
+
+
+def ema_projection_update(learner):
+    """g_xi <- g_xi + tau (g_theta - g_xi) at the target's tau (after the optimiser steps)."""
+    net = learner.spr_net
+    call("riqn_ema_f32", net.proj_numel, ptr(net._flat), ptr(learner.spr_ema_projection), learner.target_ema)
 
 
 def _bf(rows, cols, dev):
@@ -145,8 +170,11 @@ def transition_backward(net, ims, saved, out, dout, gw1_pad):
 def targets(learner, window, debug=None):
     """t_k of one step, (K*B, 128) with rows k*B + b: the online trunk (no gradient) over independent shifts of
     s_{t+1} .. s_{t+K} = window[:, k:k+history] (drawn after the step's shifts of s_t and s_{t+n}, under SPR_SHIFT_SEED
-    and without moving the shift counters, or the parity hook's ``"spr_shifts"`` (K*B, 2) int32), then g."""
-    on, K, H = learner.online_net, learner.spr[0], learner.history
+    and without moving the shift counters, or the parity hook's ``"spr_shifts"`` (K*B, 2) int32), then g.  Under
+    target_ema the EMA target network's trunk and the EMA projection instead (BBF's target encoder)."""
+    ema = learner.target_ema is not None
+    on = learner.target_net if ema else learner.online_net
+    K, H = learner.spr[0], learner.history
     B, dev = window.shape[0], on._flat.device
     x = torch.empty(K * B, H, 84, 84, dtype=torch.uint8, device=dev)
     shifts = None
@@ -161,7 +189,7 @@ def targets(learner, window, debug=None):
     if getattr(on, "_strip_ops", None) is None or getattr(on, "_static_ops_dirty", True):
         on._refresh_tc_operands(h_done=True)         # the trunk's images, as the loss core would build them
     net = learner.spr_net
-    t = project(net.views(net._flat), on.trunk(x))
+    t = project(net.views(learner.spr_ema_projection if ema else net._flat), on.trunk(x))
     if debug is not None:
         debug.update(spr_shifts=shifts, spr_targets=t)
     return t
