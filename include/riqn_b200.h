@@ -51,6 +51,17 @@ typedef struct riqn_dyn_state {
   double is_beta;                  /* priority_weight beta (annealed by the caller, launch_learner.py:167)  */
 } riqn_dyn_state;
 
+/* Update horizon of one learner step under n-step and discount annealing (BBF), kept in DEVICE memory beside
+ * riqn_dyn_state so that a captured step follows the schedule on replay.  One host writer (dynstate.HorizonState)
+ * fills it with one async copy per step and guarantees 1 <= n_step <= the entry point's n_max; the entry points keep
+ * n_step in 1..n_max all the same. */
+#define RIQN_MAX_HORIZON 16
+typedef struct riqn_horizon_state {
+  int n_step;                              /* this step's n                                                    */
+  float gamma_n;                           /* fl32(gamma ** n_step), the power taken in double on the host     */
+  double gamma_pow[RIQN_MAX_HORIZON];      /* gamma ** k in double for k < n_step (ReplayMemory._gamma_pow)    */
+} riqn_horizon_state;
+
 /* ------------------------------------------------------------------------------------------------
  * Conv trunk                                     replaces nn.Conv2d x3 + ReLU, rainbowiqn/model.py:65-67,115-118
  * ---------------------------------------------------------------------------------------------- */
@@ -652,6 +663,12 @@ int riqn_sumtree_stratified(int n, unsigned long long seed, unsigned long long s
 int riqn_sumtree_sample(int n, long capacity, int actor_capacity, const double* tree, const double* values,
                         const long long* index_actor, int history, int n_step, long long* tree_idx,
                         long long* data_idx, double* priorities, void* stream);
+/* riqn_sumtree_sample with the valid-index shift at n_step = hz->n_step, read on the device (kept in 1..n_max): bit for
+ * bit riqn_sumtree_sample at that n_step.  Returns cudaErrorInvalidValue, writing nothing, for the arguments
+ * riqn_sumtree_sample refuses, n_max outside 1..RIQN_MAX_HORIZON or a NULL hz; n <= 0 does nothing. */
+int riqn_sumtree_sample_horizon(int n, long capacity, int actor_capacity, const double* tree, const double* values,
+                                const long long* index_actor, int history, int n_max, const riqn_horizon_state* hz,
+                                long long* tree_idx, long long* data_idx, double* priorities, void* stream);
 /* Importance-sampling weights (sample_byte :465-475); n_nonpositive (device int, may be NULL) counts the
  * priorities <= 0 that were replaced by 1/capacity (:446-456).  With dyn != NULL, dyn->is_capacity and dyn->is_beta
  * replace current_capacity and priority_weight.  Returns cudaErrorInvalidValue, writing nothing, for n < 1, a NULL
@@ -698,6 +715,18 @@ int riqn_frame_gather(int batch, int actor_capacity, int history, int n_step, co
                       const unsigned char* s_frames, const int* s_timestep, const int* s_action, const float* s_reward,
                       const unsigned char* s_nonterminal, const double* gamma_pow, unsigned char* window,
                       long long* actions, float* returns, float* nonterminals, void* stream);
+/* Transition assembly at this step's n = hz->n_step, read on the device (kept in 1..n_max): frames (batch, 2*history,
+ * 84, 84) uint8 holds the states in frames[:, :history] and the next states in frames[:, history:], at offsets that do
+ * not depend on n.  The slots, blank frames, float64 return sum_{k<n} hz->gamma_pow[k] r_{t+k}, actions and 0/1
+ * nonterminals are riqn_frame_gather's at n_step = n (with gamma_pow = hz->gamma_pow), bit for bit, and the next states
+ * its window[:, n:n+history]; discounts[b] = fl32(hz->gamma_n * nonterminals[b]), the per-transition bootstrap factor a
+ * loss kernel takes in place of the nonterminals with gamma_n = 1.  Returns cudaErrorInvalidValue, writing nothing, for
+ * actor_capacity, history or n_max < 1, history + n_max > 16, or a NULL pointer; batch <= 0 does nothing. */
+int riqn_frame_gather_horizon(int batch, int actor_capacity, int history, int n_max, const long long* data_idx,
+                              const unsigned char* s_frames, const int* s_timestep, const int* s_action,
+                              const float* s_reward, const unsigned char* s_nonterminal, const riqn_horizon_state* hz,
+                              unsigned char* frames, long long* actions, float* returns, float* nonterminals,
+                              float* discounts, void* stream);
 /* SPR's K-step sequence (Schwarzer et al., ICLR 2021): window (batch, history+K, 84, 84) uint8 with the slots and blank
  * frames of riqn_frame_gather at n_step = K (so window[:, :history] is its states, bit for bit), actions (batch, K) int64
  * a_t .. a_{t+K-1} as stored (actions[:, 0] is riqn_frame_gather's), and valid (batch, K) uint8: valid[b, k-1] = 1 iff

@@ -129,12 +129,14 @@ SIGNATURES = {
     "riqn_adamw_step": [C.c_long, _P, _P, _P, _P, C.c_int] + [C.c_float] * 6 + [_P, _P],
     "riqn_sumtree_stratified": [C.c_int, C.c_ulonglong, C.c_ulonglong, _P, _P, _P, _P],
     "riqn_sumtree_sample": [C.c_int, C.c_long, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P],
-    "riqn_sumtree_is_weights": [C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P, _P, _P],
+    "riqn_sumtree_sample_horizon": [C.c_int, C.c_long, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P],
+    "riqn_sumtree_is_weights":[C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P, _P, _P],
     "riqn_sumtree_update": [C.c_int, C.c_long, _P, _P, _P, C.c_float, C.c_int, _P, _P, _P, _P],
     "riqn_sumtree_update_demo": [C.c_int, C.c_long, _P, _P, _P, C.c_float, C.c_int, _P, _P, _P, C.c_longlong, C.c_float,
                                  _P],
     "riqn_replay_append": [C.c_int, C.c_int, C.c_int, C.c_int] + [_P] * 11,
     "riqn_frame_gather": [C.c_int, C.c_int, C.c_int, C.c_int] + [_P] * 12,
+    "riqn_frame_gather_horizon": [C.c_int, C.c_int, C.c_int, C.c_int] + [_P] * 13,
     "riqn_split_bf16_multi": [C.c_int, C.POINTER(SplitJob), _P],
     "riqn_split_bf16": [C.c_long, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P],
     "riqn_gemm_bf16_tc": [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_long, C.c_int, _P, _P, _P, C.c_int, _P, _P, C.c_int, _P],

@@ -13,7 +13,9 @@ large-margin loss on demonstrations (dqfd.py), ``random_shift`` for the learner'
 (augment.py), ``curl`` for CURL's contrastive loss on the trunk (curl.py), ``spr`` for SPR's self-predictive loss on the
 trunk (spr.py), ``reset`` (reset_interval, reset_shrink) with ``updates`` / ``resets`` for the learner's periodic
 network resets (reset.py), ``target_ema`` (tau) for the learner's EMA target network (target.py) and ``adamw`` (the
-weight decay) for AdamW in every optimiser the agent builds.  The networks FQF, CURL and SPR train beside the DQN and
+weight decay) for AdamW in every optimiser the agent builds, ``horizon_anneal`` (n0, gamma0, steps) for the learner's
+update-horizon and discount annealing (horizon.py), and ``horizon()`` / ``gamma_n()`` for the (n, gamma) the loss cores
+train at.  The networks FQF, CURL and SPR train beside the DQN and
 their optimisers are set by those modules' ``build`` (None when off), and ``sides`` lists them (arena.Side).  The
 networks are
 rainbow_iqn_apex_b200.model.DQN (CUDA) and the optimiser is the arena Adam; checkpoints keep the reference schema
@@ -114,6 +116,20 @@ class Agent:
         self.updates = self.resets = 0
         if self.reset is not None and checkpoint is not None and "reset_state" in checkpoint:
             self.updates, self.resets = (int(x) for x in checkpoint["reset_state"])
+        self._discounts_fed = False   # the loss cores' nonterminals are per-transition discounts (Learner, horizon_anneal)
+
+    def horizon(self):
+        """(n, gamma) of the agent's updates: multi_step and discount (a Learner anneals them under horizon_anneal)."""
+        return self.n, self.discount
+
+    def gamma_n(self):
+        """The gamma^n every loss core hands its kernel, which multiplies the nonterminals by it: 1.0 while a step feeds
+        the per-transition discounts fl32(gamma^n) * nt in their place (Learner under horizon_anneal), otherwise
+        gamma ** n of horizon()."""
+        if self._discounts_fed:
+            return 1.0
+        n, gamma = self.horizon()
+        return float(gamma ** n)
 
     def set_risk(self, measure, eta=None):
         """Act, and pick the double-DQN target action a*, under a distortion risk measure (IQN paper, section 3.1):

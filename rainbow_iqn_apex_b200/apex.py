@@ -306,7 +306,13 @@ class ApexTopology:
             route_priorities(mem, self.shard, self.counts, sample, loss)
 
     def maybe_publish(self, agent):
-        """learner.py:28-36 / actor.py:36-39 every ``publish_every`` learner steps, as one broadcast of the flat arena."""
+        """learner.py:28-36 / actor.py:36-39 every ``publish_every`` learner steps, as one broadcast of the flat arena.
+        Refuses an agent under horizon_anneal on every rank, before the collective: the shards assemble their
+        transitions at the fixed multi_step and discount, which an annealing learner does not train at."""
+        if getattr(agent, "horizon_anneal", None) is not None:
+            raise ValueError("horizon_anneal = 1 anneals the learner's update horizon n, but the Ape-X shards assemble "
+                             "every transition at the fixed multi_step: train an annealing learner from its own replay "
+                             "(Learner.learn / learn_and_update)")
         self.steps += 1
         if self.steps % self.publish_every == 0:
             parallel.publish_parameters(agent, src=0, group=self.group)

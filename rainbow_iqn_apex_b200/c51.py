@@ -101,7 +101,7 @@ def loss_core(agent, states, actions, returns, next_states, nonterminals, debug=
                                target_out)
     else:
         args = (ptr(log_ps), ptr(pns), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals), ptr(agent.support),
-                float(agent.discount ** agent.n), float(agent.Vmin), float(agent.Vmax), float(agent.delta_z))
+                agent.gamma_n(), float(agent.Vmin), float(agent.Vmax), float(agent.delta_z))
         eps = getattr(agent, "value_rescaling", None)
         if eps is None:
             call("riqn_c51_loss_fwd_bwd", B, A, atoms, *args, ptr(loss), ptr(dq), ptr(m_out))

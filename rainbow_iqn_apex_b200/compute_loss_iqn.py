@@ -51,7 +51,7 @@ def _quantile_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, 
     """The double-DQN quantile-Huber loss kernel: riqn_iqn_loss_fwd_bwd, or against the transformed target
     h(R + gamma^n nt h^-1(Z)) under value rescaling (riqn_iqn_loss_fwd_bwd_h)."""
     args = (ptr(q_on), ptr(q_tgt), ptr(tau), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals),
-            float(agent.discount ** agent.n), float(agent.kappa))
+            agent.gamma_n(), float(agent.kappa))
     outs = (ptr(loss), ptr(dtheta), ptr(theta_out), ptr(target_out))
     eps = getattr(agent, "value_rescaling", None)
     if eps is None:
@@ -196,7 +196,7 @@ def _munchausen_core(agent, states, actions, returns, next_states, nonterminals,
         target_out = torch.empty(B, Np, device=dev)
         bonus_out = torch.empty(B, device=dev)
     call("riqn_miqn_loss_fwd_bwd", B, N, Np, A, ptr(q_on), ptr(q_tgt), ptr(tau), ptr(actions), ptr(returns),
-         ptr(nonterminals), float(agent.discount ** agent.n), float(agent.kappa), alpha, entropy_tau, l0, ptr(loss),
+         ptr(nonterminals), agent.gamma_n(), float(agent.kappa), alpha, entropy_tau, l0, ptr(loss),
          ptr(dtheta), ptr(theta_out), ptr(target_out), ptr(bonus_out))
     if debug is not None:
         debug.update(bonus=bonus_out, theta=theta_out, target=target_out, q_tgt=q_tgt, q_on=q_on, tau=tau, keep=keep)

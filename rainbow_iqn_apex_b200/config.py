@@ -19,6 +19,7 @@ MAX_SIGMA_RATIO = 1000.0   # riqn_hl_gauss_loss_fwd_bwd
 MAX_BATCH = 4096           # riqn_curl_infonce_fwd_bwd, riqn_spr_cosine_fwd_bwd
 MAX_SPR_STEPS = 12         # riqn_spr_cosine_fwd_bwd; riqn_sequence_gather's history + K <= 16 at history 4
 MAX_SPR_ACTIONS = 64       # riqn_spr_pack: the one-hot planes share conv1's 128 input channels with the latent's 64
+MAX_WINDOW = 16            # riqn_frame_gather_horizon: history + n <= 16
 _LOG2E = 1.4426950408889634
 
 
@@ -108,6 +109,10 @@ FIELDS = {
     "target_ema_tau": (0.005, real(lambda x: 0.0 < x <= 1.0, "in (0, 1]")),      # BBF's two
     "adamw": (0, switch),
     "adamw_weight_decay": (0.1, real(lambda x: x >= 0.0, ">= 0")),
+    "horizon_anneal": (0, switch),
+    "horizon_anneal_n": (10, integer(1, MAX_WINDOW - 1)),          # BBF's three; the end values are multi_step and
+    "horizon_anneal_gamma": (0.97, real(lambda x: 0.0 < x < 1.0, "in (0, 1)", exact=True)),      # discount
+    "horizon_anneal_steps": (10000, integer(1, math.inf)),
     "demo_segments": (0, integer(0, math.inf)),                   # at most nb_actor (read_demo)
     "demo_priority_bonus": (0.0, real(lambda x: x >= 0.0, ">= 0")),
 }
@@ -159,15 +164,16 @@ def read_risk(head, loss, measure, eta=None):
 
 def read(args, action_space):
     """Validate the optional fields of ``args`` and return what the agent stores, as a dict: qr_dqn (N or None); per
-    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr, reset, target_ema, adamw) None
-    when off, else its parameter or the tuple of its parameters; random_shift (the pad, or None); risk
-    (model.check_risk's); and the "head" and the "loss" variant (or None) they select.  Resets, the EMA target
-    (target_ema: tau) and AdamW (adamw: the weight decay lambda) combine with every head and variant; AdamW needs
-    lr * lambda < 1 for the agent's lr and, under FQF, for fqf_fraction_lr, as the float32 values the optimiser receives."""
+    variant switch (munchausen, fqf, mmd, hl_gauss, cql, dqfd, value_rescaling, curl, spr, reset, target_ema, adamw,
+    horizon_anneal) None when off, else its parameter or the tuple of its parameters; random_shift (the pad, or None);
+    risk (model.check_risk's); and the "head" and the "loss" variant (or None) they select.  Resets, the EMA target
+    (target_ema: tau), AdamW (adamw: the weight decay lambda) and n-step and discount annealing (horizon_anneal: n0,
+    gamma0, steps) combine with every head and variant; AdamW needs lr * lambda < 1 for the agent's lr and, under FQF,
+    for fqf_fraction_lr, as the float32 values the optimiser receives."""
     head, n = read_head(args, action_space)
     v = {"qr_dqn": n}
     for name in ("munchausen", "fqf", "mmd", "hl_gauss", "cql", "dqfd", "value_rescaling", "curl", "spr", "reset",
-                 "target_ema", "adamw"):
+                 "target_ema", "adamw", "horizon_anneal"):
         v[name] = None
         if field(args, name):
             params = tuple(field(args, f) for f in FIELDS if f.startswith(name + "_"))
@@ -207,8 +213,25 @@ def read(args, action_space):
             if not 0.0 <= _f32(lr) * v["adamw"] < 1.0:       # riqn_adamw_step's decay 1 - lr * lambda in (0, 1]
                 raise ValueError(f"adamw_weight_decay decays by 1 - {name} * adamw_weight_decay, which must be in (0, 1]: "
                                  f"{name} = {lr!r}, adamw_weight_decay = {v['adamw']!r}")
+    if v["horizon_anneal"] is not None:
+        _read_anneal_ends(args, v["horizon_anneal"][0])
     v["risk"] = read_risk(head, loss, getattr(args, "risk_measure", "neutral"), getattr(args, "risk_eta", None))
     return dict(v, head=head, loss=loss)
+
+
+def _read_anneal_ends(args, n0):
+    """The checks horizon_anneal adds on the fixed fields its schedule ends at: multi_step an integer >= 1, discount in
+    (0, 1) (the schedule takes log(1 - discount)), and max(horizon_anneal_n, multi_step) + history_length at most 16
+    (the gather's window)."""
+    n1 = integer(1, MAX_WINDOW - 1)("multi_step", args.multi_step)
+    gamma1 = args.discount
+    if isinstance(gamma1, bool) or not isinstance(gamma1, numbers.Real) or not 0.0 < gamma1 < 1.0:
+        raise ValueError(f"horizon_anneal anneals 1 - discount in log space: discount must be a real number in (0, 1), "
+                         f"got {gamma1!r}")
+    history = args.history_length
+    if max(n0, n1) + history > MAX_WINDOW:
+        raise ValueError(f"max(horizon_anneal_n, multi_step) + history_length must be at most {MAX_WINDOW} (the gather's "
+                         f"window), got max({n0}, {n1}) + {history}")
 
 
 def read_demo(args):

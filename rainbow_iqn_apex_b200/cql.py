@@ -29,7 +29,7 @@ def cql_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonter
     td = torch.empty(B, device=dev)
     pi = torch.empty(B, agent.action_space, device=dev)
     args = (ptr(q_on), ptr(q_tgt), ptr(tau), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals),
-            float(agent.discount ** agent.n), float(agent.kappa), agent.cql)
+            agent.gamma_n(), float(agent.kappa), agent.cql)
     outs = (ptr(loss), ptr(td), ptr(pi), ptr(dtheta), ptr(gap_out), ptr(theta_out), ptr(target_out))
     eps = getattr(agent, "value_rescaling", None)
     if eps is None:

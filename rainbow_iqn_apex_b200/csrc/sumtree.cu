@@ -43,10 +43,14 @@ __global__ void stratified_kernel(int n, uint64_t seed, uint64_t stream, const d
 // One warp per query.  The warp prefetches the whole 5-level subtree under the current node (62 nodes,
 // two coalesced 8-byte loads per lane), then walks it with shuffles: 5 levels per dependent memory
 // round trip instead of 1, using exactly the reference's stored node values and comparison order.
+// HZ: the shift's n_step is this step's hz->n_step, read on the device and kept in 1..n_step (the by-value n_max).
+template <bool HZ>
 __global__ void sumtree_sample_kernel(int n, long C, int actor_cap, const double* __restrict__ tree,
                                       const double* __restrict__ values, const int64_t* __restrict__ index_actor,
-                                      int history, int n_step, int64_t* __restrict__ tree_idx,
-                                      int64_t* __restrict__ data_idx, double* __restrict__ priorities) {
+                                      int history, int n_step, const riqn_horizon_state* __restrict__ hz,
+                                      int64_t* __restrict__ tree_idx, int64_t* __restrict__ data_idx,
+                                      double* __restrict__ priorities) {
+  if constexpr (HZ) n_step = min(max(hz->n_step, 1), n_step);
   const int lane = threadIdx.x & 31;
   const long q = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (q >= n) return;
@@ -388,6 +392,39 @@ __global__ void replay_append_kernel(int n, int actor_cap, int id_actor, int sta
   }
 }
 
+// The window of sample d (redis_memory.py:347-369,479-541): ring slots idx-history+1 .. idx-history+L of the actor's
+// segment, the blank frames across episode boundaries (:494-499) and the nonterminal flags after blanking (one thread).
+__device__ __forceinline__ void window_slots(long d, int actor_cap, int history, int L,
+                                             const int32_t* __restrict__ s_timestep,
+                                             const uint8_t* __restrict__ s_nonterminal, long* slots, int* blank, int* nt) {
+  const long actor = d / actor_cap;
+  int ts[16];
+  for (int k = 0; k < L; ++k) {
+    long pos = (k + d - history + 1) % actor_cap;
+    if (pos < 0) pos += actor_cap;
+    slots[k] = pos + actor * actor_cap;
+    ts[k] = s_timestep[slots[k]];
+    nt[k] = s_nonterminal[slots[k]];
+    blank[k] = 0;
+  }
+  for (int t = history - 2; t >= 0; --t)
+    if (ts[t + 1] == 0) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
+  for (int t = history; t < L; ++t)
+    if (!nt[t - 1]) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
+}
+
+// The n-step return sum_k gamma^k r_{t+k} in float64, in the reference's order (:516-518).
+__device__ __forceinline__ double n_step_return(int history, int n_step, const long* slots, const int* blank,
+                                                const float* __restrict__ s_reward, const double* gamma_pow) {
+  double ret = 0.0;
+  for (int k = 0; k < n_step; ++k) {
+    const int t = history + k - 1;
+    const double r = blank[t] ? 0.0 : (double)s_reward[slots[t]];
+    ret = __dadd_rn(ret, __dmul_rn(gamma_pow[k], r));   // python: sum(discount**k * reward), no FMA
+  }
+  return ret;
+}
+
 // Transition assembly (redis_memory.py:347-369,479-541): 7-frame window idx-3..idx+3 inside the actor's
 // ring, blank frames across episode boundaries, n-step return in float64, output the uint8 window
 // (B, history+n, 84, 84): states = window[:, :history], next_states = window[:, n:n+history].
@@ -402,28 +439,9 @@ __global__ void frame_gather_kernel(int B, int actor_cap, int history, int n_ste
   __shared__ long slots[16];
   __shared__ int blank[16];
   if (threadIdx.x == 0) {
-    const long d = data_idx[b];
-    const long actor = d / actor_cap;
-    int ts[16], nt[16];
-    for (int k = 0; k < L; ++k) {
-      long pos = (k + d - history + 1) % actor_cap;
-      if (pos < 0) pos += actor_cap;
-      slots[k] = pos + actor * actor_cap;
-      ts[k] = s_timestep[slots[k]];
-      nt[k] = s_nonterminal[slots[k]];
-      blank[k] = 0;
-    }
-    for (int t = history - 2; t >= 0; --t)
-      if (ts[t + 1] == 0) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
-    for (int t = history; t < L; ++t)
-      if (!nt[t - 1]) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
-    double ret = 0.0;
-    for (int k = 0; k < n_step; ++k) {
-      const int t = history + k - 1;
-      const double r = blank[t] ? 0.0 : (double)s_reward[slots[t]];
-      ret = __dadd_rn(ret, __dmul_rn(gamma_pow[k], r));   // python: sum(discount**k * reward), no FMA
-    }
-    returns[b] = (float)ret;
+    int nt[16];
+    window_slots(data_idx[b], actor_cap, history, L, s_timestep, s_nonterminal, slots, blank, nt);
+    returns[b] = (float)n_step_return(history, n_step, slots, blank, s_reward, gamma_pow);
     actions[b] = s_action[slots[history - 1]];
     nonterminals[b] = nt[L - 1] ? 1.f : 0.f;
   }
@@ -434,6 +452,42 @@ __global__ void frame_gather_kernel(int B, int actor_cap, int history, int n_ste
     uint4 v = make_uint4(0, 0, 0, 0);
     if (!blank[k]) v = reinterpret_cast<const uint4*>(s_frames + slots[k] * FRAME_BYTES)[o];
     reinterpret_cast<uint4*>(window + ((long)b * L + k) * FRAME_BYTES)[o] = v;
+  }
+}
+
+// frame_gather_kernel at this step's n = hz->n_step (kept in 1..n_max), read on the device, with a window of a fixed
+// 2 * history frames: frames[:, :history] are the states and frames[:, history:] the next states (window frames
+// n .. n+history-1), so their offsets do not depend on n.  discounts[b] = fl32(gamma^n) * nt_b.
+__global__ void frame_gather_horizon_kernel(int B, int actor_cap, int history, int n_max,
+                                            const int64_t* __restrict__ data_idx, const uint8_t* __restrict__ s_frames,
+                                            const int32_t* __restrict__ s_timestep, const int32_t* __restrict__ s_action,
+                                            const float* __restrict__ s_reward, const uint8_t* __restrict__ s_nonterminal,
+                                            const riqn_horizon_state* __restrict__ hz, uint8_t* __restrict__ frames,
+                                            int64_t* __restrict__ actions, float* __restrict__ returns,
+                                            float* __restrict__ nonterminals, float* __restrict__ discounts) {
+  const int b = blockIdx.x;
+  const int n_step = min(max(hz->n_step, 1), n_max);
+  const int L = history + n_step;
+  __shared__ long slots[16];
+  __shared__ int blank[16];
+  if (threadIdx.x == 0) {
+    int nt[16];
+    window_slots(data_idx[b], actor_cap, history, L, s_timestep, s_nonterminal, slots, blank, nt);
+    returns[b] = (float)n_step_return(history, n_step, slots, blank, s_reward, hz->gamma_pow);
+    actions[b] = s_action[slots[history - 1]];
+    const float ntf = nt[L - 1] ? 1.f : 0.f;
+    nonterminals[b] = ntf;
+    discounts[b] = __fmul_rn(hz->gamma_n, ntf);
+  }
+  __syncthreads();
+  constexpr int V = FRAME_BYTES / 16;
+  const int F = 2 * history;
+  for (int t = threadIdx.x; t < F * V; t += blockDim.x) {
+    const int k = t / V, o = t % V;
+    const int w = k < history ? k : k - history + n_step;      // the window frame this output frame holds
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (!blank[w]) v = reinterpret_cast<const uint4*>(s_frames + slots[w] * FRAME_BYTES)[o];
+    reinterpret_cast<uint4*>(frames + ((long)b * F + k) * FRAME_BYTES)[o] = v;
   }
 }
 
@@ -452,19 +506,8 @@ __global__ void sequence_gather_kernel(int B, int actor_cap, int history, int K,
   if (threadIdx.x == 0) {
     const long d = data_idx[b];
     const long actor = d / actor_cap;
-    int ts[16], nt[16];
-    for (int k = 0; k < L; ++k) {
-      long pos = (k + d - history + 1) % actor_cap;
-      if (pos < 0) pos += actor_cap;
-      slots[k] = pos + actor * actor_cap;
-      ts[k] = s_timestep[slots[k]];
-      nt[k] = s_nonterminal[slots[k]];
-      blank[k] = 0;
-    }
-    for (int t = history - 2; t >= 0; --t)
-      if (ts[t + 1] == 0) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
-    for (int t = history; t < L; ++t)
-      if (!nt[t - 1]) { blank[t] = 1; ts[t] = 0; nt[t] = 0; }
+    int nt[16];
+    window_slots(d, actor_cap, history, L, s_timestep, s_nonterminal, slots, blank, nt);
     long head = (index_actor[actor] - d % actor_cap) % actor_cap;       // distance from p to the write head
     if (head < 0) head += actor_cap;
     for (int k = 0; k < K; ++k) {
@@ -504,8 +547,24 @@ RIQN_API int riqn_sumtree_sample(int n, long capacity, int actor_capacity, const
     return (int)cudaErrorInvalidValue;
   if (n <= 0) return 0;
   const int warps_per_block = 4;
-  sumtree_sample_kernel<<<riqn_cdiv(n, warps_per_block), warps_per_block * 32, 0, (cudaStream_t)stream>>>(
-      n, capacity, actor_capacity, tree, values, (const int64_t*)index_actor, history, n_step, (int64_t*)tree_idx,
+  sumtree_sample_kernel<false><<<riqn_cdiv(n, warps_per_block), warps_per_block * 32, 0, (cudaStream_t)stream>>>(
+      n, capacity, actor_capacity, tree, values, (const int64_t*)index_actor, history, n_step, nullptr,
+      (int64_t*)tree_idx, (int64_t*)data_idx, priorities);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_sumtree_sample_horizon(int n, long capacity, int actor_capacity, const double* tree,
+                                         const double* values, const long long* index_actor, int history, int n_max,
+                                         const riqn_horizon_state* hz, long long* tree_idx, long long* data_idx,
+                                         double* priorities, void* stream) {
+  riqn::note_launches(1);
+  if (capacity < 1 || actor_capacity < 1 || capacity % actor_capacity != 0 || history < 0 || n_max < 1 ||
+      n_max > RIQN_MAX_HORIZON || !tree || !values || !index_actor || !hz || !tree_idx || !data_idx || !priorities)
+    return (int)cudaErrorInvalidValue;
+  if (n <= 0) return 0;
+  const int warps_per_block = 4;
+  sumtree_sample_kernel<true><<<riqn_cdiv(n, warps_per_block), warps_per_block * 32, 0, (cudaStream_t)stream>>>(
+      n, capacity, actor_capacity, tree, values, (const int64_t*)index_actor, history, n_max, hz, (int64_t*)tree_idx,
       (int64_t*)data_idx, priorities);
   return (int)cudaGetLastError();
 }
@@ -600,6 +659,23 @@ RIQN_API int riqn_frame_gather(int batch, int actor_capacity, int history, int n
                                                                (const int64_t*)data_idx, s_frames, s_timestep, s_action,
                                                                s_reward, s_nonterminal, gamma_pow, window,
                                                                (int64_t*)actions, returns, nonterminals);
+  return (int)cudaGetLastError();
+}
+
+RIQN_API int riqn_frame_gather_horizon(int batch, int actor_capacity, int history, int n_max, const long long* data_idx,
+                                       const unsigned char* s_frames, const int* s_timestep, const int* s_action,
+                                       const float* s_reward, const unsigned char* s_nonterminal,
+                                       const riqn_horizon_state* hz, unsigned char* frames, long long* actions,
+                                       float* returns, float* nonterminals, float* discounts, void* stream) {
+  riqn::note_launches(1);
+  if (actor_capacity < 1 || history < 1 || n_max < 1 || history + n_max > 16 || !data_idx || !s_frames ||
+      !s_timestep || !s_action || !s_reward || !s_nonterminal || !hz || !frames || !actions || !returns ||
+      !nonterminals || !discounts)
+    return (int)cudaErrorInvalidValue;
+  if (batch <= 0) return 0;
+  frame_gather_horizon_kernel<<<batch, 256, 0, (cudaStream_t)stream>>>(
+      batch, actor_capacity, history, n_max, (const int64_t*)data_idx, s_frames, s_timestep, s_action, s_reward,
+      s_nonterminal, hz, frames, (int64_t*)actions, returns, nonterminals, discounts);
   return (int)cudaGetLastError();
 }
 

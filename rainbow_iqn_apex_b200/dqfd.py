@@ -44,7 +44,7 @@ def dqfd_loss(agent, B, N, Np, q_on, q_tgt, tau, actions, a_star, returns, nonte
     a_hat = torch.empty(B, dtype=torch.int64, device=dev)
     margin, lam = agent.dqfd
     args = (ptr(q_on), ptr(q_tgt), ptr(tau), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals), ptr(demo),
-            float(agent.discount ** agent.n), float(agent.kappa), margin, lam)
+            agent.gamma_n(), float(agent.kappa), margin, lam)
     outs = (ptr(loss), ptr(td), ptr(dtheta), ptr(margin_out), ptr(a_hat), ptr(theta_out), ptr(target_out))
     eps = getattr(agent, "value_rescaling", None)
     if eps is None:

@@ -18,7 +18,7 @@ def hl_gauss_loss(agent, B, log_ps, pns, actions, a_star, returns, nonterminals,
     """The HL-Gauss cross-entropy at ratio ``agent.hl_gauss``: riqn_hl_gauss_loss_fwd_bwd, or the transformed target
     h(R + gamma^n nt E[h^-1(Z)]) under value rescaling (riqn_hl_gauss_loss_fwd_bwd_h)."""
     args = (ptr(log_ps), ptr(pns), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals), ptr(agent.support),
-            float(agent.discount ** agent.n), float(agent.Vmin), float(agent.Vmax), agent.hl_gauss)
+            agent.gamma_n(), float(agent.Vmin), float(agent.Vmax), agent.hl_gauss)
     outs = (ptr(loss), ptr(dq), ptr(m_out), ptr(target_out))
     eps = getattr(agent, "value_rescaling", None)
     if eps is None:

@@ -23,6 +23,14 @@ of one's own around loss.backward().
 Under target_ema (target.py) every step ends with the EMA of the target network, after the optimisers and the sides'
 after_step hooks, eagerly and in every captured graph.  Under adamw every optimiser is AdamW; a captured graph holds
 each one's decay 1 - lr * weight_decay by value, so a replay after an lr or weight_decay change raises.
+
+Under horizon_anneal (horizon.py) the learner anneals its update horizon n and discount gamma over the updates since the
+last reset (or construction; a resumed run starts the schedule again).  Before every step that samples from a replay
+(learn(mem, None) and learn_and_update, eager, warmed up or replayed from enable_cuda_graph's graph) it writes that
+step's (n, gamma) into its device horizon state, and the step samples through ReplayMemory.sample_horizon and hands the
+loss core the per-transition discounts with gamma^n = 1.  horizon() gives the next step's (n, gamma); learn_on_batch on
+a batch the caller assembled at horizon() trains at gamma^n of horizon() with the batch's own nonterminals.  The batch and
+learn graphs and a queued batch (learn with an mp_queue) take batches assembled at a fixed n, and refuse.
 """
 import contextlib
 import io
@@ -30,9 +38,9 @@ from typing import NamedTuple
 
 import torch
 
-from . import augment, reset, target
+from . import augment, horizon, reset, target
 from .agent import Agent
-from .dynstate import DynState
+from .dynstate import DynState, HorizonState
 
 MODEL_WEIGHT_STR = "model_weight"      # rainbowiqn/constants.py:18
 STEP_LEARNER_STR = "step_learner:"     # rainbowiqn/constants.py:14
@@ -58,13 +66,58 @@ class Learner(Agent):
         self.capture_collectives = True  # data parallel: capture the all-reduces in the step graphs (enable_cuda_graph)
         self._dyn = None           # the riqn_dyn_state every step graph of this learner reads (built at the first capture)
         self._dyn_on = False       # the struct is attached: a step is being warmed up or captured
+        self._horizon = self._horizon_base = None
+        if self.horizon_anneal is not None:
+            # the riqn_horizon_state every annealed step reads, and the updates count at the schedule's start
+            self._horizon = HorizonState(self.online_net._flat.device, max(self.horizon_anneal[0], self.n))
+            self._horizon_base = self.updates
 
     def learn(self, mem_redis, mp_queue):
-        sample = mem_redis.get_sample_from_mp_queue(mp_queue)
+        if self._horizon is not None:
+            if mp_queue is not None:
+                self._refuse_anneal("learn with an mp_queue")
+            self._horizon.write(*self.horizon())
+        sample = self._sample(mem_redis, mp_queue)
         idxs, states, actions, returns, next_states, nonterminals, weights = sample
-        loss = self.learn_on_batch(states, actions, returns, next_states, nonterminals, weights,
-                                   demo=self._demo_mask(mem_redis, idxs), sequence=self._sequence(mem_redis, idxs))
+        with self._feeding_discounts():
+            loss = self.learn_on_batch(states, actions, returns, next_states, nonterminals, weights,
+                                       demo=self._demo_mask(mem_redis, idxs), sequence=self._sequence(mem_redis, idxs))
         return idxs, loss
+
+    def _sample(self, mem, mp_queue):
+        """The step's sample: ReplayMemory.get_sample_from_mp_queue, or under horizon_anneal ReplayMemory.sample_horizon at
+        the horizon state's (n, gamma), with the discounts in the nonterminals' place."""
+        if self._horizon is None:
+            return mem.get_sample_from_mp_queue(mp_queue)
+        return mem.sample_horizon(mem.batch_size, self._horizon)
+
+    @contextlib.contextmanager
+    def _feeding_discounts(self):
+        """Under horizon_anneal, the loss cores run inside this with gamma^n = 1 (Agent.gamma_n): the step's sample carries
+        the per-transition discounts in the nonterminals' place."""
+        self._discounts_fed = self._horizon is not None
+        try:
+            yield
+        finally:
+            self._discounts_fed = False
+
+    def horizon(self):
+        """(n, gamma) of the next step: under horizon_anneal the schedule's (horizon.py) at the updates since the last
+        reset, otherwise (multi_step, discount).  For logging, and for callers that assemble learn_on_batch's batch."""
+        return self._horizon_at(0)
+
+    def _horizon_at(self, ahead):
+        """(n, gamma) of the step ``ahead`` steps after the next (a capture's warm-up steps count updates only at its
+        end)."""
+        if self._horizon is None:
+            return super().horizon()
+        return horizon.schedule(self.horizon_anneal, self.n, self.discount, self.updates - self._horizon_base + ahead)
+
+    def _refuse_anneal(self, what):
+        if self._horizon is not None:
+            raise ValueError(f"horizon_anneal = 1 anneals the update horizon n from step to step: {what} takes batches "
+                             "assembled at a fixed n; step the learner with learn(mem, None) / learn_and_update (and "
+                             "enable_cuda_graph), or pass learn_on_batch a batch assembled at horizon()")
 
     def _demo_mask(self, mem, idxs):
         """Under DQfD, the demonstration flags of the sampled tree indices ``idxs`` (ReplayMemory.demo_mask: None when the
@@ -100,6 +153,8 @@ class Learner(Agent):
         the reset (the next one draws from the next streams)."""
         reset.reset(self, self.resets)
         self.resets += 1
+        if self._horizon is not None:
+            self._horizon_base = self.updates        # the horizon schedule starts again
 
     def _count_updates(self, n):
         """Count ``n`` optimiser steps; under resets, reset once if one of them completed a reset_interval."""
@@ -153,13 +208,16 @@ class Learner(Agent):
                 side.after_step(self)
         target.update(self)
 
-    def _write_dyn(self, mem):
+    def _write_dyn(self, mem, ahead=0):
         """Stage the next step's device scalars: the Adam bias corrections of every optimiser, and the fill and beta of the
-        replay memory ``mem`` ((1, 0) for a step without one)."""
+        replay memory ``mem`` ((1, 0) for a step without one); under horizon_anneal, the (n, gamma) of the step ``ahead``
+        steps after the next (_horizon_at)."""
         nss, sbc = self.optimiser.bias_corrections(self.optimiser._step + 1)
         more = tuple(o.bias_corrections(o._step + 1) for o in self._optimisers()[1:])
         capacity, beta = (1.0, 0.0) if mem is None else (mem.transitions.get_current_capacity(), mem.priority_weight)
         self._dyn.write(nss, sbc, capacity, beta, *more)
+        if self._horizon is not None:
+            self._horizon.write(*self._horizon_at(ahead))
 
     def compute_gradients(self, states, actions, returns, next_states, nonterminals, weights, debug=None, demo=None,
                           sequence=None):
@@ -259,9 +317,10 @@ class Learner(Agent):
     def _step_pre(self, mem):
         """sample -> three forwards -> loss -> backward (gradients in the arena)."""
         self._reset_step_streams(mem)
-        idxs, states, actions, returns, next_states, nonterminals, weights = mem.get_sample_from_mp_queue(None)
-        loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights,
-                                      demo=self._demo_mask(mem, idxs), sequence=self._sequence(mem, idxs))
+        idxs, states, actions, returns, next_states, nonterminals, weights = self._sample(mem, None)
+        with self._feeding_discounts():
+            loss = self.compute_gradients(states, actions, returns, next_states, nonterminals, weights,
+                                          demo=self._demo_mask(mem, idxs), sequence=self._sequence(mem, idxs))
         return idxs, loss
 
     def _step_post(self, mem, idxs, loss, allreduce=True):
@@ -286,8 +345,8 @@ class Learner(Agent):
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                for _ in range(warmup):                  # eager warm-up on a side stream (allocator, attributes)
-                    self._write_dyn(mem)
+                for k in range(warmup):                  # eager warm-up on a side stream (allocator, attributes)
+                    self._write_dyn(mem, k)
                     post(pre(), True)
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
@@ -355,6 +414,7 @@ class Learner(Agent):
         nonterminals, weights) device tensors defining the shapes.  Requires enable_cuda_graph(mem) first.  Not under
         SPR: the host batch carries no sequences."""
         self._refuse_spr("enable_batch_graph")
+        self._refuse_anneal("enable_batch_graph")
         g = self._graphs.get("replay")
         assert g is not None and mem is g.mem
         inputs = tuple(t.clone() for t in example)
@@ -376,6 +436,7 @@ class Learner(Agent):
             raise RuntimeError("the learn graph takes batches gathered from the actor shards, which carry no demonstration "
                                "flags: a DQfD learner steps from its own replay (enable_cuda_graph / enable_batch_graph)")
         self._refuse_spr("enable_learn_graph")
+        self._refuse_anneal("enable_learn_graph")
         inputs = tuple(t.contiguous().clone() for t in example)
 
         def pre():

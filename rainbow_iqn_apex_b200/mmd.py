@@ -21,7 +21,7 @@ def mmd_loss(agent, B, N, q_on, q_tgt, actions, a_star, returns, nonterminals, l
     bw = agent.mmd
     hb = (ctypes.c_float * len(bw))(*bw)      # read by the call: a captured graph holds the values
     args = (ptr(q_on), ptr(q_tgt), ptr(actions), ptr(a_star), ptr(returns), ptr(nonterminals),
-            float(agent.discount ** agent.n), len(bw), hb)
+            agent.gamma_n(), len(bw), hb)
     outs = (ptr(loss), ptr(dtheta), ptr(theta_out), ptr(target_out))
     eps = getattr(agent, "value_rescaling", None)
     if eps is None:

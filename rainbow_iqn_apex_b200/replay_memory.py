@@ -167,10 +167,11 @@ class SegmentTree:
         self.append_arrays(id_actor, actor_index_in_replay_memory, ts, fr, ac, rw, dn, priorities, T_actor)
 
     # -------------------------------------------------------------- sampling
-    def find_multiple_values(self, history_length, n_step_length, batch_size, samples=None):
+    def find_multiple_values(self, history_length, n_step_length, batch_size, samples=None, hz=None):
         """redis_memory.py:267-331.  Returns device tensors (priorities f64, data_idx, tree_idx) and the
         device-resident total is read by the weights kernel; ``samples`` (float64) injects the stratified
-        values, otherwise they are drawn on the device."""
+        values, otherwise they are drawn on the device.  ``hz``: a dynstate.HorizonState whose n the valid-index shift
+        reads on the device in place of ``n_step_length`` (riqn_sumtree_sample_horizon), or None."""
         dev = self.device
         if samples is None:
             samples = torch.empty(batch_size, dtype=torch.float64, device=dev)
@@ -185,8 +186,13 @@ class SegmentTree:
         tree_idx = torch.empty(batch_size, dtype=torch.int64, device=dev)
         data_idx = torch.empty(batch_size, dtype=torch.int64, device=dev)
         pri = torch.empty(batch_size, dtype=torch.float64, device=dev)
-        call("riqn_sumtree_sample", batch_size, self.full_capacity, self.actor_capacity, ptr(self.tree), ptr(samples),
-             ptr(self.index_actor), history_length, n_step_length, ptr(tree_idx), ptr(data_idx), ptr(pri))
+        if hz is None:
+            call("riqn_sumtree_sample", batch_size, self.full_capacity, self.actor_capacity, ptr(self.tree), ptr(samples),
+                 ptr(self.index_actor), history_length, n_step_length, ptr(tree_idx), ptr(data_idx), ptr(pri))
+        else:
+            call("riqn_sumtree_sample_horizon", batch_size, self.full_capacity, self.actor_capacity, ptr(self.tree),
+                 ptr(samples), ptr(self.index_actor), history_length, hz.n_max, hz.ptr(), ptr(tree_idx), ptr(data_idx),
+                 ptr(pri))
         return pri, data_idx, tree_idx
 
 
@@ -216,17 +222,17 @@ class ReplayMemory:
         if self.demo_segments > 0:
             self.demo_leaf = (args.nb_actor - self.demo_segments) * args.actor_capacity + self.capacity - 1
 
-    def sample_indices(self, batch_size, samples=None):
+    def sample_indices(self, batch_size, samples=None, hz=None):
         """find_multiple_values + importance weights (redis_memory.py:424-475), including the reference's resample loop:
         while some sampled priority is <= 0 (a slot next to a write head of a partially filled segment) the batch is
         drawn again, up to 10 more times, 11 draws in all (:432-438); after that -- and always inside a captured CUDA
         graph or with injected ``samples``, where a host-side retry is impossible -- the reference's final fallback
         applies (:446-456: those probabilities become 1/capacity).  The count of such samples is left in
-        ``last_nonpositive`` (device int)."""
+        ``last_nonpositive`` (device int).  ``hz``: see SegmentTree.find_multiple_values."""
         tr = self.transitions
         retry = samples is None and tr._dyn is None and not torch.cuda.is_current_stream_capturing()
         for attempt in range(11 if retry else 1):
-            pri, data_idx, tree_idx = tr.find_multiple_values(self.history, self.n, batch_size, samples)
+            pri, data_idx, tree_idx = tr.find_multiple_values(self.history, self.n, batch_size, samples, hz)
             w64 = torch.empty(batch_size, dtype=torch.float64, device=self.device)
             w32 = torch.empty(batch_size, dtype=torch.float32, device=self.device)
             self.last_nonpositive = torch.empty(1, dtype=torch.int32, device=self.device)    # written (not accumulated) by the kernel
@@ -258,6 +264,31 @@ class ReplayMemory:
              ptr(tr.timestep), ptr(tr.action), ptr(tr.reward), ptr(tr.nonterminal), ptr(self._gamma_pow), ptr(window),
              ptr(actions), ptr(returns), ptr(nonterminals))
         return window, actions, returns, nonterminals
+
+    def assemble_horizon(self, data_idx, hz):
+        """assemble_window at the n of the dynstate.HorizonState ``hz``, read on the device (riqn_frame_gather_horizon):
+        frames (B, 2 * history, 84, 84) uint8, states = frames[:, :history] and next_states = frames[:, history:], with
+        actions, returns, the 0/1 nonterminals and discounts = fl32(gamma^n) * nonterminals."""
+        tr = self.transitions
+        if not tr.store_frames:
+            raise RuntimeError("this replay was built with store_frames=False (tree only): nothing to assemble")
+        B = data_idx.numel()
+        frames = torch.empty(B, 2 * self.history, 84, 84, dtype=torch.uint8, device=self.device)
+        actions = torch.empty(B, dtype=torch.int64, device=self.device)
+        returns, nonterminals, discounts = (torch.empty(B, dtype=torch.float32, device=self.device) for _ in range(3))
+        call("riqn_frame_gather_horizon", B, tr.actor_capacity, self.history, hz.n_max, ptr(data_idx), ptr(tr.frames),
+             ptr(tr.timestep), ptr(tr.action), ptr(tr.reward), ptr(tr.nonterminal), hz.ptr(), ptr(frames), ptr(actions),
+             ptr(returns), ptr(nonterminals), ptr(discounts))
+        return frames, actions, returns, nonterminals, discounts
+
+    def sample_horizon(self, batch_size, hz):
+        """sample() at the update horizon the dynstate.HorizonState ``hz`` holds on the device (a learner under
+        horizon_anneal): (tree_idxs, states u8, actions, returns, next_states u8, discounts, weights), the sampler's shift
+        and the transitions at hz's n, and discounts = fl32(gamma^n) * nonterminal in place of the nonterminals."""
+        tree_idx, data_idx, _, _, w32 = self.sample_indices(batch_size, hz=hz)
+        frames, actions, returns, _, discounts = self.assemble_horizon(data_idx, hz)
+        h = self.history
+        return tree_idx, frames[:, :h], actions, returns, frames[:, h:], discounts, w32
 
     def sample_sequence(self, tree_idx, K):
         """SPR's K-step sequence of the sampled tree indices ``tree_idx`` (data index tree_idx - capacity + 1), as device
