@@ -639,8 +639,8 @@ int riqn_adam_step(long n, float* params, const float* grads, float* exp_avg, fl
 /* One AdamW step (torch.optim.AdamW, non-amsgrad): first params[i] = fl(params[i] * d) with d = fl32(1 - lr *
  * weight_decay) computed in double, then riqn_adam_step's update on the decayed params in the same pass (its bias
  * corrections read from dyn when dyn != NULL; d is always taken by value).  weight_decay = 0 gives riqn_adam_step's
- * bits.  n >= 1, non-NULL params / grads / exp_avg / exp_avg_sq, a finite weight_decay >= 0 and d in (0, 1], else
- * cudaErrorInvalidValue with nothing written. */
+ * bits.  n >= 1, step >= 1, non-NULL params / grads / exp_avg / exp_avg_sq, a finite weight_decay >= 0 and d in
+ * (0, 1], else cudaErrorInvalidValue with nothing written. */
 int riqn_adamw_step(long n, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int step, float lr,
                     float beta1, float beta2, float eps, float weight_decay, float grad_scale, const riqn_dyn_state* dyn,
                     void* stream);

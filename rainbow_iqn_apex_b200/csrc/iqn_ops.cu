@@ -2052,7 +2052,9 @@ RIQN_API int riqn_adam_step(long n, float* params, const float* grads, float* ex
 RIQN_API int riqn_adamw_step(long n, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int step,
                              float lr, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
                              const riqn_dyn_state* dyn, void* stream) {
-  if (n < 1 || !params || !grads || !exp_avg || !exp_avg_sq || !isfinite(weight_decay) || weight_decay < 0.f)
+  // step < 1 would make bc1 = 0 (or negative) and the step size -inf or of the wrong sign
+  if (n < 1 || step < 1 || !params || !grads || !exp_avg || !exp_avg_sq || !isfinite(weight_decay) ||
+      weight_decay < 0.f)
     return (int)cudaErrorInvalidValue;
   const float decay = (float)(1.0 - (double)lr * (double)weight_decay);
   if (!(decay > 0.f) || !(decay <= 1.f)) return (int)cudaErrorInvalidValue;

@@ -91,11 +91,12 @@ def test_refused_calls_write_nothing(cuda_dev):
     calls = [dict(n=0), dict(n=-5), dict(p=None), dict(g=None), dict(m=None), dict(v=None), dict(wd=-1e-9),
              dict(wd=-math.inf), dict(wd=math.inf), dict(wd=math.nan), dict(wd=1000.0),      # lr wd = 1: d = 0
              dict(wd=2000.0), dict(lr=-1e-3, wd=0.1),                                        # d > 1
-             dict(lr=math.nan, wd=0.1), dict(lr=math.inf, wd=0.1)]
+             dict(lr=math.nan, wd=0.1), dict(lr=math.inf, wd=0.1),
+             dict(step=0), dict(step=-1), dict(step=0, wd=0.0)]                              # bc1 = 1 - b1^step <= 0
     for c in calls:
-        a = dict(n=n, p=P.p, g=G.p, m=M.p, v=V.p, lr=lr, wd=0.1)
+        a = dict(n=n, p=P.p, g=G.p, m=M.p, v=V.p, lr=lr, wd=0.1, step=1)
         a.update(c)
-        rc = _raw("riqn_adamw_step", a["n"], a["p"], a["g"], a["m"], a["v"], 1, a["lr"], eps, a["wd"], 1.0)
+        rc = _raw("riqn_adamw_step", a["n"], a["p"], a["g"], a["m"], a["v"], a["step"], a["lr"], eps, a["wd"], 1.0)
         assert rc == 1, (c, rc)                                            # cudaErrorInvalidValue
     torch.cuda.synchronize()
     for o, t in zip((P, G, M, V), before):
