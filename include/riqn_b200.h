@@ -14,8 +14,7 @@
  *     from the device's stream-ordered pool on `stream` and released on `stream` before the call returns
  *     (cudaMallocAsync / cudaFreeAsync): no host synchronisation, no state shared between calls or streams, and
  *     inside a CUDA graph capture it becomes part of the graph;
- *   - results are bitwise reproducible: no sum across thread blocks uses float atomics (except in the fp32
- *     CUDA-core cross-check GEMM and the col2im of riqn_conv_bwd / riqn_conv_bwd_tc);
+ *   - results are bitwise reproducible: no sum across thread blocks uses float atomics;
  *   - fp32 tensors row-major.  tau, q and dtheta use the reference's quantile-major rows r = q * batch + b
  *     (rainbowiqn/model.py:149, compute_loss_iqn.py:238-310); the head-internal matrices (cos, x, h, dh, dz and
  *     their bf16 images) use sample-major rows r' = b * num_quantiles + q, which makes the Hadamard operand
@@ -92,7 +91,8 @@ int riqn_conv_fwd(const riqn_conv_geom* g, const void* in, int in_is_u8, const f
 /* Backward of the above: dout is dL/d(out) (post-ReLU), `out` the forward output (ReLU mask).
  * dw/dbias are ACCUMULATED into (zero them first, like zero_grad -- learner.py:22); din (may be NULL
  * for the first layer) is overwritten with dL/d(in).  dY (B*OH*OW, Cout) and dcol (like col) are
- * workspaces. */
+ * workspaces.  dw += the split-K product dY^T col: each split an fp32 fmaf chain over its rows ascending, the splits
+ * added in split order, the sum added once; din[b, c, ih, iw] = the fp32 sum over (kh, kw) ascending of dcol. */
 int riqn_conv_bwd(const riqn_conv_geom* g, const float* dout, const float* out, const float* col, const float* w,
                   float* dY, float* dcol, float* dw, float* dbias, float* din, void* stream);
 
@@ -147,7 +147,8 @@ int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, const float*
 
 /* Backward of riqn_conv_fwd_tc on the tensor cores (bf16 operands, fp32 accumulate): colT_hi as that forward wrote it;
  * wT_hi (K, Cout) bf16; dY_hi (M, Cout) and dYT_hi (Cout, M) bf16 workspaces; dcol fp32 (M, K) workspace; dw/dbias
- * accumulated, dw += wgrad_scale * (dY^T col) (the trunk passes 1); din may be NULL. */
+ * accumulated, dw += wgrad_scale * (dY^T col) (the trunk passes 1); din may be NULL; with din, dcol = dY W (non-NULL)
+ * and din[b, c, ih, iw] = the fp32 sum over (kh, kw) ascending of dcol. */
 int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const float* out, const void* colT_hi, const void* wT_hi,
                      void* dY_hi, void* dYT_hi, float* dcol, float* dw, float* dbias, float* din, float wgrad_scale,
                      void* stream);

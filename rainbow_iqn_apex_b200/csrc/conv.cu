@@ -76,42 +76,9 @@ __global__ void col2im_kernel(riqn_conv_geom g, const float* __restrict__ dcol, 
   }
 }
 
-// Same scatter with coalesced reads: one block per (sample, chunk of CC input channels) streams that sample's dcol rows
-// (the CC*KH*KW gradients of a row are contiguous) and accumulates into a shared-memory image tile, written out once.
-__global__ void col2im_tile_kernel(riqn_conv_geom g, int CC, const float* __restrict__ dcol, float* __restrict__ din) {
-  extern __shared__ float acc[];     // CC * H * W
-  const int K = g.Cin * g.KH * g.KW, khw = g.KH * g.KW, ohw = g.OH * g.OW, hw = g.H * g.W;
-  const int chunks = g.Cin / CC;
-  const long b = blockIdx.x / chunks;
-  const int c0 = (blockIdx.x % chunks) * CC;
-  for (int i = threadIdx.x; i < CC * hw; i += blockDim.x) acc[i] = 0.f;
-  __syncthreads();
-  const int per_row = CC * khw;
-  const float* base = dcol + b * ohw * (long)K + (long)c0 * khw;
-  for (int e = threadIdx.x; e < ohw * per_row; e += blockDim.x) {
-    const int m = e / per_row, j = e - m * per_row;
-    const int c = j / khw, r = j - c * khw;
-    const int kh = r / g.KW, kw = r - kh * g.KW;
-    const int oh = m / g.OW, ow = m - oh * g.OW;
-    const int ih = oh * g.stride + kh - g.pad, iw = ow * g.stride + kw - g.pad;
-    if (ih >= 0 && ih < g.H && iw >= 0 && iw < g.W) atomicAdd(&acc[c * hw + ih * g.W + iw], base[(long)m * K + j]);
-  }
-  __syncthreads();
-  float* out = din + (b * g.Cin + c0) * hw;
-  for (int i = threadIdx.x; i < CC * hw; i += blockDim.x) out[i] = acc[i];
-}
-
 static int col2im(const riqn_conv_geom* g, const float* dcol, float* din, cudaStream_t s) {
-  const int hw = g->H * g->W;
-  int CC = g->Cin;
-  while (CC > 1 && ((long)CC * hw * 4 > 16 * 1024 || g->Cin % CC)) --CC;
-  if ((long)CC * hw * 4 <= 48 * 1024) {
-    col2im_tile_kernel<<<g->B * (g->Cin / CC), 256, (size_t)CC * hw * 4, s>>>(*g, CC, dcol, din);
-  } else {
-    long total = (long)g->B * g->Cin * hw;
-    long blocks = (total + 255) / 256;
-    col2im_kernel<<<(int)(blocks > 32L * riqn_sms() ? 32L * riqn_sms() : blocks), 256, 0, s>>>(*g, dcol, din);
-  }
+  const long blocks = ((long)g->B * g->Cin * g->H * g->W + 255) / 256;
+  col2im_kernel<<<(int)(blocks > 32L * riqn_sms() ? 32L * riqn_sms() : blocks), 256, 0, s>>>(*g, dcol, din);
   return (int)cudaGetLastError();
 }
 
@@ -489,7 +456,7 @@ RIQN_API int riqn_im2col_f32(const riqn_conv_geom* g, const void* in, int in_is_
 
 RIQN_API int riqn_conv_bwd(const riqn_conv_geom* g, const float* dout, const float* out, const float* col,
                            const float* w, float* dY, float* dcol, float* dw, float* dbias, float* din, void* stream) {
-  riqn::note_launches(din ? 5 : 3);
+  riqn::note_launches(din ? 6 : 4);
   cudaStream_t s = (cudaStream_t)stream;
   const long M = (long)g->B * g->OH * g->OW;
   const int K = g->Cin * g->KH * g->KW;
@@ -499,13 +466,13 @@ RIQN_API int riqn_conv_bwd(const riqn_conv_geom* g, const float* dout, const flo
   int rc = colsum_add(M, g->Cout, dY, dbias, s);
   if (rc) return rc;
   // dW[c, k] += sum_m dY[m, c] * col[m, k]
-  EpiArgs e;
   const int tiles = ((g->Cout + 127) / 128) * ((K + 127) / 128);
   int split = (2 * riqn_sms() + tiles - 1) / tiles;
   if ((long)split * 64 > M) split = (int)((M + 63) / 64);
-  rc = gemm_f32(g->Cout, K, (int)M, dY, 1, g->Cout, col, 1, K, dw, K, EPI_ATOMIC, e, split, s);
+  rc = gemm_f32_add(g->Cout, K, (int)M, dY, 1, g->Cout, col, 1, K, dw, split, s);
   if (rc) return rc;
   if (din) {
+    EpiArgs e;
     // dcol[m, k] = sum_c dY[m, c] * W[c, k]
     rc = gemm_f32((int)M, K, g->Cout, dY, g->Cout, 1, w, 1, K, dcol, K, EPI_STORE, e, 1, s);
     if (rc) return rc;
@@ -737,12 +704,12 @@ RIQN_API int riqn_conv_bwd_strip(const riqn_conv_geom* g, const float* dout, con
 RIQN_API int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const float* out, const void* colT_hi,
                               const void* wT_hi, void* dY_hi, void* dYT_hi, float* dcol, float* dw, float* dbias, float* din,
                               float wgrad_scale, void* stream) {
-  riqn::note_launches(din ? 4 : 2);
+  riqn::note_launches(din ? 5 : 3);
   cudaStream_t s = (cudaStream_t)stream;
   const long M = (long)g->B * g->OH * g->OW;
   const int K = g->Cin * g->KH * g->KW;
   const int ohw = g->OH * g->OW;
-  if (M % 8 || g->Cout % 8) return (int)cudaErrorInvalidValue;
+  if (M % 8 || g->Cout % 8 || (din && !dcol)) return (int)cudaErrorInvalidValue;
   const long tiles = (M + 63) / 64;
   const int slots = g->Cout <= 64 ? (int)(tiles < 4L * riqn_sms() ? tiles : 4L * riqn_sms()) : (int)((M + 256 * 8 - 1) / (256 * 8));
   StreamScratch dbias_part;
@@ -766,24 +733,12 @@ RIQN_API int riqn_conv_bwd_tc(const riqn_conv_geom* g, const float* dout, const 
                         nullptr, nullptr, nullptr, split, s, &ex);
   if (rc) return rc;
   if (din) {
-    // dcol[m, k] = sum_c dY[m, c] * W[c, k]
-    if (g->pad == 0) {
-      // fused col2im: the accumulators are added straight into din (never materialising dcol)
-      RIQN_CUDA(cudaMemsetAsync(din, 0, sizeof(float) * (size_t)g->B * g->Cin * g->H * g->W, s));
-      TcExtra ci;
-      ci.ohw = ohw;
-      ci.ci_h = g->H; ci.ci_w = g->W; ci.ci_cin = g->Cin; ci.ci_kh = g->KH; ci.ci_kw = g->KW;
-      ci.ci_stride = g->stride; ci.ci_ow = g->OW;
-      rc = gemm_bf16_tc((int)M, K, g->Cout, (const bf16*)dY_hi, nullptr, (const bf16*)wT_hi, nullptr, din, K, TC_COL2IM,
-                        nullptr, nullptr, nullptr, 1, s, &ci);
-      if (rc) return rc;
-    } else {
-      rc = gemm_bf16_tc((int)M, K, g->Cout, (const bf16*)dY_hi, nullptr, (const bf16*)wT_hi, nullptr, dcol, K, TC_STORE,
-                        nullptr, nullptr, nullptr, 1, s, nullptr);
-      if (rc) return rc;
-      rc = col2im(g, dcol, din, s);
-      if (rc) return rc;
-    }
+    // dcol[m, k] = sum_c dY[m, c] * W[c, k], then din gathers it in a fixed order
+    rc = gemm_bf16_tc((int)M, K, g->Cout, (const bf16*)dY_hi, nullptr, (const bf16*)wT_hi, nullptr, dcol, K, TC_STORE,
+                      nullptr, nullptr, nullptr, 1, s, nullptr);
+    if (rc) return rc;
+    rc = col2im(g, dcol, din, s);
+    if (rc) return rc;
   }
   return 0;
 }

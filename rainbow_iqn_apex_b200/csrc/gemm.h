@@ -13,7 +13,6 @@ enum Epi {
   EPI_BIAS_RELU = 1,       // C = relu(acc + bias[n])
   EPI_BIAS_RELU_NCHW = 2,  // m = b*ohw + p ; C[(b*N + n)*ohw + p] = relu(acc + bias[n])
   EPI_EMBED = 3,           // C = feat[(m / batch)*N + n] * relu(acc + bias[n]), batch = rows per sample (model.py:146-151)
-  EPI_ATOMIC = 4,          // C += alpha*acc (atomicAdd; split-K capable)
   EPI_NOISY_WGRAD = 5,     // C += acc ; out2 += acc * eps[m,n]  (dL/dmu, dL/dsigma of NoisyLinear; split 1 only)
   EPI_BIAS = 6,            // C = acc + bias[n]
   EPI_SLAB = 7,            // C[z * slab + m*ldc + n] = acc of split z (split-K partials, summed by the caller in split order)
@@ -30,16 +29,19 @@ struct EpiArgs {
   long slab = 0;
 };
 
-// fp32 CUDA-core GEMM with arbitrary operand strides.  Returns a cudaError_t as int.  split_k > 1 (EPI_ATOMIC, EPI_SLAB
-// only) cuts K into gemm_f32_splits(K, split_k) chunks of gemm_f32_kchunk(K, split_k), one grid z-slice each.
+// fp32 CUDA-core GEMM with arbitrary operand strides.  Returns a cudaError_t as int.  split_k > 1 (EPI_SLAB only) cuts K
+// into gemm_f32_splits(K, split_k) chunks of gemm_f32_kchunk(K, split_k), one grid z-slice each.
 int gemm_f32_kchunk(int K, int split_k);
 int gemm_f32_splits(int K, int split_k);
 int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,
              float* C, long ldc, int epi, const EpiArgs& e, int split_k, cudaStream_t stream);
+// C (M, N row-major) += A B^T, split-K: each split an fmaf chain over its k ascending, the splits added in split order
+int gemm_f32_add(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk, float* C,
+                 int split_k, cudaStream_t stream);
 
 // ---- wgmma / TMA path (gemm_tc.cu) ---------------------------------------------------------------------------
 enum TcEpi { TC_STORE = 0, TC_BIAS_RELU = 1, TC_ATOMIC = 2, TC_NOISY_WGRAD = 3, TC_BIAS_RELU_NCHW = 4, TC_EMBED = 5,
-             TC_COL2IM = 6, TC_CONV = 7, TC_CONV_DGRAD = 8 };
+             TC_CONV = 7, TC_CONV_DGRAD = 8 };
 
 struct TcExtra {
   int ohw = 1;
@@ -47,9 +49,7 @@ struct TcExtra {
   const float* feat = nullptr;
   int batch = 1;
   __nv_bfloat16 *o_hi = nullptr, *o_lo = nullptr, *o_hiT = nullptr, *o_loT = nullptr;
-  // TC_COL2IM: row m = (b, oh, ow), column n = (c, kh, kw); C is the NCHW image gradient (pad == 0), accumulated into
-  // (ci_G > 0: rows live on the G x G strip grid, m = (b, gy, gx); only gy < ci_oh, gx < ci_ow are real)
-  int ci_h = 0, ci_w = 0, ci_cin = 0, ci_kh = 0, ci_kw = 0, ci_stride = 0, ci_ow = 0, ci_G = 0, ci_oh = 0;
+  int ci_h = 0, ci_w = 0, ci_cin = 0, ci_stride = 0;     // TC_CONV_DGRAD: the image din (see below)
   // Strip convolution (TC_CONV): A is the space-to-depth image (B*G*G rows of strip_kc*64 values); k-block kb reads rows
   // m0 + dy*G + dx (shift = kb / strip_kc = dy*strip_t + dx), columns (kb % strip_kc)*64.  Row m = (b, gy, gx) on the
   // G x G grid is a real output iff gy < cv_oh and gx < cv_ow; C is the NCHW fp32 output (relu(acc + bias)); nx_hi / nx_lo
@@ -98,7 +98,7 @@ int gemm_bf16_tc(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bflo
 //   * and the wide tiles fill the SMs (at least one per SM), or take at most half as many rounds of CTAs as the 128-wide
 //     ones (the 1024 x 3136 weight gradient: 104 wide tiles in one round against 200 narrow ones in two).
 // These are the NoisyLinear head's forward, data gradient and weight gradient.  Everything else runs 128x{128,64,32}
-// tiles: split-bf16 x3, the convolutions, the embedding, col2im, narrow outputs, split products and small products that
+// tiles: split-bf16 x3, the convolutions, the embedding, narrow outputs, split products and small products that
 // would leave SMs idle.
 //
 // Split-K over a persistent grid of one CTA per SM: every split writes its partial product to scratch and one pass adds

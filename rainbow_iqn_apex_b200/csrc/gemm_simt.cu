@@ -25,8 +25,6 @@ __device__ __forceinline__ void epi_one(float v, int m, int n, int N, float* __r
     C[((long)b * N + n) * e.ohw + p] = fmaxf(v + e.bias[n], 0.f);
   } else if (EPI == EPI_EMBED) {
     C[(long)m * ldc + n] = e.feat[(long)(m / e.batch) * N + n] * fmaxf(v + e.bias[n], 0.f);
-  } else if (EPI == EPI_ATOMIC) {
-    atomicAdd(&C[(long)m * ldc + n], e.alpha * v);
   } else if (EPI == EPI_NOISY_WGRAD) {        // split 1 only: one block owns the element
     C[(long)m * ldc + n] += v;
     e.out2[(long)m * ldc + n] += __fmul_rn(v, e.eps[(long)m * ldc + n]);
@@ -179,18 +177,34 @@ int gemm_f32_splits(int K, int split_k) {
 int gemm_f32(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk,
              float* C, long ldc, int epi, const EpiArgs& e, int split_k, cudaStream_t s) {
   if (M <= 0 || N <= 0) return 0;
-  if (split_k > 1 && epi != EPI_ATOMIC && epi != EPI_SLAB) return (int)cudaErrorInvalidValue;
+  if (split_k > 1 && epi != EPI_SLAB) return (int)cudaErrorInvalidValue;
   switch (epi) {
     case EPI_STORE: return launch_epi<EPI_STORE>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_BIAS: return launch_epi<EPI_BIAS>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_BIAS_RELU: return launch_epi<EPI_BIAS_RELU>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_BIAS_RELU_NCHW: return launch_epi<EPI_BIAS_RELU_NCHW>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_EMBED: return launch_epi<EPI_EMBED>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
-    case EPI_ATOMIC: return launch_epi<EPI_ATOMIC>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_NOISY_WGRAD: return launch_epi<EPI_NOISY_WGRAD>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
     case EPI_SLAB: return launch_epi<EPI_SLAB>(M, N, K, A, sAm, sAk, B, sBn, sBk, C, ldc, e, split_k, s);
   }
   return (int)cudaErrorInvalidValue;
+}
+
+// C (M, N row-major) += A B^T with K cut as gemm_f32_kchunk does: every split stores its partial product in its own slab
+// of stream scratch (EPI_SLAB) and sum_slots_add adds the slabs in split order onto C, so the sum does not depend on
+// which split finishes first.  Two launches.
+int gemm_f32_add(int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBn, long sBk, float* C,
+                 int split_k, cudaStream_t s) {
+  if (M <= 0 || N <= 0) return 0;
+  const long n = (long)M * N;
+  const int splits = gemm_f32_splits(K, split_k);
+  StreamScratch part;
+  RIQN_CUDA(part.alloc((size_t)splits * n, s));
+  EpiArgs e;
+  e.slab = n;
+  const int rc = gemm_f32(M, N, K, A, sAm, sAk, B, sBn, sBk, part.p, N, EPI_SLAB, e, split_k, s);
+  if (rc) return rc;
+  return sum_slots_add(splits, (int)n, part.p, C, s);
 }
 
 }  // namespace riqn

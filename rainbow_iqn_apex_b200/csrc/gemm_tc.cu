@@ -395,7 +395,7 @@ struct alignas(64) TcArgs {
   float alpha;           // TC_ATOMIC: scale applied to the accumulator
   int vec_acc;           // TC_ATOMIC / TC_NOISY_WGRAD: C (out2, eps) rows are 16-byte aligned -> vectorised accumulate
   int ohw;               // TC_BIAS_RELU_NCHW: m = b*ohw + p -> C[(b*N + n)*ohw + p]
-  int ci_h, ci_w, ci_cin, ci_kh, ci_kw, ci_stride, ci_ow, ci_G, ci_oh;   // TC_COL2IM geometry (pad == 0)
+  int ci_h, ci_w, ci_cin, ci_stride;   // TC_CONV_DGRAD: the NCHW image din
   const float* feat;     // TC_EMBED: (samples, N) conv features, row m uses feat[m / batch] (batch = rows per sample)
   int batch;
   bf16 *o_hi, *o_lo;     // TC_EMBED: bf16 hi / lo images of the result, row-major (M, N)   (may be null)
@@ -800,7 +800,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 #pragma unroll
           for (int j = 0; j < 32; ++j)
             if (n0 + j < p.N) cb[(long)j * p.ohw] = fmaxf(__uint_as_float(v[j]) + p.bias[n0 + j], 0.f);
-        } else if (EPI == TC_COL2IM || EPI == TC_CONV || EPI == TC_CONV_DGRAD) {
+        } else if (EPI == TC_CONV || EPI == TC_CONV_DGRAD) {
           // handled below with the whole warp
         } else if (!(p.vec_acc && n0 + 32 <= p.N)) {
           float* crow = p.C + (long)m * p.ldc + n0;
@@ -861,31 +861,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 #pragma unroll
           for (int i = 0; i < 8; ++i)
             if (orow[i] >= 0 && dstb != nullptr) *reinterpret_cast<uint4*>(dstb + orow[i] + (piece & 3) * 8) = pc[i];
-        }
-      }
-      if (EPI == TC_COL2IM && n0 < p.N) {
-        // din[b, c, oh*s + kh, ow*s + kw] += dcol[m, (c, kh, kw)]: lane j decodes column n0 + j once, the offsets are
-        // broadcast by shuffle; lanes = consecutive output pixels, so one red instruction touches a few lines
-        const int khw = p.ci_kh * p.ci_kw;
-        const int kcol = n0 + lane;
-        int coff = -1;
-        if (kcol < p.N) {
-          const int c = kcol / khw, r = kcol - c * khw;
-          const int kh = r / p.ci_kw, kw = r - kh * p.ci_kw;
-          coff = (c * p.ci_h + kh) * p.ci_w + kw;
-        }
-        bool row_ok = m < p.M;
-        const int mm = row_ok ? m : 0;
-        const int b = mm / p.ohw, pp = mm - b * p.ohw;                 // ohw = G*G on the strip grid
-        const int rw = p.ci_G ? p.ci_G : p.ci_ow;
-        const int oh = pp / rw, ow = pp - oh * rw;
-        if (p.ci_G) row_ok = row_ok && oh < p.ci_oh && ow < p.ci_ow;   // grid rows beyond the real outputs carry zeros
-        float* base = p.C + ((long)b * p.ci_cin * p.ci_h + oh * p.ci_stride) * p.ci_w + ow * p.ci_stride;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int off = __shfl_sync(0xffffffffu, coff, j);
-          if (row_ok && off >= 0)
-            asm volatile("red.global.add.f32 [%0], %1;" ::"l"(base + off), "f"(__uint_as_float(v[j])) : "memory");
         }
       }
       if (EPI == TC_CONV_DGRAD && n0 < p.N) {
@@ -1141,14 +1116,11 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
   p.vec_acc = (ldc % 4 == 0) && (reinterpret_cast<uintptr_t>(C) & 15) == 0 && (reinterpret_cast<uintptr_t>(out2) & 15) == 0 &&
               (reinterpret_cast<uintptr_t>(eps) & 15) == 0;
   p.ohw = ex ? ex->ohw : 1; p.feat = ex ? ex->feat : nullptr; p.batch = ex ? ex->batch : 1;
-  p.ci_h = ex ? ex->ci_h : 0; p.ci_w = ex ? ex->ci_w : 0; p.ci_cin = ex ? ex->ci_cin : 0; p.ci_kh = ex ? ex->ci_kh : 0;
-  p.ci_kw = ex ? ex->ci_kw : 0; p.ci_stride = ex ? ex->ci_stride : 0; p.ci_ow = ex ? ex->ci_ow : 0;
-  p.ci_G = ex ? ex->ci_G : 0; p.ci_oh = ex ? ex->ci_oh : 0;
+  p.ci_h = ex ? ex->ci_h : 0; p.ci_w = ex ? ex->ci_w : 0; p.ci_cin = ex ? ex->ci_cin : 0; p.ci_stride = ex ? ex->ci_stride : 0;
   p.strip_t = ex ? ex->strip_t : 0; p.strip_G = ex ? ex->strip_G : 0; p.strip_kc = ex ? ex->strip_kc : 0;
   p.cv_oh = ex ? ex->cv_oh : 0; p.cv_ow = ex ? ex->cv_ow : 0; p.nx_s = ex ? ex->nx_s : 0; p.nx_G = ex ? ex->nx_G : 0;
   p.nx_hi = ex ? ex->nx_hi : nullptr; p.nx_lo = ex ? ex->nx_lo : nullptr;
   p.mn_major = mn ? ex->mn_major : 0; p.wg_t = ex ? ex->wg_t : 0; p.wg_G = ex ? ex->wg_G : 0; p.wg_kc = ex ? ex->wg_kc : 0;
-  if (epi == TC_COL2IM && (ex == nullptr || p.ci_kh * p.ci_kw * p.ci_cin != N || split3 || split2)) return (int)cudaErrorInvalidValue;
   p.o_hi = ex ? ex->o_hi : nullptr; p.o_lo = ex ? ex->o_lo : nullptr;
   p.o_hiT = ex ? ex->o_hiT : nullptr; p.o_loT = ex ? ex->o_loT : nullptr;
   p.fmt = ex ? ex->fmt : 0;
@@ -1214,7 +1186,6 @@ int gemm_bf16_tc(int M, int N, int K, const bf16* A_hi, const bf16* A_lo, const 
     } else {
       switch (epi) {
         case TC_STORE: RIQN_TC_NARROW(1, TC_STORE); RIQN_TC_GO(1, TC_STORE);
-        case TC_COL2IM: RIQN_TC_GO(1, TC_COL2IM);
         case TC_CONV_DGRAD:
           if (bn == 64) return launch_tc<1, TC_CONV_DGRAD, 64>(ma_hi, ma_lo, mb_hi, mb_lo, p, s);
           RIQN_TC_GO(1, TC_CONV_DGRAD);

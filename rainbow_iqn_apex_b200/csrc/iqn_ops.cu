@@ -1587,7 +1587,7 @@ RIQN_API int riqn_quantile_embed_bwd_tc(int batch, int num_quantiles, int embed_
 RIQN_API int riqn_quantile_embed_bwd(int batch, int num_quantiles, int embed_dim, int feat_dim, const float* x,
                                      const float* feat, const float* cosv, float* dx_inout, float* dfeat,
                                      float* grad_iqn_w, float* grad_iqn_b, void* stream) {
-  riqn::note_launches(3);
+  riqn::note_launches(4);
   cudaStream_t s = (cudaStream_t)stream;
   const long R = (long)batch * num_quantiles;
   embed_bwd_elem_kernel<<<riqn_cdiv((long)batch * feat_dim, 256), 256, 0, s>>>(batch, num_quantiles, feat_dim, x, feat,
@@ -1595,13 +1595,11 @@ RIQN_API int riqn_quantile_embed_bwd(int batch, int num_quantiles, int embed_dim
   RIQN_LAUNCH_CHECK();
   int rc = colsum_add(R, feat_dim, dx_inout, grad_iqn_b, s);
   if (rc) return rc;
-  EpiArgs e;
   const int tiles = (feat_dim + 127) / 128;
   int split = (3 * riqn_sms() + tiles - 1) / tiles;
   if ((long)split * 64 > R) split = (int)((R + 63) / 64);
   // dWe[f, i] += sum_r dpre[r, f] * cos[r, i]
-  return gemm_f32(feat_dim, embed_dim, (int)R, dx_inout, 1, feat_dim, cosv, 1, embed_dim, grad_iqn_w, embed_dim,
-                  EPI_ATOMIC, e, split, s);
+  return gemm_f32_add(feat_dim, embed_dim, (int)R, dx_inout, 1, feat_dim, cosv, 1, embed_dim, grad_iqn_w, split, s);
 }
 
 RIQN_API int riqn_noisy_linear_fwd(long rows, int in_features, int out_features, const float* x, const float* w_eff,
@@ -1787,15 +1785,14 @@ RIQN_API int riqn_z_wgrad(long rows, int hidden, int action_space, const float* 
                           const float* eps_b_za, float* g_mu_zv, float* g_sig_zv, float* g_bmu_zv, float* g_bsig_zv,
                           float* g_mu_za, float* g_sig_za, float* g_bmu_za, float* g_bsig_za, void* stream) {
   if (action_space < 1 || action_space > 31) return (int)cudaErrorInvalidValue;   // dwz_scratch has 32 rows
-  riqn::note_launches(3);
+  riqn::note_launches(4);
   cudaStream_t s = (cudaStream_t)stream;
   const int W = 2 * hidden;
   RIQN_CUDA(cudaMemsetAsync(dwz_scratch, 0, sizeof(float) * 32 * W, s));
   RIQN_CUDA(cudaMemsetAsync(dbz_scratch, 0, sizeof(float) * 32, s));
-  EpiArgs e;
   int split = 32;
   if ((long)split * 64 > rows) split = (int)((rows + 63) / 64);
-  int rc = gemm_f32(32, W, (int)rows, dz, 1, 32, h, 1, W, dwz_scratch, W, EPI_ATOMIC, e, split, s);
+  int rc = gemm_f32_add(32, W, (int)rows, dz, 1, 32, h, 1, W, dwz_scratch, split, s);
   if (rc) return rc;
   rc = colsum_add(rows, 32, dz, dbz_scratch, s);
   if (rc) return rc;

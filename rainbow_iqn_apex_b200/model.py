@@ -686,15 +686,24 @@ class DQN(nn.Module):
                       x_hiT=bf(FEAT, R) if (bwd_tc and not mn) else None,
                       x_loT=bf(FEAT, R) if (bwd_tc and bwd == "bf16x3") else None,
                       cos_hi=bf(R, E), cos_lo=bf(R, E) if x3 else None, cosT_hi=None, mn=mn)
-            if need_x32:
+            if need_x32 or R % 2:
                 xt = torch.empty(R, FEAT, device=dev)
                 cosv = torch.empty(R, E, device=dev)
             elif tc["x_hiT"] is not None:                        # transposed images are split from the fp32 matrix
                 xt = torch.empty(R, FEAT, device=dev)
-            call("riqn_quantile_embed_fwd_tc", B, num_quantiles, E, FEAT, ptr(tau), ptr(feat), ptr(self._iqn_ops[0]),
-                 ptr(self._iqn_ops[1]), ptr(self.iqn_fc.bias), ptr(tc["cos_hi"]), ptr(tc["cos_lo"]), ptr(tc["cosT_hi"]),
-                 ptr(xt), ptr(tc["x_hi"]), ptr(tc["x_lo"]), ptr(tc["x_hiT"]), ptr(tc["x_loT"]), 1 if f16 else 0)
-            if need_x32:   # fp32 cos for the CUDA-core dW_e product
+            if R % 2:
+                # the tensor-core embedding takes an even row count: the fp32 embedding, and the head product's operand
+                # images split from its x (fp16 mode: x_hi = fp16(x), x_lo = bf16(x), as that embedding's epilogue writes)
+                call("riqn_quantile_embed_fwd", B, num_quantiles, E, FEAT, ptr(tau), ptr(feat), ptr(self.iqn_fc.weight),
+                     ptr(self.iqn_fc.bias), ptr(cosv), ptr(xt))
+                call("riqn_split_bf16", R, FEAT, ptr(xt), ptr(tc["x_hi"]), ptr(tc["x_lo"]), ptr(tc["x_hiT"]),
+                     ptr(tc["x_loT"]), 1 if f16 else 0)
+            else:
+                call("riqn_quantile_embed_fwd_tc", B, num_quantiles, E, FEAT, ptr(tau), ptr(feat), ptr(self._iqn_ops[0]),
+                     ptr(self._iqn_ops[1]), ptr(self.iqn_fc.bias), ptr(tc["cos_hi"]), ptr(tc["cos_lo"]),
+                     ptr(tc["cosT_hi"]), ptr(xt), ptr(tc["x_hi"]), ptr(tc["x_lo"]), ptr(tc["x_hiT"]), ptr(tc["x_loT"]),
+                     1 if f16 else 0)
+            if need_x32 and R % 2 == 0:   # fp32 cos for the CUDA-core dW_e product
                 call("riqn_quantile_embed_fwd", B, num_quantiles, E, FEAT, ptr(tau), ptr(feat), ptr(self.iqn_fc.weight),
                      ptr(self.iqn_fc.bias), ptr(cosv), ptr(xt))
             tc["h_hi"] = bf(R, 2 * hid) if (bwd_tc and R % 2 == 0) else None   # bf16 image of h for the z-layer weight gradient

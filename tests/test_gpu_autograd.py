@@ -105,7 +105,7 @@ def _relu_flips(d, x, nq, tau, acts):
 
 
 @pytest.mark.parametrize("mode", MODES)
-@pytest.mark.parametrize("batch,nq", [(32, 8), (512, 64)])
+@pytest.mark.parametrize("batch,nq", [(32, 8), (512, 64), (13, 13)])     # 13 x 13: the fp32 trunk and head backwards
 def test_iqn_dense_upstream_gradient_vs_oracle(cuda_dev, precision, batch, nq, mode):
     precision(*mode)
     params, noise, x, tau, G, q_ref, p_or, acts = _iqn_case(batch, nq)
@@ -171,7 +171,7 @@ def test_reference_iqn_loss_by_hand_matches_learner(cuda_dev):
 
 # ----------------------------------------------------------------------------------------------------------------- C51
 @pytest.mark.parametrize("log", [True, False])
-@pytest.mark.parametrize("batch", [32, 512])
+@pytest.mark.parametrize("batch", [32, 512, 13])                        # 13: the fp32 trunk backward
 def test_c51_dense_upstream_gradient_vs_oracle(cuda_dev, batch, log):
     seed = 77 + batch
     params, noise = net.make_params(seed, rainbow_only=True), net.make_noise(seed + 1, rainbow_only=True)

@@ -9,15 +9,15 @@ Method (as tests/test_gpu_c51_kernels.py):
   hi + lo).  Input rounding is never part of a comparison;
 * exact regime: small-integer pixels, activations and output gradients and weights that are small integers times a
   power of two keep every product and partial sum exact in fp32 (the generators assert that every sum stays below
-  2^24 of its finest grid), so the kernel has to match float64 bit for bit, also where float atomics add in any order
-  (riqn_conv_bwd, the col2im of riqn_conv_bwd_tc).  A second exact case puts a non-zero lo image on one operand, so the
+  2^24 of its finest grid), so the kernel has to match float64 bit for bit in any summation order.  A second exact case puts a non-zero lo image on one operand, so the
   hi.lo and lo.hi products are checked bit for bit too;
 * random regime: each element is held to c * K * 2^-24 * sum|a_i b_i| (K = the reduction length) plus the output
   rounding; each test prints its worst err/bound ratio;
 * outputs that are one rounding (dYg, dY_hi / dYT_hi, the next layer's block images, every im2col image, the fp32 dY,
   riqn_split_bf16_scaled) are bitwise in both regimes;
 * overwritten outputs start as NaN, accumulated outputs (dw, dbias) from a non-zero pattern, every buffer carries
-  canaries past its end, entry points without float atomics are called twice at B = 512 and must agree bit for bit,
+  canaries past its end, entry points are called twice in the random regime and must agree bit for bit (no float
+  atomic takes part in any sum; tests/test_gpu_fallback_paths.py pins the order of the fp32 and col2im sums),
   and every documented rejection returns cudaErrorInvalidValue and writes nothing.
 """
 import zlib
@@ -615,8 +615,8 @@ BWD_TC = {"conv2": (32, 20, 64, 4, 2, 0), "conv3": (64, 9, 64, 3, 1, 0), "cout96
 @pytest.mark.parametrize("name", list(BWD_TC))
 def test_conv_bwd_tc(cuda_dev, name, B, regime):
     """dY_hi / dYT_hi bitwise; dw (split over every SM, added in split order) and dbias accumulated from a prefill;
-    din bitwise in the exact regime (float atomics, exact sums) and bounded in the random one.  A second call without
-    din writes the same dYT_hi, dw and dbias and leaves dY_hi alone."""
+    din (dcol gathered in a fixed order) bitwise in the exact regime and bounded in the random one, where a second call
+    is bitwise the first.  A call without din writes the same dYT_hi, dw and dbias and leaves dY_hi alone."""
     dev = cuda_dev
     cin, h, cout, k, s, pad = BWD_TC[name]
     oh = out_size(h, k, s, pad)
@@ -669,6 +669,9 @@ def test_conv_bwd_tc(cuda_dev, name, B, regime):
         check_bound(f"dw {tag}", o["dw"].f32(), dw_ref, C_BOUND * (M + 2) * U * (S_mag.ravel() + np.abs(pre_w)))
         check_bound(f"dbias {tag}", o["db"].f32(), db_ref, C_BOUND * (M + 2) * U * db_mag)
         check_bound(f"din {tag}", din, din_ref, C_BOUND * (cout + k * k) * U * din_mag)
+        again = run(True)
+        for key in o:
+            assert_bits(f"second call {key}", again[key].bits(), o[key].bits())
     o2 = run(False)
     assert torch.isnan(o2["dY"].t[:o2["dY"].n].float()).all(), "dY_hi written without din"
     for key in ("dYT", "dw", "db"):
@@ -689,6 +692,9 @@ def test_conv_bwd_tc_rejections(cuda_dev):
     bufs = [v.t for v in o.values()]
     _expect_rejected("riqn_conv_bwd_tc", args(geom(1, 64, 9, 64, 3, 1, 0)), bufs)     # M = 49, M % 8
     _expect_rejected("riqn_conv_bwd_tc", args(geom(8, 64, 9, 60, 3, 1, 0)), bufs)     # Cout % 8
+    no_dcol = list(args(geom(8, 64, 9, 64, 3, 1, 0)))
+    no_dcol[7] = None
+    _expect_rejected("riqn_conv_bwd_tc", tuple(no_dcol), bufs)                       # din without dcol
     assert_canaries(o)
 
 
@@ -703,8 +709,8 @@ F32_CASES = [(n, B, r) for n in F32_GEOMS for B in (1, 3, 8, 512) for r in ("exa
 @pytest.mark.parametrize("name,B,regime", F32_CASES, ids=[f"{n}-B{b}-{r}" for n, b, r in F32_CASES])
 def test_conv_fp32(cuda_dev, name, B, regime):
     """riqn_im2col_f32 and riqn_conv_fwd's col: bitwise (a gather and a correctly rounded /255); riqn_conv_fwd's out;
-    riqn_conv_bwd's dY bitwise, dbias / dw accumulated (float atomics: bitwise in the exact regime), din through
-    col2im"""
+    riqn_conv_bwd's dY bitwise, dbias / dw accumulated (bitwise in the exact regime), din through col2im; in the random
+    regime a second backward call is bitwise the first"""
     dev = cuda_dev
     cin, h, cout, k, s, pad = F32_GEOMS[name]
     oh = out_size(h, k, s, pad)
@@ -745,13 +751,18 @@ def test_conv_fp32(cuda_dev, name, B, regime):
     dout, out = grads(rs, (B, cout, oh, oh), regime)
     dy = masked(dout, out)
     pre_w, pre_b = prefills(cout * K, regime, rs), prefills(cout, regime, rs)
-    o = {"dY": Out(M * cout, dev), "dcol": Out(M * K, dev), "dw": Out(cout * K, dev, fill=pre_w),
-         "db": Out(cout, dev, fill=pre_b), "din": Out(B * cin * h * h, dev)}
     doutd, outd = to_dev(dout, dev), to_dev(out, dev)
-    lib_call("riqn_conv_bwd", g, dptr(doutd), dptr(outd), col.p, dptr(wd), o["dY"].p, o["dcol"].p, o["dw"].p, o["db"].p,
-             o["din"].p)
-    torch.cuda.synchronize()
-    assert_canaries(o)
+
+    def bwd():
+        o = {"dY": Out(M * cout, dev), "dcol": Out(M * K, dev), "dw": Out(cout * K, dev, fill=pre_w),
+             "db": Out(cout, dev, fill=pre_b), "din": Out(B * cin * h * h, dev)}
+        lib_call("riqn_conv_bwd", g, dptr(doutd), dptr(outd), col.p, dptr(wd), o["dY"].p, o["dcol"].p, o["dw"].p,
+                 o["db"].p, o["din"].p)
+        torch.cuda.synchronize()
+        assert_canaries(o)
+        return o
+
+    o = bwd()
     assert_bits(f"dY {tag}", o["dY"].bits(), f32_bits(dy.transpose(0, 2, 3, 1)).ravel())
     dw_ref = pre_w.astype(np.float64) + wgrad64(x, dy, w.shape, s, pad).ravel()
     dw_mag = np.abs(pre_w) + wgrad64(np.abs(x), np.abs(dy), w.shape, s, pad).ravel()
@@ -770,6 +781,9 @@ def test_conv_fp32(cuda_dev, name, B, regime):
         check_bound(f"dw {tag}", o["dw"].f32(), dw_ref, C_BOUND * (M + 2) * U * dw_mag)
         check_bound(f"dbias {tag}", o["db"].f32(), db_ref, C_BOUND * (M + 2) * U * db_mag)
         check_bound(f"din {tag}", din, din_ref, C_BOUND * (cout + k * k) * U * din_mag)
+        again = bwd()
+        for key in o:
+            assert_bits(f"second call {key}", again[key].bits(), o[key].bits())
 
 
 # ---------------------------------------------------------------------------------------------- 7. small helpers
